@@ -2,7 +2,7 @@
 
 ``codings.build(name, **kw)`` resolves the launcher's ``--code`` flag:
 ``sgd``/``dense``/``lossless`` (dense pass-through), ``svd`` (spectral ATOMO),
-``entrywise`` (entry-wise ATOMO), ``qsgd``, ``terngrad``, ``qsvd``, ``bsvd`` (block-spectral: the estimator of the sm_100a bf16 engine).
+``entrywise`` (entry-wise ATOMO), ``qsgd``, ``terngrad``, ``qsvd``, ``bsvd`` (block-spectral: the estimator of the sm_90a bf16 engine).
 """
 from .coding import Coding, available, build, register
 from . import utils, sampling

@@ -1,6 +1,6 @@
 """Block-spectral ATOMO (``--code bsvd``): the estimator of the overlapped bf16 engine, in plain PyTorch.
 
-The reference SVD-codes every tensor whole (``/root/reference/src/codings/svd.py:79-118``).  The sm_100a engine
+The reference SVD-codes every tensor whole (``/root/reference/src/codings/svd.py:79-118``).  The sm_90a engine
 (``csrc/v2_encode.cu``) never forms an SVD of a wide matrix: it splits a tensor into *units* whose small side has at
 most 64 columns and diagonalises each unit's Gram matrix with an in-kernel Jacobi solver —
 
@@ -60,7 +60,7 @@ class BlockSVD(Coding):
     def __init__(self, rank: int = 3, random_sample: bool = True, prob_rule: str = "reference",
                  scheme: str = "bernoulli", block_cols: int = 32, generator: Optional[torch.Generator] = None,
                  allocation: str = "per_block", *args, **kwargs):
-        """``allocation="per_block"`` is what the sm_100a engine does today (every block samples with its own budget
+        """``allocation="per_block"`` is what the sm_90a engine does today (every block samples with its own budget
         ``ceil(rank / blocks)``).  ``"global"`` treats the atoms of ALL blocks of a tensor as one atom set with
         ``p_i = min(1, rank * sigma_i / sum_all sigma)`` — ATOMO's optimal allocation for this decomposition, ``rank``
         expected atoms per tensor instead of per block; still unbiased (any probabilities are).  It needs one number

@@ -21,7 +21,7 @@ probability ``frac``; the reference rounds up with ``1-frac``), the level never
 overflows into the sign bits, and buckets need not divide the tensor (the tail
 bucket is zero-padded).  The code is a flat dict of tensors
 (``words`` int64 ``[B, L]``, ``norms`` fp32 ``[B]``) — the same layout the
-sm_100a kernel (``csrc/qsgd_kernels.cu``) writes into PS peer memory.
+sm_90a kernel (``csrc/qsgd_kernels.cu``) writes into PS peer memory.
 """
 from __future__ import annotations
 

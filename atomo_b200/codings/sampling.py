@@ -24,7 +24,7 @@ Two sampling schemes:
   probabilities and a single ``u ~ U[0,1)``.  Marginal inclusion probability is
   exactly ``p_i`` (so the estimator stays unbiased) and the number of kept
   atoms is ``floor``/``ceil`` of ``sum p`` — *fixed-length messages*, which is
-  what lets the B200 path use static peer-memory slots and CUDA graphs.
+  what lets the H100 path use static peer-memory slots and CUDA graphs.
 """
 from __future__ import annotations
 
@@ -91,7 +91,7 @@ def sample_atoms(
     """Return the (sorted) indices of the kept atoms.
 
     ``allow_empty=True`` accepts a draw that keeps nothing (the unbiased choice: the reference's redraw-until-
-    non-empty, svd.py:65-66, over-weights small budgets; the sm_100a engine does not redraw either).
+    non-empty, svd.py:65-66, over-weights small budgets; the sm_90a engine does not redraw either).
 
     ``uniforms`` (same length as ``probs`` for bernoulli, length >= 1 for
     systematic) overrides the RNG — the CUDA kernels accept the same override

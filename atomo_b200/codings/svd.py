@@ -16,7 +16,7 @@ matricized as ``(n, 1)`` instead of crashing, tensors stay ``torch.Tensor``
 are selectable (``sampling.py``).  This per-tensor class is the oracle and the
 gloo/NCCL-path coder (it runs ``torch.linalg.svd`` on whatever device the
 gradient lives on); the fused engine encodes ALL layers at once with the
-sm_100a kernels of ``csrc/svd_kernels.cu`` and is tested against this class.
+sm_90a kernels of ``csrc/svd_kernels.cu`` and is tested against this class.
 """
 from __future__ import annotations
 
@@ -74,7 +74,7 @@ def gram_basis(mat32: torch.Tensor):
 def thin_svd(mat32: torch.Tensor, gram_route: bool = True):
     """``(u, s, vT)`` of a 2-D fp32 matrix.  Tall-skinny (or short-fat) matrices — every convolution under the
     reference's matricization has 18..98 columns and 10^3..10^5 rows — go through the Gram matrix of the small side,
-    exactly like the sm_100a kernels: ``V`` = eigenvectors of ``A^T A``, ``sigma_i = ||A v_i||`` measured on the
+    exactly like the sm_90a kernels: ``V`` = eigenvectors of ``A^T A``, ``sigma_i = ||A v_i||`` measured on the
     product itself, ``u_i = A v_i / sigma_i``.  Two streaming passes over the matrix instead of LAPACK's
     bidiagonalisation (131072 x 18 on 4 CPU threads: 16 ms instead of 28 ms).  ``u_i sigma_i`` is ``A v_i`` by
     construction and ``V`` is a complete orthonormal basis, so the atoms reproduce the matrix exactly even where fp32

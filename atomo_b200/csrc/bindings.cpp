@@ -54,13 +54,14 @@ void atomo_launch_param_bcast(const float* src, float* const* params_peer, float
                               int self_rank, long long numel, cudaStream_t stream);
 void atomo_launch_set_flags(int* const* flag_peer, int nranks, int value, cudaStream_t stream);
 // bn_kernels.cu
-void atomo_launch_bn_forward(const void* x, const void* res, void* y, long long R, int C, float* acc,
+long long atomo_bn_partial_floats(long long R, int C);
+void atomo_launch_bn_forward(const void* x, const void* res, void* y, long long R, int C, float* acc, float* part,
                              const float* gamma, const float* beta, float* save_mean, float* save_invstd,
                              float* running_mean, float* running_var, float eps, float momentum, int relu,
-                             int zero_acc, cudaStream_t stream);
+                             cudaStream_t stream);
 void atomo_launch_bn_backward(const void* dy, const void* x, const void* y, void* dx, void* dres, long long R, int C,
-                              const float* mean, const float* invstd, const float* gamma, float* acc, float* dgamma,
-                              float* dbeta, int relu, int zero_acc, cudaStream_t stream);
+                              const float* mean, const float* invstd, const float* gamma, float* acc, float* part,
+                              float* dgamma, float* dbeta, int relu, cudaStream_t stream);
 // v2_encode.cu / v2_ps.cu (overlapped, sharded bf16 engine)
 int atomo_v2_unit_bytes();
 int atomo_v2_ctrl_bytes();
@@ -201,33 +202,36 @@ void check_nhwc_bf16(const torch::Tensor& t, const char* name) {
 void bn_forward(const torch::Tensor& x, c10::optional<torch::Tensor> res, torch::Tensor y, torch::Tensor acc,
                 const torch::Tensor& gamma, const torch::Tensor& beta, torch::Tensor save_mean,
                 torch::Tensor save_invstd, c10::optional<torch::Tensor> running_mean,
-                c10::optional<torch::Tensor> running_var, double eps, double momentum, bool relu, bool zero_acc) {
+                c10::optional<torch::Tensor> running_var, double eps, double momentum, bool relu) {
   check_nhwc_bf16(x, "x");
   check_nhwc_bf16(y, "y");
   if (res.has_value()) check_nhwc_bf16(*res, "residual");
   c10::cuda::CUDAGuard guard(x.device());
   const long long R = x.numel() / x.size(1);
+  // per-CTA partial sums (stream-ordered caching allocator: also valid inside a CUDA-graph capture)
+  auto part = torch::empty({atomo_bn_partial_floats(R, (int)x.size(1))}, acc.options());
   atomo_launch_bn_forward(x.data_ptr(), res.has_value() ? res->data_ptr() : nullptr, y.data_ptr(), R, (int)x.size(1),
-                          acc.data_ptr<float>(), gamma.data_ptr<float>(), beta.data_ptr<float>(),
+                          acc.data_ptr<float>(), part.data_ptr<float>(), gamma.data_ptr<float>(), beta.data_ptr<float>(),
                           save_mean.data_ptr<float>(), save_invstd.data_ptr<float>(),
                           running_mean.has_value() ? running_mean->data_ptr<float>() : nullptr,
                           running_var.has_value() ? running_var->data_ptr<float>() : nullptr, (float)eps,
-                          (float)momentum, relu ? 1 : 0, zero_acc ? 1 : 0, cur_stream());
+                          (float)momentum, relu ? 1 : 0, cur_stream());
 }
 
 void bn_backward(const torch::Tensor& dy, const torch::Tensor& x, const torch::Tensor& y, torch::Tensor dx,
                  c10::optional<torch::Tensor> dres, const torch::Tensor& mean, const torch::Tensor& invstd,
-                 const torch::Tensor& gamma, torch::Tensor acc, torch::Tensor dgamma, torch::Tensor dbeta, bool relu,
-                 bool zero_acc) {
+                 const torch::Tensor& gamma, torch::Tensor acc, torch::Tensor dgamma, torch::Tensor dbeta, bool relu) {
   check_nhwc_bf16(dy, "dy");
   check_nhwc_bf16(x, "x");
   check_nhwc_bf16(dx, "dx");
   c10::cuda::CUDAGuard guard(x.device());
   const long long R = x.numel() / x.size(1);
+  auto part = torch::empty({atomo_bn_partial_floats(R, (int)x.size(1))}, acc.options());
   atomo_launch_bn_backward(dy.data_ptr(), x.data_ptr(), y.data_ptr(), dx.data_ptr(),
                            dres.has_value() ? dres->data_ptr() : nullptr, R, (int)x.size(1), mean.data_ptr<float>(),
                            invstd.data_ptr<float>(), gamma.data_ptr<float>(), acc.data_ptr<float>(),
-                           dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), relu ? 1 : 0, zero_acc ? 1 : 0, cur_stream());
+                           part.data_ptr<float>(), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), relu ? 1 : 0,
+                           cur_stream());
 }
 
 void skinny_gemm(const torch::Tensor& tiles, int ntiles, torch::Tensor ctrl, int grid) {
@@ -382,7 +386,7 @@ void v2_bcast_bytes(uint64_t src, uint64_t peer, uint64_t mc, int nranks, int se
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "atomo_b200 native runtime: symmetric NVLink heap + sm_100a gradient-coding kernels";
+  m.doc() = "atomo_b200 native runtime: symmetric NVLink heap + sm_90a gradient-coding kernels";
   // heap
   m.def("heap_last_error", []() { return std::string(atomo_heap_last_error()); });
   m.def("heap_multicast_supported", &atomo_heap_multicast_supported);

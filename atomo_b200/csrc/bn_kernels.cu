@@ -1,8 +1,8 @@
-// Fused training-mode BatchNorm (+ residual add) (+ ReLU) for NHWC bf16 activations (sm_100a).
+// Fused training-mode BatchNorm (+ residual add) (+ ReLU) for NHWC bf16 activations (sm_90a).
 //
-// ResNet-18 on 32x32 inputs is memory/latency bound on B200: the stock path spends ~35% of the
+// ResNet-18 on 32x32 inputs is memory/latency bound: the stock path spends a large share of the
 // step in batch_norm_collect_statistics / transform_input / backward_reduce / backward_elemt plus
-// separate add and ReLU kernels (profiles/step_kernels_*).  Here the whole
+// separate add and ReLU kernels.  Here the whole
 //      y = relu( gamma * (x - mean) / sqrt(var + eps) + beta  [+ residual] )
 // is two passes over x (statistics, then normalise+add+ReLU in one sweep) and the backward is two
 // passes (per-channel reductions of dy*mask and dy*mask*xhat, then dx [+ d_residual] in one sweep).
@@ -39,10 +39,14 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
   return v;
 }
 
+// The per-channel reductions are deterministic: every reduction CTA writes its partial sums to its own row of
+// `part` ([gridDim.x][2C], no atomics) and bn_sum_partials_kernel adds the rows in a fixed order, so a step
+// computes the same bits on every run.
+
 // ---- pass 1 (forward): per-channel sum and sum of squares -------------------------------------------
-// acc layout: [0..C) sum, [C..2C) sumsq   (zeroed by the launcher)
+// part row layout: [0..C) sum, [C..2C) sumsq
 __global__ void __launch_bounds__(BN_THREADS)
-bn_stats_kernel(const uint4* __restrict__ x, long long R, int C, float* __restrict__ acc) {
+bn_stats_kernel(const uint4* __restrict__ x, long long R, int C, float* __restrict__ part) {
   extern __shared__ float red[];  // [RL][C] x 2
   const int CG = C >> 3;
   const int RL = BN_THREADS / CG;
@@ -83,8 +87,8 @@ bn_stats_kernel(const uint4* __restrict__ x, long long R, int C, float* __restri
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float a = 0.f, b = 0.f;
     for (int k = 0; k < RL; ++k) { a += red[k * C + c]; b += red[RL * C + k * C + c]; }
-    atomicAdd(acc + c, a);
-    atomicAdd(acc + C + c, b);
+    part[(long long)blockIdx.x * 2 * C + c] = a;
+    part[(long long)blockIdx.x * 2 * C + C + c] = b;
   }
 }
 
@@ -141,7 +145,7 @@ bn_apply_kernel(const uint4* __restrict__ x, const uint4* __restrict__ res, uint
 __global__ void __launch_bounds__(BN_THREADS)
 bn_bwd_reduce_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, const uint4* __restrict__ y,
                      long long R, int C, const float* __restrict__ mean, const float* __restrict__ invstd,
-                     float* __restrict__ acc, int relu) {
+                     float* __restrict__ part, int relu) {
   extern __shared__ float red[];
   const int CG = C >> 3;
   const int RL = BN_THREADS / CG;
@@ -198,8 +202,8 @@ bn_bwd_reduce_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, 
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float a = 0.f, b = 0.f;
     for (int k = 0; k < RL; ++k) { a += red[k * C + c]; b += red[RL * C + k * C + c]; }
-    atomicAdd(acc + c, a);
-    atomicAdd(acc + C + c, b);
+    part[(long long)blockIdx.x * 2 * C + c] = a;
+    part[(long long)blockIdx.x * 2 * C + C + c] = b;
   }
 }
 
@@ -246,11 +250,34 @@ bn_bwd_apply_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, c
   }
 }
 
+// acc[col] = sum over p = 0..P-1 of part[p][col] (W = 2C columns), always in the same order: 32 columns per CTA,
+// 32 warps each summing every 32nd row (few dependent loads per thread), then the 32 warp sums in warp order
+constexpr int BN_SUM_THREADS = 1024;
+__global__ void __launch_bounds__(BN_SUM_THREADS)
+bn_sum_partials_kernel(const float* __restrict__ part, int P, int W, float* __restrict__ acc) {
+  __shared__ float red[BN_SUM_THREADS / 32][32];
+  const int lane = threadIdx.x & 31, g = threadIdx.x >> 5;
+  const int col = blockIdx.x * 32 + lane;
+  float s = 0.f;
+  if (col < W) {
+#pragma unroll 4
+    for (int p = g; p < P; p += BN_SUM_THREADS / 32) s += __ldg(part + (long long)p * W + col);
+  }
+  red[g][lane] = s;
+  __syncthreads();
+  if (g == 0 && col < W) {
+    float t = red[0][lane];
+#pragma unroll
+    for (int k = 1; k < BN_SUM_THREADS / 32; ++k) t += red[k][lane];
+    acc[col] = t;
+  }
+}
+
 extern "C" {
 
 static int bn_grid(long long work_items, int per_block) {
   long long g = (work_items + per_block - 1) / per_block;
-  if (g > 148 * 8) g = 148 * 8;
+  if (g > num_sms() * 8) g = num_sms() * 8;
   if (g < 1) g = 1;
   return (int)g;
 }
@@ -258,9 +285,9 @@ static int bn_grid(long long work_items, int per_block) {
 // launch ~2 waves of CTAs instead of 32 latency-bound ones
 static int g_bn_reduce_ctas = 0;
 static int bn_reduce_grid(long long R, int RL) {
-  // Every CTA ends with 2C global atomics, so the grid is capped at a few CTAs per SM (round 1 launched up to
-  // 1024 CTAs of one row per thread for the 2-4 MB layers: ~0.5 M atomics, slower than the 16 MB layers);
-  // the row loops keep 4-6 loads in flight per thread instead.
+  // Every CTA ends with a 2C-float partial that bn_sum_partials_kernel reads back, so the grid is capped at a few
+  // CTAs per SM (round 1 launched up to 1024 CTAs of one row per thread for the 2-4 MB layers, with global atomics:
+  // slower than the 16 MB layers); the row loops keep 4-6 loads in flight per thread instead.
   if (g_bn_reduce_ctas == 0) {
     const char* e = getenv("ATOMO_BN_REDUCE_CTAS");
     g_bn_reduce_ctas = e != nullptr ? atoi(e) : 296;
@@ -271,14 +298,24 @@ static int bn_reduce_grid(long long R, int RL) {
   return (int)(g < 1 ? 1 : g);
 }
 
-void atomo_launch_bn_forward(const void* x, const void* res, void* y, long long R, int C, float* acc,
+// floats of the `part` scratch the launchers below need for a layer of R rows x C channels
+long long atomo_bn_partial_floats(long long R, int C) {
+  return (long long)bn_reduce_grid(R, BN_THREADS / (C / 8)) * 2 * C;
+}
+
+static void bn_sum_partials(const float* part, int P, int C, float* acc, cudaStream_t stream) {
+  bn_sum_partials_kernel<<<(2 * C + 31) / 32, BN_SUM_THREADS, 0, stream>>>(part, P, 2 * C, acc);
+}
+
+// acc (2C floats) is overwritten with the layer's sums; part holds atomo_bn_partial_floats(R, C) floats
+void atomo_launch_bn_forward(const void* x, const void* res, void* y, long long R, int C, float* acc, float* part,
                              const float* gamma, const float* beta, float* save_mean, float* save_invstd,
                              float* running_mean, float* running_var, float eps, float momentum, int relu,
-                             int zero_acc, cudaStream_t stream) {
+                             cudaStream_t stream) {
   const int CG = C / 8, RL = BN_THREADS / CG;
-  if (zero_acc) cudaMemsetAsync(acc, 0, sizeof(float) * 2 * C, stream);
   const int g1 = bn_reduce_grid(R, RL);
-  bn_stats_kernel<<<g1, BN_THREADS, 2 * RL * C * sizeof(float), stream>>>((const uint4*)x, R, C, acc);
+  bn_stats_kernel<<<g1, BN_THREADS, 2 * RL * C * sizeof(float), stream>>>((const uint4*)x, R, C, part);
+  bn_sum_partials(part, g1, C, acc, stream);
   const int g2 = bn_grid(R * CG, BN_THREADS * 2);
   bn_apply_kernel<<<g2, BN_THREADS, 2 * C * sizeof(float), stream>>>((const uint4*)x, (const uint4*)res, (uint4*)y, R,
                                                                      C, acc, gamma, beta, save_mean, save_invstd,
@@ -286,14 +323,14 @@ void atomo_launch_bn_forward(const void* x, const void* res, void* y, long long 
 }
 
 void atomo_launch_bn_backward(const void* dy, const void* x, const void* y, void* dx, void* dres, long long R, int C,
-                              const float* mean, const float* invstd, const float* gamma, float* acc, float* dgamma,
-                              float* dbeta, int relu, int zero_acc, cudaStream_t stream) {
+                              const float* mean, const float* invstd, const float* gamma, float* acc, float* part,
+                              float* dgamma, float* dbeta, int relu, cudaStream_t stream) {
   const int CG = C / 8, RL = BN_THREADS / CG;
-  if (zero_acc) cudaMemsetAsync(acc, 0, sizeof(float) * 2 * C, stream);
   const int g1 = bn_reduce_grid(R, RL);
   bn_bwd_reduce_kernel<<<g1, BN_THREADS, 2 * RL * C * sizeof(float), stream>>>((const uint4*)dy, (const uint4*)x,
                                                                                (const uint4*)y, R, C, mean, invstd,
-                                                                               acc, relu);
+                                                                               part, relu);
+  bn_sum_partials(part, g1, C, acc, stream);
   const int g2 = bn_grid(R * CG, BN_THREADS * 2);
   bn_bwd_apply_kernel<<<g2, BN_THREADS, 5 * C * sizeof(float), stream>>>((const uint4*)dy, (const uint4*)x,
                                                                          (const uint4*)y, (uint4*)dx, (uint4*)dres, R,

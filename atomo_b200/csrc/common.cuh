@@ -1,4 +1,4 @@
-// Shared device helpers for the atomo_b200 sm_100a kernels.
+// Shared device helpers for the atomo_b200 sm_90a kernels.
 //
 // * system-scope acquire/release accessors used for cross-GPU flags living in
 //   NVLink peer memory (the replacement for the reference's MPI tag handshakes,
@@ -12,6 +12,19 @@
 #include <stdint.h>
 
 namespace atomo {
+
+// SMs of the current device: the grid caps of the grid-stride launches are a few resident CTAs per SM
+// (132 on an H100 SXM).  Queried once per process; an engine process drives one device.
+inline int num_sms() {
+  static int n = 0;
+  if (n < 1) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    if (n < 1) n = 132;
+  }
+  return n;
+}
 
 // ----------------------------------------------------------------------------
 // Descriptor tables (built once on the host by runtime/engine.py, resident in HBM)

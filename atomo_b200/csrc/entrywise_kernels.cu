@@ -1,5 +1,5 @@
 // K3/K4 — entry-wise ATOMO (standard-basis atoms) fused with the worker->PS push,
-// and the PS-side scatter-add (sm_100a).
+// and the PS-side scatter-add (sm_90a).
 //
 // Reference: the scheme is the ATOMO recipe applied to the standard basis
 // (README.md:5-7; only the L1 indicator exists in code, codings/utils.py:7-8).
@@ -143,7 +143,7 @@ void atomo_launch_entrywise_encode(const float* grad, const void* layers, const 
                                    int capacity, int* local_count, int* push_flag_peer, void* ctrl,
                                    int worker_index, const float* ext_uniforms, int signal, cudaStream_t stream) {
   cudaMemsetAsync(l1, 0, sizeof(float) * nlayers, stream);
-  int grid = ntiles < 148 * 4 ? ntiles : 148 * 4;
+  int grid = ntiles < num_sms() * 4 ? ntiles : num_sms() * 4;
   if (grid < 1) grid = 1;
   entrywise_l1_kernel<<<grid, EW_THREADS, 0, stream>>>(grad, (const LayerDesc*)layers, (const TileDesc*)tiles,
                                                         ntiles, l1);
@@ -157,7 +157,7 @@ void atomo_launch_entrywise_scatter(const int* const* idx, const float* const* v
                                     void* ctrl, long long timeout_ticks, cudaStream_t stream) {
   cudaMemsetAsync(out_sum, 0, sizeof(float) * numel, stream);
   int grid = (capacity + EW_THREADS - 1) / EW_THREADS;
-  if (grid > 148 * 4) grid = 148 * 4;
+  if (grid > num_sms() * 4) grid = num_sms() * 4;
   if (grid < 1) grid = 1;
   entrywise_scatter_kernel<<<grid, EW_THREADS, 0, stream>>>(idx, val, count, W, capacity, out_sum, numel,
                                                              push_flags, (Ctrl*)ctrl, timeout_ticks);

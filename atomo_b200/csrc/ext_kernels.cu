@@ -1,9 +1,9 @@
 // Subspace-iteration route for square-ish layers (fc, 1x1 convolutions) — the part of K1 the
 // reference does with a full LAPACK SVD of e.g. a 4096 x 9216 matrix on the host (svd.py:95).
 //
-//   Y = A X          (skinny GEMM, tcgen05 — gemm_kernels.cu)        m x l
+//   Y = A X          (skinny GEMM, wgmma — gemm_kernels.cu)          m x l
 //   Q = orth(Y)      (gram + eig_sample(top-l) + project on the aux plan: Q = Y V / sigma)
-//   B = A^T Q        (skinny GEMM, tcgen05)                          n x l
+//   B = A^T Q        (skinny GEMM, wgmma)                            n x l
 //   B = Ub S Vb^T    (gram + eig_sample(ATOMO sampling) + project on the aux plan)
 //   A ~ (Q Vb) S Ub^T: this file's kernel forms U = Q Vb for the sampled atoms and stores
 //   (U, S/p, Ub^T) straight into the PS slot over NVLink.

@@ -1,4 +1,4 @@
-// K2/K7/K8/K9 — parameter-server side, one persistent kernel (sm_100a).
+// K2/K7/K8/K9 — parameter-server side, one persistent kernel (sm_90a).
 //
 // Reference pipeline (SURVEY.md 2.5 K2/K7/K8/K9, call stack 3.2): MPI waitany over
 // P x (W-1) pickles -> np.dot(np.dot(u, diag(s)), vT) per (layer, worker)
@@ -438,7 +438,7 @@ void atomo_launch_param_bcast(const float* src, float* const* params_peer, float
                               int self_rank, long long numel, cudaStream_t stream) {
   const long long n4 = numel / 4;
   int grid = (int)((n4 + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > num_sms() * 8) grid = num_sms() * 8;
   if (grid < 1) grid = 1;
   param_bcast_kernel<<<grid, 256, 0, stream>>>(src, params_peer, params_mc, nranks, self_rank, n4);
 }

@@ -1,5 +1,5 @@
 // K5/K6 — QSGD / TernGrad quantize + bit-pack fused with the worker->PS push,
-// and the PS-side unpack + aggregate (sm_100a).
+// and the PS-side unpack + aggregate (sm_90a).
 //
 // Reference (SURVEY.md 2.5 K5/K6): numpy encode with a Python loop over the
 // floor(64/(2+q)) sections (codings/qsgd.py:19-87), or ~15 separate torch CUDA
@@ -157,7 +157,7 @@ void atomo_launch_qsgd_encode(const float* grad, long long numel, int bucket, in
                               const void* ctrl, int worker_index, const float* ext_uniforms, cudaStream_t stream) {
   const long long nb = (numel + bucket - 1) / bucket;
   long long grid = (nb + Q_WARPS - 1) / Q_WARPS;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > num_sms() * 8) grid = num_sms() * 8;
   if (grid < 1) grid = 1;
   qsgd_encode_kernel<<<(int)grid, Q_WARPS * 32, 0, stream>>>(grad, numel, bucket, q, terngrad, clip_ptr, words_out,
                                                               norms_out, (const Ctrl*)ctrl, worker_index,
@@ -169,7 +169,7 @@ void atomo_launch_qsgd_decode_sum(const unsigned long long* const* words, const 
                                   const int* push_flags, void* ctrl, long long timeout_ticks, cudaStream_t stream) {
   const long long nb = (numel + bucket - 1) / bucket;
   long long grid = (nb + Q_WARPS - 1) / Q_WARPS;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > num_sms() * 8) grid = num_sms() * 8;
   if (grid < 1) grid = 1;
   qsgd_decode_sum_kernel<<<(int)grid, Q_WARPS * 32, 0, stream>>>(words, norms, W, numel, bucket, q, terngrad,
                                                                   out_sum, nb, push_flags, (Ctrl*)ctrl,

@@ -1,4 +1,4 @@
-// K1 — spectral-ATOMO encode fused with the worker->PS push (sm_100a).
+// K1 — spectral-ATOMO encode fused with the worker->PS push (sm_90a).
 //
 // Reference pipeline (SURVEY.md 2.5 K1): per tensor, host LAPACK SVD
 // (codings/svd.py:95) -> Python Bernoulli loop (svd.py:49-67) -> pickle ->

@@ -1,5 +1,5 @@
 // Worker side of the overlapped engine: spectral-ATOMO encode of ONE backward group, fused with the push
-// into the parameter-server owners' HBM over NVLink (sm_100a).
+// into the parameter-server owners' HBM over NVLink (sm_90a).
 //
 // Reference pipeline per tensor (SURVEY.md 2.5 K1): D2H copy -> numpy LAPACK SVD (codings/svd.py:95) ->
 // Python Bernoulli loop (svd.py:49-67) -> pickle -> MPI isend (distributed_worker.py:313-335), strictly after
@@ -149,15 +149,18 @@ __device__ void mat_gram(const __nv_bfloat16* gb, const Unit2& u, int r0, int nr
     }
   __syncthreads();
   const int nb = npad >> 2, NB = nb * nb;
-  const int RG = max(1, (int)blockDim.x / NB);
+  // RG row groups; their partial blocks are added into `red` one group after the other (not with atomics), so the
+  // Gram matrix has the same bits on every run
+  const int RG = min(16, max(1, (int)blockDim.x / NB));
   const int blk = tid % NB, grp = tid / NB;
   const int bi = blk / nb, bj = blk - bi * nb;
-  if (grp < RG && bi <= bj) {
-    float acc[4][4];
+  const bool active = grp < RG && bi <= bj;
+  float acc[4][4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i)
+  for (int i = 0; i < 4; ++i)
 #pragma unroll
-      for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+  if (active) {
     for (int r = grp; r < nr; r += RG) {
       const float4 a = *reinterpret_cast<const float4*>(&smf[r * npad + 4 * bi]);
       const float4 b = *reinterpret_cast<const float4*>(&smf[r * npad + 4 * bj]);
@@ -167,13 +170,18 @@ __device__ void mat_gram(const __nv_bfloat16* gb, const Unit2& u, int r0, int nr
 #pragma unroll
         for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
     }
+  }
+  for (int g = 0; g < RG; ++g) {
+    if (active && grp == g) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i)
+      for (int i = 0; i < 4; ++i)
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int r = 4 * bi + i, c = 4 * bj + j;
-        if (r <= c && c < n) atomicAdd(&red[r * npad + c], acc[i][j]);
-      }
+        for (int j = 0; j < 4; ++j) {
+          const int r = 4 * bi + i, c = 4 * bj + j;
+          if (r <= c && c < n) red[r * npad + c] += acc[i][j];
+        }
+    }
+    __syncthreads();
   }
 }
 

@@ -1,4 +1,4 @@
-// Parameter-server side of the overlapped / sharded engine (sm_100a): one launch per backward group and owner.
+// Parameter-server side of the overlapped / sharded engine (sm_90a): one launch per backward group and owner.
 //
 // Reference (SURVEY.md 2.5 K2/K7/K8/K9): rank 0 alone waits for P x (W-1) pickles, decodes each with two
 // np.dot calls (codings/svd.py:173), accumulates in float64, steps the optimizer (optim/sgd.py:57-90,
@@ -560,7 +560,7 @@ void atomo_v2_launch_bcast_bytes(const void* src, void* const* peer, void* mc, i
                                  cudaStream_t stream) {
   const long long n16 = nbytes / 16;
   int grid = (int)((n16 + 255) / 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > num_sms() * 8) grid = num_sms() * 8;
   if (grid < 1) grid = 1;
   v2_bcast_bytes_kernel<<<grid, 256, 0, stream>>>((const uint4*)src, (uint4* const*)peer, (uint4*)mc, nranks, self, n16);
 }

@@ -9,7 +9,7 @@ A residual block is described by a tuple of ``(kernel, channels, stride)`` conv 
 parameter names (``conv1, bn1, ..., shortcut.0, shortcut.1``, ``layer1..4``, ``linear``) and therefore the
 ``parameters()`` order match the reference, so the per-tensor coders see the same 62 tensors for ResNet-18.
 Every normalisation layer is a :class:`~atomo_b200.ops.fused_bn.BNAct`: BN + residual add + ReLU is one call
-(and one fused sm_100a kernel pair when enabled).
+(and one fused sm_90a kernel pair when enabled).
 """
 from typing import Sequence, Tuple
 

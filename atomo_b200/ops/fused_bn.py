@@ -25,13 +25,12 @@ class _FusedBNFn(torch.autograd.Function):
         C = _load()
         y = torch.empty_like(x, memory_format=torch.channels_last)
         nch = x.size(1)
-        # acc_* are slices of a per-model arena the engine zeroes ONCE per step; without an arena
-        # (stand-alone use) each call zeroes its own scratch
+        # acc_* are slices of a per-model arena (the kernels overwrite them with the layer's sums); without an
+        # arena (stand-alone use) each call uses its own scratch
         acc = acc_fwd if acc_fwd is not None else torch.empty(2 * nch, dtype=torch.float32, device=x.device)
         mean = torch.empty(nch, dtype=torch.float32, device=x.device)
         invstd = torch.empty(nch, dtype=torch.float32, device=x.device)
-        C.bn_forward(x, residual, y, acc, weight, bias, mean, invstd, running_mean, running_var, eps, momentum, relu,
-                     acc_fwd is None)
+        C.bn_forward(x, residual, y, acc, weight, bias, mean, invstd, running_mean, running_var, eps, momentum, relu)
         ctx.save_for_backward(x, y, weight, mean, invstd)
         ctx.relu = relu
         ctx.has_res = residual is not None
@@ -53,11 +52,11 @@ class _FusedBNFn(torch.autograd.Function):
             # the engine owns the gradient buffers: dgamma / dbeta are written in place by the kernel and autograd
             # sees no gradient for weight / bias (no AccumulateGrad add kernels for the 2 x #BN vectors)
             dgamma, dbeta = ctx.grad_sink
-            C.bn_backward(dy, x, y, dx, dres, mean, invstd, weight, acc, dgamma, dbeta, ctx.relu, ctx.acc_bwd is None)
+            C.bn_backward(dy, x, y, dx, dres, mean, invstd, weight, acc, dgamma, dbeta, ctx.relu)
             return dx, None, None, None, None, dres, None, None, None, None, None, None
         dgamma = torch.empty(nch, dtype=torch.float32, device=x.device)
         dbeta = torch.empty(nch, dtype=torch.float32, device=x.device)
-        C.bn_backward(dy, x, y, dx, dres, mean, invstd, weight, acc, dgamma, dbeta, ctx.relu, ctx.acc_bwd is None)
+        C.bn_backward(dy, x, y, dx, dres, mean, invstd, weight, acc, dgamma, dbeta, ctx.relu)
         return dx, dgamma, dbeta, None, None, dres, None, None, None, None, None, None
 
 
@@ -97,8 +96,8 @@ def enable_fused_bn(module: nn.Module, enabled: bool = True, arena_device=None):
     """Switch every ``BNAct`` of ``module`` to the fused kernels.
 
     Returns ``(count, arena)``.  With ``arena_device`` one fp32 scratch tensor holds the per-channel
-    reduction accumulators of every layer (forward and backward halves); the caller must zero it once
-    per training step *before* the forward pass (one memset instead of two per layer).
+    reduction accumulators of every layer (forward and backward halves); the kernels overwrite a layer's
+    slice with its sums, so it needs no zeroing.
     """
     mods = [m for m in module.modules() if isinstance(m, BNAct)]
     arena = None

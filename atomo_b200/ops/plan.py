@@ -1,4 +1,4 @@
-"""Host-side planning for the grouped sm_100a kernels.
+"""Host-side planning for the grouped sm_90a kernels.
 
 Turns a model's parameter list into the descriptor tables the kernels walk
 (``csrc/common.cuh``: ``LayerDesc``, ``TileDesc``, ``Ctrl``) and the slot layout
@@ -15,7 +15,7 @@ Routing (what the reference does per tensor vs. what is sent here):
 * 1-D tensors (BN, biases; rank <= 2) travel dense: coding them costs more
   bytes than the tensor itself (SURVEY.md 2.4, consequence 2);
 * square-ish layers (fc, 1x1 convs) -> ``ROUTE_LOWRANK_EXT`` when ``subspace``
-  is on: randomized range finder of width ``sketch`` on the tcgen05 skinny
+  is on: randomized range finder of width ``sketch`` on the wgmma skinny
   GEMMs, then the same Gram/Jacobi machinery on auxiliary plans (``ExtPlan``);
   otherwise dense.
 """

@@ -1,4 +1,4 @@
-"""Fused B200 engine: the whole PS training step on NVLink peer memory.
+"""Fused H100 engine: the whole PS training step on NVLink peer memory.
 
 Where the reference runs (SURVEY.md 3.2/3.3) ``Bcast(float64) x P -> fwd/bwd ->
 host SVD x P -> pickle -> isend x P -> waitany -> np.dot decode -> SGD`` with
@@ -255,15 +255,16 @@ class FusedEngine:
             Q = self.aux_y["arena"][qo:qo + l.rows * sk].view(l.rows, sk)
             self.ext_views.append((A, Xt, Y, B, Q))
         if self.gemm_impl == "auto":
-            self.gemm_impl = "tcgen05"
-        if self.gemm_impl == "tcgen05":
+            self.gemm_impl = "wgmma"
+        if self.gemm_impl == "wgmma":
             self._setup_gemm_tiles()
 
     def _setup_gemm_tiles(self):
-        """Tile tables of the grouped tcgen05 skinny GEMMs (csrc/gemm_kernels.cu: struct GemmTile)."""
+        """Tile tables of the grouped wgmma skinny GEMMs (csrc/gemm_kernels.cu: struct GemmTile)."""
         import struct
         assert self.C.gemm_tile_bytes() == 72
         gp = self.flat_grads.data_ptr()
+        sm = torch.cuda.get_device_properties(self.device).multi_processor_count
 
         def vec_mode(base_elems, sa_i, sa_k):
             if sa_k == 1 and sa_i % 4 == 0 and base_elems % 4 == 0:
@@ -277,8 +278,8 @@ class FusedEngine:
                                atomic)
 
         def ksplits(ntiles, K):
-            """split the reduction so that a handful of output tiles still fills the 148 SMs"""
-            want = -(-296 // max(ntiles, 1))
+            """split the reduction so that a handful of output tiles still fills every SM (two CTAs each)"""
+            want = -(-2 * sm // max(ntiles, 1))
             return max(1, min(want, K // 128))
 
         layers = self.plan.ext.layers
@@ -319,7 +320,7 @@ class FusedEngine:
         self.ext_b_all = self.ext_scratch[ext.b_range[0]:ext.b_range[1]]
 
     def _gemm_fwd(self, from_b: bool = False):
-        if self.gemm_impl == "tcgen05":
+        if self.gemm_impl == "wgmma":
             if self.gemm_fwd_atomic:
                 self.ext_y_all.zero_()   # split-K partial sums are accumulated with atomics
             self.C.skinny_gemm(self.t_gemm_fwd_b if from_b else self.t_gemm_fwd_x, self.n_fwd_tiles, self.ctrl,
@@ -330,7 +331,7 @@ class FusedEngine:
         return 0
 
     def _gemm_bwd(self):
-        if self.gemm_impl == "tcgen05":
+        if self.gemm_impl == "wgmma":
             if self.gemm_bwd_atomic:
                 self.ext_b_all.zero_()
             self.C.skinny_gemm(self.t_gemm_bwd, self.n_bwd_tiles, self.ctrl, self.gemm_grid)
@@ -356,14 +357,14 @@ class FusedEngine:
         n = 0
         xr = ext.xt_range
         self.ext_scratch[xr[0]:xr[1]].normal_()          # fresh Gaussian test matrices X for every layer
-        n += self._gemm_fwd()                            # Y = A X            (tcgen05 skinny GEMM)
+        n += self._gemm_fwd()                            # Y = A X            (wgmma skinny GEMM)
         sk = ext.layers[0].sketch
         n += self._aux_factorize(self.aux_y, sk, False, 0)       # Q = orth(Y)
         for _ in range(self.power_iters):                # optional power iterations: Y = A (A^T Q)
             n += self._gemm_bwd()
             n += self._gemm_fwd(from_b=True)
             n += self._aux_factorize(self.aux_y, sk, False, 0)
-        n += self._gemm_bwd()                            # B = A^T Q          (tcgen05 skinny GEMM)
+        n += self._gemm_bwd()                            # B = A^T Q          (wgmma skinny GEMM)
         n += self._aux_factorize(self.aux_b, self.svd_rank, self.random_sample, self.worker_index)
         self.C.ext_finalize(self.t_ext_descs, self.t_fin_tiles, len(ext.fin_tiles), self.aux_y["arena"],
                             self.aux_b["arena"], self.heap.region_ptr("arena", 0), self.plan.arena_floats,

@@ -4,7 +4,7 @@ The reference moves every parameter tensor separately (P broadcasts, P sends
 per step).  Here all parameters of a model live in ONE contiguous fp32 buffer
 (each tensor 128-byte aligned) and ``nn.Parameter.data`` / ``.grad`` are views
 into it, so a broadcast is one transfer, the PS update is one kernel, and on
-the B200 path the buffer can sit in the symmetric NVLink heap with zero copies.
+the H100 path the buffer can sit in the symmetric NVLink heap with zero copies.
 """
 from __future__ import annotations
 

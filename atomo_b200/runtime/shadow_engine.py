@@ -1,4 +1,4 @@
-"""Overlapped, sharded bf16 engine — the B200 headline path (``--backend p2p`` with ``--dtype bf16``).
+"""Overlapped, sharded bf16 engine — the H100 headline path (``--backend p2p`` with ``--dtype bf16``).
 
 Differences against ``runtime/engine.py`` (round 1: fp32 flat parameters, encode after the whole backward,
 one central PS kernel at the end of the step):

@@ -1,6 +1,6 @@
 """Launcher flag surface (parity: ``add_fit_args``,
 ``/root/reference/src/distributed_nn.py:31-82`` — every flag of SURVEY.md 2.7 is
-kept with its default) plus the B200-specific additions."""
+kept with its default) plus the H100-specific additions."""
 from __future__ import annotations
 
 import argparse
@@ -29,7 +29,7 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
     p.add_argument("--log-interval", type=int, default=10, metavar="N")
     p.add_argument("--network", type=str, default="LeNet", metavar="N")
     p.add_argument("--code", type=str, default="sgd",
-                   help="sgd | svd | qsgd | terngrad | entrywise | qsvd | bsvd (block-spectral: the estimator the sm_100a "
+                   help="sgd | svd | qsgd | terngrad | entrywise | qsvd | bsvd (block-spectral: the estimator the sm_90a "
                         "bf16 engine applies under --code svd, as a plain PyTorch coder)")
     p.add_argument("--bucket-size", type=int, default=512)
     p.add_argument("--dataset", type=str, default="MNIST", metavar="N")

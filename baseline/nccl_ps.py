@@ -5,7 +5,7 @@ pip-installable, default coder module missing — DESIGN.md), so BASELINE.md nam
 this as the bar: the same synchronous-PS protocol and the same per-tensor
 spectral-ATOMO coder, with MPI replaced by NCCL and LAPACK by
 ``torch.linalg.svd`` (cuSOLVER) on the GPU — i.e. what a straightforward port of
-``sync_replicas_master_nn.py`` / ``distributed_worker.py`` gives on a B200 box:
+``sync_replicas_master_nn.py`` / ``distributed_worker.py`` gives on an H100 box:
 
   rank 0 = dedicated PS (like the reference), ranks 1..N-1 = workers;
   per step: ``dist.broadcast`` of the flat fp32 parameters -> eager fp32
@@ -14,7 +14,7 @@ spectral-ATOMO coder, with MPI replaced by NCCL and LAPACK by
   decodes ``(u*s)@vT`` per (layer, worker), averages, ``optim.SGD.step``.
 
 With one GPU the PS and the single worker share the device (no communication).
-None of the sm_100a kernels, the symmetric heap or CUDA graphs are used here.
+None of the sm_90a kernels, the symmetric heap or CUDA graphs are used here.
 """
 from __future__ import annotations
 

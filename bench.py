@@ -12,6 +12,15 @@ sides, max over ranks).  ``e2e`` repeats the measurement through the public
 ``FusedEngine.train_step(x, y)`` API with the batch coming from pinned host
 memory every step and the loss read back to the host every step.
 
+``--dump-outputs DIR`` writes, after the timed steps, what the last step computed: ``loss.npy``
+(loss, prec@1, prec@5 as returned by ``train_step``) and ``params.npy`` (rank 0's model state after the
+step, every floating-point ``state_dict`` entry flattened in order, float32; a fixed seeded sample when it
+exceeds 64 MB).  Inputs, initial weights and coder seeds are fixed, so two builds run with the same
+arguments can be compared output for output: the step is bitwise reproducible (cuDNN runs deterministic,
+heuristically chosen algorithms and the project's kernels reduce in a fixed order).  ``--cudnn-benchmark``
+lets cuDNN autotune instead, which can pick different algorithms, and so different last bits (and, through
+the coder's Bernoulli draws, different atoms), from run to run.
+
 ``--impl reference`` reports the reference arm (not installable here: Python-2 /
 mpi4py / missing module — see DESIGN.md); ``--impl nccl-baseline`` runs the
 reference *algorithm* re-hosted on torch.distributed/NCCL + torch.linalg.svd
@@ -39,7 +48,7 @@ def metric_name(args):
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--steps", type=int, default=50, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", type=str, default="atomo_b200", choices=["atomo_b200", "reference", "nccl-baseline"])
     ap.add_argument("--network", type=str, default="ResNet18")
@@ -69,16 +78,40 @@ def parse():
     ap.add_argument("--sampling", type=str, default="bernoulli")
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-channels-last", dest="channels_last", action="store_false", default=True,
-                    help="activations are NHWC by default (2.3x faster convs/BN on B200)")
+                    help="activations are NHWC by default (faster convs/BN than NCHW)")
     ap.add_argument("--dataset", type=str, default="Cifar10", choices=["Cifar10", "ImageNet", "MNIST"])
     ap.add_argument("--quantization-level", type=int, default=4)
     ap.add_argument("--entry-budget", type=float, default=0.05)
     ap.add_argument("--subspace", type=str, default="auto", choices=["auto", "on", "off"])
     ap.add_argument("--fused-bn", type=str, default="auto", choices=["auto", "on", "off"])
-    ap.add_argument("--no-cudnn-benchmark", dest="cudnn_benchmark", action="store_false", default=True)
+    ap.add_argument("--cudnn-benchmark", dest="cudnn_benchmark", action="store_true", default=False,
+                    help="let cuDNN autotune its algorithms: the choice (and so the outputs) can differ from run to run")
+    ap.add_argument("--no-cudnn-benchmark", dest="cudnn_benchmark", action="store_false")
     ap.add_argument("--momentum", type=float, default=0.9)
     ap.add_argument("--lr", type=float, default=0.01)
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's outputs as DIR/<name>.npy")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    return args
+
+
+DUMP_MAX_BYTES = 64 * 2 ** 20
+
+
+def dump_outputs(out_dir, stats, model):
+    """What one train_step hands its caller: the returned stats and the model state it updated in place."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), stats.detach().float().cpu().numpy())
+    flat = torch.cat([t.detach().float().reshape(-1).cpu() for t in model.state_dict().values() if t.is_floating_point()])
+    cap = (DUMP_MAX_BYTES - 4096) // 4
+    if flat.numel() > cap:   # fixed seeded sample of the entries (same indices for the same model)
+        g = torch.Generator().manual_seed(0)
+        flat = flat[torch.randperm(flat.numel(), generator=g)[:cap].sort().values]
+    np.save(os.path.join(out_dir, "params.npy"), flat.numpy())
 
 
 class ClockSampler(threading.Thread):
@@ -167,6 +200,7 @@ def main():
 
     torch.manual_seed(0)
     torch.backends.cudnn.benchmark = args.cudnn_benchmark
+    torch.backends.cudnn.deterministic = True
     ncls = 1000 if args.dataset == "ImageNet" else 10
     model = build_model(args.network, ncls, args.dataset)
     engine = args.engine
@@ -285,6 +319,8 @@ def main():
     h2d = host_x[0].numel() * host_x[0].element_size() + host_y[0].numel() * host_y[0].element_size()
     check_error("after the end-to-end loop")
     err = 0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, stats, eng.model)
 
     if rank == 0:
         pm = eng.ps_mode
@@ -303,7 +339,7 @@ def main():
                        "coded_units": getattr(eng.plan, "n_coded", None),
                        "fused_bn_layers": eng.fused_bn_layers, "cuda_graph": not args.no_graph,
                        "heap": eng.heap.mode, "nvls_multicast": eng.heap.has_multicast,
-                       "l2": "no explicit flush: per-step working set %.0f MB > 126 MB L2" % work_mb,
+                       "l2": "no explicit flush: per-step working set %.0f MB > 50 MB L2 (H100)" % work_mb,
                        "optimizer": "%s fused in PS kernel" % ("momentum-SGD" if args.optimizer == "sgd" else "Adam"), "final_loss": round(losses[-1], 4),
                        "device_error": err},
             "clocks": clocks,

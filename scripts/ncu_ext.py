@@ -1,4 +1,4 @@
-"""Tiny driver for ncu: runs the subspace route (tcgen05 skinny GEMMs) and the fused BN kernels a few times."""
+"""Tiny driver for ncu: runs the subspace route (wgmma skinny GEMMs) and the fused BN kernels a few times."""
 import os
 import sys
 

@@ -1,12 +1,11 @@
 #!/bin/bash
-# Race / memory checks for the sm_100a kernels (run on a GPU box; SURVEY 5.2).  compute-sanitizer does not
+# Race / memory checks for the sm_90a kernels (run on a GPU box; SURVEY 5.2).  compute-sanitizer does not
 # see cross-device races: those are covered by tests/test_gpu_v2.py (replicas must stay bit-identical, protocol
 # fuzz with randomized delays) and by the step-stamped flag protocol (flags are never reset, only compared).
 #
 #   scripts/sanitize.sh [memcheck|synccheck|racecheck ...]      default: memcheck synccheck
 #
-# Notes from the round-2 runs (logs under profiles/r2/sanitizer_*.log):
-#  * memcheck + synccheck over both kernel families finish in ~6 min on one B200;
+# Notes from earlier runs:
 #  * racecheck does NOT finish within 15 min on the v2 kernels (every shared-memory access is tracked): run it on a
 #    single test (-k gram) with its own timeout, never inside a budgeted 8-GPU call;
 #  * the CUDA-graph capture test is excluded: cudaStreamBeginCapture makes the sanitizer report API errors

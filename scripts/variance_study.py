@@ -4,7 +4,7 @@ whole-tensor spectral coder?  For real gradients (one backward pass of the named
 matrix-shaped parameter, estimate the relative variance E||decode - g||^2 / ||g||^2 and the bytes on the wire of
 
   svd  r   whole-tensor SVD atoms (reference estimator, needs a full SVD of the matrix per step)
-  bsvd r   the sm_100a engine's estimator (3x3 convs whole; fc / 1x1 layers in <= 32-column blocks)
+  bsvd r   the sm_90a engine's estimator (3x3 convs whole; fc / 1x1 layers in <= 32-column blocks)
 
     python scripts/variance_study.py --network ResNet18 --rank 3 --out docs/experiments/variance_resnet18.md
 """

@@ -1,16 +1,16 @@
-"""In-tree build of the atomo_b200 native extension for sm_100a.
+"""In-tree build of the atomo_b200 native extension for sm_90a (H100).
 
     python setup.py build_ext --inplace      ->  atomo_b200/_C*.so
 
 The arch is passed as an explicit -gencode (bypassing torch's arch list);
--lineinfo keeps ncu's source page mapped to the .cu files.
+-lineinfo keeps profiler source views mapped to the .cu files.
 """
 import os
 
 from setuptools import setup
 from torch.utils.cpp_extension import BuildExtension, CUDAExtension
 
-os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
 here = os.path.dirname(os.path.abspath(__file__))
 src = os.path.join("atomo_b200", "csrc")
 sources = [os.path.join(src, f) for f in (
@@ -18,7 +18,7 @@ sources = [os.path.join(src, f) for f in (
     "entrywise_kernels.cu", "ext_kernels.cu", "gemm_kernels.cu", "bn_kernels.cu", "v2_encode.cu", "v2_ps.cu")]
 
 nvcc_flags = ["-O3", "-lineinfo", "-std=c++17", "--use_fast_math",
-              "-gencode", "arch=compute_100a,code=sm_100a"]
+              "-gencode", "arch=compute_90a,code=sm_90a"]
 
 setup(
     name="atomo_b200",

@@ -15,7 +15,7 @@ except ImportError:  # hypothesis is optional: the fuzz files skip themselves wi
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA GPU (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA GPU (run on an H100 with -m gpu)")
     config.addinivalue_line("markers", "multigpu: test needs >= 2 GPUs")
 
 

@@ -80,9 +80,9 @@ def test_clock_sampler_shape_without_a_gpu():
 
 
 def test_built_extension_is_the_profiled_one():
-    """Evidence integrity: every kernel of the built extension is instruction-identical to its committed SASS listing
-    (profiles/sass/, taken from the build that ran the GPU tests, benches and ncu captures).  Skipped when the
-    extension has not been built yet or cuobjdump is not on PATH."""
+    """Evidence integrity: every kernel of the built extension is instruction-identical to the committed SASS
+    manifest (profiles/sass/kernels.json, taken from the build that ran the GPU tests and the benchmark).  Skipped
+    when the extension has not been built yet or cuobjdump is not on PATH."""
     import glob
     import shutil
     import pytest

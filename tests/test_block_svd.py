@@ -1,4 +1,4 @@
-"""Block-spectral coder (codings/block_svd.py): the estimator of the sm_100a bf16 engine as a PyTorch oracle."""
+"""Block-spectral coder (codings/block_svd.py): the estimator of the sm_90a bf16 engine as a PyTorch oracle."""
 import pytest
 import torch
 

@@ -2,7 +2,7 @@
 """Cluster manager (parity: ``/root/reference/tools/pytorch_ec2.py``).
 
 The reference provisions EC2 spot instances with boto3 and drives them over
-paramiko (``command_map`` at pytorch_ec2.py:938-951).  A B200 deployment is a
+paramiko (``command_map`` at pytorch_ec2.py:938-951).  An H100 deployment is a
 fixed set of HGX nodes, so "provisioning" becomes inventory: the same command
 names operate on a host list (``--hosts a,b,c``, a hostfile, or ``SLURM_NODELIST``
 expanded by the scheduler) over ssh (paramiko), or on ``localhost`` directly.
