@@ -55,13 +55,12 @@ void atomo_launch_param_bcast(const float* src, float* const* params_peer, float
 void atomo_launch_set_flags(int* const* flag_peer, int nranks, int value, cudaStream_t stream);
 // bn_kernels.cu
 long long atomo_bn_partial_floats(long long R, int C);
-void atomo_launch_bn_forward(const void* x, const void* res, void* y, long long R, int C, float* acc, float* part,
-                             const float* gamma, const float* beta, float* save_mean, float* save_invstd,
-                             float* running_mean, float* running_var, float eps, float momentum, int relu,
-                             cudaStream_t stream);
-void atomo_launch_bn_backward(const void* dy, const void* x, const void* y, void* dx, void* dres, long long R, int C,
+void atomo_launch_bn_forward(const void* x, const void* res, void* y, void* mask, long long R, int C, float* acc,
+                             float* part, const float* gamma, const float* beta, float* save_mean, float* save_invstd,
+                             float* running_mean, float* running_var, float eps, float momentum, cudaStream_t stream);
+void atomo_launch_bn_backward(const void* dy, const void* x, const void* mask, void* dx, void* dres, long long R, int C,
                               const float* mean, const float* invstd, const float* gamma, float* acc, float* part,
-                              float* dgamma, float* dbeta, int relu, cudaStream_t stream);
+                              float* dgamma, float* dbeta, cudaStream_t stream);
 // v2_encode.cu / v2_ps.cu (overlapped, sharded bf16 engine)
 int atomo_v2_unit_bytes();
 int atomo_v2_ctrl_bytes();
@@ -199,39 +198,53 @@ void check_nhwc_bf16(const torch::Tensor& t, const char* name) {
   TORCH_CHECK(t.size(1) % 8 == 0 && t.size(1) <= 2048, name, ": C must be a multiple of 8 (<= 2048)");
 }
 
-void bn_forward(const torch::Tensor& x, c10::optional<torch::Tensor> res, torch::Tensor y, torch::Tensor acc,
-                const torch::Tensor& gamma, const torch::Tensor& beta, torch::Tensor save_mean,
-                torch::Tensor save_invstd, c10::optional<torch::Tensor> running_mean,
-                c10::optional<torch::Tensor> running_var, double eps, double momentum, bool relu) {
+// the ReLU mask of a fused BN layer: uint8, one byte (8 channel bits) per 8 channels of each row
+void check_relu_mask(const torch::Tensor& mask, const torch::Tensor& x) {
+  TORCH_CHECK(mask.is_cuda() && mask.scalar_type() == torch::kUInt8 && mask.is_contiguous(),
+              "mask must be a contiguous CUDA uint8 tensor");
+  TORCH_CHECK(mask.numel() == x.numel() / 8, "mask must hold numel(x) / 8 bytes");
+}
+
+// y = bn(x) [+ res]; with a mask, y is ReLU'd and the mask receives its y > 0 bits
+void bn_forward(const torch::Tensor& x, c10::optional<torch::Tensor> res, torch::Tensor y,
+                c10::optional<torch::Tensor> mask, torch::Tensor acc, const torch::Tensor& gamma,
+                const torch::Tensor& beta, torch::Tensor save_mean, torch::Tensor save_invstd,
+                c10::optional<torch::Tensor> running_mean, c10::optional<torch::Tensor> running_var, double eps,
+                double momentum) {
   check_nhwc_bf16(x, "x");
   check_nhwc_bf16(y, "y");
   if (res.has_value()) check_nhwc_bf16(*res, "residual");
+  if (mask.has_value()) check_relu_mask(*mask, x);
   c10::cuda::CUDAGuard guard(x.device());
   const long long R = x.numel() / x.size(1);
   // per-CTA partial sums (stream-ordered caching allocator: also valid inside a CUDA-graph capture)
   auto part = torch::empty({atomo_bn_partial_floats(R, (int)x.size(1))}, acc.options());
-  atomo_launch_bn_forward(x.data_ptr(), res.has_value() ? res->data_ptr() : nullptr, y.data_ptr(), R, (int)x.size(1),
-                          acc.data_ptr<float>(), part.data_ptr<float>(), gamma.data_ptr<float>(), beta.data_ptr<float>(),
+  atomo_launch_bn_forward(x.data_ptr(), res.has_value() ? res->data_ptr() : nullptr, y.data_ptr(),
+                          mask.has_value() ? mask->data_ptr() : nullptr, R, (int)x.size(1), acc.data_ptr<float>(),
+                          part.data_ptr<float>(), gamma.data_ptr<float>(), beta.data_ptr<float>(),
                           save_mean.data_ptr<float>(), save_invstd.data_ptr<float>(),
                           running_mean.has_value() ? running_mean->data_ptr<float>() : nullptr,
                           running_var.has_value() ? running_var->data_ptr<float>() : nullptr, (float)eps,
-                          (float)momentum, relu ? 1 : 0, cur_stream());
+                          (float)momentum, cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
-void bn_backward(const torch::Tensor& dy, const torch::Tensor& x, const torch::Tensor& y, torch::Tensor dx,
+// mask: the ReLU mask bn_forward wrote, or None for a layer without ReLU
+void bn_backward(const torch::Tensor& dy, const torch::Tensor& x, c10::optional<torch::Tensor> mask, torch::Tensor dx,
                  c10::optional<torch::Tensor> dres, const torch::Tensor& mean, const torch::Tensor& invstd,
-                 const torch::Tensor& gamma, torch::Tensor acc, torch::Tensor dgamma, torch::Tensor dbeta, bool relu) {
+                 const torch::Tensor& gamma, torch::Tensor acc, torch::Tensor dgamma, torch::Tensor dbeta) {
   check_nhwc_bf16(dy, "dy");
   check_nhwc_bf16(x, "x");
   check_nhwc_bf16(dx, "dx");
+  if (mask.has_value()) check_relu_mask(*mask, x);
   c10::cuda::CUDAGuard guard(x.device());
   const long long R = x.numel() / x.size(1);
   auto part = torch::empty({atomo_bn_partial_floats(R, (int)x.size(1))}, acc.options());
-  atomo_launch_bn_backward(dy.data_ptr(), x.data_ptr(), y.data_ptr(), dx.data_ptr(),
+  atomo_launch_bn_backward(dy.data_ptr(), x.data_ptr(), mask.has_value() ? mask->data_ptr() : nullptr, dx.data_ptr(),
                            dres.has_value() ? dres->data_ptr() : nullptr, R, (int)x.size(1), mean.data_ptr<float>(),
                            invstd.data_ptr<float>(), gamma.data_ptr<float>(), acc.data_ptr<float>(),
-                           part.data_ptr<float>(), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), relu ? 1 : 0,
-                           cur_stream());
+                           part.data_ptr<float>(), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 
 void skinny_gemm(const torch::Tensor& tiles, int ntiles, torch::Tensor ctrl, int grid) {

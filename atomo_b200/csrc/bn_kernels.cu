@@ -8,6 +8,15 @@
 // passes (per-channel reductions of dy*mask and dy*mask*xhat, then dx [+ d_residual] in one sweep).
 // All tensors are viewed as [R = N*H*W][C] with C % 8 == 0; every access is a 16-byte vector of
 // 8 bf16 channels; statistics are accumulated in fp32.
+//
+// With ReLU the forward also writes a 1-bit mask, uint8 [R][C/8]: bit i of byte e is (y > 0) for channel i of the
+// bf16 vector y[e] it stored, so the backward reads 1 bit per element instead of re-reading y (2 bytes).
+//
+// Each layer runs two chains of three kernels (stats -> sum_partials -> apply, bwd_reduce -> sum_partials ->
+// bwd_apply).  The second and third kernel of a chain are launched with programmatic dependent launch: their CTAs
+// are scheduled while the predecessor drains, and they wait (griddepcontrol.wait) before any global read or write,
+// so every result is the same as in plain stream order.  The first kernel of a chain follows a cuDNN kernel and
+// is launched plainly.
 #include <cuda_bf16.h>
 #include <stdlib.h>
 
@@ -38,6 +47,11 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
   for (int i = 0; i < 4; ++i) p[i] = __floats2bfloat162_rn(f[2 * i], f[2 * i + 1]);
   return v;
 }
+
+// programmatic dependent launch: wait until the previous kernel in the stream has completed and its writes are
+// visible (a no-op in a plain launch) / allow the next kernel's CTAs to be scheduled from now on
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;"); }
 
 // The per-channel reductions are deterministic: every reduction CTA writes its partial sums to its own row of
 // `part` ([gridDim.x][2C], no atomics) and bn_sum_partials_kernel adds the rows in a fixed order, so a step
@@ -83,6 +97,7 @@ bn_stats_kernel(const uint4* __restrict__ x, long long R, int C, float* __restri
       red[RL * C + rl * C + cg * 8 + i] = q[i];
     }
   }
+  pdl_launch_dependents();
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float a = 0.f, b = 0.f;
@@ -92,13 +107,15 @@ bn_stats_kernel(const uint4* __restrict__ x, long long R, int C, float* __restri
   }
 }
 
-// ---- pass 2 (forward): normalise + affine (+ residual) (+ ReLU); block 0 also finalises the statistics ----
+// ---- pass 2 (forward): normalise + affine (+ residual) (+ ReLU and its mask); block 0 also finalises the statistics
 __global__ void __launch_bounds__(BN_THREADS)
-bn_apply_kernel(const uint4* __restrict__ x, const uint4* __restrict__ res, uint4* __restrict__ y, long long R, int C,
-                const float* __restrict__ acc, const float* __restrict__ gamma, const float* __restrict__ beta,
-                float* __restrict__ save_mean, float* __restrict__ save_invstd, float* __restrict__ running_mean,
-                float* __restrict__ running_var, float eps, float momentum, int relu) {
+bn_apply_kernel(const uint4* __restrict__ x, const uint4* __restrict__ res, uint4* __restrict__ y,
+                uint8_t* __restrict__ mask, long long R, int C, const float* __restrict__ acc,
+                const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ save_mean,
+                float* __restrict__ save_invstd, float* __restrict__ running_mean, float* __restrict__ running_var,
+                float eps, float momentum, int relu) {
   extern __shared__ float tab[];  // scale[C], shift[C]
+  pdl_wait();
   const float invR = 1.f / (float)R;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     const float mean = acc[c] * invR;
@@ -137,13 +154,24 @@ bn_apply_kernel(const uint4* __restrict__ x, const uint4* __restrict__ res, uint
 #pragma unroll
       for (int i = 0; i < 8; ++i) o[i] = fmaxf(o[i], 0.f);
     }
-    y[e] = pack8(o);
+    const uint4 out = pack8(o);
+    y[e] = out;
+    if (relu) {
+      // the bits come from the stored bf16 values (a positive fp32 o can round to bf16 zero), compared exactly as
+      // the backward compared y before it read the mask
+      float yv[8];
+      unpack8(out, yv);
+      unsigned m = 0;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) m |= (yv[i] > 0.f ? 1u : 0u) << i;
+      mask[e] = (uint8_t)m;
+    }
   }
 }
 
 // ---- pass 1 (backward): per-channel sum(dy*mask) and sum(dy*mask*xhat) ------------------------------------------
 __global__ void __launch_bounds__(BN_THREADS)
-bn_bwd_reduce_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, const uint4* __restrict__ y,
+bn_bwd_reduce_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, const uint8_t* __restrict__ mask,
                      long long R, int C, const float* __restrict__ mean, const float* __restrict__ invstd,
                      float* __restrict__ part, int relu) {
   extern __shared__ float red[];
@@ -156,13 +184,14 @@ bn_bwd_reduce_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, 
   if (rl < RL) {
     const long long stride = (long long)gridDim.x * RL;
     long long r = (long long)blockIdx.x * RL + rl;
-    for (; r + stride < R; r += 2 * stride) {   // 2 rows x 3 tensors = 6 independent 16-byte loads in flight
-      uint4 dv[2], xq[2], yq[2];
+    for (; r + stride < R; r += 2 * stride) {   // 2 rows x 3 tensors = 6 independent loads in flight
+      uint4 dv[2], xq[2];
+      unsigned mq[2];
 #pragma unroll
       for (int k = 0; k < 2; ++k) {
         dv[k] = __ldg(dy + (r + k * stride) * CG + cg);
         xq[k] = __ldg(x + (r + k * stride) * CG + cg);
-        if (relu) yq[k] = __ldg(y + (r + k * stride) * CG + cg);
+        if (relu) mq[k] = __ldg(mask + (r + k * stride) * CG + cg);
       }
 #pragma unroll
       for (int k = 0; k < 2; ++k) {
@@ -170,10 +199,8 @@ bn_bwd_reduce_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, 
         unpack8(dv[k], d);
         unpack8(xq[k], xv);
         if (relu) {
-          float yv[8];
-          unpack8(yq[k], yv);
 #pragma unroll
-          for (int i = 0; i < 8; ++i) d[i] = yv[i] > 0.f ? d[i] : 0.f;
+          for (int i = 0; i < 8; ++i) d[i] = (mq[k] >> i) & 1u ? d[i] : 0.f;
         }
 #pragma unroll
         for (int i = 0; i < 8; ++i) { s[i] += d[i]; q[i] = fmaf(d[i], (xv[i] - mu[i]) * is[i], q[i]); }
@@ -184,10 +211,9 @@ bn_bwd_reduce_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, 
       unpack8(__ldg(dy + r * CG + cg), d);
       unpack8(__ldg(x + r * CG + cg), xv);
       if (relu) {
-        float yv[8];
-        unpack8(__ldg(y + r * CG + cg), yv);
+        const unsigned m = __ldg(mask + r * CG + cg);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) d[i] = yv[i] > 0.f ? d[i] : 0.f;
+        for (int i = 0; i < 8; ++i) d[i] = (m >> i) & 1u ? d[i] : 0.f;
       }
 #pragma unroll
       for (int i = 0; i < 8; ++i) { s[i] += d[i]; q[i] = fmaf(d[i], (xv[i] - mu[i]) * is[i], q[i]); }
@@ -198,6 +224,7 @@ bn_bwd_reduce_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, 
       red[RL * C + rl * C + cg * 8 + i] = q[i];
     }
   }
+  pdl_launch_dependents();
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float a = 0.f, b = 0.f;
@@ -209,11 +236,12 @@ bn_bwd_reduce_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, 
 
 // ---- pass 2 (backward): dx (and the masked dy for the residual branch); block 0 writes dgamma / dbeta ----------
 __global__ void __launch_bounds__(BN_THREADS)
-bn_bwd_apply_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, const uint4* __restrict__ y,
+bn_bwd_apply_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, const uint8_t* __restrict__ mask,
                     uint4* __restrict__ dx, uint4* __restrict__ dres, long long R, int C,
                     const float* __restrict__ mean, const float* __restrict__ invstd, const float* __restrict__ gamma,
                     const float* __restrict__ acc, float* __restrict__ dgamma, float* __restrict__ dbeta, int relu) {
   extern __shared__ float tab[];  // mean[C], invstd[C], a[C] = gamma*invstd, b[C] = sum_dy/R, c[C] = sum_dy_xhat/R
+  pdl_wait();
   const float invR = 1.f / (float)R;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     tab[c] = mean[c];
@@ -235,10 +263,9 @@ bn_bwd_apply_kernel(const uint4* __restrict__ dy, const uint4* __restrict__ x, c
     unpack8(__ldg(dy + e), d);
     unpack8(__ldg(x + e), xv);
     if (relu) {
-      float yv[8];
-      unpack8(__ldg(y + e), yv);
+      const unsigned m = __ldg(mask + e);
 #pragma unroll
-      for (int i = 0; i < 8; ++i) d[i] = yv[i] > 0.f ? d[i] : 0.f;
+      for (int i = 0; i < 8; ++i) d[i] = (m >> i) & 1u ? d[i] : 0.f;
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -259,10 +286,12 @@ bn_sum_partials_kernel(const float* __restrict__ part, int P, int W, float* __re
   const int lane = threadIdx.x & 31, g = threadIdx.x >> 5;
   const int col = blockIdx.x * 32 + lane;
   float s = 0.f;
+  pdl_wait();
   if (col < W) {
 #pragma unroll 4
     for (int p = g; p < P; p += BN_SUM_THREADS / 32) s += __ldg(part + (long long)p * W + col);
   }
+  pdl_launch_dependents();
   red[g][lane] = s;
   __syncthreads();
   if (g == 0 && col < W) {
@@ -271,6 +300,25 @@ bn_sum_partials_kernel(const float* __restrict__ part, int P, int W, float* __re
     for (int k = 1; k < BN_SUM_THREADS / 32; ++k) t += red[k][lane];
     acc[col] = t;
   }
+}
+
+// Launch with programmatic stream serialization: the grid may be scheduled while the previous kernel in the stream
+// is still running, so the kernel must call pdl_wait() before its first global read or write.  A launch error is
+// reported by cudaGetLastError(), as for a <<<>>> launch.
+template <typename... Params, typename... Args>
+static void launch_pdl(void (*kernel)(Params...), int grid, int block, size_t smem, cudaStream_t stream,
+                       Args... args) {
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(block);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  cudaLaunchKernelEx(&cfg, kernel, args...);
 }
 
 extern "C" {
@@ -304,38 +352,39 @@ long long atomo_bn_partial_floats(long long R, int C) {
 }
 
 static void bn_sum_partials(const float* part, int P, int C, float* acc, cudaStream_t stream) {
-  bn_sum_partials_kernel<<<(2 * C + 31) / 32, BN_SUM_THREADS, 0, stream>>>(part, P, 2 * C, acc);
+  launch_pdl(bn_sum_partials_kernel, (2 * C + 31) / 32, BN_SUM_THREADS, 0, stream, part, P, 2 * C, acc);
 }
 
-// acc (2C floats) is overwritten with the layer's sums; part holds atomo_bn_partial_floats(R, C) floats
-void atomo_launch_bn_forward(const void* x, const void* res, void* y, long long R, int C, float* acc, float* part,
-                             const float* gamma, const float* beta, float* save_mean, float* save_invstd,
-                             float* running_mean, float* running_var, float eps, float momentum, int relu,
-                             cudaStream_t stream) {
+// acc (2C floats) is overwritten with the layer's sums; part holds atomo_bn_partial_floats(R, C) floats.  With a mask
+// (uint8 [R][C/8]) the output is ReLU'd and the mask receives its y > 0 bits.
+void atomo_launch_bn_forward(const void* x, const void* res, void* y, void* mask, long long R, int C, float* acc,
+                             float* part, const float* gamma, const float* beta, float* save_mean, float* save_invstd,
+                             float* running_mean, float* running_var, float eps, float momentum, cudaStream_t stream) {
   const int CG = C / 8, RL = BN_THREADS / CG;
   const int g1 = bn_reduce_grid(R, RL);
   bn_stats_kernel<<<g1, BN_THREADS, 2 * RL * C * sizeof(float), stream>>>((const uint4*)x, R, C, part);
   bn_sum_partials(part, g1, C, acc, stream);
   const int g2 = bn_grid(R * CG, BN_THREADS * 2);
-  bn_apply_kernel<<<g2, BN_THREADS, 2 * C * sizeof(float), stream>>>((const uint4*)x, (const uint4*)res, (uint4*)y, R,
-                                                                     C, acc, gamma, beta, save_mean, save_invstd,
-                                                                     running_mean, running_var, eps, momentum, relu);
+  launch_pdl(bn_apply_kernel, g2, BN_THREADS, 2 * C * sizeof(float), stream, (const uint4*)x, (const uint4*)res,
+             (uint4*)y, (uint8_t*)mask, R, C, (const float*)acc, gamma, beta, save_mean, save_invstd, running_mean,
+             running_var, eps, momentum, mask != nullptr ? 1 : 0);
 }
 
-void atomo_launch_bn_backward(const void* dy, const void* x, const void* y, void* dx, void* dres, long long R, int C,
+// mask: the forward's ReLU mask, or nullptr for a layer without ReLU
+void atomo_launch_bn_backward(const void* dy, const void* x, const void* mask, void* dx, void* dres, long long R, int C,
                               const float* mean, const float* invstd, const float* gamma, float* acc, float* part,
-                              float* dgamma, float* dbeta, int relu, cudaStream_t stream) {
+                              float* dgamma, float* dbeta, cudaStream_t stream) {
   const int CG = C / 8, RL = BN_THREADS / CG;
+  const int relu = mask != nullptr ? 1 : 0;
   const int g1 = bn_reduce_grid(R, RL);
   bn_bwd_reduce_kernel<<<g1, BN_THREADS, 2 * RL * C * sizeof(float), stream>>>((const uint4*)dy, (const uint4*)x,
-                                                                               (const uint4*)y, R, C, mean, invstd,
-                                                                               part, relu);
+                                                                               (const uint8_t*)mask, R, C, mean,
+                                                                               invstd, part, relu);
   bn_sum_partials(part, g1, C, acc, stream);
   const int g2 = bn_grid(R * CG, BN_THREADS * 2);
-  bn_bwd_apply_kernel<<<g2, BN_THREADS, 5 * C * sizeof(float), stream>>>((const uint4*)dy, (const uint4*)x,
-                                                                         (const uint4*)y, (uint4*)dx, (uint4*)dres, R,
-                                                                         C, mean, invstd, gamma, acc, dgamma, dbeta,
-                                                                         relu);
+  launch_pdl(bn_bwd_apply_kernel, g2, BN_THREADS, 5 * C * sizeof(float), stream, (const uint4*)dy, (const uint4*)x,
+             (const uint8_t*)mask, (uint4*)dx, (uint4*)dres, R, C, mean, invstd, gamma, (const float*)acc, dgamma,
+             dbeta, relu);
 }
 }
 }  // namespace atomo

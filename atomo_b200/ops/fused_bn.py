@@ -30,9 +30,11 @@ class _FusedBNFn(torch.autograd.Function):
         acc = acc_fwd if acc_fwd is not None else torch.empty(2 * nch, dtype=torch.float32, device=x.device)
         mean = torch.empty(nch, dtype=torch.float32, device=x.device)
         invstd = torch.empty(nch, dtype=torch.float32, device=x.device)
-        C.bn_forward(x, residual, y, acc, weight, bias, mean, invstd, running_mean, running_var, eps, momentum, relu)
-        ctx.save_for_backward(x, y, weight, mean, invstd)
-        ctx.relu = relu
+        # with ReLU the kernel also writes y > 0 as one bit per element (a byte per 8 channels), which the backward
+        # reads instead of y
+        mask = torch.empty(x.numel() // 8, dtype=torch.uint8, device=x.device) if relu else None
+        C.bn_forward(x, residual, y, mask, acc, weight, bias, mean, invstd, running_mean, running_var, eps, momentum)
+        ctx.save_for_backward(x, mask, weight, mean, invstd)
         ctx.has_res = residual is not None
         ctx.acc_bwd = acc_bwd
         ctx.grad_sink = grad_sink
@@ -41,7 +43,7 @@ class _FusedBNFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         C = _load()
-        x, y, weight, mean, invstd = ctx.saved_tensors
+        x, mask, weight, mean, invstd = ctx.saved_tensors
         if not dy.is_contiguous(memory_format=torch.channels_last):
             dy = dy.contiguous(memory_format=torch.channels_last)
         nch = x.size(1)
@@ -52,11 +54,11 @@ class _FusedBNFn(torch.autograd.Function):
             # the engine owns the gradient buffers: dgamma / dbeta are written in place by the kernel and autograd
             # sees no gradient for weight / bias (no AccumulateGrad add kernels for the 2 x #BN vectors)
             dgamma, dbeta = ctx.grad_sink
-            C.bn_backward(dy, x, y, dx, dres, mean, invstd, weight, acc, dgamma, dbeta, ctx.relu)
+            C.bn_backward(dy, x, mask, dx, dres, mean, invstd, weight, acc, dgamma, dbeta)
             return dx, None, None, None, None, dres, None, None, None, None, None, None
         dgamma = torch.empty(nch, dtype=torch.float32, device=x.device)
         dbeta = torch.empty(nch, dtype=torch.float32, device=x.device)
-        C.bn_backward(dy, x, y, dx, dres, mean, invstd, weight, acc, dgamma, dbeta, ctx.relu)
+        C.bn_backward(dy, x, mask, dx, dres, mean, invstd, weight, acc, dgamma, dbeta)
         return dx, dgamma, dbeta, None, None, dres, None, None, None, None, None, None
 
 

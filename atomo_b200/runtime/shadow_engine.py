@@ -399,8 +399,6 @@ class ShadowEngine:
         self._nlaunch += 1
         if self.is_worker:
             self.vgrads.zero_()
-            if self.bn_arena is not None:
-                self.bn_arena.zero_()
             for p in self.w_params:
                 p.grad = None
             self._pending, self._fired = list(self.group_size), 0

@@ -56,7 +56,39 @@ def main():
     print("largest gaps between consecutive main-stream kernels:")
     for g, n1, n2 in gaps:
         print("  %6.1f us  after %s  before %s" % (g, n1, n2))
+    bn_chains(step)
     eng.close()
+
+
+def bn_chains(step):
+    """Fused-BN chains of the step (stats -> sum_partials -> apply, bwd_reduce -> sum_partials -> bwd_apply): kernel
+    time, the gaps on the two edges of each chain, and the chain's span from first start to last end.  A kernel
+    launched as a programmatic dependent can start before its predecessor ends (negative gap) and then counts its
+    wait as kernel time, so the span is the figure to compare."""
+    bn = [e for e in step if "bn_" in e.name]
+    chains, cur = {"fwd": [], "bwd": []}, None
+    for e in bn:
+        if "bn_stats_kernel" in e.name or "bn_bwd_reduce_kernel" in e.name:
+            cur = [e]
+            chains["bwd" if "bwd" in e.name else "fwd"].append(cur)
+        elif cur is not None:
+            cur.append(e)
+    print("fused BN: %d kernels, %.1f us of kernel time" % (len(bn), sum(e.device_time for e in bn)))
+    for kind, cs in chains.items():
+        cs = [c for c in cs if len(c) == 3]
+        if not cs:
+            continue
+        busy = sum(e.device_time for c in cs for e in c)
+        span = sum(c[2].time_range.end - c[0].time_range.start for c in cs)
+        g1 = [c[1].time_range.start - c[0].time_range.end for c in cs]
+        g2 = [c[2].time_range.start - c[1].time_range.end for c in cs]
+        print("  %s: %d chains, kernel time %.1f us, span %.1f us, edge gaps %.1f + %.1f us (mean %.2f / %.2f)"
+              % (kind, len(cs), busy, span, sum(g1), sum(g2), sum(g1) / len(cs), sum(g2) / len(cs)))
+        for i, c in enumerate(cs):
+            print("    %2d: span %6.1f  kernels %s  gaps %5.1f %5.1f"
+                  % (i, c[2].time_range.end - c[0].time_range.start,
+                     " ".join("%5.1f" % e.device_time for e in c),
+                     c[1].time_range.start - c[0].time_range.end, c[2].time_range.start - c[1].time_range.end))
 
 
 if __name__ == "__main__":
