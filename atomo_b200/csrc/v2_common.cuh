@@ -8,11 +8,16 @@
 namespace atomo {
 namespace v2 {
 
-enum Kind : int { KIND_SLAB = 1, KIND_MAT = 2, KIND_DENSE16 = 3, KIND_VEC = 4 };
+enum Kind : int { KIND_SLAB = 1, KIND_MAT = 2, KIND_DENSE16 = 3, KIND_VEC = 4, KIND_QSGD = 5 };
 
 // One coding unit: a conv gradient in [O][K][I] (channels_last) layout ("SLAB": row (o,ri), column (b,k) of the
 // reference's (O*I/2, 2K) matricization is X_o[k][2ri+b]), a <=64-column block of a 2-D matrix ("MAT"), or a
 // dense chunk (bf16 weight sent dense / fp32 vector).
+//
+// QSGD / TernGrad units ("QSGD", v2_qsgd.cu: one per >= 2-D weight, buckets over the physical element order) reuse
+// the fields:  K = bucket (elements), I = q (quantization level), rows = buckets, cols = L (uint64 words per
+// bucket), rs = 1 for TernGrad (0 for QSGD), cs = buckets per PS tile, ps_rows = elements per PS tile,
+// ts_index = index among the QSGD units (TernGrad clip / stats counter).
 struct Unit2 {
   long long w_off;      // element offset of the unit's base in wshadow / master / momentum (VEC: in vparams)
   long long g_off;      // element offset inside the parameter's own gradient tensor
@@ -143,6 +148,13 @@ __host__ __device__ inline long long slot2_u_off(int rcap, int cols) {
 // QSVD slots: int8 U occupies rows*rcap/4 floats (rounded to 4), then rows fp32 scales (max |u| of the row)
 __host__ __device__ inline long long slot2_scale_off(int rows, int rcap, int cols) {
   return slot2_u_off(rcap, cols) + (((long long)rows * rcap / 4 + 3) & ~3LL);
+}
+
+// QSGD slots (floats, from Unit2::slot_off inside one worker arena):
+//   int32 step stamp per PS tile [n_ps, padded to 4] | fp32 bucket norms [rows, padded to 4] | uint64 words [rows][cols]
+__host__ __device__ inline long long qsgd_norms_off(int n_ps) { return ((long long)n_ps + 3) & ~3LL; }
+__host__ __device__ inline long long qsgd_words_off(int n_ps, int rows) {
+  return qsgd_norms_off(n_ps) + (((long long)rows + 3) & ~3LL);
 }
 
 }  // namespace v2

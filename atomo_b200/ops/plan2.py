@@ -22,6 +22,9 @@ What changes against ``ops/plan.py`` (the fp32-flat plan of round 1):
 * **Owners.**  Parameter-server work is sharded: PS tile ``j`` of a group belongs to owner ``j % n_owners``;
   a worker stores the ``U`` rows of a tile into that owner's arena only.  ``n_owners == 1`` is the
   reference's centralized PS.
+* **Quantizing codes** (``code="qsgd" | "terngrad"``, see :func:`build_plan2`): every >= 2-D weight is one
+  ``QSGD`` unit whose buckets are quantized and bit-packed by the workers straight into the owners' arenas; the
+  owners decode, sum and step the optimizer in one launch per group.
 
 Pure Python (unit-testable on CPU).  Struct layouts mirror ``csrc/v2_common.cuh``.
 """
@@ -31,7 +34,7 @@ import struct
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
-KIND_SLAB, KIND_MAT, KIND_DENSE16, KIND_VEC = 1, 2, 3, 4
+KIND_SLAB, KIND_MAT, KIND_DENSE16, KIND_VEC, KIND_QSGD = 1, 2, 3, 4, 5
 RCAP_MAX = 32
 MAX_COLS = 64
 BLOCK_COLS = 32               # column-block width of MAT units (Jacobi cost ~ cols^3 sits in the encode launch)
@@ -43,6 +46,9 @@ MAX_WORKERS = 16
 MAX_GROUPS = 8
 W_ALIGN = 64                  # bf16 elements (128 B)
 V_ALIGN = 32                  # fp32 elements (128 B)
+QSGD_TILE_ELEMS = 4096        # a QSGD PS / encode tile holds max(1, 4096 // bucket) whole buckets
+QSGD_MAX_BUCKET = 1024        # one warp quantizes one bucket, staged in shared memory
+QSGD_MAX_LEVEL = 14           # (sign + 1) << q | level must fit 16 bits
 
 UNIT_FMT = "<4q20i"           # 112 bytes, mirrors struct Unit2
 TILE_FMT = "<4i"              # unit, a, b, owner
@@ -71,6 +77,26 @@ def slot_floats(rows: int, cols: int, rcap: int, ubits: int = 0) -> int:
 def slot_scale_off(rows: int, cols: int, rcap: int) -> int:
     """Float offset (inside the slot) of the per-row scales of an int8 U."""
     return slot_u_off(rcap, cols) + _round_up(rows * rcap // 4, 4)
+
+
+def qsgd_words_per_bucket(bucket: int, q: int) -> int:
+    """``L = ceil(bucket / E)`` 64-bit words per bucket, ``E = 64 // (2 + q)`` codes per word (codings/qsgd.py)."""
+    e = 64 // (2 + q)
+    return (bucket + e - 1) // e
+
+
+def qsgd_norms_off(n_ps: int) -> int:
+    """Float offset (inside a QSGD slot) of the bucket norms: after one int32 step stamp per PS tile."""
+    return _round_up(n_ps, 4)
+
+
+def qsgd_words_off(n_ps: int, buckets: int) -> int:
+    """Float offset (inside a QSGD slot) of the uint64 words (16-byte aligned)."""
+    return qsgd_norms_off(n_ps) + _round_up(buckets, 4)
+
+
+def qsgd_slot_floats(n_ps: int, buckets: int, words_per_bucket: int) -> int:
+    return _round_up(qsgd_words_off(n_ps, buckets) + 2 * buckets * words_per_bucket, 32)
 
 
 def slot_capacity(cols: int, rank: int, systematic: bool) -> int:
@@ -133,7 +159,7 @@ class Unit2:
     own0: int = 0
     ps_tile0: int = 0
     n_ps: int = 0
-    ts_index: int = -1      # index among coded units (vsel / selcount / counters)
+    ts_index: int = -1      # index among coded units (vsel / selcount / counters); QSGD: among QSGD units
     ubits: int = 0          # 0: U stored fp32; 8: QSVD, U stochastically rounded to int8 with a per-row scale
 
     def pack(self) -> bytes:
@@ -165,7 +191,7 @@ class Plan2:
     stage_total: int        # bf16 elements of the dense-16 staging region
     arena_floats: int
     gpart_floats: int
-    n_coded: int
+    n_coded: int            # units with per-unit device state (coded SLAB / MAT units, or the QSGD units)
     rank: int
     code: str
 
@@ -180,10 +206,15 @@ class Plan2:
         return sum(4 * (4 + u.rcap + u.rcap * u.cols) + (u.rows * (u.rcap + 4) if u.ubits == 8 else 4 * u.rows * u.rcap)
                    for u in self.units if u.coded)
 
+    def qsgd_bytes(self) -> int:
+        """Bytes of quantized gradient a worker pushes per step: the uint64 words and fp32 norms of every bucket
+        (the same sizes as ``codings.qsgd``'s ``words`` and ``norms``)."""
+        return sum(8 * u.rows * u.cols + 4 * u.rows for u in self.units if u.kind == KIND_QSGD)
+
     def expected_factor_bytes(self) -> float:
         """Bytes actually stored per worker and step for the expected number of atoms (U is written in groups
-        of 4 atoms)."""
-        tot = 0.0
+        of 4 atoms); for the quantizing codes the words and norms of the QSGD units."""
+        tot = float(self.qsgd_bytes())
         for u in self.units:
             if u.coded:
                 atoms = min(u.budget if u.budget > 0 else u.cols, u.cols)
@@ -192,7 +223,8 @@ class Plan2:
         return tot
 
     def dense_bytes(self) -> int:
-        return sum((2 if u.kind == KIND_DENSE16 else 4) * u.numel for u in self.units if not u.coded)
+        return sum((2 if u.kind == KIND_DENSE16 else 4) * u.numel for u in self.units
+                   if not u.coded and u.kind != KIND_QSGD)
 
 
 def default_groups(shapes: Sequence[Sequence[int]], n_groups: int) -> List[int]:
@@ -238,8 +270,39 @@ def default_groups(shapes: Sequence[Sequence[int]], n_groups: int) -> List[int]:
 
 def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 3, systematic: bool = False,
                 n_owners: int = 1, n_groups: int = 4, groups: Optional[Sequence[int]] = None,
-                block_cols: int = BLOCK_COLS, min_coded_numel: int = 256) -> Plan2:
+                block_cols: int = BLOCK_COLS, min_coded_numel: int = 256, quantization_level: int = 4,
+                bucket_size: int = 512) -> Plan2:
+    """Plan of the bf16 engine for ``code`` in ``svd | qsvd | sgd | qsgd | terngrad``.
+
+    ``qsgd`` / ``terngrad``: every >= 2-D weight (the 3-channel stem and the fc layers included) is exactly one
+    ``KIND_QSGD`` unit; there are no ``DENSE16`` units.  1-D parameters stay ``KIND_VEC`` (fp32, summed by
+    ``multimem.ld_reduce``) exactly as under ``svd`` — unlike the round-1 engine, which quantizes the BN and bias
+    vectors too.  Per tensor:
+
+    * buckets run over the PHYSICAL element order of the bf16 weight (``[O][kh][kw][I]`` for convs, the order
+      of ``wshadow`` and of the gradients); ``bucket = min(bucket_size, numel)`` exactly as
+      ``codings/qsgd.py::_bucketize``, the tail bucket is zero-padded;
+    * packing is the coder's: ``E = 64 // (2 + q)`` codes per word, section-major, ``L = ceil(bucket / E)``
+      words per bucket.  The result is the coder's estimator applied to the physical-order flat tensor: it is
+      not bit-identical to the round-1 path, which buckets the logical OIHW order;
+    * one PS tile (also one encode CTA) holds ``max(1, 4096 // bucket)`` whole buckets; tile ``j`` of a group
+      belongs to owner ``j % n_owners`` as for every other kind.  ``ps_tiles`` entries are (unit, first element,
+      element count, owner);
+    * the unit's slot in a worker arena (same offset in every owner's arena; a worker writes only the tiles that
+      owner owns) holds one int32 step stamp per PS tile, the fp32 norms of all buckets and the 16-byte aligned
+      uint64 words of all buckets (``qsgd_norms_off`` / ``qsgd_words_off``).
+
+    ``Unit2`` fields of a QSGD unit: ``K`` = bucket, ``I`` = q, ``rows`` = buckets, ``cols`` = words per bucket,
+    ``rs`` = 1 for TernGrad, ``cs`` = buckets per tile, ``ps_rows`` = elements per tile (``csrc/v2_common.cuh``).
+    """
     shapes = [tuple(int(d) for d in s) for s in shapes]
+    quant = code in ("qsgd", "terngrad")
+    if quant:
+        q, bsz = int(quantization_level), int(bucket_size)
+        if not 1 <= q <= QSGD_MAX_LEVEL:
+            raise ValueError("quantization_level must be in [1, %d]" % QSGD_MAX_LEVEL)
+        if not (32 <= bsz <= QSGD_MAX_BUCKET and bsz % 8 == 0):
+            raise ValueError("bucket_size must be a multiple of 8 in [32, %d]" % QSGD_MAX_BUCKET)
     ubits = 0
     if code == "qsvd":          # QSVD: spectral atoms with quantized left factors (README.md:141-142 of the reference)
         code, ubits = "svd", 8
@@ -273,6 +336,14 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             add(Unit2(0, KIND_VEC, p.index, -1, p.off, 0, numel=p.numel, group=p.group))
             continue
         s = p.shape
+        if quant:
+            bucket = min(bsz, p.numel)
+            nb = (p.numel + bucket - 1) // bucket
+            bpt = max(1, QSGD_TILE_ELEMS // bucket)
+            add(Unit2(0, KIND_QSGD, p.index, p.widx, p.off, 0, rows=nb, cols=qsgd_words_per_bucket(bucket, q),
+                      K=bucket, I=q, rs=1 if code == "terngrad" else 0, cs=bpt, numel=p.numel, group=p.group,
+                      ps_rows=bpt * bucket))
+            continue
         coded = code == "svd" and p.numel >= min_coded_numel
         if coded and len(s) == 4 and s[2] * s[3] > 1:
             o, i, kh, kw = s
@@ -339,8 +410,21 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             elif u.kind == KIND_DENSE16:
                 for e0 in range(0, u.numel, 8192):     # staging copy tiles
                     enc_tiles.append((u.index, e0, min(8192, u.numel - e0), 0))
+            elif u.kind == KIND_QSGD:                 # encode tiles = PS tiles (one destination owner per CTA)
+                for j, e0 in enumerate(range(0, u.numel, u.ps_rows)):
+                    enc_tiles.append((u.index, e0, min(u.ps_rows, u.numel - e0), j))
             u.n_enc = len(enc_tiles) - u.enc_tile0
-            if u.coded:
+            if u.kind == KIND_QSGD:
+                u.ts_index = n_coded
+                n_coded += 1
+                u.ps_tile0 = len(ps_by_group[g])
+                for e0 in range(0, u.numel, u.ps_rows):
+                    ps_by_group[g].append((u.index, e0, min(u.ps_rows, u.numel - e0)))
+                u.n_ps = len(ps_by_group[g]) - u.ps_tile0
+                u.own0 = u.ps_tile0 % n_owners
+                u.slot_off = slot_off
+                slot_off += qsgd_slot_floats(u.n_ps, u.rows, u.cols)
+            elif u.coded:
                 u.ts_index = n_coded
                 n_coded += 1
                 u.ubits = ubits

@@ -6,8 +6,10 @@ Counterpart of the role dispatch in ``/root/reference/src/distributed_nn.py:243-
 checkpoints in the ``model_step_<N>`` layout, and the reference's log lines with REAL per-phase numbers taken from
 device-side timers (``Comp`` / ``Encode`` / ``Comm`` on the worker line, ``Decode Cost`` / ``Gather`` on the PS line).
 
-Engine choice: ``--dtype bf16`` with ``--code svd|sgd`` runs the overlapped, sharded ``ShadowEngine``; everything
-else (fp32, qsgd / terngrad / entrywise) runs the fp32-flat ``FusedEngine``.
+Engine choice (``--engine auto``): ``--dtype bf16`` with ``--code svd|qsvd|sgd`` runs the overlapped, sharded
+``ShadowEngine``; everything else (fp32, qsgd / terngrad / entrywise) runs the fp32-flat ``FusedEngine``.
+``--engine shadow`` also runs ``--code qsgd|terngrad`` on ``ShadowEngine`` (bf16 only); ``--engine fused`` always
+picks ``FusedEngine``.
 """
 from __future__ import annotations
 
@@ -30,18 +32,33 @@ class _HostEvent:
 
 
 def _build_engine(args, model, rank, world):
-    shadow = args.dtype == "bf16" and args.code.lower() in ("svd", "qsvd", "sgd", "dense", "lossless")
+    engine = getattr(args, "engine", "auto")
+    code = args.code.lower()
+    if engine == "auto":
+        shadow = args.dtype == "bf16" and code in ("svd", "qsvd", "sgd", "dense", "lossless")
+    elif engine == "shadow":
+        if args.dtype != "bf16":
+            raise SystemExit("--engine shadow trains bf16 weights: it needs --dtype bf16 (fp32 runs on --engine fused)")
+        if code not in ("svd", "qsvd", "sgd", "dense", "lossless", "qsgd", "terngrad"):
+            raise SystemExit("--engine shadow runs --code svd|qsvd|sgd|qsgd|terngrad; --code %s runs on --engine fused"
+                             % args.code)
+        shadow = True
+    else:
+        shadow = False
     if shadow:
         from .shadow_engine import ShadowEngine
+        kw = {}
+        if code in ("qsgd", "terngrad"):
+            kw = dict(quantization_level=args.quantization_level, bucket_size=args.bucket_size)
         return ShadowEngine(model, rank, world, code=args.code, svd_rank=args.svd_rank, lr=args.lr,
                             momentum=args.momentum, weight_decay=args.weight_decay, nesterov=args.nesterov,
                             optimizer=args.optimizer, ps_mode=args.ps_mode, groups=args.groups, sampling=args.sampling,
                             prob_rule=args.prob_rule, seed=args.seed, num_aggregate=args.num_aggregate,
-                            timeout_s=args.flag_timeout), "shadow"
+                            timeout_s=args.flag_timeout, **kw), "shadow"
     from .engine import FusedEngine
     if args.optimizer != "sgd":
-        raise SystemExit("--optimizer adam on the p2p backend needs --dtype bf16 with --code svd|sgd (ShadowEngine); "
-                         "the fp32-flat engine fuses momentum-SGD only")
+        raise SystemExit("--optimizer adam on the p2p backend needs --dtype bf16 with --code svd|sgd, or --engine "
+                         "shadow with --code qsgd|terngrad (ShadowEngine); the fp32-flat engine fuses momentum-SGD only")
     ps_mode = "colocated" if args.ps_mode == "sharded" else args.ps_mode
     return FusedEngine(model, rank, world, code=args.code, svd_rank=args.svd_rank, lr=args.lr, momentum=args.momentum,
                        weight_decay=args.weight_decay, nesterov=args.nesterov, ps_mode=ps_mode,

@@ -18,6 +18,10 @@ one central PS kernel at the end of the step):
   optimizer and multicasts its shard; nobody is the serial tail.  ``'colocated'`` (rank 0 owns everything,
   all ranks train) and ``'dedicated'`` (rank 0 only serves, like the reference's rank 0) keep the centralized
   topology of ``src/sync_replicas_master_nn.py``.
+* **Quantizing codes** (``code="qsgd" | "terngrad"``): every weight tensor is one QSGD unit of the plan; its
+  buckets are quantized and bit-packed by the workers during backward straight into the owners' arenas
+  (``csrc/v2_qsgd.cu``, TernGrad adds a per-tensor clip launch), and the owners decode, sum and step the
+  optimizer in one launch per group.  BN and bias vectors stay fp32 (``multimem.ld_reduce``).
 * Optimizers fused in the PS epilogue: momentum-SGD (``src/optim/sgd.py:57-90``), Adam / AMSGrad
   (``src/optim/adam.py:37-94``).
 
@@ -56,7 +60,8 @@ class ShadowEngine:
                  criterion: Optional[nn.Module] = None, device: Optional[torch.device] = None,
                  ps_grid: int = 0, overlap: bool = True, fused_bn: bool = True, num_aggregate: int = 0,
                  warm_start: bool = True, max_sweeps: int = 1, main_priority: int = 0, debug_jitter_us: float = 0.0,
-                 side_priority: int = -1, resample_empty: bool = False):
+                 side_priority: int = -1, resample_empty: bool = False, quantization_level: int = 4,
+                 bucket_size: int = 512):
         self.C = load_ext()
         C = self.C
         assert C.v2_unit_bytes() == P2.UNIT_BYTES and C.v2_ctrl_bytes() == P2.CTRL2_BYTES
@@ -64,9 +69,16 @@ class ShadowEngine:
         self.device = device or torch.device("cuda", torch.cuda.current_device())
         dev = self.device
         self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
-        if self.code not in ("svd", "sgd", "qsvd"):
-            raise ValueError("ShadowEngine codes: svd | qsvd | sgd (qsgd / terngrad / entrywise run on FusedEngine)")
+        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad"):
+            raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad (entrywise runs on FusedEngine)")
         self.svd_rank = int(svd_rank)
+        self.quant = self.code in ("qsgd", "terngrad")
+        self.quantization_level, self.bucket_size = int(quantization_level), int(bucket_size)
+        if self.quant:
+            if not 1 <= self.quantization_level <= P2.QSGD_MAX_LEVEL:
+                raise ValueError("quantization_level must be in [1, %d]" % P2.QSGD_MAX_LEVEL)
+            if not (32 <= self.bucket_size <= P2.QSGD_MAX_BUCKET and self.bucket_size % 8 == 0):
+                raise ValueError("bucket_size must be a multiple of 8 in [32, %d]" % P2.QSGD_MAX_BUCKET)
         if world == 1:
             ps_mode = "colocated"
         self.ps_mode = ps_mode
@@ -110,7 +122,8 @@ class ShadowEngine:
         self.params = list(self.model.parameters())
         shapes = [tuple(p.shape) for p in self.params]
         self.plan = P2.build_plan2(shapes, self.code, self.svd_rank, self.systematic, n_owners=self.n_owners,
-                                   n_groups=groups if overlap else 1)
+                                   n_groups=groups if overlap else 1, quantization_level=self.quantization_level,
+                                   bucket_size=self.bucket_size)
         pl = self.plan
         self.G = pl.n_groups
 
@@ -204,12 +217,20 @@ class ShadowEngine:
         # eigenbasis of the previous step per coded unit (Jacobi warm start); identity to begin with
         self.max_sweeps = int(max_sweeps) if warm_start else 0
         self.vprev = None
-        if warm_start:
+        if warm_start and not self.quant:
             self.vprev = z(nc * P2.MAX_COLS * P2.MAX_COLS)
             for u in pl.units:
                 if u.coded:
                     o = u.ts_index * P2.MAX_COLS * P2.MAX_COLS
                     self.vprev[o:o + u.cols * u.cols].copy_(torch.eye(u.cols, device=dev).reshape(-1))
+        # QSGD: largest level / bucket of the plan (checked by the bindings), TernGrad clip per unit + its partials
+        qunits = [u for u in pl.units if u.kind == P2.KIND_QSGD]
+        self.q_max_level = max((u.I for u in qunits), default=0)
+        self.q_max_bucket = max((u.K for u in qunits), default=0)
+        self.clip = self.clip_partials = None
+        if self.code == "terngrad":
+            self.clip = z(nc)
+            self.clip_partials = torch.zeros(2 * max(len(pl.enc_tiles), 1), dtype=torch.float64, device=dev)
         self.counters = torch.zeros(nc + 2 * P2.MAX_GROUPS + 8, dtype=torch.int32, device=dev)
         self.cnt_enc_group = self.counters.data_ptr() + 4 * nc
         self.cnt_ps_group = self.cnt_enc_group + 4 * P2.MAX_GROUPS
@@ -311,6 +332,21 @@ class ShadowEngine:
             lo, hi = self.w_range[g]
             if hi > lo:   # pageable source: staged synchronously, safe against the host table changing next step
                 self.t_gptr[lo:hi].copy_(torch.from_numpy(self.host_gptr[lo:hi].copy()))
+        if nt > 0 and self.quant:
+            # quantize + push straight into the owners' arenas; the encode launch raises the group's push flag
+            if self.clip is not None:
+                C.v2_qsgd_stats(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
+                                self.clip_partials.data_ptr(), self.counters.data_ptr(), self.clip.data_ptr(),
+                                self.tstats.data_ptr(), g)
+                self._nlaunch += 1
+            C.v2_qsgd_encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
+                             self.clip.data_ptr() if self.clip is not None else 0, self.t_arena_peer.data_ptr(),
+                             self.t_sig_owner.data_ptr(), self.n_owners, pl.arena_floats, self.worker_index, g,
+                             self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g, 0, self.tstats.data_ptr(),
+                             self._fired == self.G, self.clip is None, self.q_max_level, self.q_max_bucket,
+                             self.code == "terngrad")
+            self._nlaunch += 1
+            return
         if nt > 0 and self.code in ("svd", "qsvd"):
             C.v2_encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
                         self.gpart.data_ptr(), self.counters.data_ptr(), self.vsel.data_ptr(),
@@ -339,6 +375,17 @@ class ShadowEngine:
         C, pl = self.C, self.plan
         t0, nt = pl.ps_range[g][self.owner_index]
         p = lambda t: t.data_ptr() if t is not None else 0
+        if self.quant:
+            C.v2_ps_qsgd(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g, final,
+                         self.owner_index, p(self.master), p(self.mom), p(self.sq), p(self.sqmax), p(self.vmom),
+                         p(self.vsq), p(self.vsqmax), self.wshadow_mc, self.t_wshadow_peer.data_ptr(),
+                         self.vparams.data_ptr(), self.vparams_mc, self.t_vparams_peer.data_ptr(), self.vgrads_mc,
+                         self.t_vgrads_peer.data_ptr(), self.heap.region_ptr("arena"), pl.arena_floats,
+                         self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
+                         self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
+                         max(1, min(self.ps_grid, max(nt, 1))), self.q_max_level, self.q_max_bucket)
+            self._nlaunch += 1
+            return
         C.v2_ps(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g, final,
                 self.owner_index, p(self.master), p(self.mom), p(self.sq), p(self.sqmax), p(self.vmom), p(self.vsq),
                 p(self.vsqmax), self.wshadow_mc, self.t_wshadow_peer.data_ptr(), self.vparams.data_ptr(),
@@ -495,7 +542,7 @@ class ShadowEngine:
             u = pl.units[ui]
             if u.kind == P2.KIND_VEC:
                 mv[u.w_off + a:u.w_off + a + b] = 1
-            elif u.kind == P2.KIND_DENSE16:
+            elif u.kind in (P2.KIND_DENSE16, P2.KIND_QSGD):     # QSGD tiles: (first element, element count)
                 mw[u.w_off + a:u.w_off + a + b] = 1
             elif u.kind == P2.KIND_SLAB:
                 half = u.I // 2
@@ -567,6 +614,8 @@ class ShadowEngine:
         os.replace(tmp, path)
         side = {"step": step, "lr": self.lr, "mom_w": mom.cpu(), "mom_v": vm.cpu(), "code": self.code,
                 "svd_rank": self.svd_rank, "engine": "shadow"}
+        if self.quant:
+            side.update(quantization_level=self.quantization_level, bucket_size=self.bucket_size)
         side.update(adam_state)
         torch.save(side, path + "_optim.tmp")
         os.replace(path + "_optim.tmp", path + "_optim")

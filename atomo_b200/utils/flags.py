@@ -68,6 +68,10 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
     p.add_argument("--ps-mode", type=str, default="sharded", choices=["sharded", "colocated", "dedicated"],
                    help="p2p backend: sharded = every GPU trains and owns 1/N of the PS tiles (bf16 engine); "
                         "colocated = rank 0 hosts the whole PS and also trains; dedicated = rank 0 only serves")
+    p.add_argument("--engine", type=str, default="auto", choices=["auto", "shadow", "fused"],
+                   help="p2p backend: auto = the overlapped sharded bf16 engine for --dtype bf16 with --code "
+                        "svd|qsvd|sgd, the fp32-flat engine otherwise; shadow = the bf16 engine (also --code "
+                        "qsgd|terngrad, needs --dtype bf16); fused = the fp32-flat engine")
     p.add_argument("--groups", type=int, default=5, help="p2p/bf16: backward groups pushed while backward runs")
     p.add_argument("--shrinkage-freq", type=int, default=50, help="steps between LR shrinkages (reference: 50)")
     p.add_argument("--flag-timeout", type=float, default=120.0,
