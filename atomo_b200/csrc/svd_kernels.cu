@@ -10,7 +10,8 @@
 //   gram_kernel      : G_tile = A_tile^T A_tile           (pass 1 over the gradient)
 //   eig_sample_kernel: G = sum tiles; V,lambda = Jacobi(G); sigma = sqrt(lambda);
 //                      p_i = min(1, r sigma_i / sum sigma) (or water-filled);
-//                      Philox Bernoulli / systematic sampling;
+//                      Philox Bernoulli / systematic sampling (spectral_sample.cuh,
+//                      shared with the bf16 engine's v2_encode_kernel);
 //                      header, s_a = sigma_a/p_a and V rows -> PS slot (peer store)
 //   project_push     : U[:,a] = A v_a / sigma_a            (pass 2, L2-resident)
 //                      float4 peer stores of U into the PS slot; the last CTA
@@ -19,7 +20,7 @@
 // Because V is a complete orthonormal basis of the skinny dimension,
 // sum_i (A v_i) v_i^T == A exactly, so the estimator is unbiased even when the
 // fp32 Gram/Jacobi eigenvectors are only approximately the singular vectors.
-#include "common.cuh"
+#include "spectral_sample.cuh"
 
 namespace atomo {
 
@@ -27,7 +28,6 @@ constexpr int GRAM_THREADS = 256;
 constexpr int GRAM_CHUNK = 64;   // rows staged per iteration
 constexpr int EIG_THREADS = 256;
 constexpr int PROJ_THREADS = 128;
-constexpr int MAX_SWEEPS = 12;
 
 // ----------------------------------------------------------------------------
 // stage a chunk of tall rows into shared memory: sm[r*stride + c] = A[row0+r][c]
@@ -125,36 +125,15 @@ struct EncodeCfg {
   int waterfill;      // 0 -> reference single clip, 1 -> paper's water-filling
   int systematic;     // 0 -> independent Bernoulli, 1 -> systematic sampling
   int worker_index;   // index of this worker's arena on the PS
-  int use_ext_uniforms;
 };
-
-constexpr int GS = TS_MAX_COLS + 1;  // padded row stride of G / V in shared memory
-
-__device__ __forceinline__ void rr_pair(int ne, int rnd, int k, int& p, int& q) {
-  // round-robin tournament over `ne` (even) players: ne/2 disjoint pairs per round
-  const int m = ne - 1;
-  int a, b;
-  if (k == 0) { a = rnd % m; b = m; }
-  else { a = (rnd + k) % m; b = (rnd - k + m) % m; }
-  p = min(a, b); q = max(a, b);
-}
 
 __global__ void __launch_bounds__(1024)
 eig_sample_kernel(const LayerDesc* __restrict__ layers, const int* __restrict__ ts_layers,
                   const float* __restrict__ gpart, float* __restrict__ vsel, int* __restrict__ selcount,
                   float* __restrict__ sigma_out, float* ps_arena_peer, long long arena_floats, const Ctrl* ctrl,
                   const float* __restrict__ ext_uniforms, EncodeCfg cfg) {
-  __shared__ float G[TS_MAX_COLS * GS];
-  __shared__ float V[TS_MAX_COLS * GS];
-  __shared__ float rc[TS_MAX_COLS / 2], rs[TS_MAX_COLS / 2];
-  __shared__ int rp[TS_MAX_COLS / 2], rq[TS_MAX_COLS / 2];
-  __shared__ float sig[TS_MAX_COLS], prob[TS_MAX_COLS], uni[TS_MAX_COLS];
-  __shared__ int order[TS_MAX_COLS];  // order[k] = index of k-th largest sigma
-  __shared__ int sel[RCAP_MAX];
-  __shared__ float selscale[RCAP_MAX];
-  __shared__ int s_maxrel;
-  __shared__ float s_gmax;
-  __shared__ int s_count, s_done;
+  __shared__ float G[TS_MAX_COLS * SPECTRAL_PITCH];
+  __shared__ float V[TS_MAX_COLS * SPECTRAL_PITCH];
 
   const int layer_id = ts_layers[blockIdx.x];
   const LayerDesc L = layers[layer_id];
@@ -164,7 +143,6 @@ eig_sample_kernel(const LayerDesc* __restrict__ layers, const int* __restrict__ 
 
   // ---- G = sum of tile partials (padded to an even size with a zero row/col); V = I ----------
   const int ne = n + (n & 1);
-  const int npairs = ne >> 1;
   for (int e = tid; e < ne * ne; e += blockDim.x) {
     const int i = e / ne, j = e - i * ne;
     float s = 0.f;
@@ -172,233 +150,39 @@ eig_sample_kernel(const LayerDesc* __restrict__ layers, const int* __restrict__ 
       const float* gp = gpart + L.gpart_off + i * n + j;
       for (int t = 0; t < L.ntiles; ++t) s += gp[(long long)t * n * n];
     }
-    G[i * GS + j] = s;
-    V[i * GS + j] = (i == j) ? 1.f : 0.f;
+    G[i * SPECTRAL_PITCH + j] = s;
+    V[i * SPECTRAL_PITCH + j] = (i == j) ? 1.f : 0.f;
   }
   __syncthreads();
   // symmetrize (partials are accumulated in different orders for (i,j)/(j,i))
   for (int e = tid; e < n * n; e += blockDim.x) {
     int i = e / n, j = e - i * n;
     if (i < j) {
-      float v = 0.5f * (G[i * GS + j] + G[j * GS + i]);
-      G[i * GS + j] = v;
-      G[j * GS + i] = v;
+      float v = 0.5f * (G[i * SPECTRAL_PITCH + j] + G[j * SPECTRAL_PITCH + i]);
+      G[i * SPECTRAL_PITCH + j] = v;
+      G[j * SPECTRAL_PITCH + i] = v;
     }
   }
   __syncthreads();
 
-  // ---- cyclic Jacobi, round-robin (parallel) ordering, fused two-sided update ------------------
-  // All ne/2 pairs of a round are disjoint, so G' = J^T G J decomposes into independent 2x2
-  // blocks: block (k1,k2) = J_k1^T * G[{p1,q1}][{p2,q2}] * J_k2 — one thread per block, one
-  // barrier between "compute rotations" and "apply", none between the row and column halves.
-  // The padded dummy index only ever meets zeros, so its rotations are the identity.
-  if (tid == 0) {
-    float g = 0.f;
-    for (int i = 0; i < n; ++i) g = fmaxf(g, fabsf(G[i * GS + i]));
-    s_gmax = g;
-  }
-  __syncthreads();
-  const float gmax = s_gmax;
-  if (n > 1 && gmax > 0.f) {
-    for (int sweep = 0; sweep < MAX_SWEEPS; ++sweep) {
-      if (tid == 0) s_maxrel = 0;
-      __syncthreads();
-      for (int rnd = 0; rnd < ne - 1; ++rnd) {
-        if (tid < npairs) {
-          int p, q;
-          rr_pair(ne, rnd, tid, p, q);
-          float c = 1.f, s = 0.f;
-          const float apq = G[p * GS + q], app = G[p * GS + p], aqq = G[q * GS + q];
-          const float scale = sqrtf(fabsf(app * aqq));
-          // rotate unless the coupling is below fp32 noise (relative to the pair and to the spectrum)
-          if (fabsf(apq) > 1e-7f * scale && fabsf(apq) > 3e-7f * gmax) {
-            const float tau = (aqq - app) / (2.f * apq);
-            const float t = (tau >= 0.f ? 1.f : -1.f) / (fabsf(tau) + sqrtf(1.f + tau * tau));
-            c = rsqrtf(1.f + t * t);
-            s = t * c;
-            atomicMax(&s_maxrel, __float_as_int(fabsf(apq) / gmax));
-          }
-          rp[tid] = p; rq[tid] = q; rc[tid] = c; rs[tid] = s;
-        }
-        __syncthreads();
-        const int nblk = npairs * npairs;
-        for (int e = tid; e < nblk + npairs * ne; e += blockDim.x) {
-          if (e < nblk) {
-            const int k1 = e / npairs, k2 = e - k1 * npairs;
-            const int p1 = rp[k1], q1 = rq[k1], p2 = rp[k2], q2 = rq[k2];
-            const float c1 = rc[k1], s1 = rs[k1], c2 = rc[k2], s2 = rs[k2];
-            const float a = G[p1 * GS + p2], b = G[p1 * GS + q2], c_ = G[q1 * GS + p2], d = G[q1 * GS + q2];
-            // left: rows (p1,q1) <- J1^T
-            const float ra = c1 * a - s1 * c_, rb = c1 * b - s1 * d;
-            const float rc_ = s1 * a + c1 * c_, rd = s1 * b + c1 * d;
-            // right: cols (p2,q2) <- J2
-            G[p1 * GS + p2] = c2 * ra - s2 * rb;
-            G[p1 * GS + q2] = s2 * ra + c2 * rb;
-            G[q1 * GS + p2] = c2 * rc_ - s2 * rd;
-            G[q1 * GS + q2] = s2 * rc_ + c2 * rd;
-          } else {
-            const int f = e - nblk;
-            const int k = f / ne, i = f - k * ne;
-            const int p = rp[k], q = rq[k];
-            const float c = rc[k], s = rs[k];
-            const float vp = V[i * GS + p], vq = V[i * GS + q];
-            V[i * GS + p] = c * vp - s * vq;
-            V[i * GS + q] = s * vp + c * vq;
-          }
-        }
-        __syncthreads();
-      }
-      // quadratic convergence: couplings below 1e-3 at the start of a sweep are ~1e-6 after it.  Every thread reads
-      // the shared value BEFORE thread 0 may reset it for the next sweep (else a slow warp can leave the loop alone
-      // and desynchronise all later barriers).
-      const float mr = __int_as_float(s_maxrel);
-      __syncthreads();
-      if (mr < 1e-3f) break;
-    }
-  }
-  __syncthreads();
-
-  // ---- singular values, descending order --------------------------------------
-  if (tid < n) sig[tid] = sqrtf(fmaxf(G[tid * GS + tid], 0.f));
-  __syncthreads();
-  if (tid < n) {
-    const float me = sig[tid];
-    int rank_ = 0;
-    for (int j = 0; j < n; ++j) {
-      const float o = sig[j];
-      rank_ += (o > me) || (o == me && j < tid);
-    }
-    order[rank_] = tid;
-  }
-  __syncthreads();
-
-  // ---- inclusion probabilities ---------------------------------------------------
+  // ---- Jacobi, sampling (an empty draw is always redrawn), vsel[blockIdx.x] = V[:, sel] / sigma ------------
   const int rcap = L.rcap;
-  if (tid == 0) {
-    float total = 0.f;
-    for (int i = 0; i < n; ++i) total += sig[i];
-    const float smax = sig[order[0]];
-    int count = 0;
-    if (!(smax >= 1e-6f)) {
-      // degenerate spectrum (svd.py:50-51): send atom 0 with probability 1
-      sel[0] = order[0]; selscale[0] = 1.f; count = 1;
-      for (int i = 0; i < n; ++i) prob[i] = 0.f;
-      prob[order[0]] = 1.f;
-      s_done = 1;
-    } else if (!cfg.random_sample) {
-      const int k = min(min(cfg.rank > 0 ? cfg.rank : n, n), rcap);
-      for (int a = 0; a < k; ++a) { sel[a] = order[a]; selscale[a] = 1.f; }
-      count = k;
-      s_done = 1;
-    } else {
-      if (cfg.rank == 0) {
-        for (int i = 0; i < n; ++i) prob[i] = fminf(sig[i] / smax, 1.f);
-      } else if (!cfg.waterfill) {
-        for (int i = 0; i < n; ++i) prob[i] = fminf((float)cfg.rank * sig[i] / total, 1.f);
-      } else {
-        // water-filling over the sorted spectrum: pin the largest atoms to 1
-        float budget = fminf((float)cfg.rank, (float)n);
-        float rest = total;
-        int pinned = 0;
-        while (pinned < n) {
-          const float s0 = sig[order[pinned]];
-          if (rest > 0.f && (budget - pinned) * s0 >= rest && (budget - pinned) > 0.f) {
-            rest -= s0; ++pinned;
-          } else break;
-        }
-        for (int k = 0; k < n; ++k) {
-          const int i = order[k];
-          prob[i] = (k < pinned) ? 1.f : (rest > 0.f ? fminf((budget - pinned) * sig[i] / rest, 1.f) : 0.f);
-        }
-      }
-      s_done = 0;
-    }
-    s_count = count;
-  }
-  __syncthreads();
+  const SampleCfg scfg{(float)cfg.rank, rcap, cfg.random_sample, cfg.waterfill, cfg.systematic, 1,
+                       ext_uniforms, &ctrl->seed, layer_id,
+                       ((uint32_t)cfg.worker_index << 24) ^ (uint32_t)step};
+  const Spectrum sp = eig_sample(G, V, n, false, 0, scfg, blockIdx.x, vsel, nullptr, 0, false);
+  const int count = sp.count;
 
-  // ---- sampling ----------------------------------------------------------------------
-  if (!s_done) {
-    for (int attempt = 0; attempt < 16 && !s_done; ++attempt) {
-      if (tid < n) {
-        float u;
-        if (cfg.use_ext_uniforms && attempt == 0) {
-          u = ext_uniforms[(long long)blockIdx.x * TS_MAX_COLS + tid];
-        } else {
-          uint32_t r4[4];
-          Philox::gen(ctrl->seed, (uint32_t)tid, (uint32_t)attempt, (uint32_t)layer_id,
-                      ((uint32_t)cfg.worker_index << 24) ^ (uint32_t)step, r4);
-          u = Philox::to_uniform(r4[0]);
-        }
-        uni[tid] = u;
-      }
-      __syncthreads();
-      if (tid == 0) {
-        int count = 0;
-        bool overflow = false;
-        if (cfg.systematic) {
-          // one uniform, cumulative probabilities in descending-sigma order
-          const float u = uni[0];
-          float c = 0.f;
-          for (int k = 0; k < n; ++k) {
-            const int i = order[k];
-            const float lo = floorf(c + u);
-            c += prob[i];
-            const float hi = floorf(c + u);
-            if (hi > lo) {
-              if (count < rcap) { sel[count] = i; selscale[count] = 1.f / prob[i]; }
-              else overflow = true;
-              ++count;
-            }
-          }
-        } else {
-          for (int k = 0; k < n; ++k) {
-            const int i = order[k];
-            if (uni[i] < prob[i]) {
-              if (count < rcap) { sel[count] = i; selscale[count] = 1.f / prob[i]; }
-              else overflow = true;
-              ++count;
-            }
-          }
-        }
-        if (count > 0 && !overflow) { s_count = count; s_done = 1; }  // else resample (svd.py:65-66)
-      }
-      __syncthreads();
-    }
-    if (!s_done) {
-      // pathological: deterministic fallback on the most probable atoms
-      if (tid == 0) {
-        const int k = min(max(cfg.rank, 1), min(n, rcap));
-        for (int a = 0; a < k; ++a) { sel[a] = order[a]; selscale[a] = 1.f / fmaxf(prob[order[a]], 1e-6f); }
-        s_count = k; s_done = 1;
-      }
-      __syncthreads();
-    }
-  }
-  const int count = s_count;
-
-  // ---- publish: local projection basis + PS slot header / s / V -----------------------
-  // vsel[ts][c*RCAP_MAX + a] = V[c][sel_a] / sigma_a   (so  U = A * vsel)
-  float* vs = vsel + (long long)blockIdx.x * TS_MAX_COLS * RCAP_MAX;
-  for (int e = tid; e < n * RCAP_MAX; e += blockDim.x) {
-    const int c = e / RCAP_MAX, a = e - c * RCAP_MAX;
-    float v = 0.f;
-    if (a < count) {
-      const int i = sel[a];
-      // a (numerically) null direction has no left vector: emit a zero column instead of 1/0
-      v = (sig[i] > 1e-7f * sig[order[0]]) ? V[c * GS + i] / sig[i] : 0.f;
-    }
-    vs[e] = v;
-  }
+  // ---- publish: selection count, sigma, and the PS slot header / s / V ----------------------------------
   if (tid == 0) selcount[blockIdx.x] = count;
-  if (sigma_out != nullptr && tid < n) sigma_out[(long long)blockIdx.x * TS_MAX_COLS + tid] = sig[order[tid]];
+  if (sigma_out != nullptr && tid < n) sigma_out[(long long)blockIdx.x * TS_MAX_COLS + tid] = sp.sig[sp.order[tid]];
 
   float* slot = ps_arena_peer + (long long)cfg.worker_index * arena_floats + L.slot_off;
-  if (tid < rcap) slot[slot_s_off() + tid] = (tid < count) ? sig[sel[tid]] * selscale[tid] : 0.f;
+  if (tid < rcap) slot[slot_s_off() + tid] = (tid < count) ? sp.sig[sp.sel[tid]] * sp.selscale[tid] : 0.f;
   float* vout = slot + slot_v_off(rcap);
   for (int e = tid; e < rcap * n; e += blockDim.x) {
     const int a = e / n, c = e - a * n;
-    vout[e] = (a < count) ? V[c * GS + sel[a]] : 0.f;
+    vout[e] = (a < count) ? V[c * SPECTRAL_PITCH + sp.sel[a]] : 0.f;
   }
   if (tid == 0) {
     int* hdr = reinterpret_cast<int*>(slot);
@@ -501,7 +285,7 @@ void atomo_launch_eig_sample(const void* layers, const int* ts_layers, int n_ts,
   if (n_ts <= 0) return;
   if (threads < 64) threads = EIG_THREADS;
   if (threads > 1024) threads = 1024;
-  EncodeCfg cfg{rank, random_sample, waterfill, systematic, worker_index, ext_uniforms != nullptr};
+  EncodeCfg cfg{rank, random_sample, waterfill, systematic, worker_index};
   eig_sample_kernel<<<n_ts, threads, 0, stream>>>((const LayerDesc*)layers, ts_layers, gpart, vsel, selcount,
                                                         sigma_out, ps_arena_peer, arena_floats, (const Ctrl*)ctrl,
                                                         ext_uniforms, cfg);

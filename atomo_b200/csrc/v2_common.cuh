@@ -68,8 +68,8 @@ enum Err2 : int { ERR2_NONE = 0, ERR2_WAIT_PUSH = 1, ERR2_WAIT_PARAM = 2, ERR2_S
 
 constexpr int MAX_WORKERS = 16;
 constexpr int MAX_GROUPS = 8;
-constexpr int V2_MAX_COLS = 64;
-constexpr int V2_RCAP_MAX = 32;
+constexpr int V2_MAX_COLS = TS_MAX_COLS;
+constexpr int V2_RCAP_MAX = RCAP_MAX;
 // signal region (ints): push flag of (group g, worker w) at g*MAX_WORKERS + w; param flag of owner o at 256 + o;
 // aggregation mask of (group g) at 320 + g (owner-local)
 constexpr int SIG_PUSH = 0;

@@ -13,6 +13,7 @@
 //   v2_project_kernel  U = A V / sigma for the sampled atoms (second pass, L2 resident), float4 peer stores of
 //                      each row into the arena of the PS owner of that row's tile; the last CTA of the group
 //                      publishes flag[group][worker] = step on every owner with st.release.sys.
+#include "spectral_sample.cuh"
 #include "v2_common.cuh"
 
 namespace atomo {
@@ -23,8 +24,6 @@ constexpr int ENC_HDR = 128;
 constexpr int ENC_TILE_BYTES = 36 * 1024;       // tile buffer; reused for G / V (2 x 64 x 65 floats) in the eig phase
 constexpr int ENC_RED_BYTES = 64 * 64 * 4;
 constexpr int ENC_SMEM = ENC_HDR + ENC_TILE_BYTES + ENC_RED_BYTES;
-constexpr int GS2 = V2_MAX_COLS + 1;
-constexpr int MAX_SWEEPS2 = 12;
 
 struct EncCfg {
   int random_sample;
@@ -185,33 +184,15 @@ __device__ void mat_gram(const __nv_bfloat16* gb, const Unit2& u, int r0, int nr
   }
 }
 
-__device__ __forceinline__ void rr_pair2(int ne, int rnd, int k, int& p, int& q) {
-  const int m = ne - 1;
-  int a, b;
-  if (k == 0) { a = rnd % m; b = m; }
-  else { a = (rnd + k) % m; b = (rnd - k + m) % m; }
-  p = min(a, b); q = max(a, b);
-}
-
 // ------------------------------------------------------------------------------------------------------
-// Eigen-decomposition of the unit's Gram + atom sampling (svd.py:49-67 semantics, see csrc/svd_kernels.cu for
-// the round-1 stand-alone version).  Runs in the LAST encode CTA of the unit; G / V live in the tile buffer.
+// Eigen-decomposition of the unit's Gram + atom sampling (spectral_sample.cuh).  Runs in the LAST encode CTA of the
+// unit; G / V live in the tile buffer.
 // ------------------------------------------------------------------------------------------------------
 __device__ void eig_sample_unit(const EncArgs& a, const Unit2& u, int unit_id, float* G, float* V, float* Tbuf) {
-  __shared__ float rc[V2_MAX_COLS / 2], rs[V2_MAX_COLS / 2];
-  __shared__ int rp[V2_MAX_COLS / 2], rq[V2_MAX_COLS / 2];
-  __shared__ float sig[V2_MAX_COLS], prob[V2_MAX_COLS], uni[V2_MAX_COLS];
-  __shared__ int order[V2_MAX_COLS];
-  __shared__ int sel[V2_RCAP_MAX];
-  __shared__ float selscale[V2_RCAP_MAX];
-  __shared__ int s_maxrel;
-  __shared__ float s_gmax;
-  __shared__ int s_count, s_done;
-
   const int n = u.cols, tid = threadIdx.x, nthr = blockDim.x;
   const int step = a.ctrl->step;
   const int ts = u.ts_index;
-  const int ne = n + (n & 1), npairs = ne >> 1;
+  const int ne = n + (n & 1);
   // Warm start: the right-singular basis of a layer's gradient drifts slowly from step to step, so Jacobi starts
   // from last step's basis V0 (G0 = V0^T G V0 is already nearly diagonal) and needs 1-2 sweeps instead of 6-10.
   // The basis is reset to the identity every 256 steps so rounding drift of V's orthonormality cannot build up.
@@ -224,10 +205,10 @@ __device__ void eig_sample_unit(const EncArgs& a, const Unit2& u, int unit_id, f
       const float* gp = a.gpart + u.gpart_off + i * n + j;
       for (int t = 0; t < u.n_enc; ++t) s += __ldcg(gp + (long long)t * n * n);
     }
-    G[i * GS2 + j] = s;
+    G[i * SPECTRAL_PITCH + j] = s;
     float v0 = (i == j) ? 1.f : 0.f;
     if (warm && i < n && j < n) v0 = vp[i * n + j];
-    V[i * GS2 + j] = v0;
+    V[i * SPECTRAL_PITCH + j] = v0;
   }
   if (warm) {
     float* T = Tbuf;   // n x n scratch (the Gram reduction buffer of the tile phase)
@@ -235,7 +216,7 @@ __device__ void eig_sample_unit(const EncArgs& a, const Unit2& u, int unit_id, f
     for (int e = tid; e < n * n; e += nthr) {       // T = G V0
       const int i = e / n, j = e - i * n;
       float acc = 0.f;
-      for (int k = 0; k < n; ++k) acc = fmaf(G[i * GS2 + k], V[k * GS2 + j], acc);
+      for (int k = 0; k < n; ++k) acc = fmaf(G[i * SPECTRAL_PITCH + k], V[k * SPECTRAL_PITCH + j], acc);
       T[e] = acc;
     }
     __syncthreads();
@@ -244,233 +225,39 @@ __device__ void eig_sample_unit(const EncArgs& a, const Unit2& u, int unit_id, f
       if (i <= j) {
         float x = 0.f, y = 0.f;
         for (int k = 0; k < n; ++k) {
-          x = fmaf(V[k * GS2 + i], T[k * n + j], x);
-          y = fmaf(V[k * GS2 + j], T[k * n + i], y);
+          x = fmaf(V[k * SPECTRAL_PITCH + i], T[k * n + j], x);
+          y = fmaf(V[k * SPECTRAL_PITCH + j], T[k * n + i], y);
         }
         const float v = 0.5f * (x + y);
-        G[i * GS2 + j] = v;
-        G[j * GS2 + i] = v;
+        G[i * SPECTRAL_PITCH + j] = v;
+        G[j * SPECTRAL_PITCH + i] = v;
       }
     }
   }
   __syncthreads();
-  if (tid == 0) {
-    float g = 0.f;
-    for (int i = 0; i < n; ++i) g = fmaxf(g, fabsf(G[i * GS2 + i]));
-    s_gmax = g;
-  }
-  __syncthreads();
-  const float gmax = s_gmax;
-  if (n > 1 && gmax > 0.f) {
-    // warm: a.max_sweeps refinement sweeps track the slowly drifting basis; cold (first step / periodic reset): full solve
-    const int sweeps = (warm && a.max_sweeps > 0) ? min(a.max_sweeps, MAX_SWEEPS2) : MAX_SWEEPS2;
-    for (int sweep = 0; sweep < sweeps; ++sweep) {
-      if (tid == 0) s_maxrel = 0;
-      __syncthreads();
-      for (int rnd = 0; rnd < ne - 1; ++rnd) {
-        if (tid < npairs) {
-          int p, q;
-          rr_pair2(ne, rnd, tid, p, q);
-          float c = 1.f, s = 0.f;
-          const float apq = G[p * GS2 + q], app = G[p * GS2 + p], aqq = G[q * GS2 + q];
-          const float scale = sqrtf(fabsf(app * aqq));
-          if (fabsf(apq) > 1e-7f * scale && fabsf(apq) > 3e-7f * gmax) {
-            const float tau = (aqq - app) / (2.f * apq);
-            const float t = (tau >= 0.f ? 1.f : -1.f) / (fabsf(tau) + sqrtf(1.f + tau * tau));
-            c = rsqrtf(1.f + t * t);
-            s = t * c;
-            atomicMax(&s_maxrel, __float_as_int(fabsf(apq) / gmax));
-          }
-          rp[tid] = p; rq[tid] = q; rc[tid] = c; rs[tid] = s;
-        }
-        __syncthreads();
-        // two-sided update of the 2x2 blocks G[{p1,q1}][{p2,q2}] ...
-        {
-          int k1 = tid / npairs, k2 = tid - k1 * npairs;
-          const int dk1 = nthr / npairs, dk2 = nthr - dk1 * npairs;
-          while (k1 < npairs) {
-            const int p1 = rp[k1], q1 = rq[k1], p2 = rp[k2], q2 = rq[k2];
-            const float c1 = rc[k1], s1 = rs[k1], c2 = rc[k2], s2 = rs[k2];
-            const float x = G[p1 * GS2 + p2], y = G[p1 * GS2 + q2], z = G[q1 * GS2 + p2], w = G[q1 * GS2 + q2];
-            const float ra = c1 * x - s1 * z, rb = c1 * y - s1 * w;
-            const float rc_ = s1 * x + c1 * z, rd = s1 * y + c1 * w;
-            G[p1 * GS2 + p2] = c2 * ra - s2 * rb;
-            G[p1 * GS2 + q2] = s2 * ra + c2 * rb;
-            G[q1 * GS2 + p2] = c2 * rc_ - s2 * rd;
-            G[q1 * GS2 + q2] = s2 * rc_ + c2 * rd;
-            k1 += dk1; k2 += dk2;
-            if (k2 >= npairs) { k2 -= npairs; ++k1; }
-          }
-        }
-        // ... and the column rotations of V (row i, pair k)
-        {
-          int k = tid / ne, i = tid - k * ne;
-          const int dk = nthr / ne, di = nthr - dk * ne;
-          while (k < npairs) {
-            const int p = rp[k], q = rq[k];
-            const float c = rc[k], sn = rs[k];
-            const float vp_ = V[i * GS2 + p], vq = V[i * GS2 + q];
-            V[i * GS2 + p] = c * vp_ - sn * vq;
-            V[i * GS2 + q] = sn * vp_ + c * vq;
-            k += dk; i += di;
-            if (i >= ne) { i -= ne; ++k; }
-          }
-        }
-        __syncthreads();
-      }
-      // Every thread must have read s_maxrel before thread 0 resets it for the next sweep: without this barrier a
-      // slow warp can see the reset value, leave the loop alone and desynchronise every barrier that follows
-      // (observed as random illegal-address / illegal-instruction faults once this kernel shared SMs with cuDNN).
-      const float mr = __int_as_float(s_maxrel);
-      __syncthreads();
-      if (mr < 1e-3f) break;
-    }
-  }
-  __syncthreads();
-  if (tid < n) {
-    float d = G[tid * GS2 + tid];
-    if (!(d >= 0.f) || !(d <= 3.0e38f)) {          // NaN / Inf / negative: flag it, treat the direction as empty
-      if (!(d > -1e-3f * gmax)) atomicOr(const_cast<int*>(&a.ctrl->error), ERR2_NONFINITE);
-      d = 0.f;
-    }
-    sig[tid] = sqrtf(d);
-    order[tid] = tid;
-  }
-  __syncthreads();
-  if (tid < n) {
-    const float me = sig[tid];
-    int rk = 0;
-    for (int j = 0; j < n; ++j) {
-      const float o = sig[j];
-      rk += (o > me) || (o == me && j < tid);
-    }
-    order[rk] = tid;
-  }
-  __syncthreads();
+  // warm: a.max_sweeps refinement sweeps track the slowly drifting basis; cold (first step / periodic reset): full solve.
+  // Stores vsel[ts], the projection basis of v2_project_kernel.
+  const SampleCfg cfg{u.budget, u.rcap, a.cfg.random_sample, a.cfg.waterfill, a.cfg.systematic, a.cfg.resample_empty,
+                      a.ext_uniforms, &a.ctrl->seed, unit_id, ((uint32_t)a.cfg.worker << 24) ^ (uint32_t)step};
+  const Spectrum sp = eig_sample(G, V, n, warm, a.max_sweeps, cfg, ts, a.vsel, const_cast<int*>(&a.ctrl->error),
+                                 ERR2_NONFINITE, true);
+  const int count = sp.count, rcap = u.rcap;
 
-  const int rcap = u.rcap;
-  const float budget = u.budget;
-  if (tid == 0) {
-    float total = 0.f;
-    for (int i = 0; i < n; ++i) total += sig[i];
-    const float smax = sig[order[0]];
-    int count = 0;
-    if (!(smax >= 1e-6f)) {
-      sel[0] = order[0]; selscale[0] = 1.f; count = 1;
-      for (int i = 0; i < n; ++i) prob[i] = 0.f;
-      prob[order[0]] = 1.f;
-      s_done = 1;
-    } else if (!a.cfg.random_sample) {
-      const int k = min(min(budget > 0.f ? (int)budget : n, n), rcap);
-      for (int x = 0; x < k; ++x) { sel[x] = order[x]; selscale[x] = 1.f; }
-      count = k;
-      s_done = 1;
-    } else {
-      if (budget <= 0.f) {
-        for (int i = 0; i < n; ++i) prob[i] = fminf(sig[i] / smax, 1.f);
-      } else if (!a.cfg.waterfill) {
-        for (int i = 0; i < n; ++i) prob[i] = fminf(budget * sig[i] / total, 1.f);
-      } else {
-        const float bud = fminf(budget, (float)n);
-        float rest = total;
-        int pinned = 0;
-        while (pinned < n) {
-          const float s0 = sig[order[pinned]];
-          if (rest > 0.f && (bud - pinned) * s0 >= rest && (bud - pinned) > 0.f) { rest -= s0; ++pinned; }
-          else break;
-        }
-        for (int k = 0; k < n; ++k) {
-          const int i = order[k];
-          prob[i] = (k < pinned) ? 1.f : (rest > 0.f ? fminf((bud - pinned) * sig[i] / rest, 1.f) : 0.f);
-        }
-      }
-      s_done = 0;
-    }
-    s_count = count;
-  }
-  __syncthreads();
-  if (!s_done) {
-    for (int attempt = 0; attempt < 16 && !s_done; ++attempt) {
-      if (tid < n) {
-        float x;
-        if (a.ext_uniforms != nullptr && attempt == 0) {
-          x = a.ext_uniforms[(long long)ts * V2_MAX_COLS + tid];
-        } else {
-          uint32_t r4[4];
-          Philox::gen(a.ctrl->seed, (uint32_t)tid, (uint32_t)attempt, (uint32_t)unit_id,
-                      ((uint32_t)a.cfg.worker << 24) ^ (uint32_t)step, r4);
-          x = Philox::to_uniform(r4[0]);
-        }
-        uni[tid] = x;
-      }
-      __syncthreads();
-      if (tid == 0) {
-        int count = 0;
-        bool overflow = false;
-        if (a.cfg.systematic) {
-          const float x = uni[0];
-          float c = 0.f;
-          for (int k = 0; k < n; ++k) {
-            const int i = order[k];
-            const float lo = floorf(c + x);
-            c += prob[i];
-            const float hi = floorf(c + x);
-            if (hi > lo) {
-              if (count < rcap) { sel[count] = i; selscale[count] = 1.f / prob[i]; }
-              else overflow = true;
-              ++count;
-            }
-          }
-        } else {
-          for (int k = 0; k < n; ++k) {
-            const int i = order[k];
-            if (uni[i] < prob[i]) {
-              if (count < rcap) { sel[count] = i; selscale[count] = 1.f / prob[i]; }
-              else overflow = true;
-              ++count;
-            }
-          }
-        }
-        if ((count > 0 || !a.cfg.resample_empty) && !overflow) { s_count = count; s_done = 1; }
-      }
-      __syncthreads();
-    }
-    if (!s_done) {
-      if (tid == 0) {
-        const int k = min(max((int)budget, 1), min(n, rcap));
-        for (int x = 0; x < k; ++x) { sel[x] = order[x]; selscale[x] = 1.f / fmaxf(prob[order[x]], 1e-6f); }
-        s_count = k; s_done = 1;
-      }
-      __syncthreads();
-    }
-  }
-  const int count = s_count;
-
-  // ---- publish: local projection basis, and header / s / V into every owner's slot (peer stores) ----
-  float* vs = a.vsel + (long long)ts * V2_MAX_COLS * V2_RCAP_MAX;
-  for (int e = tid; e < n * V2_RCAP_MAX; e += nthr) {
-    const int c = e / V2_RCAP_MAX, x = e - c * V2_RCAP_MAX;
-    float v = 0.f;
-    if (x < count) {
-      const int i = sel[x];
-      v = (sig[i] > 1e-7f * sig[order[0]]) ? V[c * GS2 + i] / sig[i] : 0.f;
-    }
-    vs[e] = v;
-  }
+  // ---- publish: selection count, next step's warm start, and header / s / V into every owner's slot ----
   if (tid == 0) a.selcount[ts] = count;
   if (vp != nullptr)
-    for (int e = tid; e < n * n; e += nthr) vp[e] = V[(e / n) * GS2 + (e % n)];
-  if (a.sigma_out != nullptr && tid < n) a.sigma_out[(long long)ts * V2_MAX_COLS + tid] = sig[order[tid]];
+    for (int e = tid; e < n * n; e += nthr) vp[e] = V[(e / n) * SPECTRAL_PITCH + (e % n)];
+  if (a.sigma_out != nullptr && tid < n) a.sigma_out[(long long)ts * V2_MAX_COLS + tid] = sp.sig[sp.order[tid]];
   // header / s / V go to every owner's slot.  Only warp 0 stores (and fences): a system-scope fence per thread
   // of the CTA costs microseconds, one per lane of a single warp is one instruction.
   if (tid < 32) {
     for (int o = 0; o < a.n_owners; ++o) {
       float* slot = a.arena_peer[o] + (long long)a.cfg.worker * a.arena_floats + u.slot_off;
-      for (int x = tid; x < rcap; x += 32) slot[4 + x] = (x < count) ? sig[sel[x]] * selscale[x] : 0.f;
+      for (int x = tid; x < rcap; x += 32) slot[4 + x] = (x < count) ? sp.sig[sp.sel[x]] * sp.selscale[x] : 0.f;
       float* vout = slot + 4 + rcap;
       for (int e = tid; e < rcap * n; e += 32) {
         const int x = e / n, c = e - x * n;
-        vout[e] = (x < count) ? V[c * GS2 + sel[x]] : 0.f;
+        vout[e] = (x < count) ? V[c * SPECTRAL_PITCH + sp.sel[x]] : 0.f;
       }
       if (tid == 0) {
         int* hdr = reinterpret_cast<int*>(slot);
@@ -549,7 +336,7 @@ __global__ void __launch_bounds__(ENC_THREADS) v2_encode_kernel(const EncArgs a)
   if (s_last) {
     __threadfence();
     float* G = reinterpret_cast<float*>(tile);
-    float* V = G + V2_MAX_COLS * GS2;
+    float* V = G + V2_MAX_COLS * SPECTRAL_PITCH;
     eig_sample_unit(a, u, t.unit, G, V, red);
   }
 }
