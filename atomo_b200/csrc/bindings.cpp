@@ -105,6 +105,23 @@ void atomo_v2_launch_ps_qsgd(const void* units, const void* tiles, int tile0, in
                              long long arena_floats, int* sig, int* const* sig_peer, void* ctrl,
                              unsigned int* group_counter, long long timeout, long long* tstats, float inv_w, int grid,
                              cudaStream_t stream);
+// v2_entrywise.cu (entry-wise ATOMO units of the bf16 engine)
+void atomo_v2_launch_entry_stats(const void* units, const void* tiles, int tile0, int ntiles, const long long* gptr,
+                                 double* partials, unsigned int* unit_counters, double* l1, long long* tstats,
+                                 int group, cudaStream_t stream);
+void atomo_v2_launch_entry_encode(const void* units, const void* tiles, int tile0, int ntiles, const long long* gptr,
+                                  const double* l1, float* const* arena_peer, int* const* sig_peer, int n_owners,
+                                  long long arena_floats, int worker, int group, const void* ctrl,
+                                  unsigned int* group_counter, const float* ext_uniforms, long long* tstats,
+                                  int final_group, cudaStream_t stream);
+void atomo_v2_launch_ps_entry(const void* units, const void* tiles, int tile0, int ntiles, int W, int nranks,
+                              int group, int final_group, int owner, float* master, float* mom, float* sq,
+                              float* sqmax, float* vmom, float* vsq, float* vsqmax, void* wshadow_mc,
+                              void* const* wshadow_peer, float* vparams_local, float* vparams_mc,
+                              float* const* vparams_peer, const float* vgrads_mc, const float* const* vgrads_peer,
+                              const float* arenas, long long arena_floats, int* sig, int* const* sig_peer, void* ctrl,
+                              unsigned int* group_counter, long long timeout, long long* tstats, float inv_w, int grid,
+                              cudaStream_t stream);
 void atomo_v2_launch_advance_step(void* ctrl, cudaStream_t stream);
 void atomo_v2_launch_bcast_bytes(const void* src, void* const* peer, void* mc, int nranks, int self, long long nbytes,
                                  cudaStream_t stream);
@@ -450,6 +467,43 @@ void v2_ps_qsgd(uint64_t units, uint64_t tiles, int tile0, int ntiles, int W, in
                           cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
+// entry-wise ATOMO: the budget travels in the unit table, the L1 norms (fp64, one per entry unit) between the launches
+void v2_entry_stats(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t partials,
+                    uint64_t counters, uint64_t l1, uint64_t tstats, int group) {
+  TORCH_CHECK(partials != 0 && l1 != 0 && counters != 0, "v2_entry_stats: partials / counters / l1 required");
+  atomo_v2_launch_entry_stats(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
+                              P<double>(partials), P<unsigned int>(counters), P<double>(l1), P<long long>(tstats),
+                              group, cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+void v2_entry_encode(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t l1,
+                     uint64_t arena_peer, uint64_t sig_peer, int n_owners, int64_t arena_floats, int worker, int group,
+                     uint64_t ctrl, uint64_t group_counter, uint64_t ext_uniforms, uint64_t tstats, bool final_group) {
+  TORCH_CHECK(l1 != 0, "v2_entry_encode: needs the L1 norms of v2_entry_stats");
+  TORCH_CHECK(worker >= 0 && worker < 16, "v2_entry_encode: worker index must be in [0, 16)");
+  atomo_v2_launch_entry_encode(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
+                               P<const double>(l1), P<float* const>(arena_peer), P<int* const>(sig_peer), n_owners,
+                               arena_floats, worker, group, P<const void>(ctrl), P<unsigned int>(group_counter),
+                               P<const float>(ext_uniforms), P<long long>(tstats), final_group ? 1 : 0, cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+void v2_ps_entry(uint64_t units, uint64_t tiles, int tile0, int ntiles, int W, int nranks, int group, bool final_group,
+                 int owner, uint64_t master, uint64_t mom, uint64_t sq, uint64_t sqmax, uint64_t vmom, uint64_t vsq,
+                 uint64_t vsqmax, uint64_t wshadow_mc, uint64_t wshadow_peer, uint64_t vparams_local,
+                 uint64_t vparams_mc, uint64_t vparams_peer, uint64_t vgrads_mc, uint64_t vgrads_peer, uint64_t arenas,
+                 int64_t arena_floats, uint64_t sig, uint64_t sig_peer, uint64_t ctrl, uint64_t group_counter,
+                 int64_t timeout, uint64_t tstats, double inv_w, int grid) {
+  TORCH_CHECK(W >= 1 && W <= 16, "too many workers for v2_ps_entry");
+  atomo_v2_launch_ps_entry(P<const void>(units), P<const void>(tiles), tile0, ntiles, W, nranks, group,
+                           final_group ? 1 : 0, owner, P<float>(master), P<float>(mom), P<float>(sq), P<float>(sqmax),
+                           P<float>(vmom), P<float>(vsq), P<float>(vsqmax), P<void>(wshadow_mc),
+                           P<void* const>(wshadow_peer), P<float>(vparams_local), P<float>(vparams_mc),
+                           P<float* const>(vparams_peer), P<const float>(vgrads_mc), P<const float* const>(vgrads_peer),
+                           P<const float>(arenas), arena_floats, P<int>(sig), P<int* const>(sig_peer), P<void>(ctrl),
+                           P<unsigned int>(group_counter), timeout, P<long long>(tstats), (float)inv_w, grid,
+                           cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
 void v2_wait_params(uint64_t sig, int n_owners, uint64_t ctrl, int64_t timeout, uint64_t tstats) {
   atomo_v2_launch_wait_params(P<const int>(sig), n_owners, P<void>(ctrl), timeout, P<long long>(tstats), cur_stream());
 }
@@ -514,6 +568,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("v2_qsgd_stats", &v2_qsgd_stats);
   m.def("v2_qsgd_encode", &v2_qsgd_encode);
   m.def("v2_ps_qsgd", &v2_ps_qsgd);
+  m.def("v2_entry_stats", &v2_entry_stats);
+  m.def("v2_entry_encode", &v2_entry_encode);
+  m.def("v2_ps_entry", &v2_ps_entry);
   m.def("v2_wait_params", &v2_wait_params);
   m.def("v2_advance_step", &v2_advance_step);
   m.def("v2_bcast_bytes", &v2_bcast_bytes);

@@ -8,7 +8,7 @@
 namespace atomo {
 namespace v2 {
 
-enum Kind : int { KIND_SLAB = 1, KIND_MAT = 2, KIND_DENSE16 = 3, KIND_VEC = 4, KIND_QSGD = 5 };
+enum Kind : int { KIND_SLAB = 1, KIND_MAT = 2, KIND_DENSE16 = 3, KIND_VEC = 4, KIND_QSGD = 5, KIND_ENTRY = 6 };
 
 // One coding unit: a conv gradient in [O][K][I] (channels_last) layout ("SLAB": row (o,ri), column (b,k) of the
 // reference's (O*I/2, 2K) matricization is X_o[k][2ri+b]), a <=64-column block of a 2-D matrix ("MAT"), or a
@@ -18,6 +18,10 @@ enum Kind : int { KIND_SLAB = 1, KIND_MAT = 2, KIND_DENSE16 = 3, KIND_VEC = 4, K
 // the fields:  K = bucket (elements), I = q (quantization level), rows = buckets, cols = L (uint64 words per
 // bucket), rs = 1 for TernGrad (0 for QSGD), cs = buckets per PS tile, ps_rows = elements per PS tile,
 // ts_index = index among the QSGD units (TernGrad clip / stats counter).
+//
+// Entry-wise units ("ENTRY", v2_entrywise.cu: one per >= 2-D weight, tiles over the physical element order) use
+// budget = expected atoms s (clamped to [1, numel]), ps_rows = elements per tile (ENTRY_TILE_ELEMS),
+// ts_index = index among the entry units (L1 norm / stats counter).
 struct Unit2 {
   long long w_off;      // element offset of the unit's base in wshadow / master / momentum (VEC: in vparams)
   long long g_off;      // element offset inside the parameter's own gradient tensor
@@ -155,6 +159,18 @@ __host__ __device__ inline long long slot2_scale_off(int rows, int rcap, int col
 __host__ __device__ inline long long qsgd_norms_off(int n_ps) { return ((long long)n_ps + 3) & ~3LL; }
 __host__ __device__ inline long long qsgd_words_off(int n_ps, int rows) {
   return qsgd_norms_off(n_ps) + (((long long)rows + 3) & ~3LL);
+}
+
+// Entry-wise slots (floats, from Unit2::slot_off inside one worker arena):
+//   16-byte header per PS tile {int32 step stamp, int32 count, fp32 scale, pad} [n_ps] | per tile j, from
+//   entry_words_off(n_ps, j, ps_rows): room for ps_rows uint32 entries (the last tile: its length rounded up to 4).
+// Entry word: bits 0-11 element offset inside the tile, bit 12 set when p_i == 1 (the value is the bf16 gradient in
+// bits 16-31), else the value is copysign(scale, bf16 gradient).
+constexpr int ENTRY_TILE_ELEMS = 4096;
+constexpr uint32_t ENTRY_FLAG_EXACT = 1u << 12;
+__host__ __device__ inline long long entry_hdr_off(int j) { return 4LL * j; }
+__host__ __device__ inline long long entry_words_off(int n_ps, int j, int ps_rows) {
+  return 4LL * n_ps + (long long)j * ps_rows;
 }
 
 }  // namespace v2

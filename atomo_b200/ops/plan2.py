@@ -25,6 +25,9 @@ What changes against ``ops/plan.py`` (the fp32-flat plan of round 1):
 * **Quantizing codes** (``code="qsgd" | "terngrad"``, see :func:`build_plan2`): every >= 2-D weight is one
   ``QSGD`` unit whose buckets are quantized and bit-packed by the workers straight into the owners' arenas; the
   owners decode, sum and step the optimizer in one launch per group.
+* **Entry-wise ATOMO** (``code="entrywise"``): every >= 2-D weight is one ``ENTRY`` unit whose sampled entries are
+  compacted by the workers into 4-byte words in the owners' arenas; the owners scatter-add, average and step the
+  optimizer in one launch per group.
 
 Pure Python (unit-testable on CPU).  Struct layouts mirror ``csrc/v2_common.cuh``.
 """
@@ -34,7 +37,7 @@ import struct
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
-KIND_SLAB, KIND_MAT, KIND_DENSE16, KIND_VEC, KIND_QSGD = 1, 2, 3, 4, 5
+KIND_SLAB, KIND_MAT, KIND_DENSE16, KIND_VEC, KIND_QSGD, KIND_ENTRY = 1, 2, 3, 4, 5, 6
 RCAP_MAX = 32
 MAX_COLS = 64
 BLOCK_COLS = 32               # column-block width of MAT units (Jacobi cost ~ cols^3 sits in the encode launch)
@@ -49,6 +52,7 @@ V_ALIGN = 32                  # fp32 elements (128 B)
 QSGD_TILE_ELEMS = 4096        # a QSGD PS / encode tile holds max(1, 4096 // bucket) whole buckets
 QSGD_MAX_BUCKET = 1024        # one warp quantizes one bucket, staged in shared memory
 QSGD_MAX_LEVEL = 14           # (sign + 1) << q | level must fit 16 bits
+ENTRY_TILE_ELEMS = 4096       # entry-wise PS / encode tile: the element offset of an entry fits 12 bits
 
 UNIT_FMT = "<4q20i"           # 112 bytes, mirrors struct Unit2
 TILE_FMT = "<4i"              # unit, a, b, owner
@@ -97,6 +101,29 @@ def qsgd_words_off(n_ps: int, buckets: int) -> int:
 
 def qsgd_slot_floats(n_ps: int, buckets: int, words_per_bucket: int) -> int:
     return _round_up(qsgd_words_off(n_ps, buckets) + 2 * buckets * words_per_bucket, 32)
+
+
+def entry_hdr_off(j: int) -> int:
+    """Float offset (inside an entry slot) of PS tile ``j``'s header {int32 step stamp, int32 count, fp32 scale, pad}."""
+    return 4 * j
+
+
+def entry_words_off(n_ps: int, j: int, ps_rows: int = ENTRY_TILE_ELEMS) -> int:
+    """Float offset (inside an entry slot) of PS tile ``j``'s uint32 entries (16-byte aligned)."""
+    return 4 * n_ps + j * ps_rows
+
+
+def entry_slot_floats(numel: int, n_ps: int, ps_rows: int = ENTRY_TILE_ELEMS) -> int:
+    """Headers, then room for one entry per element of every tile (a tile never overflows)."""
+    last = numel - (n_ps - 1) * ps_rows
+    return _round_up(entry_words_off(n_ps, n_ps - 1, ps_rows) + _round_up(last, 4), 32)
+
+
+def entry_atoms(budget: float, numel: int) -> float:
+    """Expected atoms ``s`` of a tensor: ``budget * numel`` for a fraction, else ``budget``, clamped to
+    ``[1, numel]`` (``codings.entrywise.EntryWise.atoms_for``)."""
+    s = budget * numel if budget < 1.0 else budget
+    return float(min(max(s, 1.0), numel))
 
 
 def slot_capacity(cols: int, rank: int, systematic: bool) -> int:
@@ -159,7 +186,7 @@ class Unit2:
     own0: int = 0
     ps_tile0: int = 0
     n_ps: int = 0
-    ts_index: int = -1      # index among coded units (vsel / selcount / counters); QSGD: among QSGD units
+    ts_index: int = -1      # index among coded units (vsel / selcount / counters); QSGD / ENTRY: among those units
     ubits: int = 0          # 0: U stored fp32; 8: QSVD, U stochastically rounded to int8 with a per-row scale
 
     def pack(self) -> bytes:
@@ -191,7 +218,7 @@ class Plan2:
     stage_total: int        # bf16 elements of the dense-16 staging region
     arena_floats: int
     gpart_floats: int
-    n_coded: int            # units with per-unit device state (coded SLAB / MAT units, or the QSGD units)
+    n_coded: int            # units with per-unit device state (coded SLAB / MAT units, or the QSGD / ENTRY units)
     rank: int
     code: str
 
@@ -211,10 +238,16 @@ class Plan2:
         (the same sizes as ``codings.qsgd``'s ``words`` and ``norms``)."""
         return sum(8 * u.rows * u.cols + 4 * u.rows for u in self.units if u.kind == KIND_QSGD)
 
+    def entry_bytes(self) -> float:
+        """Bytes of entry-wise code a worker pushes per step: 4 per expected atom and a 16-byte header per PS tile.
+        An upper bound on the expectation (``sum(p_i) <= s``), exact when no ``p_i`` is clamped to 1."""
+        return sum(4.0 * u.budget + 16.0 * u.n_ps for u in self.units if u.kind == KIND_ENTRY)
+
     def expected_factor_bytes(self) -> float:
         """Bytes actually stored per worker and step for the expected number of atoms (U is written in groups
-        of 4 atoms); for the quantizing codes the words and norms of the QSGD units."""
-        tot = float(self.qsgd_bytes())
+        of 4 atoms); for the quantizing codes the words and norms of the QSGD units; for entry-wise ATOMO the
+        entries and tile headers."""
+        tot = float(self.qsgd_bytes()) + self.entry_bytes()
         for u in self.units:
             if u.coded:
                 atoms = min(u.budget if u.budget > 0 else u.cols, u.cols)
@@ -224,7 +257,7 @@ class Plan2:
 
     def dense_bytes(self) -> int:
         return sum((2 if u.kind == KIND_DENSE16 else 4) * u.numel for u in self.units
-                   if not u.coded and u.kind != KIND_QSGD)
+                   if not u.coded and u.kind not in (KIND_QSGD, KIND_ENTRY))
 
 
 def default_groups(shapes: Sequence[Sequence[int]], n_groups: int) -> List[int]:
@@ -271,8 +304,8 @@ def default_groups(shapes: Sequence[Sequence[int]], n_groups: int) -> List[int]:
 def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 3, systematic: bool = False,
                 n_owners: int = 1, n_groups: int = 4, groups: Optional[Sequence[int]] = None,
                 block_cols: int = BLOCK_COLS, min_coded_numel: int = 256, quantization_level: int = 4,
-                bucket_size: int = 512) -> Plan2:
-    """Plan of the bf16 engine for ``code`` in ``svd | qsvd | sgd | qsgd | terngrad``.
+                bucket_size: int = 512, entry_budget: float = 0.05) -> Plan2:
+    """Plan of the bf16 engine for ``code`` in ``svd | qsvd | sgd | qsgd | terngrad | entrywise``.
 
     ``qsgd`` / ``terngrad``: every >= 2-D weight (the 3-channel stem and the fc layers included) is exactly one
     ``KIND_QSGD`` unit; there are no ``DENSE16`` units.  1-D parameters stay ``KIND_VEC`` (fp32, summed by
@@ -294,9 +327,22 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
 
     ``Unit2`` fields of a QSGD unit: ``K`` = bucket, ``I`` = q, ``rows`` = buckets, ``cols`` = words per bucket,
     ``rs`` = 1 for TernGrad, ``cs`` = buckets per tile, ``ps_rows`` = elements per tile (``csrc/v2_common.cuh``).
+
+    ``entrywise``: every >= 2-D weight is exactly one ``KIND_ENTRY`` unit; 1-D parameters stay ``KIND_VEC`` as above
+    (the round-1 engine samples them too).  Per tensor:
+
+    * ``budget`` = the expected atom count ``s`` of ``codings.entrywise`` (:func:`entry_atoms` of ``entry_budget``);
+    * tiles of ``ENTRY_TILE_ELEMS`` elements run over the physical element order; encode tile == PS tile, and tile
+      ``j`` of a group belongs to owner ``j % n_owners``.  ``ps_tiles`` entries are (unit, first element, element
+      count, owner);
+    * the slot holds a 16-byte header per tile, then room for one uint32 entry per element of every tile
+      (:func:`entry_hdr_off` / :func:`entry_words_off`), so a tile cannot overflow.
     """
     shapes = [tuple(int(d) for d in s) for s in shapes]
     quant = code in ("qsgd", "terngrad")
+    entry = code == "entrywise"
+    if entry and not entry_budget > 0:
+        raise ValueError("entry_budget must be positive (a fraction of numel below 1, else an atom count)")
     if quant:
         q, bsz = int(quantization_level), int(bucket_size)
         if not 1 <= q <= QSGD_MAX_LEVEL:
@@ -343,6 +389,10 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             add(Unit2(0, KIND_QSGD, p.index, p.widx, p.off, 0, rows=nb, cols=qsgd_words_per_bucket(bucket, q),
                       K=bucket, I=q, rs=1 if code == "terngrad" else 0, cs=bpt, numel=p.numel, group=p.group,
                       ps_rows=bpt * bucket))
+            continue
+        if entry:
+            add(Unit2(0, KIND_ENTRY, p.index, p.widx, p.off, 0, budget=entry_atoms(float(entry_budget), p.numel),
+                      numel=p.numel, group=p.group, ps_rows=ENTRY_TILE_ELEMS))
             continue
         coded = code == "svd" and p.numel >= min_coded_numel
         if coded and len(s) == 4 and s[2] * s[3] > 1:
@@ -410,11 +460,11 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             elif u.kind == KIND_DENSE16:
                 for e0 in range(0, u.numel, 8192):     # staging copy tiles
                     enc_tiles.append((u.index, e0, min(8192, u.numel - e0), 0))
-            elif u.kind == KIND_QSGD:                 # encode tiles = PS tiles (one destination owner per CTA)
+            elif u.kind in (KIND_QSGD, KIND_ENTRY):   # encode tiles = PS tiles (one destination owner per CTA)
                 for j, e0 in enumerate(range(0, u.numel, u.ps_rows)):
                     enc_tiles.append((u.index, e0, min(u.ps_rows, u.numel - e0), j))
             u.n_enc = len(enc_tiles) - u.enc_tile0
-            if u.kind == KIND_QSGD:
+            if u.kind in (KIND_QSGD, KIND_ENTRY):
                 u.ts_index = n_coded
                 n_coded += 1
                 u.ps_tile0 = len(ps_by_group[g])
@@ -423,7 +473,10 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 u.n_ps = len(ps_by_group[g]) - u.ps_tile0
                 u.own0 = u.ps_tile0 % n_owners
                 u.slot_off = slot_off
-                slot_off += qsgd_slot_floats(u.n_ps, u.rows, u.cols)
+                if u.kind == KIND_QSGD:
+                    slot_off += qsgd_slot_floats(u.n_ps, u.rows, u.cols)
+                else:
+                    slot_off += entry_slot_floats(u.numel, u.n_ps, u.ps_rows)
             elif u.coded:
                 u.ts_index = n_coded
                 n_coded += 1

@@ -22,6 +22,10 @@ one central PS kernel at the end of the step):
   buckets are quantized and bit-packed by the workers during backward straight into the owners' arenas
   (``csrc/v2_qsgd.cu``, TernGrad adds a per-tensor clip launch), and the owners decode, sum and step the
   optimizer in one launch per group.  BN and bias vectors stay fp32 (``multimem.ld_reduce``).
+* **Entry-wise ATOMO** (``code="entrywise"``, ``entry_budget``): every weight tensor is one entry unit; a stats
+  launch takes its fp64 L1 norm, the encode launch samples entries with ``p_i = min(1, s |g_i| / ||g||_1)`` and
+  pushes them as 4-byte words (``csrc/v2_entrywise.cu``), and the owners scatter-add them in worker order and step
+  the optimizer.  BN and bias vectors stay fp32, as above.
 * Optimizers fused in the PS epilogue: momentum-SGD (``src/optim/sgd.py:57-90``), Adam / AMSGrad
   (``src/optim/adam.py:37-94``).
 
@@ -61,16 +65,24 @@ class ShadowEngine:
                  ps_grid: int = 0, overlap: bool = True, fused_bn: bool = True, num_aggregate: int = 0,
                  warm_start: bool = True, max_sweeps: int = 1, main_priority: int = 0, debug_jitter_us: float = 0.0,
                  side_priority: int = -1, resample_empty: bool = False, quantization_level: int = 4,
-                 bucket_size: int = 512):
+                 bucket_size: int = 512, entry_budget: float = 0.05):
+        self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
+        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise"):
+            raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise")
+        self.entry = self.code == "entrywise"
+        self.entry_budget = float(entry_budget)
+        if self.entry:      # checked before any CUDA work
+            if prob_rule != "reference" or sampling != "bernoulli":
+                raise ValueError("entrywise on ShadowEngine samples with prob_rule='reference' and "
+                                 "sampling='bernoulli' only (got %r / %r)" % (prob_rule, sampling))
+            if not self.entry_budget > 0:
+                raise ValueError("entry_budget must be positive (a fraction of numel below 1, else an atom count)")
         self.C = load_ext()
         C = self.C
         assert C.v2_unit_bytes() == P2.UNIT_BYTES and C.v2_ctrl_bytes() == P2.CTRL2_BYTES
         self.rank, self.world, self.group = rank, world, group
         self.device = device or torch.device("cuda", torch.cuda.current_device())
         dev = self.device
-        self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
-        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad"):
-            raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad (entrywise runs on FusedEngine)")
         self.svd_rank = int(svd_rank)
         self.quant = self.code in ("qsgd", "terngrad")
         self.quantization_level, self.bucket_size = int(quantization_level), int(bucket_size)
@@ -123,7 +135,7 @@ class ShadowEngine:
         shapes = [tuple(p.shape) for p in self.params]
         self.plan = P2.build_plan2(shapes, self.code, self.svd_rank, self.systematic, n_owners=self.n_owners,
                                    n_groups=groups if overlap else 1, quantization_level=self.quantization_level,
-                                   bucket_size=self.bucket_size)
+                                   bucket_size=self.bucket_size, entry_budget=self.entry_budget)
         pl = self.plan
         self.G = pl.n_groups
 
@@ -217,7 +229,7 @@ class ShadowEngine:
         # eigenbasis of the previous step per coded unit (Jacobi warm start); identity to begin with
         self.max_sweeps = int(max_sweeps) if warm_start else 0
         self.vprev = None
-        if warm_start and not self.quant:
+        if warm_start and not self.quant and not self.entry:
             self.vprev = z(nc * P2.MAX_COLS * P2.MAX_COLS)
             for u in pl.units:
                 if u.coded:
@@ -231,6 +243,11 @@ class ShadowEngine:
         if self.code == "terngrad":
             self.clip = z(nc)
             self.clip_partials = torch.zeros(2 * max(len(pl.enc_tiles), 1), dtype=torch.float64, device=dev)
+        # entry-wise: fp64 L1 norm per unit and its per-tile partials
+        self.l1 = self.l1_partials = None
+        if self.entry:
+            self.l1 = torch.zeros(nc, dtype=torch.float64, device=dev)
+            self.l1_partials = torch.zeros(max(len(pl.enc_tiles), 1), dtype=torch.float64, device=dev)
         self.counters = torch.zeros(nc + 2 * P2.MAX_GROUPS + 8, dtype=torch.int32, device=dev)
         self.cnt_enc_group = self.counters.data_ptr() + 4 * nc
         self.cnt_ps_group = self.cnt_enc_group + 4 * P2.MAX_GROUPS
@@ -347,6 +364,17 @@ class ShadowEngine:
                              self.code == "terngrad")
             self._nlaunch += 1
             return
+        if nt > 0 and self.entry:
+            # per-tensor L1 norms, then sample + compact + push into the owners' arenas (raises the push flag)
+            C.v2_entry_stats(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
+                             self.l1_partials.data_ptr(), self.counters.data_ptr(), self.l1.data_ptr(),
+                             self.tstats.data_ptr(), g)
+            C.v2_entry_encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
+                              self.l1.data_ptr(), self.t_arena_peer.data_ptr(), self.t_sig_owner.data_ptr(),
+                              self.n_owners, pl.arena_floats, self.worker_index, g, self.ctrl.data_ptr(),
+                              self.cnt_enc_group + 4 * g, 0, self.tstats.data_ptr(), self._fired == self.G)
+            self._nlaunch += 2
+            return
         if nt > 0 and self.code in ("svd", "qsvd"):
             C.v2_encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
                         self.gpart.data_ptr(), self.counters.data_ptr(), self.vsel.data_ptr(),
@@ -384,6 +412,17 @@ class ShadowEngine:
                          self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
                          self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
                          max(1, min(self.ps_grid, max(nt, 1))), self.q_max_level, self.q_max_bucket)
+            self._nlaunch += 1
+            return
+        if self.entry:
+            C.v2_ps_entry(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g, final,
+                          self.owner_index, p(self.master), p(self.mom), p(self.sq), p(self.sqmax), p(self.vmom),
+                          p(self.vsq), p(self.vsqmax), self.wshadow_mc, self.t_wshadow_peer.data_ptr(),
+                          self.vparams.data_ptr(), self.vparams_mc, self.t_vparams_peer.data_ptr(), self.vgrads_mc,
+                          self.t_vgrads_peer.data_ptr(), self.heap.region_ptr("arena"), pl.arena_floats,
+                          self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
+                          self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
+                          max(1, min(self.ps_grid, max(nt, 1))))
             self._nlaunch += 1
             return
         C.v2_ps(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g, final,
@@ -542,7 +581,7 @@ class ShadowEngine:
             u = pl.units[ui]
             if u.kind == P2.KIND_VEC:
                 mv[u.w_off + a:u.w_off + a + b] = 1
-            elif u.kind in (P2.KIND_DENSE16, P2.KIND_QSGD):     # QSGD tiles: (first element, element count)
+            elif u.kind in (P2.KIND_DENSE16, P2.KIND_QSGD, P2.KIND_ENTRY):   # (first element, element count)
                 mw[u.w_off + a:u.w_off + a + b] = 1
             elif u.kind == P2.KIND_SLAB:
                 half = u.I // 2
@@ -616,6 +655,8 @@ class ShadowEngine:
                 "svd_rank": self.svd_rank, "engine": "shadow"}
         if self.quant:
             side.update(quantization_level=self.quantization_level, bucket_size=self.bucket_size)
+        if self.entry:
+            side.update(entry_budget=self.entry_budget)
         side.update(adam_state)
         torch.save(side, path + "_optim.tmp")
         os.replace(path + "_optim.tmp", path + "_optim")
