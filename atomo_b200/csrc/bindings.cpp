@@ -149,6 +149,12 @@ void atomo_launch_entrywise_encode(const float* grad, const void* layers, const 
 void atomo_launch_entrywise_scatter(const int* const* idx, const float* const* val, const int* const* count, int W,
                                     int capacity, float* out_sum, long long numel, const int* push_flags,
                                     void* ctrl, long long timeout_ticks, cudaStream_t stream);
+// data_kernels.cu
+void atomo_launch_augment_gather(const void* src, int src_u8, const long long* labels, int C, int H, int W,
+                                 const int* order, long long pos0, int B, const float* mean_std, int pad, int reflect,
+                                 int augment, unsigned long long seed, int epoch, const int* ext_draws, float* x,
+                                 long long sx_n, long long sx_c, long long sx_h, long long sx_w, long long* y,
+                                 cudaStream_t stream);
 }
 
 namespace {
@@ -513,6 +519,46 @@ void v2_bcast_bytes(uint64_t src, uint64_t peer, uint64_t mc, int nranks, int se
                               cur_stream());
 }
 
+// ---------------------------------------------------------------------------------------------- training input
+// src [N, H, W, C] uint8 or fp32, labels [N] int64, order int32 (the epoch's sample order), mean_std [2, C] fp32,
+// ext_draws [B, 3] int32 (tests); writes x [B, C, H, W] fp32 at its own strides and y [B] int64.
+void augment_gather(const torch::Tensor& src, const torch::Tensor& labels, const torch::Tensor& order, int64_t pos0,
+                    const torch::Tensor& mean_std, int pad, bool reflect, bool augment, uint64_t seed, int64_t epoch,
+                    c10::optional<torch::Tensor> ext_draws, torch::Tensor x, torch::Tensor y) {
+  TORCH_CHECK(src.is_cuda() && src.dim() == 4 && src.is_contiguous(), "src must be a contiguous CUDA [N, H, W, C]");
+  const bool u8 = src.scalar_type() == torch::kUInt8;
+  TORCH_CHECK(u8 || src.scalar_type() == torch::kFloat32, "src must be uint8 or float32");
+  const int64_t N = src.size(0), H = src.size(1), W = src.size(2), C = src.size(3);
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == torch::kFloat32 && x.dim() == 4, "x must be a CUDA fp32 [B, C, H, W]");
+  const int64_t B = x.size(0);
+  TORCH_CHECK(x.size(1) == C && x.size(2) == H && x.size(3) == W, "x must be [B, C, H, W] of src's image shape");
+  TORCH_CHECK(y.is_cuda() && y.scalar_type() == torch::kInt64 && y.is_contiguous() && y.numel() == B,
+              "y must be a contiguous CUDA int64 [B]");
+  TORCH_CHECK(labels.is_cuda() && labels.scalar_type() == torch::kInt64 && labels.is_contiguous() &&
+                  labels.numel() == N, "labels must be a contiguous CUDA int64 [N]");
+  TORCH_CHECK(order.is_cuda() && order.scalar_type() == torch::kInt32 && order.is_contiguous(),
+              "order must be a contiguous CUDA int32 tensor");
+  TORCH_CHECK(pos0 >= 0 && pos0 + B <= order.numel(), "the batch runs past the end of the order");
+  TORCH_CHECK(mean_std.is_cuda() && mean_std.scalar_type() == torch::kFloat32 && mean_std.is_contiguous() &&
+                  mean_std.numel() == 2 * C, "mean_std must be a contiguous CUDA fp32 [2, C]");
+  TORCH_CHECK(pad >= 0 && (!u8 || !reflect || (pad < H && pad < W)), "reflect padding needs pad < H and pad < W");
+  TORCH_CHECK(u8 || (pad == 0 && !augment), "fp32 sources are gathered without augmentation");
+  if (ext_draws.has_value()) {
+    TORCH_CHECK(ext_draws->is_cuda() && ext_draws->scalar_type() == torch::kInt32 && ext_draws->is_contiguous() &&
+                    ext_draws->numel() == 3 * B, "ext_draws must be a contiguous CUDA int32 [B, 3]");
+  }
+  for (const torch::Tensor* t : std::initializer_list<const torch::Tensor*>{&labels, &order, &mean_std, &x, &y})
+    TORCH_CHECK(t->device() == src.device(), "all tensors must be on src's device");
+  c10::cuda::CUDAGuard guard(src.device());
+  atomo_launch_augment_gather(src.data_ptr(), u8 ? 1 : 0, static_cast<const long long*>(labels.data_ptr()), (int)C,
+                              (int)H, (int)W, order.data_ptr<int>(), pos0, (int)B, mean_std.data_ptr<float>(), pad,
+                              reflect ? 1 : 0, augment ? 1 : 0, seed, (int)epoch,
+                              ext_draws.has_value() ? ext_draws->data_ptr<int>() : nullptr, x.data_ptr<float>(),
+                              x.stride(0), x.stride(1), x.stride(2), x.stride(3), static_cast<long long*>(y.data_ptr()),
+                              cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -574,6 +620,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("v2_wait_params", &v2_wait_params);
   m.def("v2_advance_step", &v2_advance_step);
   m.def("v2_bcast_bytes", &v2_bcast_bytes);
+  m.def("augment_gather", &augment_gather, py::arg("src"), py::arg("labels"), py::arg("order"), py::arg("pos0"),
+        py::arg("mean_std"), py::arg("pad"), py::arg("reflect"), py::arg("augment"), py::arg("seed"),
+        py::arg("epoch"), py::arg("ext_draws"), py::arg("x"), py::arg("y"));
   m.def("v2_unit_bytes", &atomo_v2_unit_bytes);
   m.def("v2_ctrl_bytes", &atomo_v2_ctrl_bytes);
   m.def("v2_enc_smem", &atomo_v2_enc_smem);

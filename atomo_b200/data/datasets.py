@@ -25,6 +25,8 @@ from .synthetic import SHAPES, synthetic_pair
 
 _CIFAR_MEAN = [x / 255.0 for x in [125.3, 123.0, 113.9]]
 _CIFAR_STD = [x / 255.0 for x in [63.0, 62.1, 66.7]]
+_SVHN_MEAN, _SVHN_STD = (0.4914, 0.4822, 0.4465), (0.2023, 0.1994, 0.2010)
+_MNIST_MEAN, _MNIST_STD = (0.1307,), (0.3081,)
 
 
 def num_classes_of(name: str) -> int:
@@ -104,33 +106,49 @@ MNISTDataset = BatchDataset
 Cifar10Dataset = BatchDataset
 
 
+def real_transforms(name: str):
+    """(train, test) torchvision transforms of the real ``--dataset name`` (mnist, cifar10, cifar100, svhn,
+    imagenet).  ``data.gpu_loader`` reproduces the same pipeline on the device."""
+    from torchvision import transforms as T
+
+    k = name.lower()
+    if k == "mnist":
+        tf = T.Compose([T.ToTensor(), T.Normalize(_MNIST_MEAN, _MNIST_STD)])
+        return tf, tf
+    if k in ("cifar10", "cifar100", "imagenet"):
+        norm = T.Normalize(_CIFAR_MEAN, _CIFAR_STD)
+        size = 227 if k == "imagenet" else 32
+        pre = [T.Resize((227, 227))] if k == "imagenet" else []
+        train_tf = T.Compose(pre + [T.RandomCrop(size, padding=4, padding_mode="reflect"),
+                                    T.RandomHorizontalFlip(), T.ToTensor(), norm])
+        return train_tf, T.Compose(pre + [T.ToTensor(), norm])
+    if k == "svhn":
+        norm = T.Normalize(_SVHN_MEAN, _SVHN_STD)
+        train_tf = T.Compose([T.RandomCrop(32, padding=4), T.RandomHorizontalFlip(), T.ToTensor(), norm])
+        return train_tf, T.Compose([T.ToTensor(), norm])
+    raise ValueError("no real-data transforms for dataset %r" % name)
+
+
 def _real_pair(name: str, root: str):
     """Try to build (train, test) from files already on disk; None if absent."""
     try:
-        from torchvision import datasets as tvd, transforms as T
+        from torchvision import datasets as tvd
     except Exception:
         return None
     k = name.lower()
     try:
         if k == "mnist":
-            tf = T.Compose([T.ToTensor(), T.Normalize((0.1307,), (0.3081,))])
-            return (tvd.MNIST(os.path.join(root, "mnist_data"), train=True, download=False, transform=tf),
-                    tvd.MNIST(os.path.join(root, "mnist_data"), train=False, download=False, transform=tf))
+            train_tf, test_tf = real_transforms(k)
+            return (tvd.MNIST(os.path.join(root, "mnist_data"), train=True, download=False, transform=train_tf),
+                    tvd.MNIST(os.path.join(root, "mnist_data"), train=False, download=False, transform=test_tf))
         if k in ("cifar10", "cifar100", "imagenet"):
-            norm = T.Normalize(_CIFAR_MEAN, _CIFAR_STD)
-            size = 227 if k == "imagenet" else 32
-            pre = [T.Resize((227, 227))] if k == "imagenet" else []
-            train_tf = T.Compose(pre + [T.RandomCrop(size, padding=4, padding_mode="reflect"),
-                                        T.RandomHorizontalFlip(), T.ToTensor(), norm])
-            test_tf = T.Compose(pre + [T.ToTensor(), norm])
+            train_tf, test_tf = real_transforms(k)
             cls = tvd.CIFAR100 if k == "cifar100" else tvd.CIFAR10
             sub = "cifar100_data" if k == "cifar100" else "cifar10_data"
             return (cls(os.path.join(root, sub), train=True, download=False, transform=train_tf),
                     cls(os.path.join(root, sub), train=False, download=False, transform=test_tf))
         if k == "svhn":
-            norm = T.Normalize((0.4914, 0.4822, 0.4465), (0.2023, 0.1994, 0.2010))
-            train_tf = T.Compose([T.RandomCrop(32, padding=4), T.RandomHorizontalFlip(), T.ToTensor(), norm])
-            test_tf = T.Compose([T.ToTensor(), norm])
+            train_tf, test_tf = real_transforms(k)
             return (SVHN(os.path.join(root, "svhn_data"), "train", train_tf),
                     SVHN(os.path.join(root, "svhn_data"), "test", test_tf))
     except Exception:

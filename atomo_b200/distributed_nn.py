@@ -61,6 +61,9 @@ def run_rank(args) -> None:
     if backend == "p2p":
         from .runtime.engine import run_p2p_training
         return run_p2p_training(args)
+    if getattr(args, "gpu_data", False):
+        raise SystemExit("--gpu-data builds batches for the --backend p2p engines; the %s backend's workers read "
+                         "the CPU loader (run without --gpu-data)" % backend)
 
     if not dist.is_initialized():
         os.environ.setdefault("MASTER_ADDR", args.master_addr)

@@ -97,9 +97,17 @@ def run_p2p_training(args, device=None):
     first = eng.first_worker
     nworkers = eng.W
     shard = shard_dataset(train_set, max(rank - first, 0), nworkers, seed=args.seed)
-    loader = DataLoader(shard, batch_size=args.batch_size, shuffle=True, seed=args.seed + rank, drop_last=True,
-                        pin_memory=True, prefetch=2)
-    test_loader = torch.utils.data.DataLoader(test_set, batch_size=args.test_batch_size, shuffle=False)
+    if getattr(args, "gpu_data", False):
+        from ..data.gpu_loader import GpuLoader
+        # the layout each engine's static input has: channels_last on the shadow engine, as the CPU batches otherwise
+        loader = GpuLoader(shard, args.batch_size, args.dataset, train=True, seed=args.seed + rank, device=dev,
+                           channels_last=kind == "shadow")
+        test_loader = GpuLoader(test_set, args.test_batch_size, args.dataset, train=False, device=dev,
+                                channels_last=kind == "shadow")
+    else:
+        loader = DataLoader(shard, batch_size=args.batch_size, shuffle=True, seed=args.seed + rank, drop_last=True,
+                            pin_memory=True, prefetch=2)
+        test_loader = torch.utils.data.DataLoader(test_set, batch_size=args.test_batch_size, shuffle=False)
     x0, y0 = loader.next_batch()
     eng.prepare(x0, y0, warmup=2 if args.max_steps < 8 else 3)   # eager warm-up steps (cuDNN autotune) count as steps
     if getattr(args, "resume", False):

@@ -82,4 +82,7 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
     p.add_argument("--master-addr", type=str, default="127.0.0.1")
     p.add_argument("--master-port", type=int, default=29511)
     p.add_argument("--eval-batches", type=int, default=0, help="cap test batches per evaluation (0 = all)")
+    p.add_argument("--gpu-data", type=bool_flag, default=False,
+                   help="p2p backend: keep the rank's shard and the test set on the GPU and build every batch there "
+                        "(same sample order and augmentation as the CPU loader; not for --dataset ImageNet)")
     return p.parse_args(argv)
