@@ -122,6 +122,14 @@ void atomo_v2_launch_ps_entry(const void* units, const void* tiles, int tile0, i
                               const float* arenas, long long arena_floats, int* sig, int* const* sig_peer, void* ctrl,
                               unsigned int* group_counter, long long timeout, long long* tstats, float inv_w, int grid,
                               cudaStream_t stream);
+// v2_stats.cu (estimator statistics of the bf16 engine, --code-stats)
+int atomo_v2_stats_fields();
+int atomo_v2_stats_partials();
+void atomo_v2_launch_code_stats(const void* units, const void* tiles, int tile0, int ntiles, const long long* gptr,
+                                const float* sigma, const int* selcount, const double* l1, const float* clip,
+                                float* const* arena_peer, int n_owners, long long arena_floats, int worker,
+                                int random_sample, int waterfill, double* partials, unsigned int* unit_counters,
+                                double* acc, cudaStream_t stream);
 void atomo_v2_launch_advance_step(void* ctrl, cudaStream_t stream);
 void atomo_v2_launch_bcast_bytes(const void* src, void* const* peer, void* mc, int nranks, int self, long long nbytes,
                                  cudaStream_t stream);
@@ -493,6 +501,20 @@ void v2_entry_encode(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint
                                P<const float>(ext_uniforms), P<long long>(tstats), final_group ? 1 : 0, cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
+// estimator statistics of one group: after the group's push, on the same stream
+void v2_code_stats(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t sigma,
+                   uint64_t selcount, uint64_t l1, uint64_t clip, uint64_t arena_peer, int n_owners,
+                   int64_t arena_floats, int worker, bool random_sample, bool waterfill, uint64_t partials,
+                   uint64_t counters, uint64_t acc) {
+  TORCH_CHECK(partials != 0 && counters != 0 && acc != 0, "v2_code_stats: partials / counters / acc required");
+  TORCH_CHECK(worker >= 0 && worker < 16, "v2_code_stats: worker index must be in [0, 16)");
+  atomo_v2_launch_code_stats(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
+                             P<const float>(sigma), P<const int>(selcount), P<const double>(l1), P<const float>(clip),
+                             P<float* const>(arena_peer), n_owners, arena_floats, worker, random_sample ? 1 : 0,
+                             waterfill ? 1 : 0, P<double>(partials), P<unsigned int>(counters), P<double>(acc),
+                             cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
 void v2_ps_entry(uint64_t units, uint64_t tiles, int tile0, int ntiles, int W, int nranks, int group, bool final_group,
                  int owner, uint64_t master, uint64_t mom, uint64_t sq, uint64_t sqmax, uint64_t vmom, uint64_t vsq,
                  uint64_t vsqmax, uint64_t wshadow_mc, uint64_t wshadow_peer, uint64_t vparams_local,
@@ -617,6 +639,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("v2_entry_stats", &v2_entry_stats);
   m.def("v2_entry_encode", &v2_entry_encode);
   m.def("v2_ps_entry", &v2_ps_entry);
+  m.def("v2_code_stats", &v2_code_stats);
+  m.def("v2_stats_fields", &atomo_v2_stats_fields);
+  m.def("v2_stats_partials", &atomo_v2_stats_partials);
   m.def("v2_wait_params", &v2_wait_params);
   m.def("v2_advance_step", &v2_advance_step);
   m.def("v2_bcast_bytes", &v2_bcast_bytes);

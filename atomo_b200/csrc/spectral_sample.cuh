@@ -31,6 +31,33 @@ struct SampleCfg {
   uint32_t tag;
 };
 
+// Inclusion probabilities of a randomly sampled unit (svd.py:49-67), written by one thread: prob[i] for the n singular
+// values sig[i], where order[k] is the index of the k-th largest, total their sum and smax the largest (>= 1e-6).
+// budget <= 0: p_i = sigma_i / sigma_max; else the reference's clip p_i = min(1, budget sigma_i / total), or
+// water-filling, which pins the largest atoms to 1.  Shared by the sampler below and the estimator statistics
+// (v2_stats.cu), so both see the same p_i.
+__device__ __forceinline__ void spectral_probs(const float* sig, const int* order, int n, float budget, int waterfill,
+                                               float total, float smax, float* prob) {
+  if (budget <= 0.f) {
+    for (int i = 0; i < n; ++i) prob[i] = fminf(sig[i] / smax, 1.f);
+  } else if (!waterfill) {
+    for (int i = 0; i < n; ++i) prob[i] = fminf(budget * sig[i] / total, 1.f);
+  } else {
+    const float bud = fminf(budget, (float)n);
+    float rest = total;
+    int pinned = 0;
+    while (pinned < n) {
+      const float s0 = sig[order[pinned]];
+      if (rest > 0.f && (bud - pinned) * s0 >= rest && (bud - pinned) > 0.f) { rest -= s0; ++pinned; }
+      else break;
+    }
+    for (int k = 0; k < n; ++k) {
+      const int i = order[k];
+      prob[i] = (k < pinned) ? 1.f : (rest > 0.f ? fminf((bud - pinned) * sig[i] / rest, 1.f) : 0.f);
+    }
+  }
+}
+
 // The core's results, in shared memory; valid until the caller's kernel ends.
 struct Spectrum {
   int count;              // atoms selected
@@ -195,25 +222,7 @@ __device__ __forceinline__ Spectrum eig_sample(float* G, float* V, int n, bool w
       count = k;
       s_done = 1;
     } else {
-      if (budget <= 0.f) {
-        for (int i = 0; i < n; ++i) prob[i] = fminf(sig[i] / smax, 1.f);
-      } else if (!cfg.waterfill) {
-        for (int i = 0; i < n; ++i) prob[i] = fminf(budget * sig[i] / total, 1.f);
-      } else {
-        // water-filling over the sorted spectrum: pin the largest atoms to 1
-        const float bud = fminf(budget, (float)n);
-        float rest = total;
-        int pinned = 0;
-        while (pinned < n) {
-          const float s0 = sig[order[pinned]];
-          if (rest > 0.f && (bud - pinned) * s0 >= rest && (bud - pinned) > 0.f) { rest -= s0; ++pinned; }
-          else break;
-        }
-        for (int k = 0; k < n; ++k) {
-          const int i = order[k];
-          prob[i] = (k < pinned) ? 1.f : (rest > 0.f ? fminf((bud - pinned) * sig[i] / rest, 1.f) : 0.f);
-        }
-      }
+      spectral_probs(sig, order, n, budget, cfg.waterfill, total, smax, prob);
       s_done = 0;
     }
     s_count = count;

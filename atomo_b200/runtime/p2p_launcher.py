@@ -50,12 +50,19 @@ def _build_engine(args, model, rank, world):
         kw = {}
         if code in ("qsgd", "terngrad"):
             kw = dict(quantization_level=args.quantization_level, bucket_size=args.bucket_size)
+        if getattr(args, "code_stats", False):
+            if code == "qsvd":
+                raise SystemExit("--code-stats does not model QSVD's int8 left factors (use --code svd)")
+            kw["code_stats"] = True
         return ShadowEngine(model, rank, world, code=args.code, svd_rank=args.svd_rank, lr=args.lr,
                             momentum=args.momentum, weight_decay=args.weight_decay, nesterov=args.nesterov,
                             optimizer=args.optimizer, ps_mode=args.ps_mode, groups=args.groups, sampling=args.sampling,
                             prob_rule=args.prob_rule, seed=args.seed, num_aggregate=args.num_aggregate,
                             timeout_s=args.flag_timeout, **kw), "shadow"
     from .engine import FusedEngine
+    if getattr(args, "code_stats", False):
+        raise SystemExit("--code-stats reads the statistics of the bf16 engine (--dtype bf16, --engine auto|shadow); "
+                         "the fp32-flat engine does not compute them (run without --code-stats)")
     if args.optimizer != "sgd":
         raise SystemExit("--optimizer adam on the p2p backend needs --dtype bf16 with --code svd|sgd, or --engine "
                          "shadow with --code qsgd|terngrad (ShadowEngine); the fp32-flat engine fuses momentum-SGD only")
@@ -127,6 +134,8 @@ def run_p2p_training(args, device=None):
     ev_a.record()
     since = 0
     eng.phase_stats(reset=True)
+    if getattr(args, "code_stats", False) and eng.is_worker:
+        eng.code_stats(reset=True)              # the first record covers the logged steps only, like phase_stats
 
     def collective_barrier():
         if on_gpu:
@@ -156,8 +165,11 @@ def run_p2p_training(args, device=None):
                                   step_s, comp, enc, comm, msg_mb, p1, p5))
             if eng.is_ps or (kind == "shadow" and eng.is_owner):
                 print(master_line(cur, ph.get("ps_work_us", 0.0) / 1e6, eng.lr, ph.get("ps_wait_push_us", 0.0) / 1e6))
+            extra = {}
+            if getattr(args, "code_stats", False) and eng.is_worker:
+                extra["code_stats"] = eng.code_stats(reset=True)
             metrics.write(step=cur, loss=loss, prec1=p1, prec5=p5, step_s=step_s, comp=comp, encode=enc, comm=comm,
-                          msg_mb=msg_mb, lr=eng.lr, phase_us={k: round(float(v), 1) for k, v in ph.items()})
+                          msg_mb=msg_mb, lr=eng.lr, phase_us={k: round(float(v), 1) for k, v in ph.items()}, **extra)
             ev_a.record()
             since = 0
         if cur % args.eval_freq == 0:

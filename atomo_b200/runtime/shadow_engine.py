@@ -65,10 +65,16 @@ class ShadowEngine:
                  ps_grid: int = 0, overlap: bool = True, fused_bn: bool = True, num_aggregate: int = 0,
                  warm_start: bool = True, max_sweeps: int = 1, main_priority: int = 0, debug_jitter_us: float = 0.0,
                  side_priority: int = -1, resample_empty: bool = False, quantization_level: int = 4,
-                 bucket_size: int = 512, entry_budget: float = 0.05):
+                 bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False):
         self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
         if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise"):
             raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise")
+        if code_stats:      # checked before any CUDA work: the closed forms of code_stats() do not hold for these
+            if self.code == "qsvd":
+                raise ValueError("code_stats does not model the int8 quantization of QSVD's left factors")
+            if resample_empty:
+                raise ValueError("code_stats needs resample_empty=False: redrawing empty selections biases the "
+                                 "estimator, and the closed-form error no longer holds")
         self.entry = self.code == "entrywise"
         self.entry_budget = float(entry_budget)
         if self.entry:      # checked before any CUDA work
@@ -272,6 +278,14 @@ class ShadowEngine:
         sm = torch.cuda.get_device_properties(dev).multi_processor_count
         self.ps_grid = ps_grid or 3 * sm
         self.tstats = torch.zeros(32, dtype=torch.int64, device=dev)
+        # --code-stats: per coded unit fp64 sums over steps (v2_stats.cu), the per-tile partials and unit counters
+        self.code_stats_on = bool(code_stats)
+        self.stats_acc = self.stats_partials = self.stats_counters = None
+        if self.code_stats_on and self.code != "sgd":
+            self.stats_acc = torch.zeros(nc * C.v2_stats_fields(), dtype=torch.float64, device=dev)
+            self.stats_partials = torch.zeros(max(len(pl.enc_tiles), 1) * C.v2_stats_partials(), dtype=torch.float64,
+                                              device=dev)
+            self.stats_counters = torch.zeros(nc, dtype=torch.int32, device=dev)
         self.loss_buf = torch.zeros(3, dtype=torch.float32, device=dev)
         self.static_x = self.static_y = self.graph = None
 
@@ -328,6 +342,77 @@ class ShadowEngine:
         if reset:
             self.tstats[:9].zero_()
         return out
+
+    def code_stats(self, reset: bool = True) -> dict:
+        """Estimator statistics of this worker's code since the last reset (``code_stats=True``), as means per step:
+        per parameter tensor (the block units of a tensor summed) and for the whole model,
+
+        * ``gsq``       ``||g||^2`` of the bf16 gradient the encoder read (coded tensors; None for tensors that travel
+                        exactly: 1-D vectors in fp32, dense bf16 weights),
+        * ``mse``       the expected ``||g_hat - g||^2`` given that gradient, in closed form (exact, not sampled);
+                        ``rel_var`` = ``mse / gsq``,
+        * ``bias_sq``   TernGrad's clip bias ``||clip(g) - g||^2`` (0 for the other codes; not part of ``mse``),
+        * ``exp_atoms`` / ``atoms``  expected and realized atoms (QSGD / TernGrad: every element), exact tensors their
+                        element count,
+        * ``bytes``     realized push bytes: the spectral slot layout, ``entry_bytes()`` / ``qsgd_bytes()`` applied to
+                        the realized counts, dense bytes for exact tensors.
+
+        The whole-model ``rel_var`` is the summed ``mse`` over the summed ``gsq`` of the coded tensors.  Reading it
+        synchronises the device; ``reset`` zeroes the sums."""
+        if not self.code_stats_on:
+            raise RuntimeError("code_stats() needs ShadowEngine(..., code_stats=True)")
+        pl, nf = self.plan, self.C.v2_stats_fields()
+        acc = self.stats_acc.view(-1, nf).tolist() if self.stats_acc is not None else []
+        names = {id(p): n for n, p in self.model.named_parameters()}
+        per = {}
+        for u in pl.units:
+            q = pl.params[u.param]
+            name = names.get(id(self.params[u.param]), str(u.param))
+            t = per.setdefault(name, {"numel": q.numel, "gsq": None, "mse": 0.0, "bias_sq": 0.0, "exp_atoms": 0.0,
+                                      "atoms": 0.0, "bytes": 0.0})
+            if u.kind in (P2.KIND_SLAB, P2.KIND_MAT, P2.KIND_ENTRY, P2.KIND_QSGD) and acc:
+                gsq, mse, ex, bias, real, real4, n = acc[u.ts_index]
+                n = max(n, 1.0)
+                t["gsq"] = (t["gsq"] or 0.0) + gsq / n
+                t["mse"] += mse / n
+                t["bias_sq"] += bias / n
+                t["exp_atoms"] += ex / n
+                t["atoms"] += real / n
+                if u.kind == P2.KIND_QSGD:
+                    t["bytes"] += 8.0 * u.rows * u.cols + 4.0 * u.rows
+                elif u.kind == P2.KIND_ENTRY:
+                    t["bytes"] += 4.0 * real / n + 16.0 * u.n_ps
+                else:
+                    t["bytes"] += 4.0 * (4 + u.rcap + u.rcap * u.cols) + 4.0 * u.rows * real4 / n
+            else:       # travels exactly: fp32 vector, or a dense bf16 weight
+                t["exp_atoms"] += u.numel
+                t["atoms"] += u.numel
+                t["bytes"] += (2.0 if u.kind == P2.KIND_DENSE16 else 4.0) * u.numel
+        for t in per.values():
+            t["rel_var"] = t["mse"] / t["gsq"] if t["gsq"] else (0.0 if t["gsq"] is None else None)
+        coded = [t for t in per.values() if t["gsq"] is not None]
+        tot = {k: sum(t[k] for t in per.values()) for k in ("mse", "bias_sq", "exp_atoms", "atoms", "bytes")}
+        tot["gsq"] = sum(t["gsq"] for t in coded)
+        tot["rel_var"] = tot["mse"] / tot["gsq"] if tot["gsq"] > 0 else 0.0
+        steps = int(acc[0][-1]) if acc else 0
+        if reset and self.stats_acc is not None:
+            self.stats_acc.zero_()
+        return {"code": self.code, "steps": steps, "model": tot, "tensors": per}
+
+    def _launch_code_stats(self, g: int):
+        """Estimator statistics of group ``g``: after its push on the same stream (the gradient, this step's sigma /
+        selcount / L1 / clip and this worker's slot headers and norms are live until the next encode)."""
+        t0, nt = self.plan.enc_range[g]
+        if self.stats_acc is None or nt == 0:
+            return
+        p = lambda t: t.data_ptr() if t is not None else 0
+        spectral = self.code == "svd"
+        self.C.v2_code_stats(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
+                             self.sigma.data_ptr() if spectral else 0, self.selcount.data_ptr(), p(self.l1),
+                             p(self.clip), self.t_arena_peer.data_ptr(), self.n_owners, self.plan.arena_floats,
+                             self.worker_index, self.random_sample, self.waterfill, self.stats_partials.data_ptr(),
+                             self.stats_counters.data_ptr(), self.stats_acc.data_ptr())
+        self._nlaunch += 1
 
     # ------------------------------------------------------------------------------------------------------
     def _make_hook(self, i: int):
@@ -441,6 +526,7 @@ class ShadowEngine:
         self._fired += 1
         if not self.overlap:
             self._launch_encode(g)
+            self._launch_code_stats(g)
             if self.is_owner:
                 self._launch_ps(g, final)
             return
@@ -452,6 +538,7 @@ class ShadowEngine:
                 torch.cuda._sleep(int(self._jitter_rng.uniform(0, self._jitter_us) * 1900))
             self._launch_encode(g)
             self.ev_push[g].record(self.s_enc)
+            self._launch_code_stats(g)
             if final:
                 self.ev_enc_done.record(self.s_enc)
         if self.is_owner:

@@ -85,4 +85,8 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
     p.add_argument("--gpu-data", type=bool_flag, default=False,
                    help="p2p backend: keep the rank's shard and the test set on the GPU and build every batch there "
                         "(same sample order and augmentation as the CPU loader; not for --dataset ImageNet)")
+    p.add_argument("--code-stats", type=bool_flag, default=False,
+                   help="p2p backend, bf16 engine: per-layer estimator statistics of the code (expected squared error "
+                        "given the gradient, expected / realized atoms, realized push bytes) in every --metrics-file "
+                        "record; not for --code qsvd")
     return p.parse_args(argv)
