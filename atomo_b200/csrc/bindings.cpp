@@ -77,7 +77,7 @@ void atomo_v2_launch_project(const void* units, const void* tiles, int tile0, in
                              const float* vsel, const int* selcount, float* const* arena_peer, int* const* sig_peer,
                              int n_owners, long long arena_floats, int worker, int group, void* ctrl,
                              unsigned int* group_counter, int flags, long long* tstats, int final_group, int timed,
-                             cudaStream_t stream);
+                             float* residual, int ef_owner, cudaStream_t stream);
 void atomo_v2_launch_ps(const void* units, const void* tiles, int tile0, int ntiles, int W, int nranks, int group,
                         int final_group, int owner, float* master, float* mom, float* sq, float* sqmax, float* vmom,
                         float* vsq, float* vsqmax, void* wshadow_mc, void* const* wshadow_peer, float* vparams_local,
@@ -96,7 +96,7 @@ void atomo_v2_launch_qsgd_encode(const void* units, const void* tiles, int tile0
                                  const float* clip, float* const* arena_peer, int* const* sig_peer, int n_owners,
                                  long long arena_floats, int worker, int group, const void* ctrl,
                                  unsigned int* group_counter, const float* ext_uniforms, long long* tstats,
-                                 int final_group, int stamp_start, cudaStream_t stream);
+                                 int final_group, int stamp_start, float* residual, cudaStream_t stream);
 void atomo_v2_launch_ps_qsgd(const void* units, const void* tiles, int tile0, int ntiles, int W, int nranks, int group,
                              int final_group, int owner, float* master, float* mom, float* sq, float* sqmax,
                              float* vmom, float* vsq, float* vsqmax, void* wshadow_mc, void* const* wshadow_peer,
@@ -113,7 +113,7 @@ void atomo_v2_launch_entry_encode(const void* units, const void* tiles, int tile
                                   const double* l1, float* const* arena_peer, int* const* sig_peer, int n_owners,
                                   long long arena_floats, int worker, int group, const void* ctrl,
                                   unsigned int* group_counter, const float* ext_uniforms, long long* tstats,
-                                  int final_group, cudaStream_t stream);
+                                  int final_group, float* residual, cudaStream_t stream);
 void atomo_v2_launch_ps_entry(const void* units, const void* tiles, int tile0, int ntiles, int W, int nranks,
                               int group, int final_group, int owner, float* master, float* mom, float* sq,
                               float* sqmax, float* vmom, float* vsq, float* vsqmax, void* wshadow_mc,
@@ -121,6 +121,10 @@ void atomo_v2_launch_ps_entry(const void* units, const void* tiles, int tile0, i
                               float* const* vparams_peer, const float* vgrads_mc, const float* const* vgrads_peer,
                               const float* arenas, long long arena_floats, int* sig, int* const* sig_peer, void* ctrl,
                               unsigned int* group_counter, long long timeout, long long* tstats, float inv_w, int grid,
+                              cudaStream_t stream);
+// v2_feedback.cu (error feedback of the bf16 engine)
+int atomo_v2_ef_chunk_bytes();
+void atomo_v2_launch_ef_apply(const void* chunks, int chunk0, int nchunks, const long long* gptr, float* residual,
                               cudaStream_t stream);
 // v2_stats.cu (estimator statistics of the bf16 engine, --code-stats)
 int atomo_v2_stats_fields();
@@ -413,12 +417,14 @@ void v2_encode(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t g
 }
 void v2_project(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t vsel, uint64_t selcount,
                 uint64_t arena_peer, uint64_t sig_peer, int n_owners, int64_t arena_floats, int worker, int group,
-                uint64_t ctrl, uint64_t group_counter, int flags, uint64_t tstats, bool final_group, bool timed) {
+                uint64_t ctrl, uint64_t group_counter, int flags, uint64_t tstats, bool final_group, bool timed,
+                uint64_t residual, int ef_owner) {
+  TORCH_CHECK(residual == 0 || (ef_owner >= 0 && ef_owner < n_owners), "v2_project: ef_owner must be an owner index");
   atomo_v2_launch_project(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
                           P<const float>(vsel), P<const int>(selcount), P<float* const>(arena_peer),
                           P<int* const>(sig_peer), n_owners, arena_floats, worker, group, P<void>(ctrl),
                           P<unsigned int>(group_counter), flags, P<long long>(tstats), final_group ? 1 : 0,
-                          timed ? 1 : 0, cur_stream());
+                          timed ? 1 : 0, P<float>(residual), ef_owner, cur_stream());
 }
 void v2_ps(uint64_t units, uint64_t tiles, int tile0, int ntiles, int W, int nranks, int group, bool final_group,
            int owner, uint64_t master, uint64_t mom, uint64_t sq, uint64_t sqmax, uint64_t vmom, uint64_t vsq,
@@ -452,15 +458,17 @@ void v2_qsgd_stats(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64
 void v2_qsgd_encode(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t clip,
                     uint64_t arena_peer, uint64_t sig_peer, int n_owners, int64_t arena_floats, int worker, int group,
                     uint64_t ctrl, uint64_t group_counter, uint64_t ext_uniforms, uint64_t tstats, bool final_group,
-                    bool stamp_start, int max_level, int max_bucket, bool terngrad) {
+                    bool stamp_start, int max_level, int max_bucket, bool terngrad, uint64_t residual) {
   check_qsgd_plan(max_level, max_bucket);
   TORCH_CHECK(worker >= 0 && worker < 16, "v2_qsgd_encode: worker index must be in [0, 16)");
   TORCH_CHECK(!terngrad || clip != 0, "v2_qsgd_encode: TernGrad needs the clip buffer of v2_qsgd_stats");
+  TORCH_CHECK(!terngrad || residual == 0, "v2_qsgd_encode: no error feedback for TernGrad (the owners rescale every "
+              "worker by the shared max norm)");
   atomo_v2_launch_qsgd_encode(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
                               P<const float>(clip), P<float* const>(arena_peer), P<int* const>(sig_peer), n_owners,
                               arena_floats, worker, group, P<const void>(ctrl), P<unsigned int>(group_counter),
                               P<const float>(ext_uniforms), P<long long>(tstats), final_group ? 1 : 0,
-                              stamp_start ? 1 : 0, cur_stream());
+                              stamp_start ? 1 : 0, P<float>(residual), cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 void v2_ps_qsgd(uint64_t units, uint64_t tiles, int tile0, int ntiles, int W, int nranks, int group, bool final_group,
@@ -492,13 +500,23 @@ void v2_entry_stats(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint6
 }
 void v2_entry_encode(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t l1,
                      uint64_t arena_peer, uint64_t sig_peer, int n_owners, int64_t arena_floats, int worker, int group,
-                     uint64_t ctrl, uint64_t group_counter, uint64_t ext_uniforms, uint64_t tstats, bool final_group) {
+                     uint64_t ctrl, uint64_t group_counter, uint64_t ext_uniforms, uint64_t tstats, bool final_group,
+                     uint64_t residual) {
   TORCH_CHECK(l1 != 0, "v2_entry_encode: needs the L1 norms of v2_entry_stats");
   TORCH_CHECK(worker >= 0 && worker < 16, "v2_entry_encode: worker index must be in [0, 16)");
   atomo_v2_launch_entry_encode(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
                                P<const double>(l1), P<float* const>(arena_peer), P<int* const>(sig_peer), n_owners,
                                arena_floats, worker, group, P<const void>(ctrl), P<unsigned int>(group_counter),
-                               P<const float>(ext_uniforms), P<long long>(tstats), final_group ? 1 : 0, cur_stream());
+                               P<const float>(ext_uniforms), P<long long>(tstats), final_group ? 1 : 0,
+                               P<float>(residual), cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+// error feedback: A = g + e, bf16(A) into the gradient buffers, A - bf16(A) into the residual, for the apply chunks
+// [chunk0, chunk0 + nchunks) of the chunk table (one backward group); before the group's encode, on the same stream
+void v2_ef_apply(uint64_t chunks, int chunk0, int nchunks, uint64_t gptr, uint64_t residual) {
+  TORCH_CHECK(chunks != 0 && gptr != 0 && residual != 0, "v2_ef_apply: chunks / gptr / residual required");
+  atomo_v2_launch_ef_apply(P<const void>(chunks), chunk0, nchunks, P<const long long>(gptr), P<float>(residual),
+                           cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 // estimator statistics of one group: after the group's push, on the same stream
@@ -631,13 +649,27 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("entrywise_scatter", &entrywise_scatter);
   // v2 engine
   m.def("v2_encode", &v2_encode);
-  m.def("v2_project", &v2_project);
+  // the error-feedback residual is the last argument of the encoders (0 / absent: no epilogue)
+  m.def("v2_project", &v2_project, py::arg("units"), py::arg("tiles"), py::arg("tile0"), py::arg("ntiles"),
+        py::arg("gptr"), py::arg("vsel"), py::arg("selcount"), py::arg("arena_peer"), py::arg("sig_peer"),
+        py::arg("n_owners"), py::arg("arena_floats"), py::arg("worker"), py::arg("group"), py::arg("ctrl"),
+        py::arg("group_counter"), py::arg("flags"), py::arg("tstats"), py::arg("final_group"), py::arg("timed"),
+        py::arg("residual") = 0, py::arg("ef_owner") = 0);
   m.def("v2_ps", &v2_ps);
   m.def("v2_qsgd_stats", &v2_qsgd_stats);
-  m.def("v2_qsgd_encode", &v2_qsgd_encode);
+  m.def("v2_qsgd_encode", &v2_qsgd_encode, py::arg("units"), py::arg("tiles"), py::arg("tile0"), py::arg("ntiles"),
+        py::arg("gptr"), py::arg("clip"), py::arg("arena_peer"), py::arg("sig_peer"), py::arg("n_owners"),
+        py::arg("arena_floats"), py::arg("worker"), py::arg("group"), py::arg("ctrl"), py::arg("group_counter"),
+        py::arg("ext_uniforms"), py::arg("tstats"), py::arg("final_group"), py::arg("stamp_start"),
+        py::arg("max_level"), py::arg("max_bucket"), py::arg("terngrad"), py::arg("residual") = 0);
   m.def("v2_ps_qsgd", &v2_ps_qsgd);
   m.def("v2_entry_stats", &v2_entry_stats);
-  m.def("v2_entry_encode", &v2_entry_encode);
+  m.def("v2_entry_encode", &v2_entry_encode, py::arg("units"), py::arg("tiles"), py::arg("tile0"), py::arg("ntiles"),
+        py::arg("gptr"), py::arg("l1"), py::arg("arena_peer"), py::arg("sig_peer"), py::arg("n_owners"),
+        py::arg("arena_floats"), py::arg("worker"), py::arg("group"), py::arg("ctrl"), py::arg("group_counter"),
+        py::arg("ext_uniforms"), py::arg("tstats"), py::arg("final_group"), py::arg("residual") = 0);
+  m.def("v2_ef_apply", &v2_ef_apply);
+  m.def("v2_ef_chunk_bytes", &atomo_v2_ef_chunk_bytes);
   m.def("v2_ps_entry", &v2_ps_entry);
   m.def("v2_code_stats", &v2_code_stats);
   m.def("v2_stats_fields", &atomo_v2_stats_fields);

@@ -12,7 +12,9 @@
 //                      then stores header / s / V into every owner's slot through peer pointers.
 //   v2_project_kernel  U = A V / sigma for the sampled atoms (second pass, L2 resident), float4 peer stores of
 //                      each row into the arena of the PS owner of that row's tile; the last CTA of the group
-//                      publishes flag[group][worker] = step on every owner with st.release.sys.
+//                      publishes flag[group][worker] = step on every owner with st.release.sys.  With error
+//                      feedback (v2_feedback.cu) each row also adds A - U diag(s) V^T, the part of the coded input
+//                      the owner does not reconstruct, to the worker's fp32 residual.
 #include "spectral_sample.cuh"
 #include "v2_common.cuh"
 
@@ -365,6 +367,16 @@ struct ProjArgs {
 };
 
 constexpr int PROJ_SMEM = ENC_HDR + ENC_TILE_BYTES + V2_MAX_COLS * V2_RCAP_MAX * 4;
+// error feedback adds s_x V[x][c] (as the owner forms it) and every thread's U row
+constexpr int PROJ_EF_SMEM = PROJ_SMEM + V2_MAX_COLS * V2_RCAP_MAX * 4 + V2_RCAP_MAX * ENC_THREADS * 4;
+
+// Error feedback: U[x] s_x V[x][c] summed over the atoms in atom order with fmaf, which is the order and rounding of
+// the owner's reconstruction (v2_ps_kernel) for one worker
+__device__ __forceinline__ float ef_recon(const float* ust, const float* svc, int count) {
+  float acc = 0.f;
+  for (int x = 0; x < count; ++x) acc = fmaf(ust[x * ENC_THREADS], svc[x], acc);
+  return acc;
+}
 
 // QSVD: quantize one float4 of a U row to 4 x int8 with unbiased stochastic rounding against the row scale
 __device__ __forceinline__ int quant4_i8(const float4 v, float inv_scale127, const uint32_t (&rnd)[4]) {
@@ -381,13 +393,19 @@ __device__ __forceinline__ int quant4_i8(const float4 v, float inv_scale127, con
   return packed;
 }
 
-__global__ void __launch_bounds__(ENC_THREADS) v2_project_kernel(const ProjArgs a) {
+// EF (v2_project_ef_kernel): `residual` is the fp32 residual indexed like wshadow, `ef_owner` the owner whose copy of
+// this worker's slot (s, V) the epilogue reads (a local one if any)
+template <bool EF>
+__device__ __forceinline__ void project(const ProjArgs& a, float* residual, int ef_owner) {
   uint64_t* mbar = reinterpret_cast<uint64_t*>(enc_smem);
   uint32_t* tile = reinterpret_cast<uint32_t*>(enc_smem + ENC_HDR);
   float* vs = reinterpret_cast<float*>(enc_smem + ENC_HDR + ENC_TILE_BYTES);
+  float* sv = vs + V2_MAX_COLS * V2_RCAP_MAX;          // error feedback only: [col][atom] s_x V[x][col]
+  float* ust = sv + V2_MAX_COLS * V2_RCAP_MAX;         // error feedback only: [atom][thread] U row of the thread
   const Tile2 t = a.tiles[blockIdx.x];
   const Unit2 u = a.units[t.unit];
   const int tid = threadIdx.x;
+  const bool ef = EF && u.ubits != 8;
 
   if (u.kind == KIND_SLAB || u.kind == KIND_MAT) {
     const __nv_bfloat16* gb = reinterpret_cast<const __nv_bfloat16*>(a.gptr[u.pidx]) + u.g_off;
@@ -402,6 +420,13 @@ __global__ void __launch_bounds__(ENC_THREADS) v2_project_kernel(const ProjArgs 
     }
     const float* vsrc = a.vsel + (long long)u.ts_index * V2_MAX_COLS * V2_RCAP_MAX;
     for (int e = tid; e < n * V2_RCAP_MAX; e += blockDim.x) vs[e] = vsrc[e];
+    if (ef) {       // the slot's s and V, as the encode launch stored them
+      const float* slot = a.arena_peer[ef_owner] + (long long)a.worker * a.arena_floats + u.slot_off;
+      for (int e = tid; e < n * V2_RCAP_MAX; e += blockDim.x) {
+        const int c = e / V2_RCAP_MAX, x = e - c * V2_RCAP_MAX;
+        sv[e] = (x < count) ? slot[4 + x] * slot[4 + rcap + (long long)x * n + c] : 0.f;
+      }
+    }
     __syncthreads();
     const long long uoff = (long long)a.worker * a.arena_floats + u.slot_off + slot2_u_off(rcap, n);
     if (u.kind == KIND_SLAB) {
@@ -440,6 +465,14 @@ __global__ void __launch_bounds__(ENC_THREADS) v2_project_kernel(const ProjArgs 
           if (u.ubits != 8) {
             st_na_f4(dst + g0, a0);
             if (two) st_na_f4(dst + g0 + 1, a1);
+            if (ef) {
+              float* us = ust + 4 * g0 * ENC_THREADS + tid;
+              us[0] = a0.x; us[ENC_THREADS] = a0.y; us[2 * ENC_THREADS] = a0.z; us[3 * ENC_THREADS] = a0.w;
+              if (two) {
+                us[4 * ENC_THREADS] = a1.x; us[5 * ENC_THREADS] = a1.y;
+                us[6 * ENC_THREADS] = a1.z; us[7 * ENC_THREADS] = a1.w;
+              }
+            }
           } else if (pass == 0) {
             rowmax = fmaxf(rowmax, fmaxf(fmaxf(fabsf(a0.x), fabsf(a0.y)), fmaxf(fabsf(a0.z), fabsf(a0.w))));
             if (two) rowmax = fmaxf(rowmax, fmaxf(fmaxf(fabsf(a1.x), fabsf(a1.y)), fmaxf(fabsf(a1.z), fabsf(a1.w))));
@@ -457,6 +490,17 @@ __global__ void __launch_bounds__(ENC_THREADS) v2_project_kernel(const ProjArgs 
               q8[g0 + 1] = quant4_i8(a1, inv, rnd);
             }
             if (g0 == 0) sbase[slot2_scale_off(u.rows, rcap, n) + r] = rowmax;
+          }
+        }
+        if (ef) {     // e += A - U diag(s) V^T on the row's 2K elements (s, k, 2ri + b); float2 aligned (I % 16 == 0)
+          float* er = residual + u.w_off + (long long)(t.a + s) * K * u.I + 2 * ri;
+          for (int k = 0; k < K; ++k) {
+            const uint32_t w = col[k * pitch];
+            float2* p = reinterpret_cast<float2*>(er + (long long)k * u.I);
+            float2 e = *p;
+            e.x += bf16_lo(w) - ef_recon(ust + tid, sv + k * V2_RCAP_MAX, count);
+            e.y += bf16_hi(w) - ef_recon(ust + tid, sv + (K + k) * V2_RCAP_MAX, count);
+            *p = e;
           }
         }
       }
@@ -485,6 +529,14 @@ __global__ void __launch_bounds__(ENC_THREADS) v2_project_kernel(const ProjArgs 
           if (u.ubits != 8) {
             st_na_f4(dst + g0, a0);
             if (two) st_na_f4(dst + g0 + 1, a1);
+            if (ef) {
+              float* us = ust + 4 * g0 * ENC_THREADS + tid;
+              us[0] = a0.x; us[ENC_THREADS] = a0.y; us[2 * ENC_THREADS] = a0.z; us[3 * ENC_THREADS] = a0.w;
+              if (two) {
+                us[4 * ENC_THREADS] = a1.x; us[5 * ENC_THREADS] = a1.y;
+                us[6 * ENC_THREADS] = a1.z; us[7 * ENC_THREADS] = a1.w;
+              }
+            }
           } else if (pass == 0) {
             rowmax = fmaxf(rowmax, fmaxf(fmaxf(fabsf(a0.x), fabsf(a0.y)), fmaxf(fabsf(a0.z), fabsf(a0.w))));
             if (two) rowmax = fmaxf(rowmax, fmaxf(fmaxf(fabsf(a1.x), fabsf(a1.y)), fmaxf(fabsf(a1.z), fabsf(a1.w))));
@@ -503,6 +555,12 @@ __global__ void __launch_bounds__(ENC_THREADS) v2_project_kernel(const ProjArgs 
             }
             if (g0 == 0) sbase[slot2_scale_off(u.rows, rcap, n) + r] = rowmax;
           }
+        }
+        if (ef) {     // e += A - U diag(s) V^T on the row's n elements
+          float* er = residual + u.w_off + r * u.rs;
+          for (int c = 0; c < n; ++c)
+            er[(long long)c * u.cs] += __bfloat162float(row[(long long)c * u.cs]) -
+                                       ef_recon(ust + tid, sv + c * V2_RCAP_MAX, count);
         }
       }
     }
@@ -526,6 +584,13 @@ __global__ void __launch_bounds__(ENC_THREADS) v2_project_kernel(const ProjArgs 
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(ENC_THREADS) v2_project_kernel(const ProjArgs a) { project<false>(a, nullptr, 0); }
+// error feedback: the same encode plus the residual epilogue
+__global__ void __launch_bounds__(ENC_THREADS, 2) v2_project_ef_kernel(const ProjArgs a, float* residual,
+                                                                        int ef_owner) {
+  project<true>(a, residual, ef_owner);
 }
 
 // flag-only push of a group that has no encode tiles (dense-only configurations)
@@ -554,6 +619,7 @@ void atomo_v2_launch_encode(const void* units, const void* tiles, int tile0, int
   if (!attr) {
     cudaFuncSetAttribute(v2_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM);
     cudaFuncSetAttribute(v2_project_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PROJ_SMEM);
+    cudaFuncSetAttribute(v2_project_ef_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PROJ_EF_SMEM);
     attr = true;
   }
   EncArgs a;
@@ -570,7 +636,7 @@ void atomo_v2_launch_project(const void* units, const void* tiles, int tile0, in
                              const float* vsel, const int* selcount, float* const* arena_peer, int* const* sig_peer,
                              int n_owners, long long arena_floats, int worker, int group, void* ctrl,
                              unsigned int* group_counter, int flags, long long* tstats, int final_group, int timed,
-                             cudaStream_t stream) {
+                             float* residual, int ef_owner, cudaStream_t stream) {
   if (ntiles <= 0) {
     v2_signal_kernel<<<1, 32, 0, stream>>>(sig_peer, n_owners, group, worker, (const Ctrl2*)ctrl);
     return;
@@ -579,6 +645,7 @@ void atomo_v2_launch_project(const void* units, const void* tiles, int tile0, in
   if (!attr) {
     cudaFuncSetAttribute(v2_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM);
     cudaFuncSetAttribute(v2_project_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PROJ_SMEM);
+    cudaFuncSetAttribute(v2_project_ef_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PROJ_EF_SMEM);
     attr = true;
   }
   ProjArgs a;
@@ -586,7 +653,8 @@ void atomo_v2_launch_project(const void* units, const void* tiles, int tile0, in
   a.selcount = selcount; a.arena_peer = arena_peer; a.sig_peer = sig_peer; a.n_owners = n_owners;
   a.arena_floats = arena_floats; a.worker = worker; a.group = group; a.ctrl = (Ctrl2*)ctrl;
   a.group_counter = group_counter; a.flags = flags; a.tstats = tstats; a.final_group = final_group; a.timed = timed;
-  v2_project_kernel<<<ntiles, ENC_THREADS, PROJ_SMEM, stream>>>(a);
+  if (residual != nullptr) v2_project_ef_kernel<<<ntiles, ENC_THREADS, PROJ_EF_SMEM, stream>>>(a, residual, ef_owner);
+  else v2_project_kernel<<<ntiles, ENC_THREADS, PROJ_SMEM, stream>>>(a);
 }
 
 }  // extern "C"

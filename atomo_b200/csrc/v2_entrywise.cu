@@ -108,7 +108,14 @@ struct EEncArgs {
   const float* ext_uniforms;   // tests: uniforms indexed like wshadow, replacing Philox
   long long* tstats;
   int final_group;
+  float* residual;             // error feedback (v2_feedback.cu): fp32 residual indexed like wshadow, or nullptr
 };
+
+// Error feedback: what element x of A is owed after this push, x - g_hat (the owner's decode of the tile)
+__device__ __forceinline__ float entry_residual(uint32_t bits, uint32_t kept, uint32_t exact, float scale) {
+  const float x = __uint_as_float(bits << 16);
+  return kept ? (exact ? 0.f : x - copysignf(scale, x)) : x;
+}
 
 // The uniform of element e of a unit is word (e & 3) of Philox(seed', counter = (e >> 2, unit, step, worker)):
 // one Philox call serves 4 consecutive elements.  The seed differs from the QSGD rounding's.
@@ -117,7 +124,8 @@ __device__ __forceinline__ void entry_philox(const EEncArgs& a, int unit, long l
               (uint32_t)a.worker, r4);
 }
 
-__global__ void __launch_bounds__(EE_THREADS) v2_entry_encode_kernel(const EEncArgs a) {
+template <bool EF>
+__device__ __forceinline__ void entry_encode(const EEncArgs& a) {
   __shared__ __align__(16) uint32_t ent[ENTRY_TILE_ELEMS];
   __shared__ int wsum[EE_WARPS];
   const Tile2 t = a.tiles[blockIdx.x];
@@ -153,6 +161,23 @@ __global__ void __launch_bounds__(EE_THREADS) v2_entry_encode_kernel(const EEncA
       const float p = fabsf(__uint_as_float(bf16_bits(h, i) << 16)) * k;   // clamped to 1 below: u < 1 <= p
       if (uu < p) keep |= 1u << i;
       if (p >= 1.f) exact |= 1u << i;
+    }
+  }
+  if (EF && n > 0) {
+    float* ep = a.residual + u.w_off + e0;                   // 64-byte aligned: w_off % 64 == 0, e0 % 16 == 0
+    if (n >= EE_PER_THREAD) {
+#pragma unroll
+      for (int j = 0; j < EE_PER_THREAD / 4; ++j) {
+        float4 v = reinterpret_cast<const float4*>(ep)[j];
+        const int i = 4 * j;
+        v.x += entry_residual(bf16_bits(h, i), (keep >> i) & 1u, (exact >> i) & 1u, scale);
+        v.y += entry_residual(bf16_bits(h, i + 1), (keep >> (i + 1)) & 1u, (exact >> (i + 1)) & 1u, scale);
+        v.z += entry_residual(bf16_bits(h, i + 2), (keep >> (i + 2)) & 1u, (exact >> (i + 2)) & 1u, scale);
+        v.w += entry_residual(bf16_bits(h, i + 3), (keep >> (i + 3)) & 1u, (exact >> (i + 3)) & 1u, scale);
+        reinterpret_cast<float4*>(ep)[j] = v;
+      }
+    } else {
+      for (int i = 0; i < n; ++i) ep[i] += entry_residual(bf16_bits(h, i), (keep >> i) & 1u, (exact >> i) & 1u, scale);
     }
   }
 
@@ -209,6 +234,10 @@ __global__ void __launch_bounds__(EE_THREADS) v2_entry_encode_kernel(const EEncA
     }
   }
 }
+
+__global__ void __launch_bounds__(EE_THREADS) v2_entry_encode_kernel(const EEncArgs a) { entry_encode<false>(a); }
+// error feedback: the same encode plus the residual epilogue
+__global__ void __launch_bounds__(EE_THREADS) v2_entry_encode_ef_kernel(const EEncArgs a) { entry_encode<true>(a); }
 
 // ---- PS: scatter-add + optimizer --------------------------------------------------------------------------
 __global__ void __launch_bounds__(EPS_THREADS) v2_ps_entry_kernel(const PsArgs2 a) {
@@ -321,14 +350,15 @@ void atomo_v2_launch_entry_encode(const void* units, const void* tiles, int tile
                                   const double* l1, float* const* arena_peer, int* const* sig_peer, int n_owners,
                                   long long arena_floats, int worker, int group, const void* ctrl,
                                   unsigned int* group_counter, const float* ext_uniforms, long long* tstats,
-                                  int final_group, cudaStream_t stream) {
+                                  int final_group, float* residual, cudaStream_t stream) {
   if (ntiles <= 0) return;
   EEncArgs a;
   a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.gptr = gptr; a.l1 = l1;
   a.arena_peer = arena_peer; a.sig_peer = sig_peer; a.n_owners = n_owners; a.arena_floats = arena_floats;
   a.worker = worker; a.group = group; a.ctrl = (const Ctrl2*)ctrl; a.group_counter = group_counter;
-  a.ext_uniforms = ext_uniforms; a.tstats = tstats; a.final_group = final_group;
-  v2_entry_encode_kernel<<<ntiles, EE_THREADS, 0, stream>>>(a);
+  a.ext_uniforms = ext_uniforms; a.tstats = tstats; a.final_group = final_group; a.residual = residual;
+  if (residual != nullptr) v2_entry_encode_ef_kernel<<<ntiles, EE_THREADS, 0, stream>>>(a);
+  else v2_entry_encode_kernel<<<ntiles, EE_THREADS, 0, stream>>>(a);
 }
 
 void atomo_v2_launch_ps_entry(const void* units, const void* tiles, int tile0, int ntiles, int W, int nranks,

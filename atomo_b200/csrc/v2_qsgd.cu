@@ -42,6 +42,7 @@ struct QEncArgs {
   long long* tstats;
   int final_group;
   int stamp_start;             // 1: this launch stamps the group's encode start (no stats launch before it)
+  float* residual;             // error feedback (v2_feedback.cu, QSGD only): fp32 residual like wshadow, or nullptr
 };
 
 __device__ __forceinline__ void bf16x8(const uint4 v, float (&x)[8]) {
@@ -74,7 +75,15 @@ __device__ __forceinline__ unsigned short qsgd_code(float x, float inv, int leve
   return (unsigned short)((sgn << q) | xi);
 }
 
-__global__ void __launch_bounds__(QE_THREADS) v2_qsgd_encode_kernel(const QEncArgs a) {
+// The owner's decode of one code (v2_ps_qsgd_kernel): sign * level * (norm / levels), with the same roundings
+__device__ __forceinline__ float qsgd_dequant(uint32_t cd, int q, int levels, float scale) {
+  const float xi = (float)(int)(cd & (uint32_t)levels);
+  const float sg = (float)((int)(cd >> q) & 3) - 1.f;
+  return __fmul_rn(sg * xi, scale);
+}
+
+template <bool EF>
+__device__ __forceinline__ void qsgd_encode(const QEncArgs& a) {
   __shared__ __align__(16) unsigned short codes[QE_WARPS][QE_MAX_BUCKET];
   const Tile2 t = a.tiles[blockIdx.x];
   const Unit2 u = a.units[t.unit];
@@ -119,6 +128,8 @@ __global__ void __launch_bounds__(QE_THREADS) v2_qsgd_encode_kernel(const QEncAr
     }
     const float nrm = tern ? warp_max(acc) : sqrtf(warp_sum(acc));
     const float inv = nrm > 0.f ? (float)levels / nrm : 0.f;
+    const float dq = EF ? __fdiv_rn(nrm, (float)levels) : 0.f;   // error feedback: the owner's scale of the bucket
+    float* res = EF ? a.residual + u.w_off + e0 : nullptr;
     // pass 2: stochastic rounding into codes (the bucket is L1 resident from pass 1)
     for (int c = lane; c < nch; c += 32) {
       float x[8];
@@ -142,11 +153,26 @@ __global__ void __launch_bounds__(QE_THREADS) v2_qsgd_encode_kernel(const QEncAr
         else packed[i >> 1] = cd;
       }
       *reinterpret_cast<uint4*>(&codes[warp][8 * c]) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
+      if (EF) {                      // e += x - g_hat; 32-byte aligned (w_off % 64 == 0, e0 % 8 == 0)
+        float4* rp = reinterpret_cast<float4*>(res + 8 * c);
+        float4 r0 = rp[0], r1 = rp[1];
+        r0.x += x[0] - qsgd_dequant(packed[0] & 0xffffu, q, levels, dq);
+        r0.y += x[1] - qsgd_dequant(packed[0] >> 16, q, levels, dq);
+        r0.z += x[2] - qsgd_dequant(packed[1] & 0xffffu, q, levels, dq);
+        r0.w += x[3] - qsgd_dequant(packed[1] >> 16, q, levels, dq);
+        r1.x += x[4] - qsgd_dequant(packed[2] & 0xffffu, q, levels, dq);
+        r1.y += x[5] - qsgd_dequant(packed[2] >> 16, q, levels, dq);
+        r1.z += x[6] - qsgd_dequant(packed[3] & 0xffffu, q, levels, dq);
+        r1.w += x[7] - qsgd_dequant(packed[3] >> 16, q, levels, dq);
+        rp[0] = r0; rp[1] = r1;
+      }
     }
     for (int i = (nch << 3) + lane; i < blen; i += 32) {
       float x = __bfloat162float(src[i]);
       if (tern && clip > 0.f) x = fminf(fmaxf(x, -clip), clip);
-      codes[warp][i] = qsgd_code(x, inv, levels, q, qsgd_uniform(a, u, t.unit, e0 + i, step));
+      const unsigned short cd = qsgd_code(x, inv, levels, q, qsgd_uniform(a, u, t.unit, e0 + i, step));
+      codes[warp][i] = cd;
+      if (EF) res[i] += x - qsgd_dequant(cd, q, levels, dq);
     }
     __syncwarp();
     // section-major packing: word j holds elements j, j+L, j+2L, ... (section 0 in the MSBs); padding (zero tail of
@@ -184,6 +210,10 @@ __global__ void __launch_bounds__(QE_THREADS) v2_qsgd_encode_kernel(const QEncAr
     }
   }
 }
+
+__global__ void __launch_bounds__(QE_THREADS) v2_qsgd_encode_kernel(const QEncArgs a) { qsgd_encode<false>(a); }
+// error feedback: the same encode plus the residual epilogue
+__global__ void __launch_bounds__(QE_THREADS) v2_qsgd_encode_ef_kernel(const QEncArgs a) { qsgd_encode<true>(a); }
 
 // ---- TernGrad clip: per-tile (sum, sum of squares) in fp64, combined in tile order by the unit's last tile ----
 struct QStatArgs {
@@ -373,14 +403,16 @@ void atomo_v2_launch_qsgd_encode(const void* units, const void* tiles, int tile0
                                  const float* clip, float* const* arena_peer, int* const* sig_peer, int n_owners,
                                  long long arena_floats, int worker, int group, const void* ctrl,
                                  unsigned int* group_counter, const float* ext_uniforms, long long* tstats,
-                                 int final_group, int stamp_start, cudaStream_t stream) {
+                                 int final_group, int stamp_start, float* residual, cudaStream_t stream) {
   if (ntiles <= 0) return;
   QEncArgs a;
   a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.gptr = gptr; a.clip = clip;
   a.arena_peer = arena_peer; a.sig_peer = sig_peer; a.n_owners = n_owners; a.arena_floats = arena_floats;
   a.worker = worker; a.group = group; a.ctrl = (const Ctrl2*)ctrl; a.group_counter = group_counter;
   a.ext_uniforms = ext_uniforms; a.tstats = tstats; a.final_group = final_group; a.stamp_start = stamp_start;
-  v2_qsgd_encode_kernel<<<ntiles, QE_THREADS, 0, stream>>>(a);
+  a.residual = residual;
+  if (residual != nullptr) v2_qsgd_encode_ef_kernel<<<ntiles, QE_THREADS, 0, stream>>>(a);
+  else v2_qsgd_encode_kernel<<<ntiles, QE_THREADS, 0, stream>>>(a);
 }
 
 void atomo_v2_launch_ps_qsgd(const void* units, const void* tiles, int tile0, int ntiles, int W, int nranks, int group,

@@ -64,6 +64,9 @@ def run_rank(args) -> None:
     if getattr(args, "gpu_data", False):
         raise SystemExit("--gpu-data builds batches for the --backend p2p engines; the %s backend's workers read "
                          "the CPU loader (run without --gpu-data)" % backend)
+    if getattr(args, "error_feedback", False):
+        raise SystemExit("--error-feedback keeps its residuals in the --backend p2p bf16 engine; the %s backend's "
+                         "PyTorch coders do not (run without --error-feedback)" % backend)
     if getattr(args, "code_stats", False):
         raise SystemExit("--code-stats reads the statistics of the --backend p2p bf16 engine; the %s backend's "
                          "PyTorch coders do not compute them (run without --code-stats)" % backend)

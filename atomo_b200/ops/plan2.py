@@ -519,6 +519,28 @@ def owner_of_row(u: Unit2, row: int, n_owners: int) -> int:
     return (u.own0 + row // u.ps_rows) % n_owners
 
 
+# error feedback (csrc/v2_feedback.cu): the apply pass runs over the weight tensors of a group in chunks of
+# EF_CHUNK_ELEMS elements, one CTA each; EfChunk = {residual offset of the tensor, pointer-table index, first element,
+# element count, pad}
+EF_CHUNK_ELEMS = 8192
+EF_CHUNK_FMT = "<qiiii"
+
+
+def ef_chunks(plan: "Plan2") -> Tuple[bytes, List[Tuple[int, int]]]:
+    """Packed apply chunks of every weight tensor, grouped by backward group, and (first chunk, chunk count) per
+    group.  1-D vectors travel exactly in fp32 and have no residual."""
+    rows: List[Tuple[int, int, int, int]] = []
+    ranges: List[Tuple[int, int]] = []
+    for g in range(plan.n_groups):
+        first = len(rows)
+        for q in plan.params:
+            if q.is_w and q.group == g:
+                rows.extend((q.off, q.widx, s, min(EF_CHUNK_ELEMS, q.numel - s))
+                            for s in range(0, q.numel, EF_CHUNK_ELEMS))
+        ranges.append((first, len(rows) - first))
+    return b"".join(struct.pack(EF_CHUNK_FMT, o, w, s, c, 0) for o, w, s, c in rows), ranges
+
+
 OPT_SGD, OPT_ADAM, OPT_AMSGRAD = 0, 1, 2
 
 

@@ -54,12 +54,17 @@ def _build_engine(args, model, rank, world):
             if code == "qsvd":
                 raise SystemExit("--code-stats does not model QSVD's int8 left factors (use --code svd)")
             kw["code_stats"] = True
+        if getattr(args, "error_feedback", False):
+            kw["error_feedback"] = True      # the engine refuses codes / --num-aggregate it cannot feed back
         return ShadowEngine(model, rank, world, code=args.code, svd_rank=args.svd_rank, lr=args.lr,
                             momentum=args.momentum, weight_decay=args.weight_decay, nesterov=args.nesterov,
                             optimizer=args.optimizer, ps_mode=args.ps_mode, groups=args.groups, sampling=args.sampling,
                             prob_rule=args.prob_rule, seed=args.seed, num_aggregate=args.num_aggregate,
                             timeout_s=args.flag_timeout, **kw), "shadow"
     from .engine import FusedEngine
+    if getattr(args, "error_feedback", False):
+        raise SystemExit("--error-feedback runs on the bf16 engine (--dtype bf16, --engine auto|shadow); the fp32-flat "
+                         "engine keeps no residual (run without --error-feedback)")
     if getattr(args, "code_stats", False):
         raise SystemExit("--code-stats reads the statistics of the bf16 engine (--dtype bf16, --engine auto|shadow); "
                          "the fp32-flat engine does not compute them (run without --code-stats)")
@@ -168,6 +173,8 @@ def run_p2p_training(args, device=None):
             extra = {}
             if getattr(args, "code_stats", False) and eng.is_worker:
                 extra["code_stats"] = eng.code_stats(reset=True)
+            if getattr(args, "error_feedback", False) and eng.is_worker:
+                extra["ef_norm"] = eng.error_feedback_norm()["model"]
             metrics.write(step=cur, loss=loss, prec1=p1, prec5=p5, step_s=step_s, comp=comp, encode=enc, comm=comm,
                           msg_mb=msg_mb, lr=eng.lr, phase_us={k: round(float(v), 1) for k, v in ph.items()}, **extra)
             ev_a.record()

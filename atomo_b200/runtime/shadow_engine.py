@@ -26,6 +26,10 @@ one central PS kernel at the end of the step):
   launch takes its fp64 L1 norm, the encode launch samples entries with ``p_i = min(1, s |g_i| / ||g||_1)`` and
   pushes them as 4-byte words (``csrc/v2_entrywise.cu``), and the owners scatter-add them in worker order and step
   the optimizer.  BN and bias vectors stay fp32, as above.
+* **Error feedback** (``error_feedback=True``; svd, entrywise, qsgd): each worker keeps an fp32 residual ``e`` per
+  weight element and codes ``A = g + e``.  An apply launch per group (``csrc/v2_feedback.cu``) writes ``bf16(A)`` into
+  autograd's gradient buffer in place and keeps ``A - bf16(A)``; the encoders' epilogues add ``bf16(A) - g_hat``, the
+  part of ``A`` this push did not carry.  Nothing is discarded, only delayed.
 * Optimizers fused in the PS epilogue: momentum-SGD (``src/optim/sgd.py:57-90``), Adam / AMSGrad
   (``src/optim/adam.py:37-94``).
 
@@ -36,6 +40,7 @@ step-stamped flags in peer memory (``csrc/v2_common.cuh``); no NCCL call on the 
 from __future__ import annotations
 
 import os
+import struct
 from typing import List, Optional
 
 import numpy as np
@@ -65,10 +70,26 @@ class ShadowEngine:
                  ps_grid: int = 0, overlap: bool = True, fused_bn: bool = True, num_aggregate: int = 0,
                  warm_start: bool = True, max_sweeps: int = 1, main_priority: int = 0, debug_jitter_us: float = 0.0,
                  side_priority: int = -1, resample_empty: bool = False, quantization_level: int = 4,
-                 bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False):
+                 bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False,
+                 error_feedback: bool = False):
         self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
         if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise"):
             raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise")
+        self.error_feedback = bool(error_feedback)
+        if self.error_feedback:     # checked before any CUDA work
+            if self.code == "qsvd":
+                raise ValueError("error_feedback: QSVD rounds its int8 left factors after the residual would be "
+                                 "formed (use code='svd')")
+            if self.code == "terngrad":
+                raise ValueError("error_feedback: TernGrad's owners rescale every worker by a shared max norm, so a "
+                                 "worker cannot know what it contributed")
+            if self.code == "sgd":
+                raise ValueError("error_feedback: the dense code sends the gradient exactly; there is nothing to "
+                                 "feed back")
+            n_workers = world - 1 if (ps_mode == "dedicated" and world > 1) else world
+            if 0 < num_aggregate < n_workers:
+                raise ValueError("error_feedback needs every push counted (num_aggregate=0 or >= workers): a "
+                                 "dropped push would lose its residual credit")
         if code_stats:      # checked before any CUDA work: the closed forms of code_stats() do not hold for these
             if self.code == "qsvd":
                 raise ValueError("code_stats does not model the int8 quantization of QSVD's left factors")
@@ -286,6 +307,14 @@ class ShadowEngine:
             self.stats_partials = torch.zeros(max(len(pl.enc_tiles), 1) * C.v2_stats_partials(), dtype=torch.float64,
                                               device=dev)
             self.stats_counters = torch.zeros(nc, dtype=torch.int32, device=dev)
+        # error feedback: fp32 residual per weight element (wshadow's physical order) and the apply chunks per group
+        self.residual = self.t_ef_chunks = None
+        self.ef_range = []
+        if self.error_feedback and self.is_worker:
+            assert C.v2_ef_chunk_bytes() == struct.calcsize(P2.EF_CHUNK_FMT)
+            self.residual = z(pl.w_total)
+            chunks, self.ef_range = P2.ef_chunks(pl)
+            self.t_ef_chunks = _dev_bytes(chunks, dev)
         self.loss_buf = torch.zeros(3, dtype=torch.float32, device=dev)
         self.static_x = self.static_y = self.graph = None
 
@@ -348,7 +377,8 @@ class ShadowEngine:
         per parameter tensor (the block units of a tensor summed) and for the whole model,
 
         * ``gsq``       ``||g||^2`` of the bf16 gradient the encoder read (coded tensors; None for tensors that travel
-                        exactly: 1-D vectors in fp32, dense bf16 weights),
+                        exactly: 1-D vectors in fp32, dense bf16 weights).  With ``error_feedback=True`` the encoder
+                        reads the coded input ``bf16(g + e)``, so every statistic describes that input, not ``g``,
         * ``mse``       the expected ``||g_hat - g||^2`` given that gradient, in closed form (exact, not sampled);
                         ``rel_var`` = ``mse / gsq``,
         * ``bias_sq``   TernGrad's clip bias ``||clip(g) - g||^2`` (0 for the other codes; not part of ``mse``),
@@ -399,6 +429,16 @@ class ShadowEngine:
             self.stats_acc.zero_()
         return {"code": self.code, "steps": steps, "model": tot, "tensors": per}
 
+    def error_feedback_norm(self) -> dict:
+        """``||e||`` of this worker's error-feedback residual: per weight tensor and for the whole model
+        (``error_feedback=True``).  Reading it synchronises the device."""
+        if self.residual is None:
+            raise RuntimeError("error_feedback_norm() needs ShadowEngine(..., error_feedback=True) on a worker")
+        names = {id(p): n for n, p in self.model.named_parameters()}
+        ws = [(names.get(id(p), str(q.index)), q) for p, q in zip(self.params, self.plan.params) if q.is_w]
+        sq = torch.stack([self.residual[q.off:q.off + q.numel].double().square().sum() for _, q in ws]).tolist()
+        return {"model": float(sum(sq)) ** 0.5, "tensors": {n: v ** 0.5 for (n, _), v in zip(ws, sq)}}
+
     def _launch_code_stats(self, g: int):
         """Estimator statistics of group ``g``: after its push on the same stream (the gradient, this step's sigma /
         selcount / L1 / clip and this worker's slot headers and norms are live until the next encode)."""
@@ -434,6 +474,11 @@ class ShadowEngine:
             lo, hi = self.w_range[g]
             if hi > lo:   # pageable source: staged synchronously, safe against the host table changing next step
                 self.t_gptr[lo:hi].copy_(torch.from_numpy(self.host_gptr[lo:hi].copy()))
+        res = self.residual.data_ptr() if self.residual is not None else 0
+        if res:     # A = g + e into the gradient buffers (bf16) and the residual (its rounding remainder)
+            c0, ncs = self.ef_range[g]
+            C.v2_ef_apply(self.t_ef_chunks.data_ptr(), c0, ncs, self.t_gptr.data_ptr(), res)
+            self._nlaunch += 1
         if nt > 0 and self.quant:
             # quantize + push straight into the owners' arenas; the encode launch raises the group's push flag
             if self.clip is not None:
@@ -446,7 +491,7 @@ class ShadowEngine:
                              self.t_sig_owner.data_ptr(), self.n_owners, pl.arena_floats, self.worker_index, g,
                              self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g, 0, self.tstats.data_ptr(),
                              self._fired == self.G, self.clip is None, self.q_max_level, self.q_max_bucket,
-                             self.code == "terngrad")
+                             self.code == "terngrad", res)
             self._nlaunch += 1
             return
         if nt > 0 and self.entry:
@@ -457,7 +502,7 @@ class ShadowEngine:
             C.v2_entry_encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
                               self.l1.data_ptr(), self.t_arena_peer.data_ptr(), self.t_sig_owner.data_ptr(),
                               self.n_owners, pl.arena_floats, self.worker_index, g, self.ctrl.data_ptr(),
-                              self.cnt_enc_group + 4 * g, 0, self.tstats.data_ptr(), self._fired == self.G)
+                              self.cnt_enc_group + 4 * g, 0, self.tstats.data_ptr(), self._fired == self.G, res)
             self._nlaunch += 2
             return
         if nt > 0 and self.code in ("svd", "qsvd"):
@@ -481,7 +526,7 @@ class ShadowEngine:
                      self.vsel.data_ptr(), self.selcount.data_ptr(), self.t_arena_peer.data_ptr(),
                      self.t_sig_owner.data_ptr(), self.n_owners, pl.arena_floats, self.worker_index, g,
                      self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g, self.kflags, self.tstats.data_ptr(),
-                     self._fired == self.G, nt > 0)
+                     self._fired == self.G, nt > 0, res, max(self.owner_index, 0))
         self._nlaunch += 1
 
     def _launch_ps(self, g: int, final: bool):
@@ -712,7 +757,8 @@ class ShadowEngine:
     def save_checkpoint(self, train_dir: str, step: Optional[int] = None) -> Optional[str]:
         """Collective.  The first training rank writes ``model_step_<N>`` (fp32, trained BN statistics) and the
         ``_optim`` sidecar (momentum — for Adam / AMSGrad also the second moments —, step, LR) so a later run can
-        resume."""
+        resume.  Error-feedback residuals are per-worker state and are not written: a resumed run starts from
+        ``e = 0``."""
         from ..utils import checkpoint as ckpt
         step = (self.step - 1) if step is None else step
         sd = self.fp32_state_dict()

@@ -89,4 +89,9 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                    help="p2p backend, bf16 engine: per-layer estimator statistics of the code (expected squared error "
                         "given the gradient, expected / realized atoms, realized push bytes) in every --metrics-file "
                         "record; not for --code qsvd")
+    p.add_argument("--error-feedback", type=bool_flag, default=False,
+                   help="p2p backend, bf16 engine: every worker keeps the part of its gradient the code did not send "
+                        "(an fp32 residual per weight) and adds it to the next step's gradient before coding; --code "
+                        "svd | qsgd, every push counted (no --num-aggregate below the worker count).  Residuals are "
+                        "not checkpointed: --resume starts them from zero")
     return p.parse_args(argv)
