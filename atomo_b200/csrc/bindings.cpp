@@ -122,6 +122,22 @@ void atomo_v2_launch_ps_entry(const void* units, const void* tiles, int tile0, i
                               const float* arenas, long long arena_floats, int* sig, int* const* sig_peer, void* ctrl,
                               unsigned int* group_counter, long long timeout, long long* tstats, float inv_w, int grid,
                               cudaStream_t stream);
+// v2_topk.cu (top-k units of the bf16 engine; the PS is v2_ps_entry)
+int atomo_v2_topk_state_ints();
+int atomo_v2_topk_hist_bins();
+int atomo_v2_topk_tile_bins();
+void atomo_v2_launch_topk_select(const void* units, const void* tiles, int tile0, int ntiles, const long long* gptr,
+                                 int* hist, int* tile_counts, unsigned int* unit_counters, int* sel, long long* tstats,
+                                 int group, cudaStream_t stream);
+void atomo_v2_launch_topk_encode(const void* units, const void* tiles, int tile0, int ntiles, const long long* gptr,
+                                 const int* sel, const int* tile_counts, float* const* arena_peer,
+                                 int* const* sig_peer, int n_owners, long long arena_floats, int worker, int group,
+                                 const void* ctrl, unsigned int* group_counter, long long* tstats, int final_group,
+                                 float* residual, cudaStream_t stream);
+void atomo_v2_launch_topk_code_stats(const void* units, const void* tiles, int tile0, int ntiles,
+                                     const long long* gptr, const int* sel, const int* tile_counts,
+                                     float* const* arena_peer, int n_owners, long long arena_floats, int worker,
+                                     double* partials, unsigned int* unit_counters, double* acc, cudaStream_t stream);
 // v2_feedback.cu (error feedback of the bf16 engine)
 int atomo_v2_ef_chunk_bytes();
 void atomo_v2_launch_ef_apply(const void* chunks, int chunk0, int nchunks, const long long* gptr, float* residual,
@@ -511,6 +527,41 @@ void v2_entry_encode(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint
                                P<float>(residual), cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
+// top-k: the two selection launches (high / low magnitude bits; per-unit histogram, tile counts, state) of one group
+void v2_topk_select(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t hist,
+                    uint64_t tile_counts, uint64_t counters, uint64_t sel, uint64_t tstats, int group) {
+  TORCH_CHECK(hist != 0 && tile_counts != 0 && counters != 0 && sel != 0,
+              "v2_topk_select: hist / tile_counts / counters / sel required");
+  atomo_v2_launch_topk_select(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
+                              P<int>(hist), P<int>(tile_counts), P<unsigned int>(counters), P<int>(sel),
+                              P<long long>(tstats), group, cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+void v2_topk_encode(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t sel,
+                    uint64_t tile_counts, uint64_t arena_peer, uint64_t sig_peer, int n_owners, int64_t arena_floats,
+                    int worker, int group, uint64_t ctrl, uint64_t group_counter, uint64_t tstats, bool final_group,
+                    uint64_t residual) {
+  TORCH_CHECK(sel != 0 && tile_counts != 0, "v2_topk_encode: needs the selection of v2_topk_select");
+  TORCH_CHECK(worker >= 0 && worker < 16, "v2_topk_encode: worker index must be in [0, 16)");
+  atomo_v2_launch_topk_encode(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
+                              P<const int>(sel), P<const int>(tile_counts), P<float* const>(arena_peer),
+                              P<int* const>(sig_peer), n_owners, arena_floats, worker, group, P<const void>(ctrl),
+                              P<unsigned int>(group_counter), P<long long>(tstats), final_group ? 1 : 0,
+                              P<float>(residual), cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+void v2_topk_code_stats(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t sel,
+                        uint64_t tile_counts, uint64_t arena_peer, int n_owners, int64_t arena_floats, int worker,
+                        uint64_t partials, uint64_t counters, uint64_t acc) {
+  TORCH_CHECK(partials != 0 && counters != 0 && acc != 0 && sel != 0 && tile_counts != 0,
+              "v2_topk_code_stats: partials / counters / acc / sel / tile_counts required");
+  TORCH_CHECK(worker >= 0 && worker < 16, "v2_topk_code_stats: worker index must be in [0, 16)");
+  atomo_v2_launch_topk_code_stats(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
+                                  P<const int>(sel), P<const int>(tile_counts), P<float* const>(arena_peer), n_owners,
+                                  arena_floats, worker, P<double>(partials), P<unsigned int>(counters), P<double>(acc),
+                                  cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
 // error feedback: A = g + e, bf16(A) into the gradient buffers, A - bf16(A) into the residual, for the apply chunks
 // [chunk0, chunk0 + nchunks) of the chunk table (one backward group); before the group's encode, on the same stream
 void v2_ef_apply(uint64_t chunks, int chunk0, int nchunks, uint64_t gptr, uint64_t residual) {
@@ -668,6 +719,15 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("gptr"), py::arg("l1"), py::arg("arena_peer"), py::arg("sig_peer"), py::arg("n_owners"),
         py::arg("arena_floats"), py::arg("worker"), py::arg("group"), py::arg("ctrl"), py::arg("group_counter"),
         py::arg("ext_uniforms"), py::arg("tstats"), py::arg("final_group"), py::arg("residual") = 0);
+  m.def("v2_topk_select", &v2_topk_select);
+  m.def("v2_topk_encode", &v2_topk_encode, py::arg("units"), py::arg("tiles"), py::arg("tile0"), py::arg("ntiles"),
+        py::arg("gptr"), py::arg("sel"), py::arg("tile_counts"), py::arg("arena_peer"), py::arg("sig_peer"),
+        py::arg("n_owners"), py::arg("arena_floats"), py::arg("worker"), py::arg("group"), py::arg("ctrl"),
+        py::arg("group_counter"), py::arg("tstats"), py::arg("final_group"), py::arg("residual") = 0);
+  m.def("v2_topk_code_stats", &v2_topk_code_stats);
+  m.def("v2_topk_sizes", []() {
+    return py::make_tuple(atomo_v2_topk_state_ints(), atomo_v2_topk_hist_bins(), atomo_v2_topk_tile_bins());
+  });
   m.def("v2_ef_apply", &v2_ef_apply);
   m.def("v2_ef_chunk_bytes", &atomo_v2_ef_chunk_bytes);
   m.def("v2_ps_entry", &v2_ps_entry);

@@ -173,5 +173,15 @@ __host__ __device__ inline long long entry_words_off(int n_ps, int j, int ps_row
   return 4LL * n_ps + (long long)j * ps_rows;
 }
 
+// Top-k entry units (v2_topk.cu; same slots, budget = k): the selection state of unit ts_index is
+// sel[TOPK_STATE * ts_index + TK_*]; hist[TOPK_HI_BINS * ts_index] is the unit's histogram (all zero between launches),
+// tiles[TOPK_LO_BINS * encode tile] the tile's counts of the low magnitude bits inside the threshold's high bin.
+// A threshold of TOPK_NONE keeps nothing (all-zero or non-finite tensor).
+constexpr int TOPK_STATE = 8;
+constexpr int TOPK_HI_BINS = 256;     // magnitude bits 14..7
+constexpr int TOPK_LO_BINS = 128;     // magnitude bits 6..0
+constexpr int TOPK_NONE = 0x8000;
+enum TopkField : int { TK_BIN = 0, TK_NEED_BIN = 1, TK_T = 2, TK_NEED_TIES = 3, TK_KEFF = 4, TK_NONFINITE = 5 };
+
 }  // namespace v2
 }  // namespace atomo

@@ -33,6 +33,7 @@ Pure Python (unit-testable on CPU).  Struct layouts mirror ``csrc/v2_common.cuh`
 """
 from __future__ import annotations
 
+import math
 import struct
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
@@ -53,6 +54,7 @@ QSGD_TILE_ELEMS = 4096        # a QSGD PS / encode tile holds max(1, 4096 // buc
 QSGD_MAX_BUCKET = 1024        # one warp quantizes one bucket, staged in shared memory
 QSGD_MAX_LEVEL = 14           # (sign + 1) << q | level must fit 16 bits
 ENTRY_TILE_ELEMS = 4096       # entry-wise PS / encode tile: the element offset of an entry fits 12 bits
+TOPK_STATE_INTS, TOPK_HI_BINS, TOPK_LO_BINS = 8, 256, 128   # top-k selection state / histograms (csrc/v2_common.cuh)
 
 UNIT_FMT = "<4q20i"           # 112 bytes, mirrors struct Unit2
 TILE_FMT = "<4i"              # unit, a, b, owner
@@ -124,6 +126,11 @@ def entry_atoms(budget: float, numel: int) -> float:
     ``[1, numel]`` (``codings.entrywise.EntryWise.atoms_for``)."""
     s = budget * numel if budget < 1.0 else budget
     return float(min(max(s, 1.0), numel))
+
+
+def topk_atoms(budget: float, numel: int) -> int:
+    """``k`` of a top-k unit: ``floor(s)`` of :func:`entry_atoms` (``codings.topk.TopK.k_for``), at least 1."""
+    return int(math.floor(entry_atoms(budget, numel)))
 
 
 def slot_capacity(cols: int, rank: int, systematic: bool) -> int:
@@ -240,7 +247,8 @@ class Plan2:
 
     def entry_bytes(self) -> float:
         """Bytes of entry-wise code a worker pushes per step: 4 per expected atom and a 16-byte header per PS tile.
-        An upper bound on the expectation (``sum(p_i) <= s``), exact when no ``p_i`` is clamped to 1."""
+        An upper bound on the expectation (``sum(p_i) <= s``), exact when no ``p_i`` is clamped to 1.  Top-k: an
+        upper bound on the realized bytes, exact when every tensor has at least ``k`` non-zero entries."""
         return sum(4.0 * u.budget + 16.0 * u.n_ps for u in self.units if u.kind == KIND_ENTRY)
 
     def expected_factor_bytes(self) -> float:
@@ -305,7 +313,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 n_owners: int = 1, n_groups: int = 4, groups: Optional[Sequence[int]] = None,
                 block_cols: int = BLOCK_COLS, min_coded_numel: int = 256, quantization_level: int = 4,
                 bucket_size: int = 512, entry_budget: float = 0.05) -> Plan2:
-    """Plan of the bf16 engine for ``code`` in ``svd | qsvd | sgd | qsgd | terngrad | entrywise``.
+    """Plan of the bf16 engine for ``code`` in ``svd | qsvd | sgd | qsgd | terngrad | entrywise | topk``.
 
     ``qsgd`` / ``terngrad``: every >= 2-D weight (the 3-channel stem and the fc layers included) is exactly one
     ``KIND_QSGD`` unit; there are no ``DENSE16`` units.  1-D parameters stay ``KIND_VEC`` (fp32, summed by
@@ -337,10 +345,13 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
       count, owner);
     * the slot holds a 16-byte header per tile, then room for one uint32 entry per element of every tile
       (:func:`entry_hdr_off` / :func:`entry_words_off`), so a tile cannot overflow.
+
+    ``topk``: the units, tiles, owners, slots and headers of ``entrywise``, with ``budget = k`` (:func:`topk_atoms`, an
+    integer: the exact number of entries pushed when the tensor has at least ``k`` non-zeros).
     """
     shapes = [tuple(int(d) for d in s) for s in shapes]
     quant = code in ("qsgd", "terngrad")
-    entry = code == "entrywise"
+    entry = code in ("entrywise", "topk")
     if entry and not entry_budget > 0:
         raise ValueError("entry_budget must be positive (a fraction of numel below 1, else an atom count)")
     if quant:
@@ -391,7 +402,10 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                       ps_rows=bpt * bucket))
             continue
         if entry:
-            add(Unit2(0, KIND_ENTRY, p.index, p.widx, p.off, 0, budget=entry_atoms(float(entry_budget), p.numel),
+            s_atoms = entry_atoms(float(entry_budget), p.numel)
+            if code == "topk":
+                s_atoms = float(topk_atoms(float(entry_budget), p.numel))
+            add(Unit2(0, KIND_ENTRY, p.index, p.widx, p.off, 0, budget=s_atoms,
                       numel=p.numel, group=p.group, ps_rows=ENTRY_TILE_ELEMS))
             continue
         coded = code == "svd" and p.numel >= min_coded_numel

@@ -45,6 +45,9 @@ def build_coder(kwargs: dict, worker_side: bool):
     if code == "entrywise":
         return codings.build("entrywise", budget=kwargs.get("entry_budget", 0.05),
                              prob_rule=kwargs.get("prob_rule", "reference"))
+    if code == "topk":
+        raise ValueError("--code topk runs on the --backend p2p bf16 engine (--dtype bf16), which keeps the "
+                         "error-feedback residual; top-k without it is biased, and the gloo / nccl coders keep none")
     if code == "bsvd":
         return codings.build("bsvd", rank=kwargs.get("svd_rank", 0) or 3, random_sample=worker_side,
                              prob_rule=kwargs.get("prob_rule", "reference"),

@@ -6,10 +6,11 @@ Counterpart of the role dispatch in ``/root/reference/src/distributed_nn.py:243-
 checkpoints in the ``model_step_<N>`` layout, and the reference's log lines with REAL per-phase numbers taken from
 device-side timers (``Comp`` / ``Encode`` / ``Comm`` on the worker line, ``Decode Cost`` / ``Gather`` on the PS line).
 
-Engine choice (``--engine auto``): ``--dtype bf16`` with ``--code svd|qsvd|sgd`` runs the overlapped, sharded
+Engine choice (``--engine auto``): ``--dtype bf16`` with ``--code svd|qsvd|sgd|topk`` runs the overlapped, sharded
 ``ShadowEngine``; everything else (fp32, qsgd / terngrad / entrywise) runs the fp32-flat ``FusedEngine``.
-``--engine shadow`` also runs ``--code qsgd|terngrad`` on ``ShadowEngine`` (bf16 only); ``--engine fused`` always
-picks ``FusedEngine``.
+``--engine shadow`` also runs ``--code qsgd|terngrad`` on ``ShadowEngine`` (bf16 only) and refuses ``--code
+entrywise``, which the launcher keeps on ``FusedEngine``; ``--engine fused`` always picks ``FusedEngine``.  ``--code
+topk`` exists only on ``ShadowEngine``.
 """
 from __future__ import annotations
 
@@ -34,14 +35,17 @@ class _HostEvent:
 def _build_engine(args, model, rank, world):
     engine = getattr(args, "engine", "auto")
     code = args.code.lower()
+    if code == "topk" and (engine == "fused" or args.dtype != "bf16"):
+        raise SystemExit("--code topk runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the fp32-flat "
+                         "engine has no top-k selection")
     if engine == "auto":
-        shadow = args.dtype == "bf16" and code in ("svd", "qsvd", "sgd", "dense", "lossless")
+        shadow = args.dtype == "bf16" and code in ("svd", "qsvd", "sgd", "dense", "lossless", "topk")
     elif engine == "shadow":
         if args.dtype != "bf16":
             raise SystemExit("--engine shadow trains bf16 weights: it needs --dtype bf16 (fp32 runs on --engine fused)")
-        if code not in ("svd", "qsvd", "sgd", "dense", "lossless", "qsgd", "terngrad"):
-            raise SystemExit("--engine shadow runs --code svd|qsvd|sgd|qsgd|terngrad; --code %s runs on --engine fused"
-                             % args.code)
+        if code not in ("svd", "qsvd", "sgd", "dense", "lossless", "qsgd", "terngrad", "topk"):
+            raise SystemExit("--engine shadow runs --code svd|qsvd|sgd|qsgd|terngrad|topk; --code %s runs on --engine "
+                             "fused" % args.code)
         shadow = True
     else:
         shadow = False
@@ -50,6 +54,8 @@ def _build_engine(args, model, rank, world):
         kw = {}
         if code in ("qsgd", "terngrad"):
             kw = dict(quantization_level=args.quantization_level, bucket_size=args.bucket_size)
+        elif code == "topk":
+            kw = dict(entry_budget=args.entry_budget)
         if getattr(args, "code_stats", False):
             if code == "qsvd":
                 raise SystemExit("--code-stats does not model QSVD's int8 left factors (use --code svd)")

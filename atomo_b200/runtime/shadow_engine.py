@@ -26,7 +26,11 @@ one central PS kernel at the end of the step):
   launch takes its fp64 L1 norm, the encode launch samples entries with ``p_i = min(1, s |g_i| / ||g||_1)`` and
   pushes them as 4-byte words (``csrc/v2_entrywise.cu``), and the owners scatter-add them in worker order and step
   the optimizer.  BN and bias vectors stay fp32, as above.
-* **Error feedback** (``error_feedback=True``; svd, entrywise, qsgd): each worker keeps an fp32 residual ``e`` per
+* **Top-k** (``code="topk"``, ``entry_budget``): the entry units, slots and PS of entry-wise ATOMO with ``k =
+  floor(s)`` entries per tensor.  Two selection launches find each tensor's threshold magnitude from histograms of the
+  bf16 bits, and the encode pushes the ``k`` largest entries exactly (``csrc/v2_topk.cu``).  Deterministic and
+  biased on its own: it is the contractive code for ``error_feedback=True``.
+* **Error feedback** (``error_feedback=True``; svd, entrywise, topk, qsgd): each worker keeps an fp32 residual ``e`` per
   weight element and codes ``A = g + e``.  An apply launch per group (``csrc/v2_feedback.cu``) writes ``bf16(A)`` into
   autograd's gradient buffer in place and keeps ``A - bf16(A)``; the encoders' epilogues add ``bf16(A) - g_hat``, the
   part of ``A`` this push did not carry.  Nothing is discarded, only delayed.
@@ -73,8 +77,8 @@ class ShadowEngine:
                  bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False,
                  error_feedback: bool = False):
         self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
-        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise"):
-            raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise")
+        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk"):
+            raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise | topk")
         self.error_feedback = bool(error_feedback)
         if self.error_feedback:     # checked before any CUDA work
             if self.code == "qsvd":
@@ -96,12 +100,13 @@ class ShadowEngine:
             if resample_empty:
                 raise ValueError("code_stats needs resample_empty=False: redrawing empty selections biases the "
                                  "estimator, and the closed-form error no longer holds")
-        self.entry = self.code == "entrywise"
+        self.entry = self.code in ("entrywise", "topk")
+        self.topk = self.code == "topk"
         self.entry_budget = float(entry_budget)
         if self.entry:      # checked before any CUDA work
             if prob_rule != "reference" or sampling != "bernoulli":
-                raise ValueError("entrywise on ShadowEngine samples with prob_rule='reference' and "
-                                 "sampling='bernoulli' only (got %r / %r)" % (prob_rule, sampling))
+                raise ValueError("%s on ShadowEngine runs with prob_rule='reference' and sampling='bernoulli' only "
+                                 "(got %r / %r)" % (self.code, prob_rule, sampling))
             if not self.entry_budget > 0:
                 raise ValueError("entry_budget must be positive (a fraction of numel below 1, else an atom count)")
         self.C = load_ext()
@@ -272,7 +277,15 @@ class ShadowEngine:
             self.clip_partials = torch.zeros(2 * max(len(pl.enc_tiles), 1), dtype=torch.float64, device=dev)
         # entry-wise: fp64 L1 norm per unit and its per-tile partials
         self.l1 = self.l1_partials = None
-        if self.entry:
+        # top-k: selection state and histogram per unit (the histogram is zero between launches), tie counts per tile
+        self.topk_sel = self.topk_hist = self.topk_tiles = None
+        if self.topk:
+            n_state, n_hi, n_lo = C.v2_topk_sizes()
+            assert (n_state, n_hi, n_lo) == (P2.TOPK_STATE_INTS, P2.TOPK_HI_BINS, P2.TOPK_LO_BINS)
+            i32 = lambda n: torch.zeros(n, dtype=torch.int32, device=dev)
+            self.topk_sel, self.topk_hist = i32(nc * n_state), i32(nc * n_hi)
+            self.topk_tiles = i32(max(len(pl.enc_tiles), 1) * n_lo)
+        elif self.entry:
             self.l1 = torch.zeros(nc, dtype=torch.float64, device=dev)
             self.l1_partials = torch.zeros(max(len(pl.enc_tiles), 1), dtype=torch.float64, device=dev)
         self.counters = torch.zeros(nc + 2 * P2.MAX_GROUPS + 8, dtype=torch.int32, device=dev)
@@ -446,6 +459,14 @@ class ShadowEngine:
         if self.stats_acc is None or nt == 0:
             return
         p = lambda t: t.data_ptr() if t is not None else 0
+        if self.topk:
+            self.C.v2_topk_code_stats(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt,
+                                      self.t_gptr.data_ptr(), self.topk_sel.data_ptr(), self.topk_tiles.data_ptr(),
+                                      self.t_arena_peer.data_ptr(), self.n_owners, self.plan.arena_floats,
+                                      self.worker_index, self.stats_partials.data_ptr(),
+                                      self.stats_counters.data_ptr(), self.stats_acc.data_ptr())
+            self._nlaunch += 1
+            return
         spectral = self.code == "svd"
         self.C.v2_code_stats(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
                              self.sigma.data_ptr() if spectral else 0, self.selcount.data_ptr(), p(self.l1),
@@ -493,6 +514,18 @@ class ShadowEngine:
                              self._fired == self.G, self.clip is None, self.q_max_level, self.q_max_bucket,
                              self.code == "terngrad", res)
             self._nlaunch += 1
+            return
+        if nt > 0 and self.topk:
+            # per-tensor threshold magnitude (two histogram launches), then the k largest entries pushed exactly
+            C.v2_topk_select(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
+                             self.topk_hist.data_ptr(), self.topk_tiles.data_ptr(), self.counters.data_ptr(),
+                             self.topk_sel.data_ptr(), self.tstats.data_ptr(), g)
+            C.v2_topk_encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
+                             self.topk_sel.data_ptr(), self.topk_tiles.data_ptr(), self.t_arena_peer.data_ptr(),
+                             self.t_sig_owner.data_ptr(), self.n_owners, pl.arena_floats, self.worker_index, g,
+                             self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g, self.tstats.data_ptr(),
+                             self._fired == self.G, res)
+            self._nlaunch += 3
             return
         if nt > 0 and self.entry:
             # per-tensor L1 norms, then sample + compact + push into the owners' arenas (raises the push flag)

@@ -30,7 +30,9 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
     p.add_argument("--network", type=str, default="LeNet", metavar="N")
     p.add_argument("--code", type=str, default="sgd",
                    help="sgd | svd | qsgd | terngrad | entrywise | qsvd | bsvd (block-spectral: the estimator the sm_90a "
-                        "bf16 engine applies under --code svd, as a plain PyTorch coder)")
+                        "bf16 engine applies under --code svd, as a plain PyTorch coder) | topk (the --entry-budget "
+                        "largest entries per tensor, sent exactly; --backend p2p --dtype bf16 only, meant for "
+                        "--error-feedback 1)")
     p.add_argument("--bucket-size", type=int, default=512)
     p.add_argument("--dataset", type=str, default="MNIST", metavar="N")
     p.add_argument("--comm-type", type=str, default="Bcast", metavar="N")
@@ -51,7 +53,8 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
     p.add_argument("--data-root", type=str, default=".")
     p.add_argument("--train-len", type=int, default=0, help="truncate the training set (0 = full)")
     p.add_argument("--test-len", type=int, default=0)
-    p.add_argument("--entry-budget", type=float, default=0.05, help="entry-wise ATOMO budget (fraction or count)")
+    p.add_argument("--entry-budget", type=float, default=0.05, help="entry-wise ATOMO / top-k budget: a fraction of each tensor's "
+                   "elements below 1, else an atom count (top-k sends floor of it)")
     p.add_argument("--sampling", type=str, default="bernoulli", choices=["bernoulli", "systematic"])
     p.add_argument("--prob-rule", type=str, default="reference", choices=["reference", "waterfill"])
     p.add_argument("--optimizer", type=str, default="sgd", choices=["sgd", "adam"])
@@ -70,7 +73,7 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "colocated = rank 0 hosts the whole PS and also trains; dedicated = rank 0 only serves")
     p.add_argument("--engine", type=str, default="auto", choices=["auto", "shadow", "fused"],
                    help="p2p backend: auto = the overlapped sharded bf16 engine for --dtype bf16 with --code "
-                        "svd|qsvd|sgd, the fp32-flat engine otherwise; shadow = the bf16 engine (also --code "
+                        "svd|qsvd|sgd|topk, the fp32-flat engine otherwise; shadow = the bf16 engine (also --code "
                         "qsgd|terngrad, needs --dtype bf16); fused = the fp32-flat engine")
     p.add_argument("--groups", type=int, default=5, help="p2p/bf16: backward groups pushed while backward runs")
     p.add_argument("--shrinkage-freq", type=int, default=50, help="steps between LR shrinkages (reference: 50)")
@@ -92,6 +95,7 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
     p.add_argument("--error-feedback", type=bool_flag, default=False,
                    help="p2p backend, bf16 engine: every worker keeps the part of its gradient the code did not send "
                         "(an fp32 residual per weight) and adds it to the next step's gradient before coding; --code "
-                        "svd | qsgd, every push counted (no --num-aggregate below the worker count).  Residuals are "
+                        "svd | entrywise | topk | qsgd (it stays bounded with svd top-k and topk, the contractive "
+                        "codes), every push counted (no --num-aggregate below the worker count).  Residuals are "
                         "not checkpointed: --resume starts them from zero")
     return p.parse_args(argv)
