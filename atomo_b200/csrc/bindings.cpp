@@ -138,6 +138,23 @@ void atomo_v2_launch_topk_code_stats(const void* units, const void* tiles, int t
                                      const long long* gptr, const int* sel, const int* tile_counts,
                                      float* const* arena_peer, int n_owners, long long arena_floats, int worker,
                                      double* partials, unsigned int* unit_counters, double* acc, cudaStream_t stream);
+// v2_sign.cu (scaled-sign units of the bf16 engine)
+void atomo_v2_launch_sign_encode(const void* units, const void* tiles, int tile0, int ntiles, const long long* gptr,
+                                 float* const* arena_peer, int* const* sig_peer, int n_owners, long long arena_floats,
+                                 int worker, int group, const void* ctrl, unsigned int* group_counter,
+                                 long long* tstats, int final_group, float* residual, cudaStream_t stream);
+void atomo_v2_launch_ps_sign(const void* units, const void* tiles, int tile0, int ntiles, int W, int nranks, int group,
+                             int final_group, int owner, float* master, float* mom, float* sq, float* sqmax,
+                             float* vmom, float* vsq, float* vsqmax, void* wshadow_mc, void* const* wshadow_peer,
+                             float* vparams_local, float* vparams_mc, float* const* vparams_peer,
+                             const float* vgrads_mc, const float* const* vgrads_peer, const float* arenas,
+                             long long arena_floats, int* sig, int* const* sig_peer, void* ctrl,
+                             unsigned int* group_counter, long long timeout, long long* tstats, float inv_w, int grid,
+                             cudaStream_t stream);
+void atomo_v2_launch_sign_code_stats(const void* units, const void* tiles, int tile0, int ntiles,
+                                     const long long* gptr, float* const* arena_peer, int n_owners,
+                                     long long arena_floats, int worker, double* partials, unsigned int* unit_counters,
+                                     double* acc, cudaStream_t stream);
 // v2_feedback.cu (error feedback of the bf16 engine)
 int atomo_v2_ef_chunk_bytes();
 void atomo_v2_launch_ef_apply(const void* chunks, int chunk0, int nchunks, const long long* gptr, float* residual,
@@ -562,6 +579,44 @@ void v2_topk_code_stats(uint64_t units, uint64_t tiles, int tile0, int ntiles, u
                                   cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
+// scaled sign: the bucket travels in the unit table; the encode is the group's only launch (it raises the push flag)
+void v2_sign_encode(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t arena_peer,
+                    uint64_t sig_peer, int n_owners, int64_t arena_floats, int worker, int group, uint64_t ctrl,
+                    uint64_t group_counter, uint64_t tstats, bool final_group, uint64_t residual) {
+  TORCH_CHECK(worker >= 0 && worker < 16, "v2_sign_encode: worker index must be in [0, 16)");
+  atomo_v2_launch_sign_encode(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
+                              P<float* const>(arena_peer), P<int* const>(sig_peer), n_owners, arena_floats, worker,
+                              group, P<const void>(ctrl), P<unsigned int>(group_counter), P<long long>(tstats),
+                              final_group ? 1 : 0, P<float>(residual), cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+void v2_ps_sign(uint64_t units, uint64_t tiles, int tile0, int ntiles, int W, int nranks, int group, bool final_group,
+                int owner, uint64_t master, uint64_t mom, uint64_t sq, uint64_t sqmax, uint64_t vmom, uint64_t vsq,
+                uint64_t vsqmax, uint64_t wshadow_mc, uint64_t wshadow_peer, uint64_t vparams_local,
+                uint64_t vparams_mc, uint64_t vparams_peer, uint64_t vgrads_mc, uint64_t vgrads_peer, uint64_t arenas,
+                int64_t arena_floats, uint64_t sig, uint64_t sig_peer, uint64_t ctrl, uint64_t group_counter,
+                int64_t timeout, uint64_t tstats, double inv_w, int grid) {
+  TORCH_CHECK(W >= 1 && W <= 16, "too many workers for v2_ps_sign");
+  atomo_v2_launch_ps_sign(P<const void>(units), P<const void>(tiles), tile0, ntiles, W, nranks, group,
+                          final_group ? 1 : 0, owner, P<float>(master), P<float>(mom), P<float>(sq), P<float>(sqmax),
+                          P<float>(vmom), P<float>(vsq), P<float>(vsqmax), P<void>(wshadow_mc),
+                          P<void* const>(wshadow_peer), P<float>(vparams_local), P<float>(vparams_mc),
+                          P<float* const>(vparams_peer), P<const float>(vgrads_mc), P<const float* const>(vgrads_peer),
+                          P<const float>(arenas), arena_floats, P<int>(sig), P<int* const>(sig_peer), P<void>(ctrl),
+                          P<unsigned int>(group_counter), timeout, P<long long>(tstats), (float)inv_w, grid,
+                          cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+void v2_sign_code_stats(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t arena_peer,
+                        int n_owners, int64_t arena_floats, int worker, uint64_t partials, uint64_t counters,
+                        uint64_t acc) {
+  TORCH_CHECK(partials != 0 && counters != 0 && acc != 0, "v2_sign_code_stats: partials / counters / acc required");
+  TORCH_CHECK(worker >= 0 && worker < 16, "v2_sign_code_stats: worker index must be in [0, 16)");
+  atomo_v2_launch_sign_code_stats(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
+                                  P<float* const>(arena_peer), n_owners, arena_floats, worker, P<double>(partials),
+                                  P<unsigned int>(counters), P<double>(acc), cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
 // error feedback: A = g + e, bf16(A) into the gradient buffers, A - bf16(A) into the residual, for the apply chunks
 // [chunk0, chunk0 + nchunks) of the chunk table (one backward group); before the group's encode, on the same stream
 void v2_ef_apply(uint64_t chunks, int chunk0, int nchunks, uint64_t gptr, uint64_t residual) {
@@ -728,6 +783,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("v2_topk_sizes", []() {
     return py::make_tuple(atomo_v2_topk_state_ints(), atomo_v2_topk_hist_bins(), atomo_v2_topk_tile_bins());
   });
+  m.def("v2_sign_encode", &v2_sign_encode, py::arg("units"), py::arg("tiles"), py::arg("tile0"), py::arg("ntiles"),
+        py::arg("gptr"), py::arg("arena_peer"), py::arg("sig_peer"), py::arg("n_owners"), py::arg("arena_floats"),
+        py::arg("worker"), py::arg("group"), py::arg("ctrl"), py::arg("group_counter"), py::arg("tstats"),
+        py::arg("final_group"), py::arg("residual") = 0);
+  m.def("v2_ps_sign", &v2_ps_sign);
+  m.def("v2_sign_code_stats", &v2_sign_code_stats);
   m.def("v2_ef_apply", &v2_ef_apply);
   m.def("v2_ef_chunk_bytes", &atomo_v2_ef_chunk_bytes);
   m.def("v2_ps_entry", &v2_ps_entry);

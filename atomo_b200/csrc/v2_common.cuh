@@ -8,7 +8,9 @@
 namespace atomo {
 namespace v2 {
 
-enum Kind : int { KIND_SLAB = 1, KIND_MAT = 2, KIND_DENSE16 = 3, KIND_VEC = 4, KIND_QSGD = 5, KIND_ENTRY = 6 };
+enum Kind : int {
+  KIND_SLAB = 1, KIND_MAT = 2, KIND_DENSE16 = 3, KIND_VEC = 4, KIND_QSGD = 5, KIND_ENTRY = 6, KIND_SIGN = 7
+};
 
 // One coding unit: a conv gradient in [O][K][I] (channels_last) layout ("SLAB": row (o,ri), column (b,k) of the
 // reference's (O*I/2, 2K) matricization is X_o[k][2ri+b]), a <=64-column block of a 2-D matrix ("MAT"), or a
@@ -18,6 +20,10 @@ enum Kind : int { KIND_SLAB = 1, KIND_MAT = 2, KIND_DENSE16 = 3, KIND_VEC = 4, K
 // the fields:  K = bucket (elements), I = q (quantization level), rows = buckets, cols = L (uint64 words per
 // bucket), rs = 1 for TernGrad (0 for QSGD), cs = buckets per PS tile, ps_rows = elements per PS tile,
 // ts_index = index among the QSGD units (TernGrad clip / stats counter).
+//
+// Scaled-sign units ("SIGN", v2_sign.cu: one per >= 2-D weight) use the QSGD fields and slot with one bit per element:
+// K = bucket, rows = buckets, cols = L = ceil(bucket / 64) uint64 words per bucket, cs = buckets per PS tile,
+// ps_rows = elements per PS tile, ts_index = index among the sign units; the slot's norms are the fp32 scales.
 //
 // Entry-wise units ("ENTRY", v2_entrywise.cu: one per >= 2-D weight, tiles over the physical element order) use
 // budget = expected atoms s (clamped to [1, numel]), ps_rows = elements per tile (ENTRY_TILE_ELEMS),

@@ -25,6 +25,8 @@ What changes against ``ops/plan.py`` (the fp32-flat plan of round 1):
 * **Quantizing codes** (``code="qsgd" | "terngrad"``, see :func:`build_plan2`): every >= 2-D weight is one
   ``QSGD`` unit whose buckets are quantized and bit-packed by the workers straight into the owners' arenas; the
   owners decode, sum and step the optimizer in one launch per group.
+* **Scaled sign** (``code="sign"``): every >= 2-D weight is one ``SIGN`` unit whose buckets are sent as one bit per
+  element and one fp32 scale, in the slot and tile geometry of the quantizing codes.
 * **Entry-wise ATOMO** (``code="entrywise"``): every >= 2-D weight is one ``ENTRY`` unit whose sampled entries are
   compacted by the workers into 4-byte words in the owners' arenas; the owners scatter-add, average and step the
   optimizer in one launch per group.
@@ -38,7 +40,7 @@ import struct
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
-KIND_SLAB, KIND_MAT, KIND_DENSE16, KIND_VEC, KIND_QSGD, KIND_ENTRY = 1, 2, 3, 4, 5, 6
+KIND_SLAB, KIND_MAT, KIND_DENSE16, KIND_VEC, KIND_QSGD, KIND_ENTRY, KIND_SIGN = 1, 2, 3, 4, 5, 6, 7
 RCAP_MAX = 32
 MAX_COLS = 64
 BLOCK_COLS = 32               # column-block width of MAT units (Jacobi cost ~ cols^3 sits in the encode launch)
@@ -53,6 +55,7 @@ V_ALIGN = 32                  # fp32 elements (128 B)
 QSGD_TILE_ELEMS = 4096        # a QSGD PS / encode tile holds max(1, 4096 // bucket) whole buckets
 QSGD_MAX_BUCKET = 1024        # one warp quantizes one bucket, staged in shared memory
 QSGD_MAX_LEVEL = 14           # (sign + 1) << q | level must fit 16 bits
+SIGN_MIN_BUCKET, SIGN_MAX_BUCKET = 64, 4096   # scaled sign: one warp per bucket, whole 64-bit words
 ENTRY_TILE_ELEMS = 4096       # entry-wise PS / encode tile: the element offset of an entry fits 12 bits
 TOPK_STATE_INTS, TOPK_HI_BINS, TOPK_LO_BINS = 8, 256, 128   # top-k selection state / histograms (csrc/v2_common.cuh)
 
@@ -225,7 +228,7 @@ class Plan2:
     stage_total: int        # bf16 elements of the dense-16 staging region
     arena_floats: int
     gpart_floats: int
-    n_coded: int            # units with per-unit device state (coded SLAB / MAT units, or the QSGD / ENTRY units)
+    n_coded: int            # units with per-unit device state (coded SLAB / MAT units, or the QSGD / ENTRY / SIGN units)
     rank: int
     code: str
 
@@ -242,8 +245,9 @@ class Plan2:
 
     def qsgd_bytes(self) -> int:
         """Bytes of quantized gradient a worker pushes per step: the uint64 words and fp32 norms of every bucket
-        (the same sizes as ``codings.qsgd``'s ``words`` and ``norms``)."""
-        return sum(8 * u.rows * u.cols + 4 * u.rows for u in self.units if u.kind == KIND_QSGD)
+        (the same sizes as ``codings.qsgd``'s ``words`` and ``norms``; for sign units ``codings.sign``'s ``words`` and
+        ``scales``)."""
+        return sum(8 * u.rows * u.cols + 4 * u.rows for u in self.units if u.kind in (KIND_QSGD, KIND_SIGN))
 
     def entry_bytes(self) -> float:
         """Bytes of entry-wise code a worker pushes per step: 4 per expected atom and a 16-byte header per PS tile.
@@ -265,7 +269,7 @@ class Plan2:
 
     def dense_bytes(self) -> int:
         return sum((2 if u.kind == KIND_DENSE16 else 4) * u.numel for u in self.units
-                   if not u.coded and u.kind not in (KIND_QSGD, KIND_ENTRY))
+                   if not u.coded and u.kind not in (KIND_QSGD, KIND_ENTRY, KIND_SIGN))
 
 
 def default_groups(shapes: Sequence[Sequence[int]], n_groups: int) -> List[int]:
@@ -313,7 +317,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 n_owners: int = 1, n_groups: int = 4, groups: Optional[Sequence[int]] = None,
                 block_cols: int = BLOCK_COLS, min_coded_numel: int = 256, quantization_level: int = 4,
                 bucket_size: int = 512, entry_budget: float = 0.05) -> Plan2:
-    """Plan of the bf16 engine for ``code`` in ``svd | qsvd | sgd | qsgd | terngrad | entrywise | topk``.
+    """Plan of the bf16 engine for ``code`` in ``svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign``.
 
     ``qsgd`` / ``terngrad``: every >= 2-D weight (the 3-channel stem and the fc layers included) is exactly one
     ``KIND_QSGD`` unit; there are no ``DENSE16`` units.  1-D parameters stay ``KIND_VEC`` (fp32, summed by
@@ -348,10 +352,17 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
 
     ``topk``: the units, tiles, owners, slots and headers of ``entrywise``, with ``budget = k`` (:func:`topk_atoms`, an
     integer: the exact number of entries pushed when the tensor has at least ``k`` non-zeros).
+
+    ``sign``: every >= 2-D weight is exactly one ``KIND_SIGN`` unit; 1-D parameters stay ``KIND_VEC``.  Buckets, tiles,
+    owners and slots are those of ``qsgd`` with ``bucket = min(bucket_size, numel)`` (``bucket_size`` a multiple of 64
+    in ``[64, 4096]``) and ``L = ceil(bucket / 64)`` words per bucket: one bit per element (``codings/sign.py``) in
+    place of the quantized codes and one fp32 scale per bucket in place of the norm.  ``Unit2`` fields: ``K`` = bucket,
+    ``rows`` = buckets, ``cols`` = L, ``cs`` = buckets per tile, ``ps_rows`` = elements per tile, ``I`` = ``rs`` = 0.
     """
     shapes = [tuple(int(d) for d in s) for s in shapes]
     quant = code in ("qsgd", "terngrad")
     entry = code in ("entrywise", "topk")
+    sign = code == "sign"
     if entry and not entry_budget > 0:
         raise ValueError("entry_budget must be positive (a fraction of numel below 1, else an atom count)")
     if quant:
@@ -360,6 +371,10 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             raise ValueError("quantization_level must be in [1, %d]" % QSGD_MAX_LEVEL)
         if not (32 <= bsz <= QSGD_MAX_BUCKET and bsz % 8 == 0):
             raise ValueError("bucket_size must be a multiple of 8 in [32, %d]" % QSGD_MAX_BUCKET)
+    if sign:
+        sbsz = int(bucket_size)
+        if not (SIGN_MIN_BUCKET <= sbsz <= SIGN_MAX_BUCKET and sbsz % 64 == 0):
+            raise ValueError("sign: bucket_size must be a multiple of 64 in [%d, %d]" % (SIGN_MIN_BUCKET, SIGN_MAX_BUCKET))
     ubits = 0
     if code == "qsvd":          # QSVD: spectral atoms with quantized left factors (README.md:141-142 of the reference)
         code, ubits = "svd", 8
@@ -400,6 +415,12 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             add(Unit2(0, KIND_QSGD, p.index, p.widx, p.off, 0, rows=nb, cols=qsgd_words_per_bucket(bucket, q),
                       K=bucket, I=q, rs=1 if code == "terngrad" else 0, cs=bpt, numel=p.numel, group=p.group,
                       ps_rows=bpt * bucket))
+            continue
+        if sign:
+            bucket = min(sbsz, p.numel)
+            bpt = max(1, QSGD_TILE_ELEMS // bucket)
+            add(Unit2(0, KIND_SIGN, p.index, p.widx, p.off, 0, rows=(p.numel + bucket - 1) // bucket,
+                      cols=(bucket + 63) // 64, K=bucket, cs=bpt, numel=p.numel, group=p.group, ps_rows=bpt * bucket))
             continue
         if entry:
             s_atoms = entry_atoms(float(entry_budget), p.numel)
@@ -474,11 +495,11 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             elif u.kind == KIND_DENSE16:
                 for e0 in range(0, u.numel, 8192):     # staging copy tiles
                     enc_tiles.append((u.index, e0, min(8192, u.numel - e0), 0))
-            elif u.kind in (KIND_QSGD, KIND_ENTRY):   # encode tiles = PS tiles (one destination owner per CTA)
+            elif u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN):   # encode tiles = PS tiles (one destination owner per CTA)
                 for j, e0 in enumerate(range(0, u.numel, u.ps_rows)):
                     enc_tiles.append((u.index, e0, min(u.ps_rows, u.numel - e0), j))
             u.n_enc = len(enc_tiles) - u.enc_tile0
-            if u.kind in (KIND_QSGD, KIND_ENTRY):
+            if u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN):
                 u.ts_index = n_coded
                 n_coded += 1
                 u.ps_tile0 = len(ps_by_group[g])
@@ -487,7 +508,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 u.n_ps = len(ps_by_group[g]) - u.ps_tile0
                 u.own0 = u.ps_tile0 % n_owners
                 u.slot_off = slot_off
-                if u.kind == KIND_QSGD:
+                if u.kind in (KIND_QSGD, KIND_SIGN):
                     slot_off += qsgd_slot_floats(u.n_ps, u.rows, u.cols)
                 else:
                     slot_off += entry_slot_floats(u.numel, u.n_ps, u.ps_rows)

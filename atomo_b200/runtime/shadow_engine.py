@@ -30,7 +30,11 @@ one central PS kernel at the end of the step):
   floor(s)`` entries per tensor.  Two selection launches find each tensor's threshold magnitude from histograms of the
   bf16 bits, and the encode pushes the ``k`` largest entries exactly (``csrc/v2_topk.cu``).  Deterministic and
   biased on its own: it is the contractive code for ``error_feedback=True``.
-* **Error feedback** (``error_feedback=True``; svd, entrywise, topk, qsgd): each worker keeps an fp32 residual ``e`` per
+* **Scaled sign** (``code="sign"``, ``bucket_size``): every weight's buckets are pushed as one bit per element and one
+  fp32 scale ``||b||_1 / |b|`` in the slots and tiles of QSGD (``csrc/v2_sign.cu``, one encode launch per group); the
+  owners decode ``+-scale``, sum in worker order and step the optimizer.  Deterministic, dense and biased on its own:
+  the contractive code of EF-SignSGD for ``error_feedback=True``.
+* **Error feedback** (``error_feedback=True``; svd, entrywise, topk, qsgd, sign): each worker keeps an fp32 residual ``e`` per
   weight element and codes ``A = g + e``.  An apply launch per group (``csrc/v2_feedback.cu``) writes ``bf16(A)`` into
   autograd's gradient buffer in place and keeps ``A - bf16(A)``; the encoders' epilogues add ``bf16(A) - g_hat``, the
   part of ``A`` this push did not carry.  Nothing is discarded, only delayed.
@@ -77,8 +81,8 @@ class ShadowEngine:
                  bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False,
                  error_feedback: bool = False):
         self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
-        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk"):
-            raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise | topk")
+        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign"):
+            raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign")
         self.error_feedback = bool(error_feedback)
         if self.error_feedback:     # checked before any CUDA work
             if self.code == "qsvd":
@@ -109,6 +113,11 @@ class ShadowEngine:
                                  "(got %r / %r)" % (self.code, prob_rule, sampling))
             if not self.entry_budget > 0:
                 raise ValueError("entry_budget must be positive (a fraction of numel below 1, else an atom count)")
+        self.sign = self.code == "sign"
+        if self.sign:       # checked before any CUDA work
+            if not (P2.SIGN_MIN_BUCKET <= int(bucket_size) <= P2.SIGN_MAX_BUCKET and int(bucket_size) % 64 == 0):
+                raise ValueError("sign: bucket_size must be a multiple of 64 in [%d, %d] (got %r)"
+                                 % (P2.SIGN_MIN_BUCKET, P2.SIGN_MAX_BUCKET, bucket_size))
         self.C = load_ext()
         C = self.C
         assert C.v2_unit_bytes() == P2.UNIT_BYTES and C.v2_ctrl_bytes() == P2.CTRL2_BYTES
@@ -261,7 +270,7 @@ class ShadowEngine:
         # eigenbasis of the previous step per coded unit (Jacobi warm start); identity to begin with
         self.max_sweeps = int(max_sweeps) if warm_start else 0
         self.vprev = None
-        if warm_start and not self.quant and not self.entry:
+        if warm_start and not self.quant and not self.entry and not self.sign:
             self.vprev = z(nc * P2.MAX_COLS * P2.MAX_COLS)
             for u in pl.units:
                 if u.coded:
@@ -395,7 +404,7 @@ class ShadowEngine:
         * ``mse``       the expected ``||g_hat - g||^2`` given that gradient, in closed form (exact, not sampled);
                         ``rel_var`` = ``mse / gsq``,
         * ``bias_sq``   TernGrad's clip bias ``||clip(g) - g||^2`` (0 for the other codes; not part of ``mse``),
-        * ``exp_atoms`` / ``atoms``  expected and realized atoms (QSGD / TernGrad: every element), exact tensors their
+        * ``exp_atoms`` / ``atoms``  expected and realized atoms (QSGD / TernGrad / sign: every element), exact tensors their
                         element count,
         * ``bytes``     realized push bytes: the spectral slot layout, ``entry_bytes()`` / ``qsgd_bytes()`` applied to
                         the realized counts, dense bytes for exact tensors.
@@ -413,7 +422,7 @@ class ShadowEngine:
             name = names.get(id(self.params[u.param]), str(u.param))
             t = per.setdefault(name, {"numel": q.numel, "gsq": None, "mse": 0.0, "bias_sq": 0.0, "exp_atoms": 0.0,
                                       "atoms": 0.0, "bytes": 0.0})
-            if u.kind in (P2.KIND_SLAB, P2.KIND_MAT, P2.KIND_ENTRY, P2.KIND_QSGD) and acc:
+            if u.kind in (P2.KIND_SLAB, P2.KIND_MAT, P2.KIND_ENTRY, P2.KIND_QSGD, P2.KIND_SIGN) and acc:
                 gsq, mse, ex, bias, real, real4, n = acc[u.ts_index]
                 n = max(n, 1.0)
                 t["gsq"] = (t["gsq"] or 0.0) + gsq / n
@@ -421,7 +430,7 @@ class ShadowEngine:
                 t["bias_sq"] += bias / n
                 t["exp_atoms"] += ex / n
                 t["atoms"] += real / n
-                if u.kind == P2.KIND_QSGD:
+                if u.kind in (P2.KIND_QSGD, P2.KIND_SIGN):
                     t["bytes"] += 8.0 * u.rows * u.cols + 4.0 * u.rows
                 elif u.kind == P2.KIND_ENTRY:
                     t["bytes"] += 4.0 * real / n + 16.0 * u.n_ps
@@ -459,6 +468,13 @@ class ShadowEngine:
         if self.stats_acc is None or nt == 0:
             return
         p = lambda t: t.data_ptr() if t is not None else 0
+        if self.sign:
+            self.C.v2_sign_code_stats(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt,
+                                      self.t_gptr.data_ptr(), self.t_arena_peer.data_ptr(), self.n_owners,
+                                      self.plan.arena_floats, self.worker_index, self.stats_partials.data_ptr(),
+                                      self.stats_counters.data_ptr(), self.stats_acc.data_ptr())
+            self._nlaunch += 1
+            return
         if self.topk:
             self.C.v2_topk_code_stats(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt,
                                       self.t_gptr.data_ptr(), self.topk_sel.data_ptr(), self.topk_tiles.data_ptr(),
@@ -513,6 +529,14 @@ class ShadowEngine:
                              self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g, 0, self.tstats.data_ptr(),
                              self._fired == self.G, self.clip is None, self.q_max_level, self.q_max_bucket,
                              self.code == "terngrad", res)
+            self._nlaunch += 1
+            return
+        if nt > 0 and self.sign:
+            # scales + sign bits pushed straight into the owners' arenas; the encode launch raises the push flag
+            C.v2_sign_encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
+                             self.t_arena_peer.data_ptr(), self.t_sig_owner.data_ptr(), self.n_owners, pl.arena_floats,
+                             self.worker_index, g, self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g,
+                             self.tstats.data_ptr(), self._fired == self.G, res)
             self._nlaunch += 1
             return
         if nt > 0 and self.topk:
@@ -575,6 +599,17 @@ class ShadowEngine:
                          self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
                          self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
                          max(1, min(self.ps_grid, max(nt, 1))), self.q_max_level, self.q_max_bucket)
+            self._nlaunch += 1
+            return
+        if self.sign:
+            C.v2_ps_sign(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g, final,
+                         self.owner_index, p(self.master), p(self.mom), p(self.sq), p(self.sqmax), p(self.vmom),
+                         p(self.vsq), p(self.vsqmax), self.wshadow_mc, self.t_wshadow_peer.data_ptr(),
+                         self.vparams.data_ptr(), self.vparams_mc, self.t_vparams_peer.data_ptr(), self.vgrads_mc,
+                         self.t_vgrads_peer.data_ptr(), self.heap.region_ptr("arena"), pl.arena_floats,
+                         self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
+                         self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
+                         max(1, min(self.ps_grid, max(nt, 1))))
             self._nlaunch += 1
             return
         if self.entry:
@@ -746,7 +781,7 @@ class ShadowEngine:
             u = pl.units[ui]
             if u.kind == P2.KIND_VEC:
                 mv[u.w_off + a:u.w_off + a + b] = 1
-            elif u.kind in (P2.KIND_DENSE16, P2.KIND_QSGD, P2.KIND_ENTRY):   # (first element, element count)
+            elif u.kind in (P2.KIND_DENSE16, P2.KIND_QSGD, P2.KIND_ENTRY, P2.KIND_SIGN):   # (first element, count)
                 mw[u.w_off + a:u.w_off + a + b] = 1
             elif u.kind == P2.KIND_SLAB:
                 half = u.I // 2
@@ -821,6 +856,8 @@ class ShadowEngine:
                 "svd_rank": self.svd_rank, "engine": "shadow"}
         if self.quant:
             side.update(quantization_level=self.quantization_level, bucket_size=self.bucket_size)
+        if self.sign:
+            side.update(bucket_size=self.bucket_size)
         if self.entry:
             side.update(entry_budget=self.entry_budget)
         side.update(adam_state)

@@ -32,7 +32,9 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                    help="sgd | svd | qsgd | terngrad | entrywise | qsvd | bsvd (block-spectral: the estimator the sm_90a "
                         "bf16 engine applies under --code svd, as a plain PyTorch coder) | topk (the --entry-budget "
                         "largest entries per tensor, sent exactly; --backend p2p --dtype bf16 only, meant for "
-                        "--error-feedback 1)")
+                        "--error-feedback 1) | sign (scaled sign: one bit per element and one fp32 scale "
+                        "||b||_1/|b| per --bucket-size bucket, a multiple of 64 in [64, 4096]; --backend p2p --dtype "
+                        "bf16 only, meant for --error-feedback 1)")
     p.add_argument("--bucket-size", type=int, default=512)
     p.add_argument("--dataset", type=str, default="MNIST", metavar="N")
     p.add_argument("--comm-type", type=str, default="Bcast", metavar="N")
@@ -73,7 +75,7 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "colocated = rank 0 hosts the whole PS and also trains; dedicated = rank 0 only serves")
     p.add_argument("--engine", type=str, default="auto", choices=["auto", "shadow", "fused"],
                    help="p2p backend: auto = the overlapped sharded bf16 engine for --dtype bf16 with --code "
-                        "svd|qsvd|sgd|topk, the fp32-flat engine otherwise; shadow = the bf16 engine (also --code "
+                        "svd|qsvd|sgd|topk|sign, the fp32-flat engine otherwise; shadow = the bf16 engine (also --code "
                         "qsgd|terngrad, needs --dtype bf16); fused = the fp32-flat engine")
     p.add_argument("--groups", type=int, default=5, help="p2p/bf16: backward groups pushed while backward runs")
     p.add_argument("--shrinkage-freq", type=int, default=50, help="steps between LR shrinkages (reference: 50)")
@@ -95,7 +97,7 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
     p.add_argument("--error-feedback", type=bool_flag, default=False,
                    help="p2p backend, bf16 engine: every worker keeps the part of its gradient the code did not send "
                         "(an fp32 residual per weight) and adds it to the next step's gradient before coding; --code "
-                        "svd | entrywise | topk | qsgd (it stays bounded with svd top-k and topk, the contractive "
-                        "codes), every push counted (no --num-aggregate below the worker count).  Residuals are "
+                        "svd | entrywise | topk | qsgd | sign (it stays bounded with svd top-k, topk and sign, the "
+                        "contractive codes), every push counted (no --num-aggregate below the worker count).  Residuals are "
                         "not checkpointed: --resume starts them from zero")
     return p.parse_args(argv)
