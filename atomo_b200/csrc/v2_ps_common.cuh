@@ -239,6 +239,37 @@ __device__ __forceinline__ void ps_vec_tile(const PsArgs2& a, const OptC& c, con
   }
 }
 
+// ---- bf16 weight tile that travels dense: the counted workers' staged copies summed in worker order, optimizer,
+// bf16 broadcast.  v2_ps_kernel keeps its own inline copy (calling this there changes its instruction schedule).
+__device__ __forceinline__ void ps_dense16_tile(const PsArgs2& a, const OptC& c, const Unit2& u, const Tile2& t,
+                                                unsigned int wmask, float inv_w) {
+  const int tid = threadIdx.x;
+  const long long e0 = u.w_off + t.a;
+  const long long s0 = (long long)u.rs + t.a;
+  const int nvec = (((e0 | s0) & 7) == 0) ? (t.b >> 3) : 0;
+  for (int v = tid; v < nvec; v += blockDim.x) {
+    float g[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) g[i] = 0.f;
+    for (int w = 0; w < a.W; ++w) {
+      if (!((wmask >> w) & 1u)) continue;
+      const uint4 y = ld_cg_u4(a.stage_peer[w] + s0 + 8LL * v);
+      const uint32_t ws[4] = {y.x, y.y, y.z, y.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i) { g[2 * i] += bf16_lo(ws[i]); g[2 * i + 1] += bf16_hi(ws[i]); }
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) g[i] *= inv_w;
+    update8(a, c, e0 + 8LL * v, g);
+  }
+  for (int i = (nvec << 3) + tid; i < t.b; i += blockDim.x) {
+    float g = 0.f;
+    for (int w = 0; w < a.W; ++w)
+      if ((wmask >> w) & 1u) g += ld_cg_bf16(a.stage_peer[w] + s0 + i);
+    update1(a, c, e0 + i, g * inv_w);
+  }
+}
+
 // ---- completion (thread 0 of every CTA): group counter; the last CTA of the final group publishes the
 // parameters of `step` (param_flag[owner] = step + 1 on every rank) ---------------------------------------------
 __device__ __forceinline__ void ps_complete(const PsArgs2& a, Ctrl2* ctrl, int step, bool bad, long long t_enter,

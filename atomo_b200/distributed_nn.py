@@ -67,6 +67,10 @@ def run_rank(args) -> None:
     if getattr(args, "error_feedback", False):
         raise SystemExit("--error-feedback keeps its residuals in the --backend p2p bf16 engine; the %s backend's "
                          "PyTorch coders do not (run without --error-feedback)" % backend)
+    if args.code.lower() == "powersgd":
+        raise SystemExit("--code powersgd runs on the --backend p2p bf16 engine (--dtype bf16), which keeps each "
+                         "worker's warm state and error-feedback residual; the %s backend's coders keep neither"
+                         % backend)
     if args.code.lower() == "sign":
         raise SystemExit("--code sign runs on the --backend p2p bf16 engine (--dtype bf16), which keeps the "
                          "error-feedback residual; scaled sign without it is biased, and the %s backend's coders keep "

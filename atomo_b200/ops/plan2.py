@@ -27,6 +27,9 @@ What changes against ``ops/plan.py`` (the fp32-flat plan of round 1):
   owners decode, sum and step the optimizer in one launch per group.
 * **Scaled sign** (``code="sign"``): every >= 2-D weight is one ``SIGN`` unit whose buckets are sent as one bit per
   element and one fp32 scale, in the slot and tile geometry of the quantizing codes.
+* **PowerSGD** (``code="powersgd"``): every >= 2-D weight with ``r (O + C) < O C`` is one ``POWER`` unit, the whole
+  ``[O][C]`` matrix of its physical layout, sent as a rank-``r`` pair ``P_hat`` / ``Q'`` from one warm-started power
+  step; the owners reconstruct ``P_hat Q'^T`` and step the optimizer.
 * **Entry-wise ATOMO** (``code="entrywise"``): every >= 2-D weight is one ``ENTRY`` unit whose sampled entries are
   compacted by the workers into 4-byte words in the owners' arenas; the owners scatter-add, average and step the
   optimizer in one launch per group.
@@ -40,7 +43,7 @@ import struct
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
-KIND_SLAB, KIND_MAT, KIND_DENSE16, KIND_VEC, KIND_QSGD, KIND_ENTRY, KIND_SIGN = 1, 2, 3, 4, 5, 6, 7
+KIND_SLAB, KIND_MAT, KIND_DENSE16, KIND_VEC, KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_POWER = 1, 2, 3, 4, 5, 6, 7, 8
 RCAP_MAX = 32
 MAX_COLS = 64
 BLOCK_COLS = 32               # column-block width of MAT units (Jacobi cost ~ cols^3 sits in the encode launch)
@@ -58,6 +61,11 @@ QSGD_MAX_LEVEL = 14           # (sign + 1) << q | level must fit 16 bits
 SIGN_MIN_BUCKET, SIGN_MAX_BUCKET = 64, 4096   # scaled sign: one warp per bucket, whole 64-bit words
 ENTRY_TILE_ELEMS = 4096       # entry-wise PS / encode tile: the element offset of an entry fits 12 bits
 TOPK_STATE_INTS, TOPK_HI_BINS, TOPK_LO_BINS = 8, 256, 128   # top-k selection state / histograms (csrc/v2_common.cuh)
+POWER_MAX_RANK = 4            # PowerSGD: rank r in [1, 4] (csrc/v2_powersgd.cu keeps r x 8 accumulators per thread)
+PW_ENC_ROWS = 8               # PowerSGD pass A (P = M Q_w, Gram partial) and the EF / stats passes: rows per tile
+PW_COL_BLOCK = 256            # PowerSGD pass B (Q' = M^T P_hat): columns per CTA, every row summed inside the CTA
+PW_PS_ROWS = 4                # PowerSGD PS tile: rows of the reconstructed matrix
+PW_GRAM = 16                  # fp64 Gram partial per pass-A tile (4 x 4)
 
 UNIT_FMT = "<4q20i"           # 112 bytes, mirrors struct Unit2
 TILE_FMT = "<4i"              # unit, a, b, owner
@@ -106,6 +114,27 @@ def qsgd_words_off(n_ps: int, buckets: int) -> int:
 
 def qsgd_slot_floats(n_ps: int, buckets: int, words_per_bucket: int) -> int:
     return _round_up(qsgd_words_off(n_ps, buckets) + 2 * buckets * words_per_bucket, 32)
+
+
+def pw_phat_off(n_ps: int) -> int:
+    """Float offset (inside a PowerSGD slot) of ``P_hat^T`` (``[r][round4(O)]``): after one int32 step stamp per PS
+    tile."""
+    return _round_up(n_ps, 4)
+
+
+def pw_q_off(n_ps: int, rows: int, rank: int) -> int:
+    """Float offset (inside a PowerSGD slot) of ``Q'^T`` (``[r][round4(C)]``)."""
+    return pw_phat_off(n_ps) + rank * _round_up(rows, 4)
+
+
+def pw_slot_floats(n_ps: int, rows: int, cols: int, rank: int) -> int:
+    return _round_up(pw_q_off(n_ps, rows, rank) + rank * _round_up(cols, 4), 32)
+
+
+def pw_scratch_floats(rows: int, cols: int, rank: int) -> int:
+    """Worker-local fp32 state of a PowerSGD unit (from ``gpart_off``): ``P^T``, ``P_hat^T`` (``[r][round4(O)]`` each),
+    ``Q'^T`` and the warm ``Q_w^T`` (``[r][round4(C)]`` each)."""
+    return 2 * rank * (_round_up(rows, 4) + _round_up(cols, 4))
 
 
 def entry_hdr_off(j: int) -> int:
@@ -231,6 +260,8 @@ class Plan2:
     n_coded: int            # units with per-unit device state (coded SLAB / MAT units, or the QSGD / ENTRY / SIGN units)
     rank: int
     code: str
+    pw_tiles: List[Tuple[int, int, int, int]] = field(default_factory=list)   # PowerSGD pass B: (unit, col0, ncols, j)
+    pw_range: List[Tuple[int, int]] = field(default_factory=list)             # per group: (first pw tile, count)
 
     def units_bytes(self) -> bytes:
         return b"".join(u.pack() for u in self.units)
@@ -249,6 +280,12 @@ class Plan2:
         ``scales``)."""
         return sum(8 * u.rows * u.cols + 4 * u.rows for u in self.units if u.kind in (KIND_QSGD, KIND_SIGN))
 
+    def powersgd_bytes(self) -> int:
+        """Bytes of PowerSGD factors a worker pushes per step: ``4 r (O + C)`` per coded tensor, ``P_hat`` and ``Q'``
+        sent once to the tensor's single owner, for any number of owners.  The 4-byte step stamps per PS tile are not
+        counted."""
+        return sum(4 * u.rcap * (u.rows + u.cols) for u in self.units if u.kind == KIND_POWER)
+
     def entry_bytes(self) -> float:
         """Bytes of entry-wise code a worker pushes per step: 4 per expected atom and a 16-byte header per PS tile.
         An upper bound on the expectation (``sum(p_i) <= s``), exact when no ``p_i`` is clamped to 1.  Top-k: an
@@ -259,7 +296,7 @@ class Plan2:
         """Bytes actually stored per worker and step for the expected number of atoms (U is written in groups
         of 4 atoms); for the quantizing codes the words and norms of the QSGD units; for entry-wise ATOMO the
         entries and tile headers."""
-        tot = float(self.qsgd_bytes()) + self.entry_bytes()
+        tot = float(self.qsgd_bytes()) + self.entry_bytes() + float(self.powersgd_bytes())
         for u in self.units:
             if u.coded:
                 atoms = min(u.budget if u.budget > 0 else u.cols, u.cols)
@@ -269,7 +306,7 @@ class Plan2:
 
     def dense_bytes(self) -> int:
         return sum((2 if u.kind == KIND_DENSE16 else 4) * u.numel for u in self.units
-                   if not u.coded and u.kind not in (KIND_QSGD, KIND_ENTRY, KIND_SIGN))
+                   if not u.coded and u.kind not in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_POWER))
 
 
 def default_groups(shapes: Sequence[Sequence[int]], n_groups: int) -> List[int]:
@@ -317,7 +354,8 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 n_owners: int = 1, n_groups: int = 4, groups: Optional[Sequence[int]] = None,
                 block_cols: int = BLOCK_COLS, min_coded_numel: int = 256, quantization_level: int = 4,
                 bucket_size: int = 512, entry_budget: float = 0.05) -> Plan2:
-    """Plan of the bf16 engine for ``code`` in ``svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign``.
+    """Plan of the bf16 engine for ``code`` in ``svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign |
+    powersgd``.
 
     ``qsgd`` / ``terngrad``: every >= 2-D weight (the 3-channel stem and the fc layers included) is exactly one
     ``KIND_QSGD`` unit; there are no ``DENSE16`` units.  1-D parameters stay ``KIND_VEC`` (fp32, summed by
@@ -358,6 +396,22 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
     in ``[64, 4096]``) and ``L = ceil(bucket / 64)`` words per bucket: one bit per element (``codings/sign.py``) in
     place of the quantized codes and one fp32 scale per bucket in place of the norm.  ``Unit2`` fields: ``K`` = bucket,
     ``rows`` = buckets, ``cols`` = L, ``cs`` = buckets per tile, ``ps_rows`` = elements per tile, ``I`` = ``rs`` = 0.
+
+    ``powersgd`` (``rank`` = r in ``[1, 4]``): every >= 2-D weight with ``r (O + C) < O C`` is exactly one ``KIND_POWER``
+    unit (``codings/powersgd.py``), the others travel ``DENSE16``; 1-D parameters stay ``KIND_VEC``.  Per unit:
+
+    * ``rows`` = O, ``cols`` = C = numel / O (row ``o`` is the contiguous physical slab of output channel ``o``),
+      ``rcap`` = ``budget`` = r, ``K`` = pass-B tiles;
+    * pass-A encode tiles (``enc_tiles``) of ``PW_ENC_ROWS`` rows: (unit, first row, rows, index in unit); each leaves a
+      16-double Gram partial (indexed by global encode tile) that the unit's last tile sums in tile order;
+    * pass-B tiles (``pw_tiles`` / ``pw_range``) of ``PW_COL_BLOCK`` columns: (unit, first column, columns, index in
+      unit); each sums ``Q' = M^T P_hat`` over all rows of its columns inside one CTA, so no ``Q'`` partials exist;
+    * PS tiles of ``PW_PS_ROWS`` rows: (unit, first row, rows, owner).  Every PS tile of a unit belongs to ONE owner,
+      ``own0`` (every tile needs all of ``Q'``, so spreading a unit over owners would send ``Q'`` to each of them); the
+      units of a group go to the owner with the fewest PowerSGD elements of that group so far (lowest index on ties);
+    * the slot holds one int32 step stamp per PS tile, ``P_hat^T`` and ``Q'^T`` (:func:`pw_phat_off` /
+      :func:`pw_q_off`), written into owner ``own0``'s arena only;
+    * ``gpart_off`` locates the worker-local scratch (:func:`pw_scratch_floats`) inside the ``gpart`` region.
     """
     shapes = [tuple(int(d) for d in s) for s in shapes]
     quant = code in ("qsgd", "terngrad")
@@ -375,6 +429,9 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
         sbsz = int(bucket_size)
         if not (SIGN_MIN_BUCKET <= sbsz <= SIGN_MAX_BUCKET and sbsz % 64 == 0):
             raise ValueError("sign: bucket_size must be a multiple of 64 in [%d, %d]" % (SIGN_MIN_BUCKET, SIGN_MAX_BUCKET))
+    power = code == "powersgd"
+    if power and not 1 <= int(rank) <= POWER_MAX_RANK:
+        raise ValueError("powersgd: svd_rank must be in [1, %d] (got %r)" % (POWER_MAX_RANK, rank))
     ubits = 0
     if code == "qsvd":          # QSVD: spectral atoms with quantized left factors (README.md:141-142 of the reference)
         code, ubits = "svd", 8
@@ -422,6 +479,13 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             add(Unit2(0, KIND_SIGN, p.index, p.widx, p.off, 0, rows=(p.numel + bucket - 1) // bucket,
                       cols=(bucket + 63) // 64, K=bucket, cs=bpt, numel=p.numel, group=p.group, ps_rows=bpt * bucket))
             continue
+        if power:
+            o = s[0]
+            c = p.numel // o
+            if rank * (o + c) < o * c:
+                add(Unit2(0, KIND_POWER, p.index, p.widx, p.off, 0, rows=o, cols=c, K=-(-c // PW_COL_BLOCK),
+                          rcap=int(rank), budget=float(rank), numel=p.numel, group=p.group, ps_rows=PW_PS_ROWS))
+                continue
         if entry:
             s_atoms = entry_atoms(float(entry_budget), p.numel)
             if code == "topk":
@@ -468,10 +532,13 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
     enc_tiles: List[Tuple[int, int, int, int]] = []
     ps_by_group: List[List[Tuple[int, int, int]]] = [[] for _ in range(n_groups)]
     enc_range, group_units = [], [[] for _ in range(n_groups)]
+    pw_tiles: List[Tuple[int, int, int, int]] = []
+    pw_range: List[Tuple[int, int]] = []
     slot_off = gpart_off = 0
     n_coded = 0
     for g in range(n_groups):
-        first = len(enc_tiles)
+        first, pw_first = len(enc_tiles), len(pw_tiles)
+        pw_load = [0] * n_owners            # PowerSGD elements of this group per owner
         for u in units:
             if u.group != g:
                 continue
@@ -498,6 +565,11 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             elif u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN):   # encode tiles = PS tiles (one destination owner per CTA)
                 for j, e0 in enumerate(range(0, u.numel, u.ps_rows)):
                     enc_tiles.append((u.index, e0, min(u.ps_rows, u.numel - e0), j))
+            elif u.kind == KIND_POWER:
+                for j, r0 in enumerate(range(0, u.rows, PW_ENC_ROWS)):
+                    enc_tiles.append((u.index, r0, min(PW_ENC_ROWS, u.rows - r0), j))
+                for j, c0 in enumerate(range(0, u.cols, PW_COL_BLOCK)):
+                    pw_tiles.append((u.index, c0, min(PW_COL_BLOCK, u.cols - c0), j))
             u.n_enc = len(enc_tiles) - u.enc_tile0
             if u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN):
                 u.ts_index = n_coded
@@ -512,6 +584,19 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                     slot_off += qsgd_slot_floats(u.n_ps, u.rows, u.cols)
                 else:
                     slot_off += entry_slot_floats(u.numel, u.n_ps, u.ps_rows)
+            elif u.kind == KIND_POWER:
+                u.ts_index = n_coded
+                n_coded += 1
+                u.ps_tile0 = len(ps_by_group[g])
+                for r0 in range(0, u.rows, u.ps_rows):
+                    ps_by_group[g].append((u.index, r0, min(u.ps_rows, u.rows - r0)))
+                u.n_ps = len(ps_by_group[g]) - u.ps_tile0
+                u.own0 = min(range(n_owners), key=lambda o: (pw_load[o], o))
+                pw_load[u.own0] += u.numel
+                u.slot_off = slot_off
+                slot_off += pw_slot_floats(u.n_ps, u.rows, u.cols, u.rcap)
+                u.gpart_off = gpart_off
+                gpart_off += pw_scratch_floats(u.rows, u.cols, u.rcap)
             elif u.coded:
                 u.ts_index = n_coded
                 n_coded += 1
@@ -532,6 +617,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 u.n_ps = len(ps_by_group[g]) - u.ps_tile0
                 u.own0 = u.ps_tile0 % n_owners
         enc_range.append((first, len(enc_tiles) - first))
+        pw_range.append((pw_first, len(pw_tiles) - pw_first))
 
     ps_tiles: List[Tuple[int, int, int, int]] = []
     ps_range: List[List[Tuple[int, int]]] = []
@@ -540,13 +626,14 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
         for o in range(n_owners):
             first = len(ps_tiles)
             for j, (ui, a, b) in enumerate(ps_by_group[g]):
-                if j % n_owners == o:
+                own = units[ui].own0 if units[ui].kind == KIND_POWER else j % n_owners
+                if own == o:
                     ps_tiles.append((ui, a, b, o))
             row.append((first, len(ps_tiles) - first))
         ps_range.append(row)
     return Plan2(params, units, enc_tiles, ps_tiles, enc_range, ps_range, group_units, n_groups, n_owners,
                  max(w_off, W_ALIGN), max(v_off, V_ALIGN), max(stage_off, W_ALIGN), max(slot_off, 32),
-                 max(gpart_off, 1), n_coded, rank, code)
+                 max(gpart_off, 1), n_coded, rank, code, pw_tiles, pw_range)
 
 
 def owner_of_row(u: Unit2, row: int, n_owners: int) -> int:

@@ -45,6 +45,9 @@ def build_coder(kwargs: dict, worker_side: bool):
     if code == "entrywise":
         return codings.build("entrywise", budget=kwargs.get("entry_budget", 0.05),
                              prob_rule=kwargs.get("prob_rule", "reference"))
+    if code == "powersgd":
+        raise ValueError("--code powersgd runs on the --backend p2p bf16 engine (--dtype bf16), which keeps each "
+                         "worker's warm state and error-feedback residual; the gloo / nccl coders keep neither")
     if code == "sign":
         raise ValueError("--code sign runs on the --backend p2p bf16 engine (--dtype bf16), which keeps the "
                          "error-feedback residual; scaled sign without it is biased, and the gloo / nccl coders keep "

@@ -6,11 +6,12 @@ Counterpart of the role dispatch in ``/root/reference/src/distributed_nn.py:243-
 checkpoints in the ``model_step_<N>`` layout, and the reference's log lines with REAL per-phase numbers taken from
 device-side timers (``Comp`` / ``Encode`` / ``Comm`` on the worker line, ``Decode Cost`` / ``Gather`` on the PS line).
 
-Engine choice (``--engine auto``): ``--dtype bf16`` with ``--code svd|qsvd|sgd|topk|sign`` runs the overlapped, sharded
+Engine choice (``--engine auto``): ``--dtype bf16`` with ``--code svd|qsvd|sgd|topk|sign|powersgd`` runs the overlapped,
+sharded
 ``ShadowEngine``; everything else (fp32, qsgd / terngrad / entrywise) runs the fp32-flat ``FusedEngine``.
 ``--engine shadow`` also runs ``--code qsgd|terngrad`` on ``ShadowEngine`` (bf16 only) and refuses ``--code
 entrywise``, which the launcher keeps on ``FusedEngine``; ``--engine fused`` always picks ``FusedEngine``.  ``--code
-topk`` and ``--code sign`` exist only on ``ShadowEngine``.
+topk``, ``--code sign`` and ``--code powersgd`` exist only on ``ShadowEngine``.
 """
 from __future__ import annotations
 
@@ -41,14 +42,21 @@ def _build_engine(args, model, rank, world):
     if code == "sign" and (engine == "fused" or args.dtype != "bf16"):
         raise SystemExit("--code sign runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the fp32-flat "
                          "engine has no scaled-sign code")
+    if code == "powersgd" and (engine == "fused" or args.dtype != "bf16"):
+        raise SystemExit("--code powersgd runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the "
+                         "fp32-flat engine has no PowerSGD code")
+    if code == "powersgd" and not 1 <= args.svd_rank <= 4:
+        raise SystemExit("--code powersgd needs --svd-rank in [1, 4] (the rank of the pushed factors; got %d)"
+                         % args.svd_rank)
     if engine == "auto":
-        shadow = args.dtype == "bf16" and code in ("svd", "qsvd", "sgd", "dense", "lossless", "topk", "sign")
+        shadow = args.dtype == "bf16" and code in ("svd", "qsvd", "sgd", "dense", "lossless", "topk", "sign",
+                                                   "powersgd")
     elif engine == "shadow":
         if args.dtype != "bf16":
             raise SystemExit("--engine shadow trains bf16 weights: it needs --dtype bf16 (fp32 runs on --engine fused)")
-        if code not in ("svd", "qsvd", "sgd", "dense", "lossless", "qsgd", "terngrad", "topk", "sign"):
-            raise SystemExit("--engine shadow runs --code svd|qsvd|sgd|qsgd|terngrad|topk|sign; --code %s runs on "
-                             "--engine fused" % args.code)
+        if code not in ("svd", "qsvd", "sgd", "dense", "lossless", "qsgd", "terngrad", "topk", "sign", "powersgd"):
+            raise SystemExit("--engine shadow runs --code svd|qsvd|sgd|qsgd|terngrad|topk|sign|powersgd; --code %s "
+                             "runs on --engine fused" % args.code)
         shadow = True
     else:
         shadow = False

@@ -34,7 +34,12 @@ one central PS kernel at the end of the step):
   fp32 scale ``||b||_1 / |b|`` in the slots and tiles of QSGD (``csrc/v2_sign.cu``, one encode launch per group); the
   owners decode ``+-scale``, sum in worker order and step the optimizer.  Deterministic, dense and biased on its own:
   the contractive code of EF-SignSGD for ``error_feedback=True``.
-* **Error feedback** (``error_feedback=True``; svd, entrywise, topk, qsgd, sign): each worker keeps an fp32 residual ``e`` per
+* **PowerSGD** (``code="powersgd"``, ``svd_rank`` = r in ``[1, 4]``): every weight matrix (``[O][C]`` in its physical
+  layout) is pushed as a rank-``r`` pair from one power step warm-started by the previous step's right factor
+  (``csrc/v2_powersgd.cu``, two encode launches per group); the owners reconstruct ``P_hat Q'^T`` in worker order and
+  step the optimizer.  Deterministic, low-rank and biased on its own: a contractive code for ``error_feedback=True``.
+  The warm state is per worker and, like the residuals, not checkpointed: a resumed run draws it afresh.
+* **Error feedback** (``error_feedback=True``; svd, entrywise, topk, qsgd, sign, powersgd): each worker keeps an fp32 residual ``e`` per
   weight element and codes ``A = g + e``.  An apply launch per group (``csrc/v2_feedback.cu``) writes ``bf16(A)`` into
   autograd's gradient buffer in place and keeps ``A - bf16(A)``; the encoders' epilogues add ``bf16(A) - g_hat``, the
   part of ``A`` this push did not carry.  Nothing is discarded, only delayed.
@@ -81,8 +86,11 @@ class ShadowEngine:
                  bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False,
                  error_feedback: bool = False):
         self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
-        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign"):
-            raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign")
+        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign", "powersgd"):
+            raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign | powersgd")
+        self.power = self.code == "powersgd"
+        if self.power and not 1 <= int(svd_rank) <= P2.POWER_MAX_RANK:      # checked before any CUDA work
+            raise ValueError("powersgd: svd_rank must be in [1, %d] (got %r)" % (P2.POWER_MAX_RANK, svd_rank))
         self.error_feedback = bool(error_feedback)
         if self.error_feedback:     # checked before any CUDA work
             if self.code == "qsvd":
@@ -270,7 +278,7 @@ class ShadowEngine:
         # eigenbasis of the previous step per coded unit (Jacobi warm start); identity to begin with
         self.max_sweeps = int(max_sweeps) if warm_start else 0
         self.vprev = None
-        if warm_start and not self.quant and not self.entry and not self.sign:
+        if warm_start and not self.quant and not self.entry and not self.sign and not self.power:
             self.vprev = z(nc * P2.MAX_COLS * P2.MAX_COLS)
             for u in pl.units:
                 if u.coded:
@@ -297,6 +305,13 @@ class ShadowEngine:
         elif self.entry:
             self.l1 = torch.zeros(nc, dtype=torch.float64, device=dev)
             self.l1_partials = torch.zeros(max(len(pl.enc_tiles), 1), dtype=torch.float64, device=dev)
+        # PowerSGD: pass-B tiles, fp64 Gram partials per pass-A tile, per-unit state (R^{-1}, mask, draw counter, unit
+        # counters); the factors and the warm Q_w live in ``gpart`` (ops/plan2.py pw_scratch_floats)
+        self.pw_state = self.pw_gram = self.t_pw_tiles = None
+        if self.power:
+            self.t_pw_tiles = _dev_bytes(P2.Plan2.tiles_bytes(pl.pw_tiles), dev)
+            self.pw_gram = torch.zeros(P2.PW_GRAM * max(len(pl.enc_tiles), 1), dtype=torch.float64, device=dev)
+            self.pw_state = torch.zeros(nc * C.v2_powersgd_state_bytes(), dtype=torch.uint8, device=dev)
         self.counters = torch.zeros(nc + 2 * P2.MAX_GROUPS + 8, dtype=torch.int32, device=dev)
         self.cnt_enc_group = self.counters.data_ptr() + 4 * nc
         self.cnt_ps_group = self.cnt_enc_group + 4 * P2.MAX_GROUPS
@@ -305,6 +320,8 @@ class ShadowEngine:
                                              beta1=betas[0], beta2=betas[1], eps=eps, opt=self.opt,
                                              num_aggregate=num_aggregate), dev)
         self.ctrl_i32, self.ctrl_f32 = self.ctrl.view(torch.int32), self.ctrl.view(torch.float32)
+        if self.power and self.is_worker:       # the warm state's first draw (Philox keyed by seed, unit, column)
+            C.v2_powersgd_init(self.t_units.data_ptr(), len(pl.units), self.gpart.data_ptr(), self.ctrl.data_ptr())
         n_w = max(len(self.w_params), 1)
         self.t_gptr = torch.zeros(n_w, dtype=torch.int64, device=dev)
         self.host_gptr = np.zeros(n_w, dtype=np.int64)
@@ -404,8 +421,8 @@ class ShadowEngine:
         * ``mse``       the expected ``||g_hat - g||^2`` given that gradient, in closed form (exact, not sampled);
                         ``rel_var`` = ``mse / gsq``,
         * ``bias_sq``   TernGrad's clip bias ``||clip(g) - g||^2`` (0 for the other codes; not part of ``mse``),
-        * ``exp_atoms`` / ``atoms``  expected and realized atoms (QSGD / TernGrad / sign: every element), exact tensors their
-                        element count,
+        * ``exp_atoms`` / ``atoms``  expected and realized atoms (QSGD / TernGrad / sign: every element; PowerSGD: the
+                        non-degenerate columns of ``P_hat``), exact tensors their element count,
         * ``bytes``     realized push bytes: the spectral slot layout, ``entry_bytes()`` / ``qsgd_bytes()`` applied to
                         the realized counts, dense bytes for exact tensors.
 
@@ -422,7 +439,7 @@ class ShadowEngine:
             name = names.get(id(self.params[u.param]), str(u.param))
             t = per.setdefault(name, {"numel": q.numel, "gsq": None, "mse": 0.0, "bias_sq": 0.0, "exp_atoms": 0.0,
                                       "atoms": 0.0, "bytes": 0.0})
-            if u.kind in (P2.KIND_SLAB, P2.KIND_MAT, P2.KIND_ENTRY, P2.KIND_QSGD, P2.KIND_SIGN) and acc:
+            if u.kind in (P2.KIND_SLAB, P2.KIND_MAT, P2.KIND_ENTRY, P2.KIND_QSGD, P2.KIND_SIGN, P2.KIND_POWER) and acc:
                 gsq, mse, ex, bias, real, real4, n = acc[u.ts_index]
                 n = max(n, 1.0)
                 t["gsq"] = (t["gsq"] or 0.0) + gsq / n
@@ -432,6 +449,8 @@ class ShadowEngine:
                 t["atoms"] += real / n
                 if u.kind in (P2.KIND_QSGD, P2.KIND_SIGN):
                     t["bytes"] += 8.0 * u.rows * u.cols + 4.0 * u.rows
+                elif u.kind == P2.KIND_POWER:
+                    t["bytes"] += 4.0 * u.rcap * (u.rows + u.cols)
                 elif u.kind == P2.KIND_ENTRY:
                     t["bytes"] += 4.0 * real / n + 16.0 * u.n_ps
                 else:
@@ -468,6 +487,13 @@ class ShadowEngine:
         if self.stats_acc is None or nt == 0:
             return
         p = lambda t: t.data_ptr() if t is not None else 0
+        if self.power:
+            self.C.v2_powersgd_code_stats(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt,
+                                          self.t_gptr.data_ptr(), self.gpart.data_ptr(), self.pw_state.data_ptr(),
+                                          self.stats_partials.data_ptr(), self.stats_counters.data_ptr(),
+                                          self.stats_acc.data_ptr())
+            self._nlaunch += 1
+            return
         if self.sign:
             self.C.v2_sign_code_stats(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt,
                                       self.t_gptr.data_ptr(), self.t_arena_peer.data_ptr(), self.n_owners,
@@ -530,6 +556,17 @@ class ShadowEngine:
                              self._fired == self.G, self.clip is None, self.q_max_level, self.q_max_bucket,
                              self.code == "terngrad", res)
             self._nlaunch += 1
+            return
+        if self.power:
+            # pass A (P = M Q_w, Gram, R^{-1}), pass B (Q' = M^T P_hat, pushes, warm state, push flag), EF pass
+            p0, npw = pl.pw_range[g]
+            C.v2_powersgd_encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt,
+                                 self.t_pw_tiles.data_ptr(), p0, npw, self.t_gptr.data_ptr(), self.gpart.data_ptr(),
+                                 self.pw_gram.data_ptr(), self.pw_state.data_ptr(), self.wstage.data_ptr(),
+                                 self.t_arena_peer.data_ptr(), self.t_sig_owner.data_ptr(), self.n_owners,
+                                 pl.arena_floats, self.worker_index, g, self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g,
+                                 self.tstats.data_ptr(), self._fired == self.G, res)
+            self._nlaunch += (1 if nt > 0 else 0) + 1 + (1 if res and nt > 0 else 0)
             return
         if nt > 0 and self.sign:
             # scales + sign bits pushed straight into the owners' arenas; the encode launch raises the push flag
@@ -599,6 +636,17 @@ class ShadowEngine:
                          self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
                          self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
                          max(1, min(self.ps_grid, max(nt, 1))), self.q_max_level, self.q_max_bucket)
+            self._nlaunch += 1
+            return
+        if self.power:
+            C.v2_ps_powersgd(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g, final,
+                             self.owner_index, p(self.master), p(self.mom), p(self.sq), p(self.sqmax), p(self.vmom),
+                             p(self.vsq), p(self.vsqmax), self.wshadow_mc, self.t_wshadow_peer.data_ptr(),
+                             self.vparams.data_ptr(), self.vparams_mc, self.t_vparams_peer.data_ptr(), self.vgrads_mc,
+                             self.t_vgrads_peer.data_ptr(), self.t_stage_peer.data_ptr(), self.heap.region_ptr("arena"),
+                             pl.arena_floats, self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
+                             self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
+                             max(1, min(self.ps_grid, max(nt, 1))))
             self._nlaunch += 1
             return
         if self.sign:
@@ -783,6 +831,8 @@ class ShadowEngine:
                 mv[u.w_off + a:u.w_off + a + b] = 1
             elif u.kind in (P2.KIND_DENSE16, P2.KIND_QSGD, P2.KIND_ENTRY, P2.KIND_SIGN):   # (first element, count)
                 mw[u.w_off + a:u.w_off + a + b] = 1
+            elif u.kind == P2.KIND_POWER:                                                # (first row, rows)
+                mw[u.w_off + a * u.cols:u.w_off + (a + b) * u.cols] = 1
             elif u.kind == P2.KIND_SLAB:
                 half = u.I // 2
                 e0 = u.w_off + (a // half) * u.K * u.I
@@ -826,7 +876,7 @@ class ShadowEngine:
         """Collective.  The first training rank writes ``model_step_<N>`` (fp32, trained BN statistics) and the
         ``_optim`` sidecar (momentum — for Adam / AMSGrad also the second moments —, step, LR) so a later run can
         resume.  Error-feedback residuals are per-worker state and are not written: a resumed run starts from
-        ``e = 0``."""
+        ``e = 0``.  Nor is PowerSGD's warm ``Q_w``: a resumed run draws it afresh."""
         from ..utils import checkpoint as ckpt
         step = (self.step - 1) if step is None else step
         sd = self.fp32_state_dict()
