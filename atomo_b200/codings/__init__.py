@@ -2,7 +2,7 @@
 
 ``codings.build(name, **kw)`` resolves the launcher's ``--code`` flag:
 ``sgd``/``dense``/``lossless`` (dense pass-through), ``svd`` (spectral ATOMO),
-``entrywise`` (entry-wise ATOMO), ``topk`` (top-k sparsification, the oracle of the bf16 engine's top-k units), ``sign`` (scaled sign, the oracle of the bf16 engine's sign units), ``powersgd`` (warm-started rank-r power iteration, the oracle of the bf16 engine's PowerSGD units), ``qsgd``, ``terngrad``, ``qsvd``, ``bsvd`` (block-spectral: the estimator of the sm_90a bf16 engine).
+``entrywise`` (entry-wise ATOMO), ``topk`` (top-k sparsification, the oracle of the bf16 engine's top-k units), ``sign`` (scaled sign, the oracle of the bf16 engine's sign units), ``powersgd`` (warm-started rank-r power iteration, the oracle of the bf16 engine's PowerSGD units), ``fp8`` (e4m3 bytes with stochastic rounding, the oracle of the bf16 engine's fp8 units), ``qsgd``, ``terngrad``, ``qsvd``, ``bsvd`` (block-spectral: the estimator of the sm_90a bf16 engine).
 """
 from .coding import Coding, available, build, register
 from . import utils, sampling
@@ -12,11 +12,12 @@ from .entrywise import EntryWise
 from .topk import TopK
 from .sign import ScaledSign
 from .powersgd import PowerSGD
+from .fp8 import FP8
 from .qsvd import QSVD
 from .block_svd import BlockSVD
 from . import lossless_compress
 from .lossless_compress import LosslessCompress
 from . import svd, qsgd, entrywise, qsvd  # noqa: F401  (module-style access like the reference)
 
-__all__ = ["Coding", "SVD", "QSGD", "TernGrad", "EntryWise", "TopK", "ScaledSign", "PowerSGD", "QSVD", "BlockSVD", "LosslessCompress",
+__all__ = ["Coding", "SVD", "QSGD", "TernGrad", "EntryWise", "TopK", "ScaledSign", "PowerSGD", "FP8", "QSVD", "BlockSVD", "LosslessCompress",
            "utils", "sampling", "build", "register", "available"]

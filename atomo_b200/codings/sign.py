@@ -29,11 +29,12 @@ from .coding import Coding, register
 SIGN_MIN_BUCKET, SIGN_MAX_BUCKET = 64, 4096
 
 
-def check_bucket_size(bucket_size: int) -> int:
+def check_bucket_size(bucket_size: int, code: str = "sign") -> int:
+    """The bucket rule of the sign and fp8 codes: a multiple of 64 in ``[64, 4096]``."""
     b = int(bucket_size)
     if not (SIGN_MIN_BUCKET <= b <= SIGN_MAX_BUCKET and b % 64 == 0):
-        raise ValueError("sign: bucket_size must be a multiple of 64 in [%d, %d] (got %r)"
-                         % (SIGN_MIN_BUCKET, SIGN_MAX_BUCKET, bucket_size))
+        raise ValueError("%s: bucket_size must be a multiple of 64 in [%d, %d] (got %r)"
+                         % (code, SIGN_MIN_BUCKET, SIGN_MAX_BUCKET, bucket_size))
     return b
 
 

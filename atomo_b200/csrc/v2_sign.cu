@@ -16,6 +16,7 @@
 //   v2_sign_code_stats_kernel  --code-stats: per tile gsq = sum x^2 and mse = sum (x - decode)^2 in fp64 with the scale
 //                              read back from this worker's slot (the error of the code is exact, not an expectation);
 //                              atoms = numel.  The unit's last tile adds the partials in tile order.
+#include "v2_bf16_load.cuh"
 #include "v2_ps_common.cuh"
 
 namespace atomo {
@@ -44,30 +45,6 @@ struct SEncArgs {
   int final_group;
   float* residual;             // error feedback: fp32 residual like wshadow, or nullptr
 };
-
-// bf16 subnormals read as signed zero, by bit operations: the code (and codings/sign.py) does not depend on how the
-// compiler's flush-to-zero treats them in the comparisons and the fp64 conversions below
-__device__ __forceinline__ float sign_ftz(float x) {
-  const uint32_t u = __float_as_uint(x);
-  return __uint_as_float((u & 0x7f800000u) ? u : (u & 0x80000000u));
-}
-
-// elements 8c .. 8c+7 of a bucket, 0 past blen: one 16-byte load for the first nch (aligned, whole) chunks, else
-// element loads
-__device__ __forceinline__ void sign_load8(const __nv_bfloat16* src, int c, int nch, int blen, float (&x)[8]) {
-  if (c < nch) {
-    const uint4 v = __ldg(reinterpret_cast<const uint4*>(src) + c);
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { x[2 * i] = sign_ftz(bf16_lo(w[i])); x[2 * i + 1] = sign_ftz(bf16_hi(w[i])); }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int e = 8 * c + i;
-      x[i] = e < blen ? sign_ftz(__bfloat162float(src[e])) : 0.f;
-    }
-  }
-}
 
 __device__ __forceinline__ float sign_decode(float x, float scale) { return x < 0.f ? -scale : scale; }
 

@@ -67,6 +67,9 @@ def run_rank(args) -> None:
     if getattr(args, "error_feedback", False):
         raise SystemExit("--error-feedback keeps its residuals in the --backend p2p bf16 engine; the %s backend's "
                          "PyTorch coders do not (run without --error-feedback)" % backend)
+    if args.code.lower() == "fp8":
+        raise SystemExit("--code fp8 runs on the --backend p2p bf16 engine (--dtype bf16) only; the %s backend has no "
+                         "fp8 coder" % backend)
     if args.code.lower() == "powersgd":
         raise SystemExit("--code powersgd runs on the --backend p2p bf16 engine (--dtype bf16), which keeps each "
                          "worker's warm state and error-feedback residual; the %s backend's coders keep neither"

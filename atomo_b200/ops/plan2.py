@@ -27,6 +27,8 @@ What changes against ``ops/plan.py`` (the fp32-flat plan of round 1):
   owners decode, sum and step the optimizer in one launch per group.
 * **Scaled sign** (``code="sign"``): every >= 2-D weight is one ``SIGN`` unit whose buckets are sent as one bit per
   element and one fp32 scale, in the slot and tile geometry of the quantizing codes.
+* **FP8** (``code="fp8"``): every >= 2-D weight is one ``FP8`` unit whose buckets are sent as one e4m3 byte per
+  element (stochastically rounded) and one power-of-two fp32 scale, in the geometry of the sign units.
 * **PowerSGD** (``code="powersgd"``): every >= 2-D weight with ``r (O + C) < O C`` is one ``POWER`` unit, the whole
   ``[O][C]`` matrix of its physical layout, sent as a rank-``r`` pair ``P_hat`` / ``Q'`` from one warm-started power
   step; the owners reconstruct ``P_hat Q'^T`` and step the optimizer.
@@ -43,7 +45,8 @@ import struct
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
-KIND_SLAB, KIND_MAT, KIND_DENSE16, KIND_VEC, KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_POWER = 1, 2, 3, 4, 5, 6, 7, 8
+KIND_SLAB, KIND_MAT, KIND_DENSE16, KIND_VEC, KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_POWER, KIND_FP8 = \
+    1, 2, 3, 4, 5, 6, 7, 8, 9
 RCAP_MAX = 32
 MAX_COLS = 64
 BLOCK_COLS = 32               # column-block width of MAT units (Jacobi cost ~ cols^3 sits in the encode launch)
@@ -58,7 +61,7 @@ V_ALIGN = 32                  # fp32 elements (128 B)
 QSGD_TILE_ELEMS = 4096        # a QSGD PS / encode tile holds max(1, 4096 // bucket) whole buckets
 QSGD_MAX_BUCKET = 1024        # one warp quantizes one bucket, staged in shared memory
 QSGD_MAX_LEVEL = 14           # (sign + 1) << q | level must fit 16 bits
-SIGN_MIN_BUCKET, SIGN_MAX_BUCKET = 64, 4096   # scaled sign: one warp per bucket, whole 64-bit words
+SIGN_MIN_BUCKET, SIGN_MAX_BUCKET = 64, 4096   # scaled sign and fp8: whole 64-bit words, at most one tile
 ENTRY_TILE_ELEMS = 4096       # entry-wise PS / encode tile: the element offset of an entry fits 12 bits
 TOPK_STATE_INTS, TOPK_HI_BINS, TOPK_LO_BINS = 8, 256, 128   # top-k selection state / histograms (csrc/v2_common.cuh)
 POWER_MAX_RANK = 4            # PowerSGD: rank r in [1, 4] (csrc/v2_powersgd.cu keeps r x 8 accumulators per thread)
@@ -257,7 +260,7 @@ class Plan2:
     stage_total: int        # bf16 elements of the dense-16 staging region
     arena_floats: int
     gpart_floats: int
-    n_coded: int            # units with per-unit device state (coded SLAB / MAT units, or the QSGD / ENTRY / SIGN units)
+    n_coded: int            # units with per-unit device state (coded SLAB / MAT units, or the QSGD / ENTRY / SIGN / FP8 units)
     rank: int
     code: str
     pw_tiles: List[Tuple[int, int, int, int]] = field(default_factory=list)   # PowerSGD pass B: (unit, col0, ncols, j)
@@ -277,8 +280,8 @@ class Plan2:
     def qsgd_bytes(self) -> int:
         """Bytes of quantized gradient a worker pushes per step: the uint64 words and fp32 norms of every bucket
         (the same sizes as ``codings.qsgd``'s ``words`` and ``norms``; for sign units ``codings.sign``'s ``words`` and
-        ``scales``)."""
-        return sum(8 * u.rows * u.cols + 4 * u.rows for u in self.units if u.kind in (KIND_QSGD, KIND_SIGN))
+        ``scales``; for fp8 units ``codings.fp8``'s ``bytes`` and ``scales``)."""
+        return sum(8 * u.rows * u.cols + 4 * u.rows for u in self.units if u.kind in (KIND_QSGD, KIND_SIGN, KIND_FP8))
 
     def powersgd_bytes(self) -> int:
         """Bytes of PowerSGD factors a worker pushes per step: ``4 r (O + C)`` per coded tensor, ``P_hat`` and ``Q'``
@@ -306,7 +309,7 @@ class Plan2:
 
     def dense_bytes(self) -> int:
         return sum((2 if u.kind == KIND_DENSE16 else 4) * u.numel for u in self.units
-                   if not u.coded and u.kind not in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_POWER))
+                   if not u.coded and u.kind not in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_POWER, KIND_FP8))
 
 
 def default_groups(shapes: Sequence[Sequence[int]], n_groups: int) -> List[int]:
@@ -355,7 +358,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 block_cols: int = BLOCK_COLS, min_coded_numel: int = 256, quantization_level: int = 4,
                 bucket_size: int = 512, entry_budget: float = 0.05) -> Plan2:
     """Plan of the bf16 engine for ``code`` in ``svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign |
-    powersgd``.
+    powersgd | fp8``.
 
     ``qsgd`` / ``terngrad``: every >= 2-D weight (the 3-channel stem and the fc layers included) is exactly one
     ``KIND_QSGD`` unit; there are no ``DENSE16`` units.  1-D parameters stay ``KIND_VEC`` (fp32, summed by
@@ -397,6 +400,10 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
     place of the quantized codes and one fp32 scale per bucket in place of the norm.  ``Unit2`` fields: ``K`` = bucket,
     ``rows`` = buckets, ``cols`` = L, ``cs`` = buckets per tile, ``ps_rows`` = elements per tile, ``I`` = ``rs`` = 0.
 
+    ``fp8``: the units, buckets, tiles, owners and slots of ``sign`` (kind ``KIND_FP8``) with ``cols`` =
+    ``ceil(bucket / 8)`` uint64 words per bucket: one e4m3 byte per element in element order, bucket ``j`` starting at
+    byte ``8 j cols``, and one power-of-two fp32 scale per bucket in place of the norm (``codings/fp8.py``).
+
     ``powersgd`` (``rank`` = r in ``[1, 4]``): every >= 2-D weight with ``r (O + C) < O C`` is exactly one ``KIND_POWER``
     unit (``codings/powersgd.py``), the others travel ``DENSE16``; 1-D parameters stay ``KIND_VEC``.  Per unit:
 
@@ -417,6 +424,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
     quant = code in ("qsgd", "terngrad")
     entry = code in ("entrywise", "topk")
     sign = code == "sign"
+    fp8 = code == "fp8"
     if entry and not entry_budget > 0:
         raise ValueError("entry_budget must be positive (a fraction of numel below 1, else an atom count)")
     if quant:
@@ -425,10 +433,11 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             raise ValueError("quantization_level must be in [1, %d]" % QSGD_MAX_LEVEL)
         if not (32 <= bsz <= QSGD_MAX_BUCKET and bsz % 8 == 0):
             raise ValueError("bucket_size must be a multiple of 8 in [32, %d]" % QSGD_MAX_BUCKET)
-    if sign:
+    if sign or fp8:
         sbsz = int(bucket_size)
         if not (SIGN_MIN_BUCKET <= sbsz <= SIGN_MAX_BUCKET and sbsz % 64 == 0):
-            raise ValueError("sign: bucket_size must be a multiple of 64 in [%d, %d]" % (SIGN_MIN_BUCKET, SIGN_MAX_BUCKET))
+            raise ValueError("%s: bucket_size must be a multiple of 64 in [%d, %d]"
+                             % (code, SIGN_MIN_BUCKET, SIGN_MAX_BUCKET))
     power = code == "powersgd"
     if power and not 1 <= int(rank) <= POWER_MAX_RANK:
         raise ValueError("powersgd: svd_rank must be in [1, %d] (got %r)" % (POWER_MAX_RANK, rank))
@@ -478,6 +487,12 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             bpt = max(1, QSGD_TILE_ELEMS // bucket)
             add(Unit2(0, KIND_SIGN, p.index, p.widx, p.off, 0, rows=(p.numel + bucket - 1) // bucket,
                       cols=(bucket + 63) // 64, K=bucket, cs=bpt, numel=p.numel, group=p.group, ps_rows=bpt * bucket))
+            continue
+        if fp8:
+            bucket = min(sbsz, p.numel)
+            bpt = max(1, QSGD_TILE_ELEMS // bucket)
+            add(Unit2(0, KIND_FP8, p.index, p.widx, p.off, 0, rows=(p.numel + bucket - 1) // bucket,
+                      cols=(bucket + 7) // 8, K=bucket, cs=bpt, numel=p.numel, group=p.group, ps_rows=bpt * bucket))
             continue
         if power:
             o = s[0]
@@ -562,7 +577,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             elif u.kind == KIND_DENSE16:
                 for e0 in range(0, u.numel, 8192):     # staging copy tiles
                     enc_tiles.append((u.index, e0, min(8192, u.numel - e0), 0))
-            elif u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN):   # encode tiles = PS tiles (one destination owner per CTA)
+            elif u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_FP8):   # encode tiles = PS tiles (one owner per CTA)
                 for j, e0 in enumerate(range(0, u.numel, u.ps_rows)):
                     enc_tiles.append((u.index, e0, min(u.ps_rows, u.numel - e0), j))
             elif u.kind == KIND_POWER:
@@ -571,7 +586,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 for j, c0 in enumerate(range(0, u.cols, PW_COL_BLOCK)):
                     pw_tiles.append((u.index, c0, min(PW_COL_BLOCK, u.cols - c0), j))
             u.n_enc = len(enc_tiles) - u.enc_tile0
-            if u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN):
+            if u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_FP8):
                 u.ts_index = n_coded
                 n_coded += 1
                 u.ps_tile0 = len(ps_by_group[g])
@@ -580,7 +595,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 u.n_ps = len(ps_by_group[g]) - u.ps_tile0
                 u.own0 = u.ps_tile0 % n_owners
                 u.slot_off = slot_off
-                if u.kind in (KIND_QSGD, KIND_SIGN):
+                if u.kind in (KIND_QSGD, KIND_SIGN, KIND_FP8):
                     slot_off += qsgd_slot_floats(u.n_ps, u.rows, u.cols)
                 else:
                     slot_off += entry_slot_floats(u.numel, u.n_ps, u.ps_rows)

@@ -6,12 +6,12 @@ Counterpart of the role dispatch in ``/root/reference/src/distributed_nn.py:243-
 checkpoints in the ``model_step_<N>`` layout, and the reference's log lines with REAL per-phase numbers taken from
 device-side timers (``Comp`` / ``Encode`` / ``Comm`` on the worker line, ``Decode Cost`` / ``Gather`` on the PS line).
 
-Engine choice (``--engine auto``): ``--dtype bf16`` with ``--code svd|qsvd|sgd|topk|sign|powersgd`` runs the overlapped,
-sharded
+Engine choice (``--engine auto``): ``--dtype bf16`` with ``--code svd|qsvd|sgd|topk|sign|powersgd|fp8`` runs the
+overlapped, sharded
 ``ShadowEngine``; everything else (fp32, qsgd / terngrad / entrywise) runs the fp32-flat ``FusedEngine``.
 ``--engine shadow`` also runs ``--code qsgd|terngrad`` on ``ShadowEngine`` (bf16 only) and refuses ``--code
 entrywise``, which the launcher keeps on ``FusedEngine``; ``--engine fused`` always picks ``FusedEngine``.  ``--code
-topk``, ``--code sign`` and ``--code powersgd`` exist only on ``ShadowEngine``.
+topk``, ``--code sign``, ``--code powersgd`` and ``--code fp8`` exist only on ``ShadowEngine``.
 """
 from __future__ import annotations
 
@@ -42,6 +42,9 @@ def _build_engine(args, model, rank, world):
     if code == "sign" and (engine == "fused" or args.dtype != "bf16"):
         raise SystemExit("--code sign runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the fp32-flat "
                          "engine has no scaled-sign code")
+    if code == "fp8" and (engine == "fused" or args.dtype != "bf16"):
+        raise SystemExit("--code fp8 runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the fp32-flat "
+                         "engine has no fp8 code")
     if code == "powersgd" and (engine == "fused" or args.dtype != "bf16"):
         raise SystemExit("--code powersgd runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the "
                          "fp32-flat engine has no PowerSGD code")
@@ -50,12 +53,13 @@ def _build_engine(args, model, rank, world):
                          % args.svd_rank)
     if engine == "auto":
         shadow = args.dtype == "bf16" and code in ("svd", "qsvd", "sgd", "dense", "lossless", "topk", "sign",
-                                                   "powersgd")
+                                                   "powersgd", "fp8")
     elif engine == "shadow":
         if args.dtype != "bf16":
             raise SystemExit("--engine shadow trains bf16 weights: it needs --dtype bf16 (fp32 runs on --engine fused)")
-        if code not in ("svd", "qsvd", "sgd", "dense", "lossless", "qsgd", "terngrad", "topk", "sign", "powersgd"):
-            raise SystemExit("--engine shadow runs --code svd|qsvd|sgd|qsgd|terngrad|topk|sign|powersgd; --code %s "
+        if code not in ("svd", "qsvd", "sgd", "dense", "lossless", "qsgd", "terngrad", "topk", "sign", "powersgd",
+                        "fp8"):
+            raise SystemExit("--engine shadow runs --code svd|qsvd|sgd|qsgd|terngrad|topk|sign|powersgd|fp8; --code %s "
                              "runs on --engine fused" % args.code)
         shadow = True
     else:
@@ -67,7 +71,7 @@ def _build_engine(args, model, rank, world):
             kw = dict(quantization_level=args.quantization_level, bucket_size=args.bucket_size)
         elif code == "topk":
             kw = dict(entry_budget=args.entry_budget)
-        elif code == "sign":
+        elif code in ("sign", "fp8"):
             kw = dict(bucket_size=args.bucket_size)
         if getattr(args, "code_stats", False):
             if code == "qsvd":

@@ -39,7 +39,11 @@ one central PS kernel at the end of the step):
   (``csrc/v2_powersgd.cu``, two encode launches per group); the owners reconstruct ``P_hat Q'^T`` in worker order and
   step the optimizer.  Deterministic, low-rank and biased on its own: a contractive code for ``error_feedback=True``.
   The warm state is per worker and, like the residuals, not checkpointed: a resumed run draws it afresh.
-* **Error feedback** (``error_feedback=True``; svd, entrywise, topk, qsgd, sign, powersgd): each worker keeps an fp32 residual ``e`` per
+* **FP8** (``code="fp8"``, ``bucket_size``): every weight's buckets are pushed as one e4m3 byte per element and one
+  power-of-two fp32 scale in the slots and tiles of sign (``csrc/v2_fp8.cu``, one encode launch per group); each
+  scaled magnitude is rounded to one of its two e4m3 neighbours with Philox draws, so the code is unbiased.  The
+  owners decode with the hardware conversion, sum in worker order and step the optimizer.
+* **Error feedback** (``error_feedback=True``; svd, entrywise, topk, qsgd, sign, powersgd, fp8): each worker keeps an fp32 residual ``e`` per
   weight element and codes ``A = g + e``.  An apply launch per group (``csrc/v2_feedback.cu``) writes ``bf16(A)`` into
   autograd's gradient buffer in place and keeps ``A - bf16(A)``; the encoders' epilogues add ``bf16(A) - g_hat``, the
   part of ``A`` this push did not carry.  Nothing is discarded, only delayed.
@@ -86,8 +90,9 @@ class ShadowEngine:
                  bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False,
                  error_feedback: bool = False):
         self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
-        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign", "powersgd"):
-            raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign | powersgd")
+        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign", "powersgd", "fp8"):
+            raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign | powersgd "
+                             "| fp8")
         self.power = self.code == "powersgd"
         if self.power and not 1 <= int(svd_rank) <= P2.POWER_MAX_RANK:      # checked before any CUDA work
             raise ValueError("powersgd: svd_rank must be in [1, %d] (got %r)" % (P2.POWER_MAX_RANK, svd_rank))
@@ -122,10 +127,11 @@ class ShadowEngine:
             if not self.entry_budget > 0:
                 raise ValueError("entry_budget must be positive (a fraction of numel below 1, else an atom count)")
         self.sign = self.code == "sign"
-        if self.sign:       # checked before any CUDA work
+        self.fp8 = self.code == "fp8"
+        if self.sign or self.fp8:       # checked before any CUDA work
             if not (P2.SIGN_MIN_BUCKET <= int(bucket_size) <= P2.SIGN_MAX_BUCKET and int(bucket_size) % 64 == 0):
-                raise ValueError("sign: bucket_size must be a multiple of 64 in [%d, %d] (got %r)"
-                                 % (P2.SIGN_MIN_BUCKET, P2.SIGN_MAX_BUCKET, bucket_size))
+                raise ValueError("%s: bucket_size must be a multiple of 64 in [%d, %d] (got %r)"
+                                 % (self.code, P2.SIGN_MIN_BUCKET, P2.SIGN_MAX_BUCKET, bucket_size))
         self.C = load_ext()
         C = self.C
         assert C.v2_unit_bytes() == P2.UNIT_BYTES and C.v2_ctrl_bytes() == P2.CTRL2_BYTES
@@ -278,7 +284,7 @@ class ShadowEngine:
         # eigenbasis of the previous step per coded unit (Jacobi warm start); identity to begin with
         self.max_sweeps = int(max_sweeps) if warm_start else 0
         self.vprev = None
-        if warm_start and not self.quant and not self.entry and not self.sign and not self.power:
+        if warm_start and not self.quant and not self.entry and not self.sign and not self.power and not self.fp8:
             self.vprev = z(nc * P2.MAX_COLS * P2.MAX_COLS)
             for u in pl.units:
                 if u.coded:
@@ -421,7 +427,7 @@ class ShadowEngine:
         * ``mse``       the expected ``||g_hat - g||^2`` given that gradient, in closed form (exact, not sampled);
                         ``rel_var`` = ``mse / gsq``,
         * ``bias_sq``   TernGrad's clip bias ``||clip(g) - g||^2`` (0 for the other codes; not part of ``mse``),
-        * ``exp_atoms`` / ``atoms``  expected and realized atoms (QSGD / TernGrad / sign: every element; PowerSGD: the
+        * ``exp_atoms`` / ``atoms``  expected and realized atoms (QSGD / TernGrad / sign / fp8: every element; PowerSGD: the
                         non-degenerate columns of ``P_hat``), exact tensors their element count,
         * ``bytes``     realized push bytes: the spectral slot layout, ``entry_bytes()`` / ``qsgd_bytes()`` applied to
                         the realized counts, dense bytes for exact tensors.
@@ -439,7 +445,8 @@ class ShadowEngine:
             name = names.get(id(self.params[u.param]), str(u.param))
             t = per.setdefault(name, {"numel": q.numel, "gsq": None, "mse": 0.0, "bias_sq": 0.0, "exp_atoms": 0.0,
                                       "atoms": 0.0, "bytes": 0.0})
-            if u.kind in (P2.KIND_SLAB, P2.KIND_MAT, P2.KIND_ENTRY, P2.KIND_QSGD, P2.KIND_SIGN, P2.KIND_POWER) and acc:
+            if u.kind in (P2.KIND_SLAB, P2.KIND_MAT, P2.KIND_ENTRY, P2.KIND_QSGD, P2.KIND_SIGN, P2.KIND_POWER,
+                          P2.KIND_FP8) and acc:
                 gsq, mse, ex, bias, real, real4, n = acc[u.ts_index]
                 n = max(n, 1.0)
                 t["gsq"] = (t["gsq"] or 0.0) + gsq / n
@@ -447,7 +454,7 @@ class ShadowEngine:
                 t["bias_sq"] += bias / n
                 t["exp_atoms"] += ex / n
                 t["atoms"] += real / n
-                if u.kind in (P2.KIND_QSGD, P2.KIND_SIGN):
+                if u.kind in (P2.KIND_QSGD, P2.KIND_SIGN, P2.KIND_FP8):
                     t["bytes"] += 8.0 * u.rows * u.cols + 4.0 * u.rows
                 elif u.kind == P2.KIND_POWER:
                     t["bytes"] += 4.0 * u.rcap * (u.rows + u.cols)
@@ -494,11 +501,11 @@ class ShadowEngine:
                                           self.stats_acc.data_ptr())
             self._nlaunch += 1
             return
-        if self.sign:
-            self.C.v2_sign_code_stats(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt,
-                                      self.t_gptr.data_ptr(), self.t_arena_peer.data_ptr(), self.n_owners,
-                                      self.plan.arena_floats, self.worker_index, self.stats_partials.data_ptr(),
-                                      self.stats_counters.data_ptr(), self.stats_acc.data_ptr())
+        if self.sign or self.fp8:
+            stats = self.C.v2_sign_code_stats if self.sign else self.C.v2_fp8_code_stats
+            stats(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
+                  self.t_arena_peer.data_ptr(), self.n_owners, self.plan.arena_floats, self.worker_index,
+                  self.stats_partials.data_ptr(), self.stats_counters.data_ptr(), self.stats_acc.data_ptr())
             self._nlaunch += 1
             return
         if self.topk:
@@ -568,12 +575,13 @@ class ShadowEngine:
                                  self.tstats.data_ptr(), self._fired == self.G, res)
             self._nlaunch += (1 if nt > 0 else 0) + 1 + (1 if res and nt > 0 else 0)
             return
-        if nt > 0 and self.sign:
-            # scales + sign bits pushed straight into the owners' arenas; the encode launch raises the push flag
-            C.v2_sign_encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
-                             self.t_arena_peer.data_ptr(), self.t_sig_owner.data_ptr(), self.n_owners, pl.arena_floats,
-                             self.worker_index, g, self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g,
-                             self.tstats.data_ptr(), self._fired == self.G, res)
+        if nt > 0 and (self.sign or self.fp8):
+            # scales + sign bits / e4m3 bytes pushed straight into the owners' arenas; the encode raises the push flag
+            encode = C.v2_sign_encode if self.sign else C.v2_fp8_encode
+            encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
+                   self.t_arena_peer.data_ptr(), self.t_sig_owner.data_ptr(), self.n_owners, pl.arena_floats,
+                   self.worker_index, g, self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g, self.tstats.data_ptr(),
+                   self._fired == self.G, res)
             self._nlaunch += 1
             return
         if nt > 0 and self.topk:
@@ -649,15 +657,15 @@ class ShadowEngine:
                              max(1, min(self.ps_grid, max(nt, 1))))
             self._nlaunch += 1
             return
-        if self.sign:
-            C.v2_ps_sign(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g, final,
-                         self.owner_index, p(self.master), p(self.mom), p(self.sq), p(self.sqmax), p(self.vmom),
-                         p(self.vsq), p(self.vsqmax), self.wshadow_mc, self.t_wshadow_peer.data_ptr(),
-                         self.vparams.data_ptr(), self.vparams_mc, self.t_vparams_peer.data_ptr(), self.vgrads_mc,
-                         self.t_vgrads_peer.data_ptr(), self.heap.region_ptr("arena"), pl.arena_floats,
-                         self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
-                         self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
-                         max(1, min(self.ps_grid, max(nt, 1))))
+        if self.sign or self.fp8:
+            ps = C.v2_ps_sign if self.sign else C.v2_ps_fp8
+            ps(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g, final,
+               self.owner_index, p(self.master), p(self.mom), p(self.sq), p(self.sqmax), p(self.vmom), p(self.vsq),
+               p(self.vsqmax), self.wshadow_mc, self.t_wshadow_peer.data_ptr(), self.vparams.data_ptr(),
+               self.vparams_mc, self.t_vparams_peer.data_ptr(), self.vgrads_mc, self.t_vgrads_peer.data_ptr(),
+               self.heap.region_ptr("arena"), pl.arena_floats, self.signals.data_ptr(), self.t_sig_all.data_ptr(),
+               self.ctrl.data_ptr(), self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(),
+               1.0 / self.W, max(1, min(self.ps_grid, max(nt, 1))))
             self._nlaunch += 1
             return
         if self.entry:
@@ -829,7 +837,7 @@ class ShadowEngine:
             u = pl.units[ui]
             if u.kind == P2.KIND_VEC:
                 mv[u.w_off + a:u.w_off + a + b] = 1
-            elif u.kind in (P2.KIND_DENSE16, P2.KIND_QSGD, P2.KIND_ENTRY, P2.KIND_SIGN):   # (first element, count)
+            elif u.kind in (P2.KIND_DENSE16, P2.KIND_QSGD, P2.KIND_ENTRY, P2.KIND_SIGN, P2.KIND_FP8):   # (first, count)
                 mw[u.w_off + a:u.w_off + a + b] = 1
             elif u.kind == P2.KIND_POWER:                                                # (first row, rows)
                 mw[u.w_off + a * u.cols:u.w_off + (a + b) * u.cols] = 1
@@ -906,7 +914,7 @@ class ShadowEngine:
                 "svd_rank": self.svd_rank, "engine": "shadow"}
         if self.quant:
             side.update(quantization_level=self.quantization_level, bucket_size=self.bucket_size)
-        if self.sign:
+        if self.sign or self.fp8:
             side.update(bucket_size=self.bucket_size)
         if self.entry:
             side.update(entry_budget=self.entry_budget)

@@ -36,7 +36,9 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "||b||_1/|b| per --bucket-size bucket, a multiple of 64 in [64, 4096]; --backend p2p --dtype "
                         "bf16 only, meant for --error-feedback 1) | powersgd (rank --svd-rank in [1, 4] factors of every "
                         "weight matrix from one warm-started power step; --backend p2p --dtype bf16 only, meant for "
-                        "--error-feedback 1)")
+                        "--error-feedback 1) | fp8 (one e4m3 byte per element, stochastically rounded and so "
+                        "unbiased, and one power-of-two fp32 scale per --bucket-size bucket, a multiple of 64 in "
+                        "[64, 4096]; --backend p2p --dtype bf16 only)")
     p.add_argument("--bucket-size", type=int, default=512)
     p.add_argument("--dataset", type=str, default="MNIST", metavar="N")
     p.add_argument("--comm-type", type=str, default="Bcast", metavar="N")
@@ -77,7 +79,7 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "colocated = rank 0 hosts the whole PS and also trains; dedicated = rank 0 only serves")
     p.add_argument("--engine", type=str, default="auto", choices=["auto", "shadow", "fused"],
                    help="p2p backend: auto = the overlapped sharded bf16 engine for --dtype bf16 with --code "
-                        "svd|qsvd|sgd|topk|sign|powersgd, the fp32-flat engine otherwise; shadow = the bf16 engine (also --code "
+                        "svd|qsvd|sgd|topk|sign|powersgd|fp8, the fp32-flat engine otherwise; shadow = the bf16 engine (also --code "
                         "qsgd|terngrad, needs --dtype bf16); fused = the fp32-flat engine")
     p.add_argument("--groups", type=int, default=5, help="p2p/bf16: backward groups pushed while backward runs")
     p.add_argument("--shrinkage-freq", type=int, default=50, help="steps between LR shrinkages (reference: 50)")
@@ -99,7 +101,7 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
     p.add_argument("--error-feedback", type=bool_flag, default=False,
                    help="p2p backend, bf16 engine: every worker keeps the part of its gradient the code did not send "
                         "(an fp32 residual per weight) and adds it to the next step's gradient before coding; --code "
-                        "svd | entrywise | topk | qsgd | sign | powersgd (it stays bounded with svd top-k, topk, sign "
-                        "and powersgd, the contractive codes), every push counted (no --num-aggregate below the worker "
+                        "svd | entrywise | topk | qsgd | sign | powersgd | fp8 (it stays bounded with svd top-k, topk, "
+                        "sign and powersgd, the contractive codes, and with fp8, whose variance is small), every push counted (no --num-aggregate below the worker "
                         "count).  Residuals (and PowerSGD's warm state) are not checkpointed: --resume starts them afresh")
     return p.parse_args(argv)

@@ -16,7 +16,7 @@ src = os.path.join("atomo_b200", "csrc")
 sources = [os.path.join(src, f) for f in (
     "bindings.cpp", "symm_heap.cpp", "svd_kernels.cu", "ps_kernels.cu", "qsgd_kernels.cu",
     "entrywise_kernels.cu", "ext_kernels.cu", "gemm_kernels.cu", "bn_kernels.cu", "v2_encode.cu", "v2_ps.cu",
-    "v2_qsgd.cu", "v2_entrywise.cu", "v2_topk.cu", "v2_sign.cu", "v2_powersgd.cu", "v2_stats.cu", "v2_feedback.cu", "data_kernels.cu")]
+    "v2_qsgd.cu", "v2_entrywise.cu", "v2_topk.cu", "v2_sign.cu", "v2_fp8.cu", "v2_powersgd.cu", "v2_stats.cu", "v2_feedback.cu", "data_kernels.cu")]
 
 nvcc_flags = ["-O3", "-lineinfo", "-std=c++17", "--use_fast_math",
               "-gencode", "arch=compute_90a,code=sm_90a"]
