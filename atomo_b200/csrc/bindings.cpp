@@ -2,6 +2,8 @@
 // Kernels live in the .cu files behind a plain C ABI; this file only adapts
 // torch tensors / raw peer pointers to those launchers on the current stream.
 #include <ATen/cuda/CUDAContext.h>
+#include <ATen/cuda/CUDAEvent.h>
+#include <c10/cuda/CUDACachingAllocator.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
 
@@ -368,6 +370,46 @@ void bn_backward(const torch::Tensor& dy, const torch::Tensor& x, c10::optional<
                            invstd.data_ptr<float>(), gamma.data_ptr<float>(), acc.data_ptr<float>(),
                            part.data_ptr<float>(), dgamma.data_ptr<float>(), dbeta.data_ptr<float>(), cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+
+// Backward of a convolution without bias whose weight gradient nobody on the current stream waits for: the input
+// gradient (if input_grad) on the current stream, then the weight gradient (if weight_grad) on `wgrad_stream`, forked
+// from the current stream after the input gradient was enqueued, so the backward chain's own GEMM is issued first.
+// Both are the at::convolution_backward calls the stock autograd node makes as one, with the same algorithm choice,
+// so the values are the same.  dy and x are marked as used on the wgrad stream: the caller frees them when this
+// returns, and the caching allocator then keeps their blocks until the weight gradient has read them.  Whoever reads
+// the weight gradient on another stream waits for the wgrad stream first.  Returns [dx, dw] (None where not asked).
+std::vector<c10::optional<torch::Tensor>> conv_backward_split(const torch::Tensor& dy, const torch::Tensor& x,
+                                                              const torch::Tensor& weight, std::vector<int64_t> stride,
+                                                              std::vector<int64_t> padding,
+                                                              std::vector<int64_t> dilation, int64_t groups,
+                                                              bool input_grad, bool weight_grad,
+                                                              uint64_t wgrad_stream) {
+  TORCH_CHECK(dy.is_cuda() && x.is_cuda() && weight.is_cuda(), "conv_backward_split: CUDA tensors expected");
+  TORCH_CHECK(wgrad_stream != 0 || !weight_grad, "conv_backward_split: a wgrad stream is required");
+  c10::cuda::CUDAGuard guard(dy.device());
+  const std::vector<int64_t> out_pad(stride.size(), 0);
+  c10::optional<torch::Tensor> dx, dw;
+  if (input_grad) {
+    dx = std::get<0>(at::convolution_backward(dy, x, weight, c10::nullopt, stride, padding, dilation, false, out_pad,
+                                              groups, {true, false, false}));
+  }
+  if (weight_grad) {
+    const c10::cuda::CUDAStream cur = c10::cuda::getCurrentCUDAStream();
+    const c10::cuda::CUDAStream side =
+        c10::cuda::getStreamFromExternal(reinterpret_cast<cudaStream_t>(wgrad_stream), dy.device().index());
+    at::cuda::CUDAEvent fork;
+    fork.record(cur);
+    fork.block(side);
+    {
+      c10::cuda::CUDAStreamGuard on_side(side);
+      dw = std::get<1>(at::convolution_backward(dy, x, weight, c10::nullopt, stride, padding, dilation, false,
+                                                out_pad, groups, {false, true, false}));
+    }
+    c10::cuda::CUDACachingAllocator::recordStream(dy.storage().data_ptr(), side);
+    c10::cuda::CUDACachingAllocator::recordStream(x.storage().data_ptr(), side);
+  }
+  return {dx, dw};
 }
 
 void skinny_gemm(const torch::Tensor& tiles, int ntiles, torch::Tensor ctrl, int grid) {
@@ -861,6 +903,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("skinny_gemm", &skinny_gemm);
   m.def("bn_forward", &bn_forward);
   m.def("bn_backward", &bn_backward);
+  m.def("conv_backward_split", &conv_backward_split);
   m.def("gemm_tile_bytes", &atomo_gemm_tile_bytes);
   m.def("gemm_smem_bytes", &atomo_gemm_smem_bytes);
   m.def("ext_desc_bytes", &atomo_ext_desc_bytes);

@@ -17,6 +17,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ..ops.fused_bn import BNAct
+from ..ops.split_conv import Conv2d
 
 Stage = Tuple[int, int, int]  # (kernel size, output channels, stride)
 
@@ -29,12 +30,12 @@ class _ResidualBlock(nn.Module):
         self.depth = len(stages)
         width = in_planes
         for i, (k, ch, s) in enumerate(stages, start=1):
-            setattr(self, "conv%d" % i, nn.Conv2d(width, ch, k, s, k // 2, bias=False))
+            setattr(self, "conv%d" % i, Conv2d(width, ch, k, s, k // 2, bias=False))
             setattr(self, "bn%d" % i, BNAct(ch))
             width = ch
         self.shortcut = nn.Sequential()  # identity unless the shape changes
         if stride != 1 or in_planes != width:
-            self.shortcut = nn.Sequential(nn.Conv2d(in_planes, width, 1, stride, bias=False), BNAct(width))
+            self.shortcut = nn.Sequential(Conv2d(in_planes, width, 1, stride, bias=False), BNAct(width))
 
     def forward(self, x):
         out = x
@@ -64,7 +65,7 @@ class ResNet(nn.Module):
     def __init__(self, block, num_blocks, num_classes=10, imagenet_stem=False):
         super().__init__()
         self.imagenet_stem = imagenet_stem
-        self.conv1 = nn.Conv2d(3, 64, 7, 2, 3, bias=False) if imagenet_stem else nn.Conv2d(3, 64, 3, 1, 1, bias=False)
+        self.conv1 = Conv2d(3, 64, 7, 2, 3, bias=False) if imagenet_stem else Conv2d(3, 64, 3, 1, 1, bias=False)
         self.bn1 = BNAct(64)
         self.in_planes = 64
         for idx, (planes, n) in enumerate(zip(self.widths, num_blocks), start=1):

@@ -367,6 +367,20 @@ class ShadowEngine:
         self.s_enc = torch.cuda.Stream(device=dev, priority=side_priority)
         self.s_ps = torch.cuda.Stream(device=dev, priority=side_priority)
         self.s_main = torch.cuda.Stream(device=dev, priority=main_priority)   # warm-up + capture stream
+        # with the fused BN, the convolutions' weight gradients run on a stream of their own, beside the backward
+        # chain (ops/split_conv.py); the encode of a group waits for it.  Same priority as the backward: the main
+        # stream is at the lowest priority by default, and the wgrad is as urgent as the rest of the backward.
+        self.s_wgrad, self.ev_wgrad, self.group_w_params, self.split_wgrad_layers = None, [], [], 0
+        if self.fused_bn_layers and self.is_worker:
+            from ..ops.split_conv import enable_split_wgrad
+            self.s_wgrad = torch.cuda.Stream(device=dev, priority=main_priority)
+            self.split_wgrad_layers = enable_split_wgrad(self.model, self.s_wgrad)
+            if self.split_wgrad_layers:
+                self.ev_wgrad = [torch.cuda.Event() for _ in range(self.G)]
+                self.group_w_params = [[p for p, q in zip(self.params, pl.params) if q.is_w and q.group == g]
+                                       for g in range(self.G)]
+            else:
+                self.s_wgrad = None
         self.ev_ready = [torch.cuda.Event() for _ in range(self.G)]
         self.ev_push = [torch.cuda.Event() for _ in range(self.G)]
         self.ev_enc_done, self.ev_ps_done = torch.cuda.Event(), torch.cuda.Event()
@@ -693,13 +707,20 @@ class ShadowEngine:
         (and, on an owner, the PS stream) off the stream backward is running on."""
         final = self._fired == self.G - 1
         self._fired += 1
+        cur = torch.cuda.current_stream(self.device)
+        if self.s_wgrad is not None:
+            # the wgrad stream runs in launch order: this event covers the weight gradients of the group
+            self.ev_wgrad[g].record(self.s_wgrad)
+            reader = cur if not self.overlap else self.s_enc
+            reader.wait_event(self.ev_wgrad[g])
+            for p in self.group_w_params[g]:
+                p.grad.record_stream(reader)
         if not self.overlap:
             self._launch_encode(g)
             self._launch_code_stats(g)
             if self.is_owner:
                 self._launch_ps(g, final)
             return
-        cur = torch.cuda.current_stream(self.device)
         self.ev_ready[g].record(cur)
         self.s_enc.wait_event(self.ev_ready[g])
         with torch.cuda.stream(self.s_enc):
@@ -744,6 +765,10 @@ class ShadowEngine:
             for p in self.w_params:
                 p.grad = None
             self._pending, self._fired = list(self.group_size), 0
+            if self.s_wgrad is not None:
+                # fork the wgrad stream here, so that it is part of a graph capture before any group records on it;
+                # the encode's waits on the last group's event join it again
+                self.s_wgrad.wait_stream(torch.cuda.current_stream(self.device))
             self._forward_backward()
             self._nlaunch += 4 * self.fused_bn_layers
             assert self._fired == self.G, "a backward group never fired (%d of %d)" % (self._fired, self.G)
