@@ -78,28 +78,42 @@ class BlockSVD(Coding):
         self.generator = generator
 
     # ------------------------------------------------------------------
-    def _code_unit(self, a: torch.Tensor, budget: float, total_sigma: Optional[float] = None):
+    def _code_unit(self, a: torch.Tensor, budget: float, total_sigma: Optional[float] = None,
+                   max_atoms: Optional[int] = None):
         """One unit ``a`` (rows x cols, fp32): Gram -> eigenvectors -> sampled atoms ``(U, s/p, V^T)``.
-        ``total_sigma`` (global allocation): nuclear-norm normaliser shared by all blocks of the tensor."""
+        ``total_sigma`` (global allocation): nuclear-norm normaliser shared by all blocks of the tensor.
+        ``max_atoms`` (the engine's slot capacity): a draw with more atoms is redrawn, as the kernel does.
+
+        The rules of the kernel (``csrc/spectral_sample.cuh``):
+
+        * ``sigma_max < 1e-6``: the top atom is sent with ``p = 1`` (the reference's rule, ``svd.py:50-51``).  This
+          estimate ``A v_0 v_0^T`` is biased by at most ``||A||_F <= sqrt(cols) sigma_max < sqrt(cols) * 1e-6``.
+        * An atom with ``sigma_i <= 1e-7 sigma_max`` (a null direction) is counted and sent, with a zero column of
+          ``U`` instead of ``A v_i / 0``.
+        """
         lam, v = torch.linalg.eigh(a.t() @ a)
         lam, v = lam.flip(0).clamp_min(0), v.flip(1)
         sigma = lam.sqrt()
-        if float(sigma[0]) < 1e-12:
-            return a.new_zeros(a.shape[0], 0), a.new_zeros(0), a.new_zeros(0, a.shape[1])
-        if self.random_sample:
+        smax = float(sigma[0])
+        cols = a.shape[1]
+        if not smax >= 1e-6:
+            idx = torch.zeros(1, dtype=torch.long)
+            scale = torch.ones(1, dtype=sigma.dtype)
+        elif self.random_sample:
             if total_sigma is not None:
                 p = (budget * sigma / total_sigma).clamp(max=1.0)
             else:
                 p = atom_probabilities(sigma, budget, self.prob_rule)
-            idx = sample_atoms(p, scheme=self.scheme, generator=self.generator, allow_empty=True)
-            idx = idx[sigma[idx] > 1e-12 * sigma[0]]
+            idx = sample_atoms(p, scheme=self.scheme, generator=self.generator, allow_empty=True,
+                               max_atoms=max_atoms)
             scale = 1.0 / p[idx].to(sigma.dtype)
         else:
-            idx = torch.arange(min(int(budget), a.shape[1]))
-            idx = idx[sigma[idx] > 1e-12 * sigma[0]]
+            k = min(int(budget) if budget > 0 else cols, cols)
+            idx = torch.arange(k if max_atoms is None else min(k, max_atoms))
             scale = torch.ones(len(idx), dtype=sigma.dtype)
         vs = v[:, idx]
-        u = (a @ vs) / sigma[idx]
+        live = sigma[idx] > 1e-7 * smax
+        u = torch.where(live, a @ vs, 0.0) / torch.where(live, sigma[idx], 1.0)
         return u.contiguous(), (sigma[idx] * scale).contiguous(), vs.t().contiguous()
 
     def encode(self, grad: torch.Tensor, **kwargs) -> dict:

@@ -75,3 +75,56 @@ def test_code_is_smaller_than_the_tensor_and_survives_the_wire():
     assert 4 * 3 * (16384 + 19) < 0.2 * g.numel() * 4                           # ~6x fewer bytes than the tensor
     back = wire.unpack(wire.pack({"codes": [code]}))["codes"][0]
     assert torch.equal(c.decode(back), c.decode(code))
+
+
+def _unit(shape_cols, sigmas, seed=4):
+    """rows x cols matrix with the given singular values (random orthonormal factors)."""
+    gen = torch.Generator().manual_seed(seed)
+    rows, cols = shape_cols
+    u = torch.linalg.qr(torch.randn(rows, cols, generator=gen, dtype=torch.float64)).Q
+    v = torch.linalg.qr(torch.randn(cols, cols, generator=gen, dtype=torch.float64)).Q
+    return ((u * torch.tensor(sigmas, dtype=torch.float64)) @ v.t()).float()
+
+
+@pytest.mark.parametrize("smax", [0.0, 1e-8, 5e-7])
+def test_degenerate_unit_sends_its_top_atom_with_probability_one(smax):
+    """sigma_max < 1e-6 (the kernel's rule, svd.py:50-51): exactly one atom, the top one, with s = sigma_0 and no 1/p
+    scale, whatever the draw; its estimate A v_0 v_0^T is off by at most ||A||_F <= sqrt(cols) * 1e-6."""
+    a = _unit((40, 6), [smax, smax / 2, smax / 4, 0, 0, 0])
+    for random_sample in (True, False):
+        c = codings.build("bsvd", rank=3, random_sample=random_sample, generator=torch.Generator().manual_seed(0))
+        for _ in range(5):
+            u, s, vT = c._code_unit(a, 3.0)
+            assert len(s) == 1 and vT.shape == (1, 6)
+            assert float(s[0]) == pytest.approx(float(torch.linalg.svdvals(a)[0]), rel=1e-3, abs=1e-12)
+            dec = (u * s) @ vT
+            assert torch.isfinite(dec).all()
+            assert float((dec - a).norm()) <= 6 ** 0.5 * 1e-6
+
+
+def test_null_atoms_are_counted_and_carry_a_zero_column():
+    """An atom with sigma_i <= 1e-7 sigma_max is sent (it counts) with a zero U column, not dropped."""
+    a = _unit((50, 5), [2.0, 1.0, 0.5, 0.0, 0.0]).double()     # fp64: the null sigmas stay below 1e-7 sigma_max
+    c = codings.build("bsvd", rank=5, random_sample=False)
+    u, s, vT = c._code_unit(a, 5.0)
+    assert len(s) == 5 and u.shape == (50, 5)
+    assert torch.equal(u[:, 3:], torch.zeros(50, 2, dtype=torch.float64))
+    assert torch.isfinite(u).all()
+    assert torch.allclose((u * s) @ vT, a, atol=1e-5)
+    cs = codings.build("bsvd", rank=5, generator=torch.Generator().manual_seed(1))   # p = 0 atoms are never drawn
+    for _ in range(10):
+        u, s, vT = cs._code_unit(a, 5.0)
+        assert torch.isfinite(u).all()
+
+
+def test_max_atoms_redraws_an_overflowing_draw():
+    """max_atoms (the engine's slot capacity): a draw with more atoms is redrawn, never truncated; without it, draws
+    above the capacity occur.  The top-k path keeps min(budget, cols, max_atoms) atoms."""
+    a = _unit((64, 18), [1.0] * 18)                  # p = 6 / 18 each: P(count > 6) ~ 0.3
+    c = codings.build("bsvd", rank=6, generator=torch.Generator().manual_seed(2))
+    capped = [len(c._code_unit(a, 6.0, max_atoms=6)[1]) for _ in range(200)]
+    free = [len(c._code_unit(a, 6.0)[1]) for _ in range(200)]
+    assert max(capped) <= 6 and max(free) > 6
+    top = codings.build("bsvd", rank=6, random_sample=False)
+    assert len(top._code_unit(a, 6.0, max_atoms=4)[1]) == 4
+    assert len(top._code_unit(a, 0.0)[1]) == 18        # budget <= 0: every atom

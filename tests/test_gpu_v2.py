@@ -89,7 +89,7 @@ class H2:
         self.wgrads[w] = grads
         return logical
 
-    def encode(self, w, random_sample=True, waterfill=False, systematic=False, uniforms=None):
+    def encode(self, w, random_sample=True, waterfill=False, systematic=False, uniforms=None, resample_empty=False):
         C, pl = self.C, self.plan
         gptr = torch.tensor([t.data_ptr() for t in self.wgrads[w]] or [0], dtype=torch.int64, device=self.dev)
         self._gptr = gptr
@@ -100,7 +100,7 @@ class H2:
                         self.t_arena_peer.data_ptr(), 1, pl.arena_floats, self.stage[w].data_ptr(), self.ctrl.data_ptr(),
                         uniforms.data_ptr() if uniforms is not None else 0,
                         self.vprev.data_ptr() if self.vprev is not None else 0, self.max_sweeps, random_sample,
-                        waterfill, systematic, w, False, 0, 0, g)
+                        waterfill, systematic, w, resample_empty, 0, 0, g)
             C.v2_project(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr.data_ptr(), self.vsel.data_ptr(),
                          self.selcount.data_ptr(), self.t_arena_peer.data_ptr(), self.t_sig_peer.data_ptr(), 1,
                          pl.arena_floats, w, g, self.ctrl.data_ptr(), self.counters.data_ptr() + 4 * (pl.n_coded + g), 0, 0,
