@@ -10,7 +10,7 @@ namespace v2 {
 
 enum Kind : int {
   KIND_SLAB = 1, KIND_MAT = 2, KIND_DENSE16 = 3, KIND_VEC = 4, KIND_QSGD = 5, KIND_ENTRY = 6, KIND_SIGN = 7,
-  KIND_POWER = 8, KIND_FP8 = 9
+  KIND_POWER = 8, KIND_FP8 = 9, KIND_HADAMARD = 10
 };
 
 // One coding unit: a conv gradient in [O][K][I] (channels_last) layout ("SLAB": row (o,ri), column (b,k) of the
@@ -28,6 +28,10 @@ enum Kind : int {
 //
 // FP8 units ("FP8", v2_fp8.cu) have the fields and slot of the sign units with one e4m3 byte per element:
 // cols = ceil(bucket / 8) uint64 words per bucket, the bytes in element order; the norms are the fp32 scales 2^-k.
+//
+// Randomized-Hadamard units ("HADAMARD", v2_hadamard.cu: one per >= 2-D weight): K = d (a power-of-two bucket),
+// I = bits (2, 4 or 8), rows = buckets, cols = d bits / 64 uint64 words per bucket, cs = buckets per PS tile,
+// ps_rows = elements per PS tile; the slot holds the step stamps, one fp32 (lo, step) pair per bucket, then the words.
 //
 // PowerSGD units ("POWER", v2_powersgd.cu: one per >= 2-D weight with r (O + C) < O C): rows = O, cols = C (row o is
 // the contiguous physical slab of output channel o), rcap = r, K = pass-B column blocks, n_enc = pass-A row tiles,

@@ -70,6 +70,9 @@ def run_rank(args) -> None:
     if args.code.lower() == "fp8":
         raise SystemExit("--code fp8 runs on the --backend p2p bf16 engine (--dtype bf16) only; the %s backend has no "
                          "fp8 coder" % backend)
+    if args.code.lower() == "hadamard":
+        raise SystemExit("--code hadamard runs on the --backend p2p bf16 engine (--dtype bf16) only; the %s backend has "
+                         "no randomized-Hadamard coder" % backend)
     if args.code.lower() == "powersgd":
         raise SystemExit("--code powersgd runs on the --backend p2p bf16 engine (--dtype bf16), which keeps each "
                          "worker's warm state and error-feedback residual; the %s backend's coders keep neither"

@@ -29,6 +29,9 @@ What changes against ``ops/plan.py`` (the fp32-flat plan of round 1):
   element and one fp32 scale, in the slot and tile geometry of the quantizing codes.
 * **FP8** (``code="fp8"``): every >= 2-D weight is one ``FP8`` unit whose buckets are sent as one e4m3 byte per
   element (stochastically rounded) and one power-of-two fp32 scale, in the geometry of the sign units.
+* **Randomized Hadamard** (``code="hadamard"``): every >= 2-D weight is one ``HADAMARD`` unit whose power-of-two
+  buckets are rotated by ``H D`` and sent as 2 / 4 / 8-bit codes between the bucket's min and max (``lo``, ``step``
+  in fp32), in the tile and owner geometry of the sign units.
 * **PowerSGD** (``code="powersgd"``): every >= 2-D weight with ``r (O + C) < O C`` is one ``POWER`` unit, the whole
   ``[O][C]`` matrix of its physical layout, sent as a rank-``r`` pair ``P_hat`` / ``Q'`` from one warm-started power
   step; the owners reconstruct ``P_hat Q'^T`` and step the optimizer.
@@ -47,6 +50,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 KIND_SLAB, KIND_MAT, KIND_DENSE16, KIND_VEC, KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_POWER, KIND_FP8 = \
     1, 2, 3, 4, 5, 6, 7, 8, 9
+KIND_HADAMARD = 10
 RCAP_MAX = 32
 MAX_COLS = 64
 BLOCK_COLS = 32               # column-block width of MAT units (Jacobi cost ~ cols^3 sits in the encode launch)
@@ -64,6 +68,8 @@ QSGD_MAX_LEVEL = 14           # (sign + 1) << q | level must fit 16 bits
 SIGN_MIN_BUCKET, SIGN_MAX_BUCKET = 64, 4096   # scaled sign and fp8: whole 64-bit words, at most one tile
 ENTRY_TILE_ELEMS = 4096       # entry-wise PS / encode tile: the element offset of an entry fits 12 bits
 TOPK_STATE_INTS, TOPK_HI_BINS, TOPK_LO_BINS = 8, 256, 128   # top-k selection state / histograms (csrc/v2_common.cuh)
+HADAMARD_BITS = (2, 4, 8)    # randomized Hadamard: whole codes per 64-bit word
+HADAMARD_MIN_BUCKET, HADAMARD_MAX_BUCKET = 64, 4096   # power-of-two buckets, one CTA transforms a whole tile
 POWER_MAX_RANK = 4            # PowerSGD: rank r in [1, 4] (csrc/v2_powersgd.cu keeps r x 8 accumulators per thread)
 PW_ENC_ROWS = 8               # PowerSGD pass A (P = M Q_w, Gram partial) and the EF / stats passes: rows per tile
 PW_COL_BLOCK = 256            # PowerSGD pass B (Q' = M^T P_hat): columns per CTA, every row summed inside the CTA
@@ -117,6 +123,27 @@ def qsgd_words_off(n_ps: int, buckets: int) -> int:
 
 def qsgd_slot_floats(n_ps: int, buckets: int, words_per_bucket: int) -> int:
     return _round_up(qsgd_words_off(n_ps, buckets) + 2 * buckets * words_per_bucket, 32)
+
+
+def hadamard_params_off(n_ps: int) -> int:
+    """Float offset (inside a hadamard slot) of the per-bucket ``(lo, step)`` fp32 pairs: after one int32 step stamp
+    per PS tile."""
+    return _round_up(n_ps, 4)
+
+
+def hadamard_words_off(n_ps: int, buckets: int) -> int:
+    """Float offset (inside a hadamard slot) of the uint64 code words (16-byte aligned)."""
+    return hadamard_params_off(n_ps) + _round_up(2 * buckets, 4)
+
+
+def hadamard_slot_floats(n_ps: int, buckets: int, words_per_bucket: int) -> int:
+    return _round_up(hadamard_words_off(n_ps, buckets) + 2 * buckets * words_per_bucket, 32)
+
+
+def hadamard_bucket(numel: int, bucket_size: int) -> int:
+    """``d = min(bucket_size, next_pow2(max(numel, 64)))`` (``codings/hadamard.py``)."""
+    n = max(int(numel), HADAMARD_MIN_BUCKET)
+    return min(int(bucket_size), 1 << (n - 1).bit_length())
 
 
 def pw_phat_off(n_ps: int) -> int:
@@ -260,7 +287,8 @@ class Plan2:
     stage_total: int        # bf16 elements of the dense-16 staging region
     arena_floats: int
     gpart_floats: int
-    n_coded: int            # units with per-unit device state (coded SLAB / MAT units, or the QSGD / ENTRY / SIGN / FP8 units)
+    n_coded: int            # units with per-unit device state (coded SLAB / MAT units, or the QSGD / ENTRY / SIGN / FP8 /
+    #                         HADAMARD units)
     rank: int
     code: str
     pw_tiles: List[Tuple[int, int, int, int]] = field(default_factory=list)   # PowerSGD pass B: (unit, col0, ncols, j)
@@ -289,6 +317,11 @@ class Plan2:
         counted."""
         return sum(4 * u.rcap * (u.rows + u.cols) for u in self.units if u.kind == KIND_POWER)
 
+    def hadamard_bytes(self) -> int:
+        """Bytes of rotated codes a worker pushes per step: the uint64 words and the fp32 ``(lo, step)`` of every
+        bucket (``codings.hadamard``'s ``words``, ``lo`` and ``step``), tail padding included."""
+        return sum(8 * u.rows * u.cols + 8 * u.rows for u in self.units if u.kind == KIND_HADAMARD)
+
     def entry_bytes(self) -> float:
         """Bytes of entry-wise code a worker pushes per step: 4 per expected atom and a 16-byte header per PS tile.
         An upper bound on the expectation (``sum(p_i) <= s``), exact when no ``p_i`` is clamped to 1.  Top-k: an
@@ -299,7 +332,7 @@ class Plan2:
         """Bytes actually stored per worker and step for the expected number of atoms (U is written in groups
         of 4 atoms); for the quantizing codes the words and norms of the QSGD units; for entry-wise ATOMO the
         entries and tile headers."""
-        tot = float(self.qsgd_bytes()) + self.entry_bytes() + float(self.powersgd_bytes())
+        tot = float(self.qsgd_bytes()) + self.entry_bytes() + float(self.powersgd_bytes()) + float(self.hadamard_bytes())
         for u in self.units:
             if u.coded:
                 atoms = min(u.budget if u.budget > 0 else u.cols, u.cols)
@@ -309,7 +342,8 @@ class Plan2:
 
     def dense_bytes(self) -> int:
         return sum((2 if u.kind == KIND_DENSE16 else 4) * u.numel for u in self.units
-                   if not u.coded and u.kind not in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_POWER, KIND_FP8))
+                   if not u.coded and u.kind not in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_POWER, KIND_FP8,
+                                                     KIND_HADAMARD))
 
 
 def default_groups(shapes: Sequence[Sequence[int]], n_groups: int) -> List[int]:
@@ -358,7 +392,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 block_cols: int = BLOCK_COLS, min_coded_numel: int = 256, quantization_level: int = 4,
                 bucket_size: int = 512, entry_budget: float = 0.05) -> Plan2:
     """Plan of the bf16 engine for ``code`` in ``svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign |
-    powersgd | fp8``.
+    powersgd | fp8 | hadamard``.
 
     ``qsgd`` / ``terngrad``: every >= 2-D weight (the 3-channel stem and the fc layers included) is exactly one
     ``KIND_QSGD`` unit; there are no ``DENSE16`` units.  1-D parameters stay ``KIND_VEC`` (fp32, summed by
@@ -404,6 +438,14 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
     ``ceil(bucket / 8)`` uint64 words per bucket: one e4m3 byte per element in element order, bucket ``j`` starting at
     byte ``8 j cols``, and one power-of-two fp32 scale per bucket in place of the norm (``codings/fp8.py``).
 
+    ``hadamard`` (``quantization_level`` = bits in ``{2, 4, 8}``, ``bucket_size`` a power of two in ``[64, 4096]``):
+    every >= 2-D weight is exactly one ``KIND_HADAMARD`` unit; 1-D parameters stay ``KIND_VEC``.  Per tensor the bucket
+    is ``d = min(bucket_size, next_pow2(max(numel, 64)))`` (:func:`hadamard_bucket`, the tail bucket zero padded); tiles
+    and owners are those of ``sign`` with ``max(1, 4096 // d)`` whole buckets per tile.  ``Unit2`` fields: ``K`` = d,
+    ``I`` = bits, ``rows`` = buckets, ``cols`` = ``d bits / 64`` uint64 words per bucket, ``cs`` = buckets per tile,
+    ``ps_rows`` = elements per tile, ``rs`` = 0.  The slot holds one int32 step stamp per PS tile, the fp32 ``(lo,
+    step)`` of every bucket and the 16-byte aligned words (:func:`hadamard_params_off` / :func:`hadamard_words_off`).
+
     ``powersgd`` (``rank`` = r in ``[1, 4]``): every >= 2-D weight with ``r (O + C) < O C`` is exactly one ``KIND_POWER``
     unit (``codings/powersgd.py``), the others travel ``DENSE16``; 1-D parameters stay ``KIND_VEC``.  Per unit:
 
@@ -438,6 +480,14 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
         if not (SIGN_MIN_BUCKET <= sbsz <= SIGN_MAX_BUCKET and sbsz % 64 == 0):
             raise ValueError("%s: bucket_size must be a multiple of 64 in [%d, %d]"
                              % (code, SIGN_MIN_BUCKET, SIGN_MAX_BUCKET))
+    had = code == "hadamard"
+    if had:
+        hbits, hbsz = int(quantization_level), int(bucket_size)
+        if hbits not in HADAMARD_BITS:
+            raise ValueError("hadamard: quantization_level (bits) must be 2, 4 or 8 (got %r)" % (quantization_level,))
+        if not (HADAMARD_MIN_BUCKET <= hbsz <= HADAMARD_MAX_BUCKET and hbsz & (hbsz - 1) == 0):
+            raise ValueError("hadamard: bucket_size must be a power of two in [%d, %d] (got %r)"
+                             % (HADAMARD_MIN_BUCKET, HADAMARD_MAX_BUCKET, bucket_size))
     power = code == "powersgd"
     if power and not 1 <= int(rank) <= POWER_MAX_RANK:
         raise ValueError("powersgd: svd_rank must be in [1, %d] (got %r)" % (POWER_MAX_RANK, rank))
@@ -493,6 +543,13 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             bpt = max(1, QSGD_TILE_ELEMS // bucket)
             add(Unit2(0, KIND_FP8, p.index, p.widx, p.off, 0, rows=(p.numel + bucket - 1) // bucket,
                       cols=(bucket + 7) // 8, K=bucket, cs=bpt, numel=p.numel, group=p.group, ps_rows=bpt * bucket))
+            continue
+        if had:
+            bucket = hadamard_bucket(p.numel, hbsz)
+            bpt = max(1, QSGD_TILE_ELEMS // bucket)
+            add(Unit2(0, KIND_HADAMARD, p.index, p.widx, p.off, 0, rows=(p.numel + bucket - 1) // bucket,
+                      cols=bucket * hbits // 64, K=bucket, I=hbits, cs=bpt, numel=p.numel, group=p.group,
+                      ps_rows=bpt * bucket))
             continue
         if power:
             o = s[0]
@@ -577,7 +634,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             elif u.kind == KIND_DENSE16:
                 for e0 in range(0, u.numel, 8192):     # staging copy tiles
                     enc_tiles.append((u.index, e0, min(8192, u.numel - e0), 0))
-            elif u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_FP8):   # encode tiles = PS tiles (one owner per CTA)
+            elif u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_FP8, KIND_HADAMARD):   # encode = PS tiles
                 for j, e0 in enumerate(range(0, u.numel, u.ps_rows)):
                     enc_tiles.append((u.index, e0, min(u.ps_rows, u.numel - e0), j))
             elif u.kind == KIND_POWER:
@@ -586,7 +643,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 for j, c0 in enumerate(range(0, u.cols, PW_COL_BLOCK)):
                     pw_tiles.append((u.index, c0, min(PW_COL_BLOCK, u.cols - c0), j))
             u.n_enc = len(enc_tiles) - u.enc_tile0
-            if u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_FP8):
+            if u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_FP8, KIND_HADAMARD):
                 u.ts_index = n_coded
                 n_coded += 1
                 u.ps_tile0 = len(ps_by_group[g])
@@ -597,6 +654,8 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 u.slot_off = slot_off
                 if u.kind in (KIND_QSGD, KIND_SIGN, KIND_FP8):
                     slot_off += qsgd_slot_floats(u.n_ps, u.rows, u.cols)
+                elif u.kind == KIND_HADAMARD:
+                    slot_off += hadamard_slot_floats(u.n_ps, u.rows, u.cols)
                 else:
                     slot_off += entry_slot_floats(u.numel, u.n_ps, u.ps_rows)
             elif u.kind == KIND_POWER:

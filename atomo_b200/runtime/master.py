@@ -48,6 +48,9 @@ def build_coder(kwargs: dict, worker_side: bool):
     if code == "fp8":
         raise ValueError("--code fp8 runs on the --backend p2p bf16 engine (--dtype bf16) only; the gloo / nccl "
                          "backends have no fp8 coder")
+    if code == "hadamard":
+        raise ValueError("--code hadamard runs on the --backend p2p bf16 engine (--dtype bf16) only; the gloo / nccl "
+                         "backends have no randomized-Hadamard coder")
     if code == "powersgd":
         raise ValueError("--code powersgd runs on the --backend p2p bf16 engine (--dtype bf16), which keeps each "
                          "worker's warm state and error-feedback residual; the gloo / nccl coders keep neither")

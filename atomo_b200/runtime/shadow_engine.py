@@ -43,7 +43,12 @@ one central PS kernel at the end of the step):
   power-of-two fp32 scale in the slots and tiles of sign (``csrc/v2_fp8.cu``, one encode launch per group); each
   scaled magnitude is rounded to one of its two e4m3 neighbours with Philox draws, so the code is unbiased.  The
   owners decode with the hardware conversion, sum in worker order and step the optimizer.
-* **Error feedback** (``error_feedback=True``; svd, entrywise, topk, qsgd, sign, powersgd, fp8): each worker keeps an fp32 residual ``e`` per
+* **Randomized Hadamard** (``code="hadamard"``, ``quantization_level`` = bits in {2, 4, 8}, ``bucket_size`` a power
+  of two): every weight's buckets are rotated by ``H D`` (Philox signs shared by all workers in a step) and pushed as
+  ``bits``-bit codes between the bucket's min and max, stochastically rounded, with an fp32 ``(lo, step)`` per bucket
+  (``csrc/v2_hadamard.cu``, one encode launch per group).  Unbiased.  The owners sum the workers' decodes in the
+  rotated domain, apply one inverse transform per bucket and step the optimizer.
+* **Error feedback** (``error_feedback=True``; svd, entrywise, topk, qsgd, sign, powersgd, fp8, hadamard): each worker keeps an fp32 residual ``e`` per
   weight element and codes ``A = g + e``.  An apply launch per group (``csrc/v2_feedback.cu``) writes ``bf16(A)`` into
   autograd's gradient buffer in place and keeps ``A - bf16(A)``; the encoders' epilogues add ``bf16(A) - g_hat``, the
   part of ``A`` this push did not carry.  Nothing is discarded, only delayed.
@@ -90,9 +95,10 @@ class ShadowEngine:
                  bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False,
                  error_feedback: bool = False):
         self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
-        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign", "powersgd", "fp8"):
+        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign", "powersgd", "fp8",
+                             "hadamard"):
             raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign | powersgd "
-                             "| fp8")
+                             "| fp8 | hadamard")
         self.power = self.code == "powersgd"
         if self.power and not 1 <= int(svd_rank) <= P2.POWER_MAX_RANK:      # checked before any CUDA work
             raise ValueError("powersgd: svd_rank must be in [1, %d] (got %r)" % (P2.POWER_MAX_RANK, svd_rank))
@@ -132,6 +138,14 @@ class ShadowEngine:
             if not (P2.SIGN_MIN_BUCKET <= int(bucket_size) <= P2.SIGN_MAX_BUCKET and int(bucket_size) % 64 == 0):
                 raise ValueError("%s: bucket_size must be a multiple of 64 in [%d, %d] (got %r)"
                                  % (self.code, P2.SIGN_MIN_BUCKET, P2.SIGN_MAX_BUCKET, bucket_size))
+        self.hadamard = self.code == "hadamard"
+        if self.hadamard:       # checked before any CUDA work
+            if int(quantization_level) not in P2.HADAMARD_BITS:
+                raise ValueError("hadamard: quantization_level (bits) must be 2, 4 or 8 (got %r)" % (quantization_level,))
+            hb = int(bucket_size)
+            if not (P2.HADAMARD_MIN_BUCKET <= hb <= P2.HADAMARD_MAX_BUCKET and hb & (hb - 1) == 0):
+                raise ValueError("hadamard: bucket_size must be a power of two in [%d, %d] (got %r)"
+                                 % (P2.HADAMARD_MIN_BUCKET, P2.HADAMARD_MAX_BUCKET, bucket_size))
         self.C = load_ext()
         C = self.C
         assert C.v2_unit_bytes() == P2.UNIT_BYTES and C.v2_ctrl_bytes() == P2.CTRL2_BYTES
@@ -284,7 +298,8 @@ class ShadowEngine:
         # eigenbasis of the previous step per coded unit (Jacobi warm start); identity to begin with
         self.max_sweeps = int(max_sweeps) if warm_start else 0
         self.vprev = None
-        if warm_start and not self.quant and not self.entry and not self.sign and not self.power and not self.fp8:
+        if warm_start and not self.quant and not self.entry and not self.sign and not self.power and not self.fp8 \
+                and not self.hadamard:
             self.vprev = z(nc * P2.MAX_COLS * P2.MAX_COLS)
             for u in pl.units:
                 if u.coded:
@@ -441,7 +456,7 @@ class ShadowEngine:
         * ``mse``       the expected ``||g_hat - g||^2`` given that gradient, in closed form (exact, not sampled);
                         ``rel_var`` = ``mse / gsq``,
         * ``bias_sq``   TernGrad's clip bias ``||clip(g) - g||^2`` (0 for the other codes; not part of ``mse``),
-        * ``exp_atoms`` / ``atoms``  expected and realized atoms (QSGD / TernGrad / sign / fp8: every element; PowerSGD: the
+        * ``exp_atoms`` / ``atoms``  expected and realized atoms (QSGD / TernGrad / sign / fp8 / hadamard: every element; PowerSGD: the
                         non-degenerate columns of ``P_hat``), exact tensors their element count,
         * ``bytes``     realized push bytes: the spectral slot layout, ``entry_bytes()`` / ``qsgd_bytes()`` applied to
                         the realized counts, dense bytes for exact tensors.
@@ -460,7 +475,7 @@ class ShadowEngine:
             t = per.setdefault(name, {"numel": q.numel, "gsq": None, "mse": 0.0, "bias_sq": 0.0, "exp_atoms": 0.0,
                                       "atoms": 0.0, "bytes": 0.0})
             if u.kind in (P2.KIND_SLAB, P2.KIND_MAT, P2.KIND_ENTRY, P2.KIND_QSGD, P2.KIND_SIGN, P2.KIND_POWER,
-                          P2.KIND_FP8) and acc:
+                          P2.KIND_FP8, P2.KIND_HADAMARD) and acc:
                 gsq, mse, ex, bias, real, real4, n = acc[u.ts_index]
                 n = max(n, 1.0)
                 t["gsq"] = (t["gsq"] or 0.0) + gsq / n
@@ -470,6 +485,8 @@ class ShadowEngine:
                 t["atoms"] += real / n
                 if u.kind in (P2.KIND_QSGD, P2.KIND_SIGN, P2.KIND_FP8):
                     t["bytes"] += 8.0 * u.rows * u.cols + 4.0 * u.rows
+                elif u.kind == P2.KIND_HADAMARD:
+                    t["bytes"] += 8.0 * u.rows * u.cols + 8.0 * u.rows
                 elif u.kind == P2.KIND_POWER:
                     t["bytes"] += 4.0 * u.rcap * (u.rows + u.cols)
                 elif u.kind == P2.KIND_ENTRY:
@@ -511,6 +528,14 @@ class ShadowEngine:
         if self.power:
             self.C.v2_powersgd_code_stats(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt,
                                           self.t_gptr.data_ptr(), self.gpart.data_ptr(), self.pw_state.data_ptr(),
+                                          self.stats_partials.data_ptr(), self.stats_counters.data_ptr(),
+                                          self.stats_acc.data_ptr())
+            self._nlaunch += 1
+            return
+        if self.hadamard:
+            self.C.v2_hadamard_code_stats(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt,
+                                          self.t_gptr.data_ptr(), self.t_arena_peer.data_ptr(), self.n_owners,
+                                          self.plan.arena_floats, self.worker_index, self.ctrl.data_ptr(),
                                           self.stats_partials.data_ptr(), self.stats_counters.data_ptr(),
                                           self.stats_acc.data_ptr())
             self._nlaunch += 1
@@ -589,9 +614,10 @@ class ShadowEngine:
                                  self.tstats.data_ptr(), self._fired == self.G, res)
             self._nlaunch += (1 if nt > 0 else 0) + 1 + (1 if res and nt > 0 else 0)
             return
-        if nt > 0 and (self.sign or self.fp8):
-            # scales + sign bits / e4m3 bytes pushed straight into the owners' arenas; the encode raises the push flag
-            encode = C.v2_sign_encode if self.sign else C.v2_fp8_encode
+        if nt > 0 and (self.sign or self.fp8 or self.hadamard):
+            # scales + sign bits / e4m3 bytes / (lo, step) + rotated codes pushed straight into the owners' arenas; the
+            # encode raises the push flag
+            encode = C.v2_sign_encode if self.sign else C.v2_fp8_encode if self.fp8 else C.v2_hadamard_encode
             encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
                    self.t_arena_peer.data_ptr(), self.t_sig_owner.data_ptr(), self.n_owners, pl.arena_floats,
                    self.worker_index, g, self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g, self.tstats.data_ptr(),
@@ -671,8 +697,8 @@ class ShadowEngine:
                              max(1, min(self.ps_grid, max(nt, 1))))
             self._nlaunch += 1
             return
-        if self.sign or self.fp8:
-            ps = C.v2_ps_sign if self.sign else C.v2_ps_fp8
+        if self.sign or self.fp8 or self.hadamard:
+            ps = C.v2_ps_sign if self.sign else C.v2_ps_fp8 if self.fp8 else C.v2_ps_hadamard
             ps(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g, final,
                self.owner_index, p(self.master), p(self.mom), p(self.sq), p(self.sqmax), p(self.vmom), p(self.vsq),
                p(self.vsqmax), self.wshadow_mc, self.t_wshadow_peer.data_ptr(), self.vparams.data_ptr(),
@@ -862,7 +888,8 @@ class ShadowEngine:
             u = pl.units[ui]
             if u.kind == P2.KIND_VEC:
                 mv[u.w_off + a:u.w_off + a + b] = 1
-            elif u.kind in (P2.KIND_DENSE16, P2.KIND_QSGD, P2.KIND_ENTRY, P2.KIND_SIGN, P2.KIND_FP8):   # (first, count)
+            elif u.kind in (P2.KIND_DENSE16, P2.KIND_QSGD, P2.KIND_ENTRY, P2.KIND_SIGN, P2.KIND_FP8,
+                            P2.KIND_HADAMARD):                                           # (first, count)
                 mw[u.w_off + a:u.w_off + a + b] = 1
             elif u.kind == P2.KIND_POWER:                                                # (first row, rows)
                 mw[u.w_off + a * u.cols:u.w_off + (a + b) * u.cols] = 1
@@ -937,7 +964,7 @@ class ShadowEngine:
         os.replace(tmp, path)
         side = {"step": step, "lr": self.lr, "mom_w": mom.cpu(), "mom_v": vm.cpu(), "code": self.code,
                 "svd_rank": self.svd_rank, "engine": "shadow"}
-        if self.quant:
+        if self.quant or self.hadamard:
             side.update(quantization_level=self.quantization_level, bucket_size=self.bucket_size)
         if self.sign or self.fp8:
             side.update(bucket_size=self.bucket_size)

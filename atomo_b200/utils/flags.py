@@ -38,7 +38,10 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "weight matrix from one warm-started power step; --backend p2p --dtype bf16 only, meant for "
                         "--error-feedback 1) | fp8 (one e4m3 byte per element, stochastically rounded and so "
                         "unbiased, and one power-of-two fp32 scale per --bucket-size bucket, a multiple of 64 in "
-                        "[64, 4096]; --backend p2p --dtype bf16 only)")
+                        "[64, 4096]; --backend p2p --dtype bf16 only) | hadamard (each --bucket-size bucket, a power "
+                        "of two in [64, 4096], rotated by random signs and a Walsh-Hadamard transform and sent as "
+                        "--quantization-level bits per element (2, 4 or 8), stochastically rounded between its min and "
+                        "max and so unbiased, plus an fp32 (lo, step) per bucket; --backend p2p --dtype bf16 only)")
     p.add_argument("--bucket-size", type=int, default=512)
     p.add_argument("--dataset", type=str, default="MNIST", metavar="N")
     p.add_argument("--comm-type", type=str, default="Bcast", metavar="N")
@@ -79,7 +82,7 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "colocated = rank 0 hosts the whole PS and also trains; dedicated = rank 0 only serves")
     p.add_argument("--engine", type=str, default="auto", choices=["auto", "shadow", "fused"],
                    help="p2p backend: auto = the overlapped sharded bf16 engine for --dtype bf16 with --code "
-                        "svd|qsvd|sgd|topk|sign|powersgd|fp8, the fp32-flat engine otherwise; shadow = the bf16 engine (also --code "
+                        "svd|qsvd|sgd|topk|sign|powersgd|fp8|hadamard, the fp32-flat engine otherwise; shadow = the bf16 engine (also --code "
                         "qsgd|terngrad, needs --dtype bf16); fused = the fp32-flat engine")
     p.add_argument("--groups", type=int, default=5, help="p2p/bf16: backward groups pushed while backward runs")
     p.add_argument("--shrinkage-freq", type=int, default=50, help="steps between LR shrinkages (reference: 50)")
@@ -101,7 +104,8 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
     p.add_argument("--error-feedback", type=bool_flag, default=False,
                    help="p2p backend, bf16 engine: every worker keeps the part of its gradient the code did not send "
                         "(an fp32 residual per weight) and adds it to the next step's gradient before coding; --code "
-                        "svd | entrywise | topk | qsgd | sign | powersgd | fp8 (it stays bounded with svd top-k, topk, "
-                        "sign and powersgd, the contractive codes, and with fp8, whose variance is small), every push counted (no --num-aggregate below the worker "
+                        "svd | entrywise | topk | qsgd | sign | powersgd | fp8 | hadamard (it stays bounded with svd "
+                        "top-k, topk, sign and powersgd, the contractive codes, and with fp8 and hadamard at 4 or 8 "
+                        "bits, whose variance is small), every push counted (no --num-aggregate below the worker "
                         "count).  Residuals (and PowerSGD's warm state) are not checkpointed: --resume starts them afresh")
     return p.parse_args(argv)
