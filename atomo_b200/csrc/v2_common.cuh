@@ -202,5 +202,106 @@ constexpr int TOPK_LO_BINS = 128;     // magnitude bits 6..0
 constexpr int TOPK_NONE = 0x8000;
 enum TopkField : int { TK_BIN = 0, TK_NEED_BIN = 1, TK_T = 2, TK_NEED_TIES = 3, TK_KEFF = 4, TK_NONFINITE = 5 };
 
+// ---- push publication (thread 0 of every encode CTA, after the CTA's final __syncthreads) ----------------------
+// The owner trusts a tile once its step stamp reads this step, and waits for the group's push flag before it reads any
+// stamp; so the payload is fenced before the stamp, and the stamps before the counter that raises the flag.
+// The stamp is stamps[j]: base and index apart, so that the address is formed after the fence, as it always was.
+__device__ __forceinline__ void enc_stamp(int* stamps, int j, int step) {
+  __threadfence_system();                                   // the tile's payload before its stamp
+  st_release_sys(stamps + j, step);
+}
+
+// The group counter; the last CTA of the launch resets it and publishes flag[group][worker] = step on every owner.
+template <class Args>
+__device__ __forceinline__ void enc_push_flag(const Args& a, int step) {
+  __threadfence_system();                                   // the stamps before the counter (and so the push flag)
+  const unsigned int old = atomicAdd(a.group_counter, 1u);
+  if (old == gridDim.x - 1) {
+    *a.group_counter = 0;
+    __threadfence_system();
+    for (int o = 0; o < a.n_owners; ++o)
+      st_release_sys(a.sig_peer[o] + SIG_PUSH + a.group * MAX_WORKERS + a.worker, step);
+    if (a.tstats != nullptr) {
+      const long long now = globaltimer_ns();
+      a.tstats[5] += now - a.tstats[9 + a.group];      // encode of this group
+      if (a.final_group) a.tstats[8] += now - a.tstats[6];          // step start -> last push published
+    }
+  }
+}
+
+// The encode arguments of the bucketed dense codes (sign, fp8, hadamard).
+struct PushArgs {
+  const Unit2* units;
+  const Tile2* tiles;          // already offset to the first tile of the group
+  const long long* gptr;       // gradient base pointers (bf16), one per weight tensor
+  float* const* arena_peer;    // [n_owners] arena base inside each owner
+  int* const* sig_peer;        // [n_owners] signal region base of each owner
+  int n_owners;
+  long long arena_floats;
+  int worker;
+  int group;
+  const Ctrl2* ctrl;
+  unsigned int* group_counter;
+  long long* tstats;
+  int final_group;
+  float* residual;             // error feedback: fp32 residual like wshadow, or nullptr
+};
+
+// ---- --code-stats layout, read by ShadowEngine.code_stats() through v2_stats_fields() / v2_stats_partials() ------
+constexpr int STAT_PART = 5;   // per encode tile: gsq, mse, exp_atoms, bias_sq, realized atoms
+constexpr int STAT_ACC = 7;    // per unit: the five sums, realized atoms (spectral: rounded up to U's groups of 4), steps
+
+// The --code-stats arguments of the codes whose stats read the per-bucket scales back from the slot (sign, fp8).
+struct ScaleStatArgs {
+  const Unit2* units;
+  const Tile2* tiles;          // already offset to the first tile of the group
+  int tile0;                   // global index of tiles[0] (partials are indexed by global encode tile)
+  const long long* gptr;
+  float* const* arena_peer;    // [n_owners] arena base inside each owner (this worker's scales)
+  int n_owners;
+  long long arena_floats;
+  int worker;
+  double* partials;            // [n_enc_tiles][STAT_PART]
+  unsigned int* unit_counters; // [n_units of the code]
+  double* acc;                 // [n_units of the code][STAT_ACC]
+};
+
+// Thread 0: the tile's partials, then the unit's counter; last = 1 in the unit's last tile, which resets the counter.
+template <class Args>
+__device__ __forceinline__ void stat_store_tile(const Args& a, const Unit2& u, double gsq, double mse, double ex,
+                                                double bias, double real, int& last) {
+  double* p = a.partials + (long long)STAT_PART * (a.tile0 + blockIdx.x);
+  p[0] = gsq;
+  p[1] = mse;
+  p[2] = ex;
+  p[3] = bias;
+  p[4] = real;
+  __threadfence();
+  const unsigned int old = atomicAdd(&a.unit_counters[u.ts_index], 1u);
+  last = (old == (unsigned int)u.n_enc - 1u) ? 1 : 0;
+  if (last) a.unit_counters[u.ts_index] = 0;
+}
+
+// The unit's last tile: the sum of every tile's partials, in tile order (the same bits on every run).
+template <class Args>
+__device__ __forceinline__ void stat_unit_sum(const Args& a, const Unit2& u, double (&sum)[STAT_PART]) {
+  __threadfence();
+#pragma unroll
+  for (int f = 0; f < STAT_PART; ++f) sum[f] = 0.0;
+  for (int k = 0; k < u.n_enc; ++k) {
+    const double* pk = a.partials + (long long)STAT_PART * (u.enc_tile0 + k);
+    for (int f = 0; f < STAT_PART; ++f) sum[f] += __ldcg(pk + f);
+  }
+}
+
+// ... added into the unit's accumulator, with the realized atoms as they are and one more step.
+template <class Args>
+__device__ __forceinline__ void stat_accumulate(const Args& a, const Unit2& u, const double (&sum)[STAT_PART]) {
+  double* acc = a.acc + (long long)STAT_ACC * u.ts_index;
+  for (int f = 0; f < STAT_PART; ++f) acc[f] += sum[f];
+  acc[5] += sum[4];
+  acc[6] += 1.0;
+}
+
 }  // namespace v2
 }  // namespace atomo

@@ -567,6 +567,7 @@ __device__ __forceinline__ void project(const ProjArgs& a, float* residual, int 
   }
 
   // ---- completion: the last CTA publishes flag[group][worker] = step on every owner -------------------
+  // enc_push_flag (v2_common.cuh) with a `timed` condition, kept inline: the helper changes this kernel's schedule
   __syncthreads();
   if (tid == 0) {
     __threadfence_system();

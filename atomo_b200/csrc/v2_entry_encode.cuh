@@ -179,21 +179,8 @@ __device__ __forceinline__ void entry_encode(const Args& a) {
   // ---- the tile's step stamp (after its entries, count and scale), then the group's push flag -----------------
   __syncthreads();
   if (tid == 0) {
-    __threadfence_system();                                   // entries + count + scale before the stamp
-    st_release_sys(hdr, step);
-    __threadfence_system();                                   // the stamp before the counter (and so the push flag)
-    const unsigned int old = atomicAdd(a.group_counter, 1u);
-    if (old == gridDim.x - 1) {
-      *a.group_counter = 0;
-      __threadfence_system();
-      for (int o = 0; o < a.n_owners; ++o)
-        st_release_sys(a.sig_peer[o] + SIG_PUSH + a.group * MAX_WORKERS + a.worker, step);
-      if (a.tstats != nullptr) {
-        const long long now = globaltimer_ns();
-        a.tstats[5] += now - a.tstats[9 + a.group];      // selection / stats + encode of this group
-        if (a.final_group) a.tstats[8] += now - a.tstats[6];          // step start -> last push published
-      }
-    }
+    enc_stamp(hdr, 0, step);
+    enc_push_flag(a, step);
   }
 }
 

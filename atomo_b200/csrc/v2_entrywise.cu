@@ -83,23 +83,15 @@ __global__ void __launch_bounds__(EPS_THREADS) v2_ps_entry_kernel(const PsArgs2 
   const int step = ctrl->step;
 
   long long t_enter = 0, t_ready = 0;
-  if (tid == 0) {
-    t_enter = globaltimer_ns();
-    unsigned int mask;
-    const bool ok = ps_wait_pushes(a, ctrl, step, mask);
-    if (!ok) atomicOr(&ctrl->error, ERR2_WAIT_PUSH);
-    s_ok = ok ? 1 : 0;
-    s_bad = 0;
-    s_mask = mask;
-    t_ready = globaltimer_ns();
-  }
-  __syncthreads();
+  ps_wait(a, ctrl, step, s_ok, s_bad, s_mask, t_enter, t_ready);
+  // the counted workers stay inline: as a helper they change this kernel's register allocation
   const bool ok = s_ok != 0;
   const unsigned int wmask = s_mask;
   const bool all_workers = wmask == (a.W >= 32 ? 0xffffffffu : ((1u << a.W) - 1u));
   const OptC c = ps_opt_consts(ctrl, step);
   const float inv_w = all_workers ? a.inv_w : 1.f / (float)max(__popc(wmask), 1);
 
+  // the tile range stays inline: with ps_tile_range next to ps_wait this kernel's register allocation changes
   const int per_cta = (a.ntiles + gridDim.x - 1) / gridDim.x;
   const int t_begin = blockIdx.x * per_cta;
   const int t_end = min(a.ntiles, t_begin + per_cta);
@@ -113,17 +105,10 @@ __global__ void __launch_bounds__(EPS_THREADS) v2_ps_entry_kernel(const PsArgs2 
     if (u.kind != KIND_ENTRY) continue;
     const int jt = t.a / u.ps_rows;
     __syncthreads();   // previous tile is done with OUT / s_use
-    if (tid == 0) {
-      unsigned int use = 0;
-      for (int w = 0; w < a.W; ++w) {
-        if (!((wmask >> w) & 1u)) continue;
-        const int* hdr = reinterpret_cast<const int*>(a.arenas + (long long)w * a.arena_floats + u.slot_off +
-                                                      entry_hdr_off(jt));
-        if (ld_cg_i(hdr) == step) use |= 1u << w;
-        else s_bad = 1;                                  // stale slot: a push of another step
-      }
-      s_use = use;
-    }
+    if (tid == 0)
+      s_use = ps_fresh_workers(a, wmask, step, s_bad, [&](int w) {
+        return reinterpret_cast<const int*>(a.arenas + (long long)w * a.arena_floats + u.slot_off + entry_hdr_off(jt));
+      });
     for (int i = tid; i < t.b; i += blockDim.x) OUT[i] = 0.f;
     __syncthreads();
     const unsigned int use = s_use;
@@ -203,17 +188,10 @@ void atomo_v2_launch_ps_entry(const void* units, const void* tiles, int tile0, i
                               const float* arenas, long long arena_floats, int* sig, int* const* sig_peer, void* ctrl,
                               unsigned int* group_counter, long long timeout, long long* tstats, float inv_w, int grid,
                               cudaStream_t stream) {
-  PsArgs2 a;
-  a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.ntiles = ntiles; a.W = W; a.nranks = nranks;
-  a.group = group; a.final_group = final_group; a.owner = owner; a.master = master; a.mom = mom; a.sq = sq;
-  a.sqmax = sqmax; a.vmom = vmom; a.vsq = vsq; a.vsqmax = vsqmax; a.wshadow_mc = (__nv_bfloat16*)wshadow_mc;
-  a.wshadow_peer = (__nv_bfloat16* const*)wshadow_peer; a.vparams_local = vparams_local; a.vparams_mc = vparams_mc;
-  a.vparams_peer = vparams_peer; a.vgrads_mc = vgrads_mc; a.vgrads_peer = vgrads_peer; a.stage_peer = nullptr;
-  a.arenas = arenas; a.arena_floats = arena_floats; a.sig = sig; a.sig_peer = sig_peer; a.ctrl = (Ctrl2*)ctrl;
-  a.group_counter = group_counter; a.timeout = timeout; a.tstats = tstats; a.inv_w = inv_w;
-  if (grid < 1) grid = 1;
-  if (ntiles > 0 && grid > ntiles) grid = ntiles;
-  v2_ps_entry_kernel<<<grid, EPS_THREADS, 0, stream>>>(a);
+  v2_ps_entry_kernel<<<ps_grid(grid, ntiles), EPS_THREADS, 0, stream>>>(
+      ps_args(units, tiles, tile0, ntiles, W, nranks, group, final_group, owner, master, mom, sq, sqmax, vmom, vsq,
+              vsqmax, wshadow_mc, wshadow_peer, vparams_local, vparams_mc, vparams_peer, vgrads_mc, vgrads_peer,
+              nullptr, arenas, arena_floats, sig, sig_peer, ctrl, group_counter, timeout, tstats, inv_w));
 }
 
 }  // extern "C"

@@ -35,27 +35,9 @@ constexpr int FE_WARPS = FE_THREADS / 32;
 constexpr int FPS_THREADS = 256;
 constexpr int F_TILE_ELEMS = 4096;
 constexpr int F_MAX_BUCKETS = F_TILE_ELEMS / 64;
-constexpr int FST_PART = 5, FST_ACC = 7;     // the partials / accumulator layout of v2_code_stats_kernel
 constexpr unsigned long long FP8_KEY_XOR = 0xF8E43A5C96D1B207ULL;   // codings/fp8.py FP8_KEY_XOR
 constexpr uint32_t FP8_SPECIAL_BITS = 0x7e800000u;   // 2^126: a bucket max at or above it (Inf, NaN) -> scale NaN
 constexpr int FP8_K_MAX = 117;                       // 2^-9 * 2^-117 = 2^-126: decoded values stay fp32 normals
-
-struct FEncArgs {
-  const Unit2* units;
-  const Tile2* tiles;          // already offset to the first tile of the group
-  const long long* gptr;       // gradient base pointers (bf16), one per weight tensor
-  float* const* arena_peer;    // [n_owners] arena base inside each owner
-  int* const* sig_peer;        // [n_owners] signal region base of each owner
-  int n_owners;
-  long long arena_floats;
-  int worker;
-  int group;
-  const Ctrl2* ctrl;
-  unsigned int* group_counter;
-  long long* tstats;
-  int final_group;
-  float* residual;             // error feedback: fp32 residual like wshadow, or nullptr
-};
 
 // scale 2^-k of a bucket from the bits of its largest magnitude: amax 2^k in (224, 448], k <= 117; 0 for an all-zero
 // bucket, NaN for a bucket holding an Inf or NaN or with amax >= 2^126
@@ -111,7 +93,7 @@ __device__ __forceinline__ void fp8_unpack4(uint32_t w, float* f) {
 }
 
 template <bool EF>
-__device__ __forceinline__ void fp8_encode(const FEncArgs& a) {
+__device__ __forceinline__ void fp8_encode(const PushArgs& a) {
   __shared__ unsigned int s_amax[F_MAX_BUCKETS];
   __shared__ float s_scale[F_MAX_BUCKETS];
   const Tile2 t = a.tiles[blockIdx.x];
@@ -204,27 +186,14 @@ __device__ __forceinline__ void fp8_encode(const FEncArgs& a) {
   // ---- the tile's step stamp (after its bytes and scales), then the group's push flag -----------------------
   __syncthreads();
   if (tid == 0) {
-    __threadfence_system();                                   // bytes + scales before the stamp
-    st_release_sys(reinterpret_cast<int*>(slot) + jt, step);
-    __threadfence_system();                                   // the stamp before the counter (and so the push flag)
-    const unsigned int old = atomicAdd(a.group_counter, 1u);
-    if (old == gridDim.x - 1) {
-      *a.group_counter = 0;
-      __threadfence_system();
-      for (int o = 0; o < a.n_owners; ++o)
-        st_release_sys(a.sig_peer[o] + SIG_PUSH + a.group * MAX_WORKERS + a.worker, step);
-      if (a.tstats != nullptr) {
-        const long long now = globaltimer_ns();
-        a.tstats[5] += now - a.tstats[9 + a.group];      // encode of this group
-        if (a.final_group) a.tstats[8] += now - a.tstats[6];          // step start -> last push published
-      }
-    }
+    enc_stamp(reinterpret_cast<int*>(slot), jt, step);
+    enc_push_flag(a, step);
   }
 }
 
-__global__ void __launch_bounds__(FE_THREADS) v2_fp8_encode_kernel(const FEncArgs a) { fp8_encode<false>(a); }
+__global__ void __launch_bounds__(FE_THREADS) v2_fp8_encode_kernel(const PushArgs a) { fp8_encode<false>(a); }
 // error feedback: the same encode plus the residual epilogue
-__global__ void __launch_bounds__(FE_THREADS) v2_fp8_encode_ef_kernel(const FEncArgs a) { fp8_encode<true>(a); }
+__global__ void __launch_bounds__(FE_THREADS) v2_fp8_encode_ef_kernel(const PushArgs a) { fp8_encode<true>(a); }
 
 // ---- PS: decode + sum + optimizer --------------------------------------------------------------------------
 __global__ void __launch_bounds__(FPS_THREADS) v2_ps_fp8_kernel(const PsArgs2 a) {
@@ -235,26 +204,14 @@ __global__ void __launch_bounds__(FPS_THREADS) v2_ps_fp8_kernel(const PsArgs2 a)
   Ctrl2* ctrl = a.ctrl;
   const int step = ctrl->step;
 
-  if (tid == 0) {
-    s_t_enter = globaltimer_ns();
-    unsigned int mask;
-    const bool ok = ps_wait_pushes(a, ctrl, step, mask);
-    if (!ok) atomicOr(&ctrl->error, ERR2_WAIT_PUSH);
-    s_ok = ok ? 1 : 0;
-    s_bad = 0;
-    s_mask = mask;
-    s_t_ready = globaltimer_ns();
-  }
-  __syncthreads();
+  ps_wait(a, ctrl, step, s_ok, s_bad, s_mask, s_t_enter, s_t_ready);
+  // the counted workers stay inline: as a helper they change this kernel's register allocation
   const bool ok = s_ok != 0;
   const unsigned int wmask = s_mask;
   const bool all_workers = wmask == (a.W >= 32 ? 0xffffffffu : ((1u << a.W) - 1u));
   const OptC c = ps_opt_consts(ctrl, step);
   const float inv_w = all_workers ? a.inv_w : 1.f / (float)max(__popc(wmask), 1);
-
-  const int per_cta = (a.ntiles + gridDim.x - 1) / gridDim.x;
-  const int t_begin = blockIdx.x * per_cta;
-  const int t_end = min(a.ntiles, t_begin + per_cta);
+  const auto [t_begin, t_end] = ps_tile_range(a);
   for (int ti = t_begin; ok && ti < t_end; ++ti) {
     const Tile2 t = a.tiles[ti];
     const Unit2 u = a.units[t.unit];
@@ -269,16 +226,7 @@ __global__ void __launch_bounds__(FPS_THREADS) v2_ps_fp8_kernel(const PsArgs2 a)
     const long long soff = qsgd_norms_off(u.n_ps) + kb0;
     const long long boff = 4LL * qsgd_words_off(u.n_ps, u.rows) + (long long)kb0 * 8 * L;   // bytes
     __syncthreads();   // previous tile is done with s_use
-    if (tid == 0) {
-      unsigned int use = 0;
-      for (int w = 0; w < a.W; ++w) {
-        if (!((wmask >> w) & 1u)) continue;
-        const int* stamps = reinterpret_cast<const int*>(a.arenas + (long long)w * a.arena_floats + u.slot_off);
-        if (ld_cg_i(stamps + jt) == step) use |= 1u << w;
-        else s_bad = 1;                                  // stale slot: a push of another step
-      }
-      s_use = use;
-    }
+    if (tid == 0) s_use = ps_fresh_workers(a, u, jt, wmask, step, s_bad);
     __syncthreads();
     const unsigned int use = s_use;
     const long long e0 = u.w_off + t.a;                  // % 64 == 0
@@ -318,21 +266,7 @@ __global__ void __launch_bounds__(FPS_THREADS) v2_ps_fp8_kernel(const PsArgs2 a)
 }
 
 // ---- --code-stats ------------------------------------------------------------------------------------------
-struct FStatArgs {
-  const Unit2* units;
-  const Tile2* tiles;          // already offset to the first tile of the group
-  int tile0;                   // global index of tiles[0] (partials are indexed by global encode tile)
-  const long long* gptr;
-  float* const* arena_peer;    // [n_owners] arena base inside each owner (this worker's scales)
-  int n_owners;
-  long long arena_floats;
-  int worker;
-  double* partials;            // [n_enc_tiles][FST_PART]
-  unsigned int* unit_counters; // [n_fp8_units]
-  double* acc;                 // [n_fp8_units][FST_ACC]
-};
-
-__global__ void __launch_bounds__(FE_THREADS) v2_fp8_code_stats_kernel(const FStatArgs a) {
+__global__ void __launch_bounds__(FE_THREADS) v2_fp8_code_stats_kernel(const ScaleStatArgs a) {
   __shared__ double red[2][FE_WARPS];
   __shared__ float s_scale[F_MAX_BUCKETS];
   __shared__ int s_last;
@@ -371,27 +305,19 @@ __global__ void __launch_bounds__(FE_THREADS) v2_fp8_code_stats_kernel(const FSt
   if (tid == 0) {
     double g = 0.0, m = 0.0;
     for (int w = 0; w < FE_WARPS; ++w) { g += red[0][w]; m += red[1][w]; }
-    double* p = a.partials + (long long)FST_PART * (a.tile0 + blockIdx.x);
-    p[0] = g;
-    p[1] = m;
-    p[2] = (double)t.b;                                   // every element is an atom
-    p[3] = 0.0;
-    p[4] = (double)t.b;
-    __threadfence();
-    const unsigned int old = atomicAdd(&a.unit_counters[u.ts_index], 1u);
-    s_last = (old == (unsigned int)u.n_enc - 1u) ? 1 : 0;
-    if (s_last) a.unit_counters[u.ts_index] = 0;
+    stat_store_tile(a, u, g, m, (double)t.b, 0.0, (double)t.b, s_last);   // every element is an atom
   }
   __syncthreads();
   if (!s_last || tid != 0) return;
+  // the unit's sum stays inline: as a helper it changes this kernel's register allocation
   __threadfence();
-  double sum[FST_PART] = {0.0, 0.0, 0.0, 0.0, 0.0};
+  double sum[STAT_PART] = {0.0, 0.0, 0.0, 0.0, 0.0};
   for (int k = 0; k < u.n_enc; ++k) {                     // tile order: the same bits on every run
-    const double* pk = a.partials + (long long)FST_PART * (u.enc_tile0 + k);
-    for (int f = 0; f < FST_PART; ++f) sum[f] += __ldcg(pk + f);
+    const double* pk = a.partials + (long long)STAT_PART * (u.enc_tile0 + k);
+    for (int f = 0; f < STAT_PART; ++f) sum[f] += __ldcg(pk + f);
   }
-  double* acc = a.acc + (long long)FST_ACC * u.ts_index;
-  for (int f = 0; f < FST_PART; ++f) acc[f] += sum[f];
+  double* acc = a.acc + (long long)STAT_ACC * u.ts_index;
+  for (int f = 0; f < STAT_PART; ++f) acc[f] += sum[f];
   acc[5] += sum[4];
   acc[6] += 1.0;
 }
@@ -403,7 +329,7 @@ void atomo_v2_launch_fp8_encode(const void* units, const void* tiles, int tile0,
                                 int worker, int group, const void* ctrl, unsigned int* group_counter,
                                 long long* tstats, int final_group, float* residual, cudaStream_t stream) {
   if (ntiles <= 0) return;
-  FEncArgs a;
+  PushArgs a;
   a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.gptr = gptr;
   a.arena_peer = arena_peer; a.sig_peer = sig_peer; a.n_owners = n_owners; a.arena_floats = arena_floats;
   a.worker = worker; a.group = group; a.ctrl = (const Ctrl2*)ctrl; a.group_counter = group_counter;
@@ -420,17 +346,10 @@ void atomo_v2_launch_ps_fp8(const void* units, const void* tiles, int tile0, int
                             long long arena_floats, int* sig, int* const* sig_peer, void* ctrl,
                             unsigned int* group_counter, long long timeout, long long* tstats, float inv_w, int grid,
                             cudaStream_t stream) {
-  PsArgs2 a;
-  a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.ntiles = ntiles; a.W = W; a.nranks = nranks;
-  a.group = group; a.final_group = final_group; a.owner = owner; a.master = master; a.mom = mom; a.sq = sq;
-  a.sqmax = sqmax; a.vmom = vmom; a.vsq = vsq; a.vsqmax = vsqmax; a.wshadow_mc = (__nv_bfloat16*)wshadow_mc;
-  a.wshadow_peer = (__nv_bfloat16* const*)wshadow_peer; a.vparams_local = vparams_local; a.vparams_mc = vparams_mc;
-  a.vparams_peer = vparams_peer; a.vgrads_mc = vgrads_mc; a.vgrads_peer = vgrads_peer; a.stage_peer = nullptr;
-  a.arenas = arenas; a.arena_floats = arena_floats; a.sig = sig; a.sig_peer = sig_peer; a.ctrl = (Ctrl2*)ctrl;
-  a.group_counter = group_counter; a.timeout = timeout; a.tstats = tstats; a.inv_w = inv_w;
-  if (grid < 1) grid = 1;
-  if (ntiles > 0 && grid > ntiles) grid = ntiles;
-  v2_ps_fp8_kernel<<<grid, FPS_THREADS, 0, stream>>>(a);
+  v2_ps_fp8_kernel<<<ps_grid(grid, ntiles), FPS_THREADS, 0, stream>>>(
+      ps_args(units, tiles, tile0, ntiles, W, nranks, group, final_group, owner, master, mom, sq, sqmax, vmom, vsq,
+              vsqmax, wshadow_mc, wshadow_peer, vparams_local, vparams_mc, vparams_peer, vgrads_mc, vgrads_peer,
+              nullptr, arenas, arena_floats, sig, sig_peer, ctrl, group_counter, timeout, tstats, inv_w));
 }
 
 void atomo_v2_launch_fp8_code_stats(const void* units, const void* tiles, int tile0, int ntiles,
@@ -438,7 +357,7 @@ void atomo_v2_launch_fp8_code_stats(const void* units, const void* tiles, int ti
                                     long long arena_floats, int worker, double* partials, unsigned int* unit_counters,
                                     double* acc, cudaStream_t stream) {
   if (ntiles <= 0) return;
-  FStatArgs a;
+  ScaleStatArgs a;
   a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.tile0 = tile0; a.gptr = gptr;
   a.arena_peer = arena_peer; a.n_owners = n_owners; a.arena_floats = arena_floats; a.worker = worker;
   a.partials = partials; a.unit_counters = unit_counters; a.acc = acc;

@@ -37,7 +37,6 @@ namespace v2 {
 constexpr int HD_THREADS = 256;
 constexpr int HD_WARPS = HD_THREADS / 32;
 constexpr int HD_TILE = 16 * HD_THREADS;                              // 4096 elements: the largest tile
-constexpr int HST_PART = 5, HST_ACC = 7;     // the partials / accumulator layout of v2_code_stats_kernel
 constexpr unsigned long long HD_ROT_KEY = 0x48D2A7E13B5C9F61ULL;     // codings/hadamard.py HADAMARD_ROT_KEY
 constexpr unsigned long long HD_Q_KEY = 0x7C1E94B2D58A3F0DULL;       // codings/hadamard.py HADAMARD_Q_KEY
 constexpr float HD_FLT_MIN = 0x1p-126f;
@@ -248,25 +247,8 @@ __device__ __forceinline__ void hd_load_codes(const unsigned char* p, int bits, 
 // 2^-log2(d), exact
 __device__ __forceinline__ float hd_inv_d(int d) { return __uint_as_float((uint32_t)(127 - (31 - __clz(d))) << 23); }
 
-struct HEncArgs {
-  const Unit2* units;
-  const Tile2* tiles;          // already offset to the first tile of the group
-  const long long* gptr;       // gradient base pointers (bf16), one per weight tensor
-  float* const* arena_peer;    // [n_owners] arena base inside each owner
-  int* const* sig_peer;        // [n_owners] signal region base of each owner
-  int n_owners;
-  long long arena_floats;
-  int worker;
-  int group;
-  const Ctrl2* ctrl;
-  unsigned int* group_counter;
-  long long* tstats;
-  int final_group;
-  float* residual;             // error feedback: fp32 residual like wshadow, or nullptr
-};
-
 template <bool EF>
-__device__ __forceinline__ void hadamard_encode(const HEncArgs& a) {
+__device__ __forceinline__ void hadamard_encode(const PushArgs& a) {
   __shared__ __align__(16) HdShared sm;
   const Tile2 t = a.tiles[blockIdx.x];
   const Unit2 u = a.units[t.unit];
@@ -344,27 +326,14 @@ __device__ __forceinline__ void hadamard_encode(const HEncArgs& a) {
   // ---- the tile's step stamp (after its codes and ranges), then the group's push flag ------------------------
   __syncthreads();
   if (tid == 0) {
-    __threadfence_system();                                   // codes + ranges before the stamp
-    st_release_sys(reinterpret_cast<int*>(slot) + jt, step);
-    __threadfence_system();                                   // the stamp before the counter (and so the push flag)
-    const unsigned int old = atomicAdd(a.group_counter, 1u);
-    if (old == gridDim.x - 1) {
-      *a.group_counter = 0;
-      __threadfence_system();
-      for (int o = 0; o < a.n_owners; ++o)
-        st_release_sys(a.sig_peer[o] + SIG_PUSH + a.group * MAX_WORKERS + a.worker, step);
-      if (a.tstats != nullptr) {
-        const long long now = globaltimer_ns();
-        a.tstats[5] += now - a.tstats[9 + a.group];      // encode of this group
-        if (a.final_group) a.tstats[8] += now - a.tstats[6];          // step start -> last push published
-      }
-    }
+    enc_stamp(reinterpret_cast<int*>(slot), jt, step);
+    enc_push_flag(a, step);
   }
 }
 
-__global__ void __launch_bounds__(HD_THREADS) v2_hadamard_encode_kernel(const HEncArgs a) { hadamard_encode<false>(a); }
+__global__ void __launch_bounds__(HD_THREADS) v2_hadamard_encode_kernel(const PushArgs a) { hadamard_encode<false>(a); }
 // error feedback: the same encode plus the residual epilogue
-__global__ void __launch_bounds__(HD_THREADS, 1) v2_hadamard_encode_ef_kernel(const HEncArgs a) {
+__global__ void __launch_bounds__(HD_THREADS, 1) v2_hadamard_encode_ef_kernel(const PushArgs a) {
   hadamard_encode<true>(a);
 }
 
@@ -378,27 +347,15 @@ __global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_kernel(const PsA
   Ctrl2* ctrl = a.ctrl;
   const int step = ctrl->step;
 
-  if (tid == 0) {
-    s_t_enter = globaltimer_ns();
-    unsigned int mask;
-    const bool ok = ps_wait_pushes(a, ctrl, step, mask);
-    if (!ok) atomicOr(&ctrl->error, ERR2_WAIT_PUSH);
-    s_ok = ok ? 1 : 0;
-    s_bad = 0;
-    s_mask = mask;
-    s_t_ready = globaltimer_ns();
-  }
-  __syncthreads();
+  ps_wait(a, ctrl, step, s_ok, s_bad, s_mask, s_t_enter, s_t_ready);
+  // the counted workers stay inline: as a helper they change this kernel's register allocation
   const bool ok = s_ok != 0;
   const unsigned int wmask = s_mask;
   const bool all_workers = wmask == (a.W >= 32 ? 0xffffffffu : ((1u << a.W) - 1u));
   const OptC c = ps_opt_consts(ctrl, step);
   const float inv_w = all_workers ? a.inv_w : 1.f / (float)max(__popc(wmask), 1);
   const unsigned long long seed = ctrl->seed;
-
-  const int per_cta = (a.ntiles + gridDim.x - 1) / gridDim.x;
-  const int t_begin = blockIdx.x * per_cta;
-  const int t_end = min(a.ntiles, t_begin + per_cta);
+  const auto [t_begin, t_end] = ps_tile_range(a);
   for (int ti = t_begin; ok && ti < t_end; ++ti) {
     const Tile2 t = a.tiles[ti];
     const Unit2 u = a.units[t.unit];
@@ -416,16 +373,7 @@ __global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_kernel(const PsA
     const long long poff = hd_params_off(u.n_ps) + 2LL * (kb0 + kb);
     const long long boff = 4LL * hd_words_off(u.n_ps, u.rows) + e0 * bits / 8;   // bytes
     __syncthreads();   // previous tile is done with s_use
-    if (tid == 0) {
-      unsigned int use = 0;
-      for (int w = 0; w < a.W; ++w) {
-        if (!((wmask >> w) & 1u)) continue;
-        const int* stamps = reinterpret_cast<const int*>(a.arenas + (long long)w * a.arena_floats + u.slot_off);
-        if (ld_cg_i(stamps + jt) == step) use |= 1u << w;
-        else s_bad = 1;                                  // stale slot: a push of another step
-      }
-      s_use = use;
-    }
+    if (tid == 0) s_use = ps_fresh_workers(a, u, jt, wmask, step, s_bad);
     __syncthreads();
     const unsigned int use = s_use;
     float g[16];
@@ -477,9 +425,9 @@ struct HStatArgs {
   long long arena_floats;
   int worker;
   const Ctrl2* ctrl;
-  double* partials;            // [n_enc_tiles][HST_PART]
+  double* partials;            // [n_enc_tiles][STAT_PART]
   unsigned int* unit_counters; // [n_hadamard_units]
-  double* acc;                 // [n_hadamard_units][HST_ACC]
+  double* acc;                 // [n_hadamard_units][STAT_ACC]
 };
 
 __global__ void __launch_bounds__(HD_THREADS) v2_hadamard_code_stats_kernel(const HStatArgs a) {
@@ -528,29 +476,13 @@ __global__ void __launch_bounds__(HD_THREADS) v2_hadamard_code_stats_kernel(cons
   if (tid == 0) {
     double g = 0.0, m = 0.0;
     for (int w = 0; w < HD_WARPS; ++w) { g += red[0][w]; m += red[1][w]; }
-    double* p = a.partials + (long long)HST_PART * (a.tile0 + blockIdx.x);
-    p[0] = g;
-    p[1] = m;
-    p[2] = (double)t.b;                                   // every element is an atom
-    p[3] = 0.0;
-    p[4] = (double)t.b;
-    __threadfence();
-    const unsigned int old = atomicAdd(&a.unit_counters[u.ts_index], 1u);
-    s_last = (old == (unsigned int)u.n_enc - 1u) ? 1 : 0;
-    if (s_last) a.unit_counters[u.ts_index] = 0;
+    stat_store_tile(a, u, g, m, (double)t.b, 0.0, (double)t.b, s_last);   // every element is an atom
   }
   __syncthreads();
   if (!s_last || tid != 0) return;
-  __threadfence();
-  double sum[HST_PART] = {0.0, 0.0, 0.0, 0.0, 0.0};
-  for (int k = 0; k < u.n_enc; ++k) {                     // tile order: the same bits on every run
-    const double* pk = a.partials + (long long)HST_PART * (u.enc_tile0 + k);
-    for (int f = 0; f < HST_PART; ++f) sum[f] += __ldcg(pk + f);
-  }
-  double* acc = a.acc + (long long)HST_ACC * u.ts_index;
-  for (int f = 0; f < HST_PART; ++f) acc[f] += sum[f];
-  acc[5] += sum[4];
-  acc[6] += 1.0;
+  double sum[STAT_PART];
+  stat_unit_sum(a, u, sum);
+  stat_accumulate(a, u, sum);
 }
 
 extern "C" {
@@ -561,7 +493,7 @@ void atomo_v2_launch_hadamard_encode(const void* units, const void* tiles, int t
                                      unsigned int* group_counter, long long* tstats, int final_group, float* residual,
                                      cudaStream_t stream) {
   if (ntiles <= 0) return;
-  HEncArgs a;
+  PushArgs a;
   a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.gptr = gptr;
   a.arena_peer = arena_peer; a.sig_peer = sig_peer; a.n_owners = n_owners; a.arena_floats = arena_floats;
   a.worker = worker; a.group = group; a.ctrl = (const Ctrl2*)ctrl; a.group_counter = group_counter;
@@ -578,17 +510,10 @@ void atomo_v2_launch_ps_hadamard(const void* units, const void* tiles, int tile0
                                  const float* arenas, long long arena_floats, int* sig, int* const* sig_peer,
                                  void* ctrl, unsigned int* group_counter, long long timeout, long long* tstats,
                                  float inv_w, int grid, cudaStream_t stream) {
-  PsArgs2 a;
-  a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.ntiles = ntiles; a.W = W; a.nranks = nranks;
-  a.group = group; a.final_group = final_group; a.owner = owner; a.master = master; a.mom = mom; a.sq = sq;
-  a.sqmax = sqmax; a.vmom = vmom; a.vsq = vsq; a.vsqmax = vsqmax; a.wshadow_mc = (__nv_bfloat16*)wshadow_mc;
-  a.wshadow_peer = (__nv_bfloat16* const*)wshadow_peer; a.vparams_local = vparams_local; a.vparams_mc = vparams_mc;
-  a.vparams_peer = vparams_peer; a.vgrads_mc = vgrads_mc; a.vgrads_peer = vgrads_peer; a.stage_peer = nullptr;
-  a.arenas = arenas; a.arena_floats = arena_floats; a.sig = sig; a.sig_peer = sig_peer; a.ctrl = (Ctrl2*)ctrl;
-  a.group_counter = group_counter; a.timeout = timeout; a.tstats = tstats; a.inv_w = inv_w;
-  if (grid < 1) grid = 1;
-  if (ntiles > 0 && grid > ntiles) grid = ntiles;
-  v2_ps_hadamard_kernel<<<grid, HD_THREADS, 0, stream>>>(a);
+  v2_ps_hadamard_kernel<<<ps_grid(grid, ntiles), HD_THREADS, 0, stream>>>(
+      ps_args(units, tiles, tile0, ntiles, W, nranks, group, final_group, owner, master, mom, sq, sqmax, vmom, vsq,
+              vsqmax, wshadow_mc, wshadow_peer, vparams_local, vparams_mc, vparams_peer, vgrads_mc, vgrads_peer,
+              nullptr, arenas, arena_floats, sig, sig_peer, ctrl, group_counter, timeout, tstats, inv_w));
 }
 
 void atomo_v2_launch_hadamard_code_stats(const void* units, const void* tiles, int tile0, int ntiles,

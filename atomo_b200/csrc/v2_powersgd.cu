@@ -41,7 +41,6 @@ constexpr int PW_COL_BLOCK = 256;
 constexpr int PW_PS_ROWS = 4;
 constexpr int PW_GRAM = 16;
 constexpr int PW_PH_CHUNK = 512;          // P_hat rows staged per round of pass B
-constexpr int PW_STAT_PART = 5, PW_STAT_ACC = 7;   // the partials / accumulator layout of v2_code_stats_kernel
 constexpr double PW_PIVOT_RTOL = 1e-12;
 constexpr unsigned long long PW_KEY_XOR = 0x70C5D1A3B2E49F17ULL;
 
@@ -361,21 +360,7 @@ __global__ void __launch_bounds__(PW_THREADS, 1) v2_powersgd_encode_b_kernel(con
     __syncthreads();
   }
   // ---- the group's push flag -----------------------------------------------------------------------------------
-  if (tid == 0) {
-    __threadfence_system();                                   // factors and stamps before the counter / push flag
-    const unsigned int old = atomicAdd(a.group_counter, 1u);
-    if (old == gridDim.x - 1) {
-      *a.group_counter = 0;
-      __threadfence_system();
-      for (int o = 0; o < a.n_owners; ++o)
-        st_release_sys(a.sig_peer[o] + SIG_PUSH + a.group * MAX_WORKERS + a.worker, step);
-      if (a.tstats != nullptr) {
-        const long long now = globaltimer_ns();
-        a.tstats[5] += now - a.tstats[9 + a.group];      // encode of this group
-        if (a.final_group) a.tstats[8] += now - a.tstats[6];          // step start -> last push published
-      }
-    }
-  }
+  if (tid == 0) enc_push_flag(a, step);                      // factors and stamps before the counter / push flag
 }
 
 // g_hat of 8 columns of row o from this worker's own factors, in the owner's fmaf order (atom order, from 0)
@@ -439,26 +424,14 @@ __global__ void __launch_bounds__(PW_THREADS) v2_ps_powersgd_kernel(const PsArgs
   Ctrl2* ctrl = a.ctrl;
   const int step = ctrl->step;
 
-  if (tid == 0) {
-    s_t_enter = globaltimer_ns();
-    unsigned int mask;
-    const bool ok = ps_wait_pushes(a, ctrl, step, mask);
-    if (!ok) atomicOr(&ctrl->error, ERR2_WAIT_PUSH);
-    s_ok = ok ? 1 : 0;
-    s_bad = 0;
-    s_mask = mask;
-    s_t_ready = globaltimer_ns();
-  }
-  __syncthreads();
+  ps_wait(a, ctrl, step, s_ok, s_bad, s_mask, s_t_enter, s_t_ready);
+  // the counted workers stay inline: as a helper they change this kernel's register allocation
   const bool ok = s_ok != 0;
   const unsigned int wmask = s_mask;
   const bool all_workers = wmask == (a.W >= 32 ? 0xffffffffu : ((1u << a.W) - 1u));
   const OptC c = ps_opt_consts(ctrl, step);
   const float inv_w = all_workers ? a.inv_w : 1.f / (float)max(__popc(wmask), 1);
-
-  const int per_cta = (a.ntiles + gridDim.x - 1) / gridDim.x;
-  const int t_begin = blockIdx.x * per_cta;
-  const int t_end = min(a.ntiles, t_begin + per_cta);
+  const auto [t_begin, t_end] = ps_tile_range(a);
   for (int ti = t_begin; ok && ti < t_end; ++ti) {
     const Tile2 t = a.tiles[ti];
     const Unit2 u = a.units[t.unit];
@@ -476,16 +449,7 @@ __global__ void __launch_bounds__(PW_THREADS) v2_ps_powersgd_kernel(const PsArgs
     const int jt = t.a / u.ps_rows;
     const long long phoff = pw_phat_off(u.n_ps), qoff = pw_q_off(u.n_ps, u.rows, r);
     __syncthreads();   // previous tile is done with sph / s_use
-    if (tid == 0) {
-      unsigned int use = 0;
-      for (int w = 0; w < a.W; ++w) {
-        if (!((wmask >> w) & 1u)) continue;
-        const int* stamps = reinterpret_cast<const int*>(a.arenas + (long long)w * a.arena_floats + u.slot_off);
-        if (ld_cg_i(stamps + jt) == step) use |= 1u << w;
-        else s_bad = 1;                                  // stale slot: a push of another step
-      }
-      s_use = use;
-    }
+    if (tid == 0) s_use = ps_fresh_workers(a, u, jt, wmask, step, s_bad);
     __syncthreads();
     const unsigned int use = s_use;
     for (int idx = tid; idx < MAX_WORKERS * PW_PS_ROWS * PW_MAXR; idx += blockDim.x) {
@@ -563,9 +527,9 @@ struct PwStatArgs {
   const long long* gptr;
   float* scratch;
   const PwState* state;
-  double* partials;            // [n_enc_tiles][PW_STAT_PART]
+  double* partials;            // [n_enc_tiles][STAT_PART]
   unsigned int* unit_counters; // [n_coded]
-  double* acc;                 // [n_coded][PW_STAT_ACC]
+  double* acc;                 // [n_coded][STAT_ACC]
 };
 
 __global__ void __launch_bounds__(PW_THREADS) v2_powersgd_code_stats_kernel(const PwStatArgs a) {
@@ -607,28 +571,21 @@ __global__ void __launch_bounds__(PW_THREADS) v2_powersgd_code_stats_kernel(cons
   if (tid == 0) {
     double g = 0.0, m = 0.0;
     for (int w = 0; w < PW_WARPS; ++w) { g += red[0][w]; m += red[1][w]; }
+    // the non-degenerate columns, counted once per unit
     const double atoms = (t.owner == 0) ? (double)__popc(a.state[u.ts_index].mask) : 0.0;
-    double* p = a.partials + (long long)PW_STAT_PART * (a.tile0 + blockIdx.x);
-    p[0] = g;
-    p[1] = m;
-    p[2] = atoms;                                         // the non-degenerate columns, counted once per unit
-    p[3] = 0.0;
-    p[4] = atoms;
-    __threadfence();
-    const unsigned int old = atomicAdd(&a.unit_counters[u.ts_index], 1u);
-    s_last = (old == (unsigned int)u.n_enc - 1u) ? 1 : 0;
-    if (s_last) a.unit_counters[u.ts_index] = 0;
+    stat_store_tile(a, u, g, m, atoms, 0.0, atoms, s_last);
   }
   __syncthreads();
   if (!s_last || tid != 0) return;
+  // the unit's sum stays inline: as a helper it changes this kernel's register allocation
   __threadfence();
-  double sum[PW_STAT_PART] = {0.0, 0.0, 0.0, 0.0, 0.0};
+  double sum[STAT_PART] = {0.0, 0.0, 0.0, 0.0, 0.0};
   for (int k = 0; k < u.n_enc; ++k) {                     // tile order: the same bits on every run
-    const double* pk = a.partials + (long long)PW_STAT_PART * (u.enc_tile0 + k);
-    for (int f = 0; f < PW_STAT_PART; ++f) sum[f] += __ldcg(pk + f);
+    const double* pk = a.partials + (long long)STAT_PART * (u.enc_tile0 + k);
+    for (int f = 0; f < STAT_PART; ++f) sum[f] += __ldcg(pk + f);
   }
-  double* acc = a.acc + (long long)PW_STAT_ACC * u.ts_index;
-  for (int f = 0; f < PW_STAT_PART; ++f) acc[f] += sum[f];
+  double* acc = a.acc + (long long)STAT_ACC * u.ts_index;
+  for (int f = 0; f < STAT_PART; ++f) acc[f] += sum[f];
   acc[5] += sum[4];
   acc[6] += 1.0;
 }
@@ -683,18 +640,10 @@ void atomo_v2_launch_ps_powersgd(const void* units, const void* tiles, int tile0
                                  const void* const* stage_peer, const float* arenas, long long arena_floats, int* sig,
                                  int* const* sig_peer, void* ctrl, unsigned int* group_counter, long long timeout,
                                  long long* tstats, float inv_w, int grid, cudaStream_t stream) {
-  PsArgs2 a;
-  a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.ntiles = ntiles; a.W = W; a.nranks = nranks;
-  a.group = group; a.final_group = final_group; a.owner = owner; a.master = master; a.mom = mom; a.sq = sq;
-  a.sqmax = sqmax; a.vmom = vmom; a.vsq = vsq; a.vsqmax = vsqmax; a.wshadow_mc = (__nv_bfloat16*)wshadow_mc;
-  a.wshadow_peer = (__nv_bfloat16* const*)wshadow_peer; a.vparams_local = vparams_local; a.vparams_mc = vparams_mc;
-  a.vparams_peer = vparams_peer; a.vgrads_mc = vgrads_mc; a.vgrads_peer = vgrads_peer;
-  a.stage_peer = (const __nv_bfloat16* const*)stage_peer;
-  a.arenas = arenas; a.arena_floats = arena_floats; a.sig = sig; a.sig_peer = sig_peer; a.ctrl = (Ctrl2*)ctrl;
-  a.group_counter = group_counter; a.timeout = timeout; a.tstats = tstats; a.inv_w = inv_w;
-  if (grid < 1) grid = 1;
-  if (ntiles > 0 && grid > ntiles) grid = ntiles;
-  v2_ps_powersgd_kernel<<<grid, PW_THREADS, 0, stream>>>(a);
+  v2_ps_powersgd_kernel<<<ps_grid(grid, ntiles), PW_THREADS, 0, stream>>>(
+      ps_args(units, tiles, tile0, ntiles, W, nranks, group, final_group, owner, master, mom, sq, sqmax, vmom, vsq,
+              vsqmax, wshadow_mc, wshadow_peer, vparams_local, vparams_mc, vparams_peer, vgrads_mc, vgrads_peer,
+              stage_peer, arenas, arena_floats, sig, sig_peer, ctrl, group_counter, timeout, tstats, inv_w));
 }
 
 void atomo_v2_launch_powersgd_code_stats(const void* units, const void* tiles, int tile0, int ntiles,

@@ -353,18 +353,10 @@ void atomo_v2_launch_ps(const void* units, const void* tiles, int tile0, int nti
     cudaFuncSetAttribute(v2_ps_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PS2_SMEM);
     attr = true;
   }
-  PsArgs2 a;
-  a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.ntiles = ntiles; a.W = W; a.nranks = nranks;
-  a.group = group; a.final_group = final_group; a.owner = owner; a.master = master; a.mom = mom; a.sq = sq;
-  a.sqmax = sqmax; a.vmom = vmom; a.vsq = vsq; a.vsqmax = vsqmax; a.wshadow_mc = (__nv_bfloat16*)wshadow_mc;
-  a.wshadow_peer = (__nv_bfloat16* const*)wshadow_peer; a.vparams_local = vparams_local; a.vparams_mc = vparams_mc;
-  a.vparams_peer = vparams_peer; a.vgrads_mc = vgrads_mc; a.vgrads_peer = vgrads_peer;
-  a.stage_peer = (const __nv_bfloat16* const*)stage_peer; a.arenas = arenas; a.arena_floats = arena_floats;
-  a.sig = sig; a.sig_peer = sig_peer; a.ctrl = (Ctrl2*)ctrl; a.group_counter = group_counter; a.timeout = timeout;
-  a.tstats = tstats; a.inv_w = inv_w;
-  if (grid < 1) grid = 1;
-  if (ntiles > 0 && grid > ntiles) grid = ntiles;
-  v2_ps_kernel<<<grid, PS2_THREADS, PS2_SMEM, stream>>>(a);
+  v2_ps_kernel<<<ps_grid(grid, ntiles), PS2_THREADS, PS2_SMEM, stream>>>(
+      ps_args(units, tiles, tile0, ntiles, W, nranks, group, final_group, owner, master, mom, sq, sqmax, vmom, vsq,
+              vsqmax, wshadow_mc, wshadow_peer, vparams_local, vparams_mc, vparams_peer, vgrads_mc, vgrads_peer,
+              stage_peer, arenas, arena_floats, sig, sig_peer, ctrl, group_counter, timeout, tstats, inv_w));
 }
 
 void atomo_v2_launch_wait_params(const int* sig, int n_owners, void* ctrl, long long timeout, long long* tstats,

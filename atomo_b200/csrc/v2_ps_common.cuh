@@ -1,6 +1,8 @@
 // Parameter-server building blocks shared by the PS kernels of the overlapped / sharded engine: the launch
-// arguments, the push wait with the --num-aggregate mask, the fp32 vector tiles and the fused optimizer epilogue
-// with its bf16 broadcast.  v2_ps.cu (spectral / dense tiles) and v2_qsgd.cu (quantized tiles) both use them.
+// arguments, the push wait with the --num-aggregate mask and the prologue around it, the stale-slot check, the fp32
+// vector and dense bf16 tiles, the fused optimizer epilogue with its bf16 broadcast, the completion, and the host
+// packing of the launch arguments.  Every v2_ps*_kernel uses them (v2_ps.cu, v2_qsgd.cu, v2_entrywise.cu, v2_sign.cu,
+// v2_fp8.cu, v2_hadamard.cu, v2_powersgd.cu); v2_ps_kernel keeps its own copies where noted.
 #pragma once
 #include "v2_common.cuh"
 
@@ -171,6 +173,58 @@ __device__ __forceinline__ bool ps_wait_pushes(const PsArgs2& a, const Ctrl2* ct
   return ok;
 }
 
+// ---- PS prologue: thread 0 waits for the pushes, then every thread reads the outcome -----------------------------
+// ok / bad / mask are the CTA's shared flags; t_enter / t_ready are thread 0's timings (shared or registers).
+__device__ __forceinline__ void ps_wait(const PsArgs2& a, Ctrl2* ctrl, int step, int& s_ok, int& s_bad,
+                                        unsigned int& s_mask, long long& t_enter, long long& t_ready) {
+  if (threadIdx.x == 0) {
+    t_enter = globaltimer_ns();
+    unsigned int mask;
+    const bool ok = ps_wait_pushes(a, ctrl, step, mask);
+    if (!ok) atomicOr(&ctrl->error, ERR2_WAIT_PUSH);
+    s_ok = ok ? 1 : 0;
+    s_bad = 0;
+    s_mask = mask;
+    t_ready = globaltimer_ns();
+  }
+  __syncthreads();
+}
+
+// The CTA's range of tiles [t_begin, t_end): consecutive tiles, the same count per CTA but for the last.
+struct PsTiles {
+  int t_begin, t_end;
+};
+
+__device__ __forceinline__ PsTiles ps_tile_range(const PsArgs2& a) {
+  const int per_cta = (a.ntiles + gridDim.x - 1) / gridDim.x;
+  PsTiles r;
+  r.t_begin = blockIdx.x * per_cta;
+  r.t_end = min(a.ntiles, r.t_begin + per_cta);
+  return r;
+}
+
+// ---- stale-slot check (thread 0, per tile): the counted workers whose stamp for the tile, stamp_of(w), is this
+// step; any other stamp is a push of another step and sets `bad` (ERR2_SLOT_STEP in ps_complete).
+template <class StampOf>
+__device__ __forceinline__ unsigned int ps_fresh_workers(const PsArgs2& a, unsigned int wmask, int step, int& bad,
+                                                         StampOf stamp_of) {
+  unsigned int use = 0;
+  for (int w = 0; w < a.W; ++w) {
+    if (!((wmask >> w) & 1u)) continue;
+    if (ld_cg_i(stamp_of(w)) == step) use |= 1u << w;
+    else bad = 1;
+  }
+  return use;
+}
+
+// ... for the slots that start with one int32 stamp per PS tile (QSGD, sign, fp8, hadamard, powersgd): stamp jt
+__device__ __forceinline__ unsigned int ps_fresh_workers(const PsArgs2& a, const Unit2& u, int jt, unsigned int wmask,
+                                                         int step, int& bad) {
+  return ps_fresh_workers(a, wmask, step, bad, [&](int w) {
+    return reinterpret_cast<const int*>(a.arenas + (long long)w * a.arena_floats + u.slot_off) + jt;
+  });
+}
+
 __device__ __forceinline__ OptC ps_opt_consts(const Ctrl2* ctrl, int step) {
   OptC c;
   c.lr = ctrl->lr; c.mu = ctrl->momentum; c.damp = ctrl->dampening; c.wd = ctrl->weight_decay;
@@ -290,6 +344,33 @@ __device__ __forceinline__ void ps_complete(const PsArgs2& a, Ctrl2* ctrl, int s
       if (a.final_group) a.tstats[7] += now - a.tstats[6];   // step start -> this owner's parameters published
     }
   }
+}
+
+// ---- host: the arguments of a PS launch (the atomo_v2_launch_ps* parameters, in order) and its grid ------------
+inline PsArgs2 ps_args(const void* units, const void* tiles, int tile0, int ntiles, int W, int nranks, int group,
+                       int final_group, int owner, float* master, float* mom, float* sq, float* sqmax, float* vmom,
+                       float* vsq, float* vsqmax, void* wshadow_mc, void* const* wshadow_peer, float* vparams_local,
+                       float* vparams_mc, float* const* vparams_peer, const float* vgrads_mc,
+                       const float* const* vgrads_peer, const void* const* stage_peer, const float* arenas,
+                       long long arena_floats, int* sig, int* const* sig_peer, void* ctrl,
+                       unsigned int* group_counter, long long timeout, long long* tstats, float inv_w) {
+  PsArgs2 a;
+  a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.ntiles = ntiles; a.W = W; a.nranks = nranks;
+  a.group = group; a.final_group = final_group; a.owner = owner; a.master = master; a.mom = mom; a.sq = sq;
+  a.sqmax = sqmax; a.vmom = vmom; a.vsq = vsq; a.vsqmax = vsqmax; a.wshadow_mc = (__nv_bfloat16*)wshadow_mc;
+  a.wshadow_peer = (__nv_bfloat16* const*)wshadow_peer; a.vparams_local = vparams_local; a.vparams_mc = vparams_mc;
+  a.vparams_peer = vparams_peer; a.vgrads_mc = vgrads_mc; a.vgrads_peer = vgrads_peer;
+  a.stage_peer = (const __nv_bfloat16* const*)stage_peer; a.arenas = arenas; a.arena_floats = arena_floats;
+  a.sig = sig; a.sig_peer = sig_peer; a.ctrl = (Ctrl2*)ctrl; a.group_counter = group_counter; a.timeout = timeout;
+  a.tstats = tstats; a.inv_w = inv_w;
+  return a;
+}
+
+// at least one CTA, at most one per tile
+inline int ps_grid(int grid, int ntiles) {
+  if (grid < 1) grid = 1;
+  if (ntiles > 0 && grid > ntiles) grid = ntiles;
+  return grid;
 }
 
 }  // namespace v2

@@ -193,21 +193,8 @@ __device__ __forceinline__ void qsgd_encode(const QEncArgs& a) {
   // ---- the tile's step stamp (after its words and norms), then the group's push flag ----------------------
   __syncthreads();
   if (tid == 0) {
-    __threadfence_system();                                   // words + norms before the stamp
-    st_release_sys(reinterpret_cast<int*>(slot) + jt, step);
-    __threadfence_system();                                   // the stamp before the counter (and so the push flag)
-    const unsigned int old = atomicAdd(a.group_counter, 1u);
-    if (old == gridDim.x - 1) {
-      *a.group_counter = 0;
-      __threadfence_system();
-      for (int o = 0; o < a.n_owners; ++o)
-        st_release_sys(a.sig_peer[o] + SIG_PUSH + a.group * MAX_WORKERS + a.worker, step);
-      if (a.tstats != nullptr) {
-        const long long now = globaltimer_ns();
-        a.tstats[5] += now - a.tstats[9 + a.group];      // encode of this group
-        if (a.final_group) a.tstats[8] += now - a.tstats[6];          // step start -> last push published
-      }
-    }
+    enc_stamp(reinterpret_cast<int*>(slot), jt, step);
+    enc_push_flag(a, step);
   }
 }
 
@@ -288,26 +275,14 @@ __global__ void __launch_bounds__(QPS_THREADS) v2_ps_qsgd_kernel(const PsArgs2 a
   const int step = ctrl->step;
 
   long long t_enter = 0, t_ready = 0;
-  if (tid == 0) {
-    t_enter = globaltimer_ns();
-    unsigned int mask;
-    const bool ok = ps_wait_pushes(a, ctrl, step, mask);
-    if (!ok) atomicOr(&ctrl->error, ERR2_WAIT_PUSH);
-    s_ok = ok ? 1 : 0;
-    s_bad = 0;
-    s_mask = mask;
-    t_ready = globaltimer_ns();
-  }
-  __syncthreads();
+  ps_wait(a, ctrl, step, s_ok, s_bad, s_mask, t_enter, t_ready);
+  // the counted workers stay inline: as a helper they change this kernel's register allocation
   const bool ok = s_ok != 0;
   const unsigned int wmask = s_mask;
   const bool all_workers = wmask == (a.W >= 32 ? 0xffffffffu : ((1u << a.W) - 1u));
   const OptC c = ps_opt_consts(ctrl, step);
   const float inv_w = all_workers ? a.inv_w : 1.f / (float)max(__popc(wmask), 1);
-
-  const int per_cta = (a.ntiles + gridDim.x - 1) / gridDim.x;
-  const int t_begin = blockIdx.x * per_cta;
-  const int t_end = min(a.ntiles, t_begin + per_cta);
+  const auto [t_begin, t_end] = ps_tile_range(a);
   for (int ti = t_begin; ok && ti < t_end; ++ti) {
     const Tile2 t = a.tiles[ti];
     const Unit2 u = a.units[t.unit];
@@ -324,16 +299,7 @@ __global__ void __launch_bounds__(QPS_THREADS) v2_ps_qsgd_kernel(const PsArgs2 a
     const int jt = kb0 / u.cs;
     const long long noff = qsgd_norms_off(u.n_ps), woff = qsgd_words_off(u.n_ps, u.rows);
     __syncthreads();   // previous tile is done with OUT / s_use
-    if (tid == 0) {
-      unsigned int use = 0;
-      for (int w = 0; w < a.W; ++w) {
-        if (!((wmask >> w) & 1u)) continue;
-        const int* stamps = reinterpret_cast<const int*>(a.arenas + (long long)w * a.arena_floats + u.slot_off);
-        if (ld_cg_i(stamps + jt) == step) use |= 1u << w;
-        else s_bad = 1;                                  // stale slot: a push of another step
-      }
-      s_use = use;
-    }
+    if (tid == 0) s_use = ps_fresh_workers(a, u, jt, wmask, step, s_bad);
     for (int i = tid; i < t.b; i += blockDim.x) OUT[i] = 0.f;
     __syncthreads();
     const unsigned int use = s_use;
@@ -423,17 +389,10 @@ void atomo_v2_launch_ps_qsgd(const void* units, const void* tiles, int tile0, in
                              long long arena_floats, int* sig, int* const* sig_peer, void* ctrl,
                              unsigned int* group_counter, long long timeout, long long* tstats, float inv_w, int grid,
                              cudaStream_t stream) {
-  PsArgs2 a;
-  a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.ntiles = ntiles; a.W = W; a.nranks = nranks;
-  a.group = group; a.final_group = final_group; a.owner = owner; a.master = master; a.mom = mom; a.sq = sq;
-  a.sqmax = sqmax; a.vmom = vmom; a.vsq = vsq; a.vsqmax = vsqmax; a.wshadow_mc = (__nv_bfloat16*)wshadow_mc;
-  a.wshadow_peer = (__nv_bfloat16* const*)wshadow_peer; a.vparams_local = vparams_local; a.vparams_mc = vparams_mc;
-  a.vparams_peer = vparams_peer; a.vgrads_mc = vgrads_mc; a.vgrads_peer = vgrads_peer; a.stage_peer = nullptr;
-  a.arenas = arenas; a.arena_floats = arena_floats; a.sig = sig; a.sig_peer = sig_peer; a.ctrl = (Ctrl2*)ctrl;
-  a.group_counter = group_counter; a.timeout = timeout; a.tstats = tstats; a.inv_w = inv_w;
-  if (grid < 1) grid = 1;
-  if (ntiles > 0 && grid > ntiles) grid = ntiles;
-  v2_ps_qsgd_kernel<<<grid, QPS_THREADS, 0, stream>>>(a);
+  v2_ps_qsgd_kernel<<<ps_grid(grid, ntiles), QPS_THREADS, 0, stream>>>(
+      ps_args(units, tiles, tile0, ntiles, W, nranks, group, final_group, owner, master, mom, sq, sqmax, vmom, vsq,
+              vsqmax, wshadow_mc, wshadow_peer, vparams_local, vparams_mc, vparams_peer, vgrads_mc, vgrads_peer,
+              nullptr, arenas, arena_floats, sig, sig_peer, ctrl, group_counter, timeout, tstats, inv_w));
 }
 
 }  // extern "C"

@@ -23,8 +23,6 @@ namespace v2 {
 
 constexpr int ST_THREADS = 256;
 constexpr int ST_WARPS = ST_THREADS / 32;
-constexpr int ST_PART = 5;              // per tile: gsq, mse, exp_atoms, bias_sq, realized atoms
-constexpr int ST_ACC = 7;               // per unit: the five sums, realized atoms rounded up to U's groups of 4, steps
 constexpr int ST_MAX_BUCKETS = 4096 / 32;
 
 struct StatArgs {
@@ -41,9 +39,9 @@ struct StatArgs {
   long long arena_floats;
   int worker;
   int random_sample, waterfill;
-  double* partials;            // [n_enc_tiles][ST_PART]
+  double* partials;            // [n_enc_tiles][STAT_PART]
   unsigned int* unit_counters; // [n_coded]
-  double* acc;                 // [n_coded][ST_ACC]
+  double* acc;                 // [n_coded][STAT_ACC]
 };
 
 __device__ __forceinline__ double warp_sum_d(double v) {
@@ -131,7 +129,7 @@ __global__ void __launch_bounds__(ST_THREADS) v2_code_stats_kernel(const StatArg
   if (lane == 0) { red[0][warp] = gsq; red[1][warp] = mse; red[2][warp] = ex; red[3][warp] = bias; }
   __syncthreads();
   if (tid == 0) {
-    double* p = a.partials + (long long)ST_PART * (a.tile0 + blockIdx.x);
+    double* p = a.partials + (long long)STAT_PART * (a.tile0 + blockIdx.x);
     for (int f = 0; f < 4; ++f) {
       double s = 0.0;
       for (int w = 0; w < ST_WARPS; ++w) s += red[f][w];
@@ -145,12 +143,8 @@ __global__ void __launch_bounds__(ST_THREADS) v2_code_stats_kernel(const StatArg
   }
   __syncthreads();
   if (!s_last || tid != 0) return;
-  __threadfence();
-  double sum[ST_PART] = {0.0, 0.0, 0.0, 0.0, 0.0};
-  for (int k = 0; k < u.n_enc; ++k) {
-    const double* pk = a.partials + (long long)ST_PART * (u.enc_tile0 + k);
-    for (int f = 0; f < ST_PART; ++f) sum[f] += __ldcg(pk + f);
-  }
+  double sum[STAT_PART];
+  stat_unit_sum(a, u, sum);
   double real4 = sum[4];
   if (u.kind == KIND_SLAB || u.kind == KIND_MAT) {
     // the sampler's probabilities on the sorted spectrum (order = identity); U is stored in groups of 4 atoms
@@ -180,16 +174,16 @@ __global__ void __launch_bounds__(ST_THREADS) v2_code_stats_kernel(const StatArg
     sum[1] = m; sum[2] = e; sum[4] = (double)cnt;
     real4 = (double)min(u.rcap, (cnt + 3) & ~3);
   }
-  double* acc = a.acc + (long long)ST_ACC * u.ts_index;
-  for (int f = 0; f < ST_PART; ++f) acc[f] += sum[f];
+  double* acc = a.acc + (long long)STAT_ACC * u.ts_index;
+  for (int f = 0; f < STAT_PART; ++f) acc[f] += sum[f];
   acc[5] += real4;
   acc[6] += 1.0;
 }
 
 extern "C" {
 
-int atomo_v2_stats_fields() { return ST_ACC; }
-int atomo_v2_stats_partials() { return ST_PART; }
+int atomo_v2_stats_fields() { return STAT_ACC; }
+int atomo_v2_stats_partials() { return STAT_PART; }
 
 void atomo_v2_launch_code_stats(const void* units, const void* tiles, int tile0, int ntiles, const long long* gptr,
                                 const float* sigma, const int* selcount, const double* l1, const float* clip,

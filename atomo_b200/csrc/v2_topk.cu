@@ -211,11 +211,8 @@ __global__ void __launch_bounds__(EE_THREADS) v2_topk_encode_ef_kernel(const TEn
 }
 
 // ---- --code-stats for top-k units ----------------------------------------------------------------------------
-// The partials / accumulator layout of v2_code_stats_kernel (v2_stats.cu: ST_PART = 5 per tile, ST_ACC = 7 per unit),
-// read by ShadowEngine.code_stats().  gsq = ||bf16(g)||^2; mse = the dropped energy, the entries below T plus the
+// The partials / accumulator layout of every --code-stats kernel (STAT_PART / STAT_ACC, v2_common.cuh).  gsq = ||bf16(g)||^2; mse = the dropped energy, the entries below T plus the
 // tile's dropped ties times T^2 (the convention of svd top-k); expected atoms = k_eff, realized = the header counts.
-constexpr int TK_ST_PART = 5, TK_ST_ACC = 7;
-
 struct TStatArgs {
   const Unit2* units;
   const Tile2* tiles;          // already offset to the first tile of the group
@@ -227,9 +224,9 @@ struct TStatArgs {
   int n_owners;
   long long arena_floats;
   int worker;
-  double* partials;            // [n_enc_tiles][TK_ST_PART]
+  double* partials;            // [n_enc_tiles][STAT_PART]
   unsigned int* unit_counters; // [n_entry_units]
-  double* acc;                 // [n_entry_units][TK_ST_ACC]
+  double* acc;                 // [n_entry_units][STAT_ACC]
 };
 
 __global__ void __launch_bounds__(EE_THREADS) v2_topk_code_stats_kernel(const TStatArgs a) {
@@ -271,7 +268,8 @@ __global__ void __launch_bounds__(EE_THREADS) v2_topk_code_stats_kernel(const TS
     const int ties = T < TOPK_NONE
         ? a.tile_counts[(long long)TOPK_LO_BINS * (a.tile0 + blockIdx.x) + (T & (TOPK_LO_BINS - 1))] : 0;
     const double tv = (double)__uint_as_float((uint32_t)T << 16);
-    double* p = a.partials + (long long)TK_ST_PART * (a.tile0 + blockIdx.x);
+    // the tile's store and the unit's sum stay inline: as helpers they change this kernel's register allocation
+    double* p = a.partials + (long long)STAT_PART * (a.tile0 + blockIdx.x);
     p[0] = g;
     p[1] = m + (double)(ties - (real - ab)) * tv * tv;    // ties not kept
     p[2] = 0.0;
@@ -285,14 +283,14 @@ __global__ void __launch_bounds__(EE_THREADS) v2_topk_code_stats_kernel(const TS
   __syncthreads();
   if (!s_last || tid != 0) return;
   __threadfence();
-  double sum[TK_ST_PART] = {0.0, 0.0, 0.0, 0.0, 0.0};
+  double sum[STAT_PART] = {0.0, 0.0, 0.0, 0.0, 0.0};
   for (int k = 0; k < u.n_enc; ++k) {                     // tile order: the same bits on every run
-    const double* pk = a.partials + (long long)TK_ST_PART * (u.enc_tile0 + k);
-    for (int f = 0; f < TK_ST_PART; ++f) sum[f] += __ldcg(pk + f);
+    const double* pk = a.partials + (long long)STAT_PART * (u.enc_tile0 + k);
+    for (int f = 0; f < STAT_PART; ++f) sum[f] += __ldcg(pk + f);
   }
   sum[2] = (double)st[TK_KEFF];
-  double* acc = a.acc + (long long)TK_ST_ACC * u.ts_index;
-  for (int f = 0; f < TK_ST_PART; ++f) acc[f] += sum[f];
+  double* acc = a.acc + (long long)STAT_ACC * u.ts_index;
+  for (int f = 0; f < STAT_PART; ++f) acc[f] += sum[f];
   acc[5] += sum[4];
   acc[6] += 1.0;
 }
