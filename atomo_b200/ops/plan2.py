@@ -43,6 +43,7 @@ Pure Python (unit-testable on CPU).  Struct layouts mirror ``csrc/v2_common.cuh`
 """
 from __future__ import annotations
 
+import hashlib
 import math
 import struct
 from dataclasses import dataclass, field
@@ -735,6 +736,24 @@ def ef_chunks(plan: "Plan2") -> Tuple[bytes, List[Tuple[int, int]]]:
                             for s in range(0, q.numel, EF_CHUNK_ELEMS))
         ranges.append((first, len(rows) - first))
     return b"".join(struct.pack(EF_CHUNK_FMT, o, w, s, c, 0) for o, w, s, c in rows), ranges
+
+
+def pw_warm_ranges(plan: "Plan2") -> List[Tuple[int, int]]:
+    """(float offset, count) in ``gpart`` of every PowerSGD unit's warm ``Q_w^T`` (``[r][round4(C)]``, the last part of
+    its :func:`pw_scratch_floats` from ``gpart_off``), in unit order.  The rest of ``gpart`` is rewritten every step
+    before it is read; ``Q_w`` is what a step hands to the next."""
+    out = []
+    for u in plan.units:
+        if u.kind == KIND_POWER:
+            n = u.rcap * _round_up(u.cols, 4)
+            out.append((u.gpart_off + pw_scratch_floats(u.rows, u.cols, u.rcap) - n, n))
+    return out
+
+
+def plan_digest(plan: "Plan2") -> str:
+    """SHA-256 of the packed unit table: it changes with the shapes, code, rank, buckets, bits, budget, groups and
+    owners, i.e. with anything that moves a unit's per-worker state."""
+    return hashlib.sha256(plan.units_bytes()).hexdigest()
 
 
 OPT_SGD, OPT_ADAM, OPT_AMSGRAD = 0, 1, 2

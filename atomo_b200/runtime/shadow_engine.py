@@ -38,7 +38,7 @@ one central PS kernel at the end of the step):
   layout) is pushed as a rank-``r`` pair from one power step warm-started by the previous step's right factor
   (``csrc/v2_powersgd.cu``, two encode launches per group); the owners reconstruct ``P_hat Q'^T`` in worker order and
   step the optimizer.  Deterministic, low-rank and biased on its own: a contractive code for ``error_feedback=True``.
-  The warm state is per worker and, like the residuals, not checkpointed: a resumed run draws it afresh.
+  The warm state is per worker and is checkpointed with the residuals (``save_checkpoint``).
 * **FP8** (``code="fp8"``, ``bucket_size``): every weight's buckets are pushed as one e4m3 byte per element and one
   power-of-two fp32 scale in the slots and tiles of sign (``csrc/v2_fp8.cu``, one encode launch per group); each
   scaled magnitude is rounded to one of its two e4m3 neighbours with Philox draws, so the code is unbiased.  The
@@ -51,7 +51,8 @@ one central PS kernel at the end of the step):
 * **Error feedback** (``error_feedback=True``; svd, entrywise, topk, qsgd, sign, powersgd, fp8, hadamard): each worker keeps an fp32 residual ``e`` per
   weight element and codes ``A = g + e``.  An apply launch per group (``csrc/v2_feedback.cu``) writes ``bf16(A)`` into
   autograd's gradient buffer in place and keeps ``A - bf16(A)``; the encoders' epilogues add ``bf16(A) - g_hat``, the
-  part of ``A`` this push did not carry.  Nothing is discarded, only delayed.
+  part of ``A`` this push did not carry.  Nothing is discarded, only delayed.  Each worker checkpoints its residual
+  and warm-start state in ``model_step_<N>_worker<R>`` (``save_checkpoint``), so a resume continues bit for bit.
 * Optimizers fused in the PS epilogue: momentum-SGD (``src/optim/sgd.py:57-90``), Adam / AMSGrad
   (``src/optim/adam.py:37-94``).
 
@@ -296,15 +297,12 @@ class ShadowEngine:
         self.selcount = torch.zeros(nc, dtype=torch.int32, device=dev)
         self.sigma = z(nc * P2.MAX_COLS)
         # eigenbasis of the previous step per coded unit (Jacobi warm start); identity to begin with
+        self.warm_start = bool(warm_start)
         self.max_sweeps = int(max_sweeps) if warm_start else 0
         self.vprev = None
         if warm_start and not self.quant and not self.entry and not self.sign and not self.power and not self.fp8 \
                 and not self.hadamard:
-            self.vprev = z(nc * P2.MAX_COLS * P2.MAX_COLS)
-            for u in pl.units:
-                if u.coded:
-                    o = u.ts_index * P2.MAX_COLS * P2.MAX_COLS
-                    self.vprev[o:o + u.cols * u.cols].copy_(torch.eye(u.cols, device=dev).reshape(-1))
+            self.vprev = z(nc * P2.MAX_COLS * P2.MAX_COLS)      # set by _fresh_worker_state()
         # QSGD: largest level / bucket of the plan (checked by the bindings), TernGrad clip per unit + its partials
         qunits = [u for u in pl.units if u.kind == P2.KIND_QSGD]
         self.q_max_level = max((u.I for u in qunits), default=0)
@@ -341,8 +339,6 @@ class ShadowEngine:
                                              beta1=betas[0], beta2=betas[1], eps=eps, opt=self.opt,
                                              num_aggregate=num_aggregate), dev)
         self.ctrl_i32, self.ctrl_f32 = self.ctrl.view(torch.int32), self.ctrl.view(torch.float32)
-        if self.power and self.is_worker:       # the warm state's first draw (Philox keyed by seed, unit, column)
-            C.v2_powersgd_init(self.t_units.data_ptr(), len(pl.units), self.gpart.data_ptr(), self.ctrl.data_ptr())
         n_w = max(len(self.w_params), 1)
         self.t_gptr = torch.zeros(n_w, dtype=torch.int64, device=dev)
         self.host_gptr = np.zeros(n_w, dtype=np.int64)
@@ -375,6 +371,8 @@ class ShadowEngine:
             self.residual = z(pl.w_total)
             chunks, self.ef_range = P2.ef_chunks(pl)
             self.t_ef_chunks = _dev_bytes(chunks, dev)
+        self.pw_warm = P2.pw_warm_ranges(pl) if self.power else []     # Q_w inside gpart (checkpointed)
+        self._fresh_worker_state()
         self.loss_buf = torch.zeros(3, dtype=torch.float32, device=dev)
         self.static_x = self.static_y = self.graph = None
 
@@ -404,6 +402,22 @@ class ShadowEngine:
         self._initial_sync()
 
     # ------------------------------------------------------------------------------------------------------
+    def _fresh_worker_state(self):
+        """Per-worker state as a new run starts it: residual ``e = 0``, the identity as the Jacobi warm start, and
+        PowerSGD's first draw of ``Q_w`` (Philox keyed by seed, unit, column) with a cleared unit state."""
+        if self.residual is not None:
+            self.residual.zero_()
+        if self.vprev is not None:
+            self.vprev.zero_()
+            for u in self.plan.units:
+                if u.coded:
+                    o = u.ts_index * P2.MAX_COLS * P2.MAX_COLS
+                    self.vprev[o:o + u.cols * u.cols].copy_(torch.eye(u.cols, device=self.device).reshape(-1))
+        if self.power and self.is_worker:
+            self.pw_state.zero_()
+            self.C.v2_powersgd_init(self.t_units.data_ptr(), len(self.plan.units), self.gpart.data_ptr(),
+                                    self.ctrl.data_ptr())
+
     def _barrier(self):
         torch.cuda.synchronize(self.device)
         if self.world > 1:
@@ -933,10 +947,32 @@ class ShadowEngine:
         return sd
 
     def save_checkpoint(self, train_dir: str, step: Optional[int] = None) -> Optional[str]:
-        """Collective.  The first training rank writes ``model_step_<N>`` (fp32, trained BN statistics) and the
-        ``_optim`` sidecar (momentum — for Adam / AMSGrad also the second moments —, step, LR) so a later run can
-        resume.  Error-feedback residuals are per-worker state and are not written: a resumed run starts from
-        ``e = 0``.  Nor is PowerSGD's warm ``Q_w``: a resumed run draws it afresh."""
+        """Collective.  Every training rank ``R`` writes ``model_step_<N>_worker<R>`` (its own state, below); after a
+        barrier the first training rank writes ``model_step_<N>`` (fp32, trained BN statistics) and the ``_optim``
+        sidecar.  So when the model file exists, its worker files exist too.  After ``load_checkpoint`` on the same
+        configuration, training continues bit for bit as if it had never stopped.
+
+        Every device buffer the engine keeps across steps is in one of these classes:
+
+        (a) owner state and BN buffers, in ``model_step_<N>`` / ``_optim``: ``master`` (``wshadow`` is rebuilt from
+            it as ``bf16(master)``, what the PS epilogue publishes), ``vparams``, ``mom`` / ``vmom``, for Adam
+            ``sq`` / ``vsq`` and for AMSGrad ``sqmax`` / ``vsqmax``, the BN running statistics, and the step and LR
+            of ``ctrl``.
+        (b) per-worker state, in ``model_step_<N>_worker<R>`` (:meth:`_worker_tensors`, physical order):
+            ``residual`` (``error_feedback``, fp32 per weight element); ``vprev`` (svd / qsvd with ``warm_start``,
+            the previous step's Jacobi basis per coded unit); PowerSGD's warm ``Q_w`` (only those ranges of
+            ``gpart``, ``ops/plan2.py`` ``pw_warm_ranges``) and ``pw_state`` (160 bytes per unit: the draw counter
+            carries over; ``R^{-1}``, the mask and the non-finite flag are rewritten by pass A before pass B reads
+            them; its unit counters are zero between launches); the device's default CUDA generator (seed and
+            offset), from which the model's dropout layers draw their masks (VGG's classifier).
+        (c) scratch, rewritten every step before it is read: the rest of ``gpart`` (Gram partials, ``P``,
+            ``P_hat``, ``Q'``), ``vsel``, ``selcount``, ``sigma``, ``clip`` / ``clip_partials``, ``l1`` /
+            ``l1_partials``, ``topk_sel``, ``topk_tiles``, ``pw_gram``, ``stats_partials``, ``vgrads``, ``wstage``,
+            the arena slots (step-stamped), the fused-BN statistics arena, ``loss_buf`` and the input staging; zero
+            between launches by design: ``counters``, ``stats_counters``, ``topk_hist``; ``signals`` carries step
+            stamps, and ``load_checkpoint`` raises the parameter flags to the resumed step.
+        (d) diagnostics that never feed the step, not saved: ``tstats`` (phase timings) and ``stats_acc``
+            (``code_stats`` sums); a resumed run starts them afresh."""
         from ..utils import checkpoint as ckpt
         step = (self.step - 1) if step is None else step
         sd = self.fp32_state_dict()
@@ -955,10 +991,13 @@ class ShadowEngine:
                     dist.all_reduce(vt, group=self.group)
                 adam_state[wname + "_w"] = self.gather_fp32(wname).cpu()
                 adam_state[wname + "_v"] = vt.cpu()
-        if self.rank != self.first_worker:
-            return None
         path = ckpt.model_path(train_dir, step)
         os.makedirs(os.path.dirname(path) or ".", exist_ok=True)
+        if self.is_worker:
+            ckpt.save_worker_state(train_dir, step, self.rank, self._worker_config(), self._worker_tensors())
+        self._barrier()         # every worker file is in place before the model file names this step
+        if self.rank != self.first_worker:
+            return None
         tmp = path + ".tmp"
         torch.save({k: v.cpu() for k, v in sd.items()}, tmp)
         os.replace(tmp, path)
@@ -975,8 +1014,55 @@ class ShadowEngine:
         os.replace(path + "_optim.tmp", path + "_optim")
         return path
 
+    def _worker_config(self) -> dict:
+        """What this worker's state depends on: a worker file is applied only where every field matches."""
+        return {"code": self.code, "plan": P2.plan_digest(self.plan), "error_feedback": self.error_feedback,
+                "warm_start": self.warm_start, "world": self.world, "ps_mode": self.ps_mode,
+                "worker": self.worker_index}
+
+    def _worker_tensors(self) -> dict:
+        """Class (b) of :meth:`save_checkpoint`: this worker's tensors that carry over between steps.  ``pw_qw`` is a
+        gathered copy of the ``Q_w`` ranges of ``gpart`` and ``cuda_rng`` the state of the device's default generator;
+        the others are the engine's own tensors."""
+        out = {}
+        if self.residual is not None:
+            out["residual"] = self.residual
+        if self.vprev is not None:
+            out["vprev"] = self.vprev
+        if self.power:
+            out["pw_qw"] = torch.cat([self.gpart[o:o + n] for o, n in self.pw_warm]) if self.pw_warm else self.gpart[:0]
+            out["pw_state"] = self.pw_state
+        out["cuda_rng"] = torch.cuda.get_rng_state(self.device)     # dropout masks draw from it (VGG's classifier)
+        return out
+
+    def _load_worker_state(self, train_dir: str, step: int) -> bool:
+        """Copy this worker's saved state into the existing tensors (no new allocation: a captured graph keeps its
+        addresses).  A missing or non-matching file leaves the state fresh (:meth:`_fresh_worker_state`), whatever
+        warm-up steps wrote into it, and the CUDA generator where it is; it prints one line."""
+        from ..utils import checkpoint as ckpt
+        state = ckpt.load_worker_state(train_dir, step, self.rank)
+        mine = self._worker_tensors()
+        bad = ["file missing"] if state is None else \
+            ckpt.worker_state_mismatch(state, step, self._worker_config(), mine)
+        if bad:
+            self._fresh_worker_state()
+            print("rank %d: per-worker state of step %d not restored (%s): residuals and warm-start state start fresh"
+                  % (self.rank, step, ", ".join(bad)), flush=True)
+            return False
+        saved = state["tensors"]
+        for name, t in mine.items():
+            if name not in ("pw_qw", "cuda_rng"):
+                t.copy_(saved[name])
+        torch.cuda.set_rng_state(saved["cuda_rng"], self.device)    # a captured graph reads seed and offset at replay
+        i = 0
+        for o, n in self.pw_warm:
+            self.gpart[o:o + n].copy_(saved["pw_qw"][i:i + n])
+            i += n
+        return True
+
     def load_checkpoint(self, train_dir: str, step: int) -> None:
-        """Collective: every rank reads the same files (shared directory) and jumps to ``step + 1``."""
+        """Collective: every rank reads the same files (shared directory) and jumps to ``step + 1``.  Each training
+        rank also restores its own worker file (:meth:`_load_worker_state`)."""
         from ..utils import checkpoint as ckpt
         self._barrier()
         path = ckpt.model_path(train_dir, step)
@@ -1010,6 +1096,8 @@ class ShadowEngine:
                         getattr(self, vname).copy_(side[vname[1:] + "_v"].to(self.device))
                 if side.get("lr") is not None:
                     self.set_lr(float(side["lr"]))
+            if self.is_worker:
+                self._load_worker_state(train_dir, step)
         self.step = step + 1
         self.ctrl_i32[0] = self.step
         self._barrier()
