@@ -217,6 +217,12 @@ void atomo_v2_launch_powersgd_code_stats(const void* units, const void* tiles, i
 int atomo_v2_ef_chunk_bytes();
 void atomo_v2_launch_ef_apply(const void* chunks, int chunk0, int nchunks, const long long* gptr, float* residual,
                               cudaStream_t stream);
+// v2_accum.cu (gradient accumulation of the bf16 engine)
+void atomo_v2_launch_accum_add(const void* wchunks, int nw, const void* vchunks, int nv, const long long* gptr,
+                               float* acc, float* vacc, float* vgrads, int first, cudaStream_t stream);
+void atomo_v2_launch_accum_fold(const void* wchunks, int nw, const void* vchunks, int nv, const long long* gptr,
+                                float* acc, float* vacc, float* vgrads, float inv_n, float* residual,
+                                cudaStream_t stream);
 // v2_stats.cu (estimator statistics of the bf16 engine, --code-stats)
 int atomo_v2_stats_fields();
 int atomo_v2_stats_partials();
@@ -850,6 +856,30 @@ void v2_ef_apply(uint64_t chunks, int chunk0, int nchunks, uint64_t gptr, uint64
                            cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
+// gradient accumulation, micro-batches before the last: acc += g over the weight chunks [0, nw) of `wchunks` (the
+// first micro-batch stores), vacc += vgrads and vgrads = 0 over the vector chunks [0, nv) of `vchunks`
+void v2_accum_add(uint64_t wchunks, int nw, uint64_t vchunks, int nv, uint64_t gptr, uint64_t acc, uint64_t vacc,
+                  uint64_t vgrads, bool first) {
+  TORCH_CHECK(nw >= 0 && nv >= 0, "v2_accum_add: negative chunk count");
+  TORCH_CHECK((nw == 0 || (wchunks != 0 && gptr != 0 && acc != 0)) && (nv == 0 || (vchunks != 0 && vacc != 0 &&
+              vgrads != 0)), "v2_accum_add: chunks / gptr / accumulators required");
+  atomo_v2_launch_accum_add(P<const void>(wchunks), nw, P<const void>(vchunks), nv, P<const long long>(gptr),
+                            P<float>(acc), P<float>(vacc), P<float>(vgrads), first ? 1 : 0, cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+// the last micro-batch, before the group's encode on the same stream: A = (acc + g) * inv_n (+ e with a residual),
+// bf16(A) into the gradient buffers, A - bf16(A) into the residual, acc = 0; vgrads = (vacc + vgrads) * inv_n,
+// vacc = 0
+void v2_accum_fold(uint64_t wchunks, int nw, uint64_t vchunks, int nv, uint64_t gptr, uint64_t acc, uint64_t vacc,
+                   uint64_t vgrads, float inv_n, uint64_t residual) {
+  TORCH_CHECK(nw >= 0 && nv >= 0, "v2_accum_fold: negative chunk count");
+  TORCH_CHECK((nw == 0 || (wchunks != 0 && gptr != 0 && acc != 0)) && (nv == 0 || (vchunks != 0 && vacc != 0 &&
+              vgrads != 0)), "v2_accum_fold: chunks / gptr / accumulators required");
+  atomo_v2_launch_accum_fold(P<const void>(wchunks), nw, P<const void>(vchunks), nv, P<const long long>(gptr),
+                             P<float>(acc), P<float>(vacc), P<float>(vgrads), inv_n, P<float>(residual),
+                             cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
 // estimator statistics of one group: after the group's push, on the same stream
 void v2_code_stats(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t sigma,
                    uint64_t selcount, uint64_t l1, uint64_t clip, uint64_t arena_peer, int n_owners,
@@ -1034,6 +1064,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("v2_powersgd_code_stats", &v2_powersgd_code_stats);
   m.def("v2_ef_apply", &v2_ef_apply);
   m.def("v2_ef_chunk_bytes", &atomo_v2_ef_chunk_bytes);
+  m.def("v2_accum_add", &v2_accum_add);
+  m.def("v2_accum_fold", &v2_accum_fold);
   m.def("v2_ps_entry", &v2_ps_entry);
   m.def("v2_code_stats", &v2_code_stats);
   m.def("v2_stats_fields", &atomo_v2_stats_fields);

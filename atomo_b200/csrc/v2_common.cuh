@@ -303,5 +303,23 @@ __device__ __forceinline__ void stat_accumulate(const Args& a, const Unit2& u, c
   acc[6] += 1.0;
 }
 
+// One chunk of the per-group element passes (error feedback, v2_feedback.cu; gradient accumulation, v2_accum.cu):
+// `count` consecutive elements of weight tensor `widx` from element `start`; the tensor's first element is residual
+// element `w_off` (ops/plan2.py: ef_chunks, the layout is mirrored there).  A vector chunk (plan2.vec_chunks) has
+// widx = -1 and `w_off` its offset in vgrads.
+struct EfChunk {
+  long long w_off;
+  int widx;
+  int start;
+  int count;
+  int pad;
+};
+static_assert(sizeof(EfChunk) == 24, "EfChunk layout must match ops/plan2.py EF_CHUNK_FMT");
+
+__device__ __forceinline__ float ef_round(float a, __nv_bfloat16& b) {
+  b = __float2bfloat16_rn(a);
+  return a - __bfloat162float(b);      // exact: the part of a that bf16 cannot hold
+}
+
 }  // namespace v2
 }  // namespace atomo

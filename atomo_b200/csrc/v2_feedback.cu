@@ -19,22 +19,6 @@ namespace v2 {
 
 constexpr int EF_THREADS = 256;
 
-// One apply chunk: `count` consecutive elements of weight tensor `widx` from element `start`; the tensor's first
-// element is residual element `w_off` (ops/plan2.py: Plan2.ef_chunks, the layout is mirrored there)
-struct EfChunk {
-  long long w_off;
-  int widx;
-  int start;
-  int count;
-  int pad;
-};
-static_assert(sizeof(EfChunk) == 24, "EfChunk layout must match ops/plan2.py EF_CHUNK_FMT");
-
-__device__ __forceinline__ float ef_round(float a, __nv_bfloat16& b) {
-  b = __float2bfloat16_rn(a);
-  return a - __bfloat162float(b);      // exact: the part of a that bf16 cannot hold
-}
-
 __global__ void __launch_bounds__(EF_THREADS) v2_ef_apply_kernel(const EfChunk* chunks, const long long* gptr,
                                                                   float* residual) {
   const EfChunk c = chunks[blockIdx.x];

@@ -738,6 +738,21 @@ def ef_chunks(plan: "Plan2") -> Tuple[bytes, List[Tuple[int, int]]]:
     return b"".join(struct.pack(EF_CHUNK_FMT, o, w, s, c, 0) for o, w, s, c in rows), ranges
 
 
+def vec_chunks(plan: "Plan2") -> Tuple[bytes, List[Tuple[int, int]]]:
+    """The 1-D vectors of every backward group as chunks of :func:`ef_chunks`' layout (``widx = -1``, offset in
+    ``vgrads``) and (first chunk, chunk count) per group: what gradient accumulation (csrc/v2_accum.cu) sums besides
+    the weights."""
+    rows: List[Tuple[int, int, int]] = []
+    ranges: List[Tuple[int, int]] = []
+    for g in range(plan.n_groups):
+        first = len(rows)
+        for q in plan.params:
+            if not q.is_w and q.group == g:
+                rows.extend((q.off, s, min(EF_CHUNK_ELEMS, q.numel - s)) for s in range(0, q.numel, EF_CHUNK_ELEMS))
+        ranges.append((first, len(rows) - first))
+    return b"".join(struct.pack(EF_CHUNK_FMT, o, -1, s, c, 0) for o, s, c in rows), ranges
+
+
 def pw_warm_ranges(plan: "Plan2") -> List[Tuple[int, int]]:
     """(float offset, count) in ``gpart`` of every PowerSGD unit's warm ``Q_w^T`` (``[r][round4(C)]``, the last part of
     its :func:`pw_scratch_floats` from ``gpart_off``), in unit order.  The rest of ``gpart`` is rewritten every step

@@ -12,7 +12,8 @@ the overlapped, sharded
 ``--engine shadow`` also runs ``--code qsgd|terngrad`` on ``ShadowEngine`` (bf16 only) and refuses ``--code
 entrywise``, which the launcher keeps on ``FusedEngine``; ``--engine fused`` always picks ``FusedEngine``.  ``--code
 topk``, ``--code sign``, ``--code powersgd``, ``--code fp8`` and ``--code hadamard`` (bits ``--quantization-level`` in
-{2, 4, 8}, a power-of-two ``--bucket-size``) exist only on ``ShadowEngine``.
+{2, 4, 8}, a power-of-two ``--bucket-size``) exist only on ``ShadowEngine``, and so does ``--accumulate-steps N``
+(``N`` micro-batches of ``--batch-size`` per step: both loaders build batches of ``N * --batch-size``).
 """
 from __future__ import annotations
 
@@ -37,6 +38,7 @@ class _HostEvent:
 def _build_engine(args, model, rank, world):
     engine = getattr(args, "engine", "auto")
     code = args.code.lower()
+    accum = getattr(args, "accumulate_steps", 1)
     if code == "topk" and (engine == "fused" or args.dtype != "bf16"):
         raise SystemExit("--code topk runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the fp32-flat "
                          "engine has no top-k selection")
@@ -83,12 +85,18 @@ def _build_engine(args, model, rank, world):
             kw["code_stats"] = True
         if getattr(args, "error_feedback", False):
             kw["error_feedback"] = True      # the engine refuses codes / --num-aggregate it cannot feed back
+        if accum != 1:
+            kw["accumulate_steps"] = accum      # the engine refuses a value below 1
         return ShadowEngine(model, rank, world, code=args.code, svd_rank=args.svd_rank, lr=args.lr,
                             momentum=args.momentum, weight_decay=args.weight_decay, nesterov=args.nesterov,
                             optimizer=args.optimizer, ps_mode=args.ps_mode, groups=args.groups, sampling=args.sampling,
                             prob_rule=args.prob_rule, seed=args.seed, num_aggregate=args.num_aggregate,
                             timeout_s=args.flag_timeout, **kw), "shadow"
     from .engine import FusedEngine
+    if accum != 1:
+        raise SystemExit("--accumulate-steps runs on the bf16 engine (--dtype bf16, --engine auto|shadow, --code "
+                         "svd|qsvd|sgd|topk|sign|powersgd|fp8|hadamard, or qsgd|terngrad with --engine shadow); the "
+                         "fp32-flat engine pushes after every backward")
     if getattr(args, "error_feedback", False):
         raise SystemExit("--error-feedback runs on the bf16 engine (--dtype bf16, --engine auto|shadow); the fp32-flat "
                          "engine keeps no residual (run without --error-feedback)")
@@ -136,15 +144,17 @@ def run_p2p_training(args, device=None):
     first = eng.first_worker
     nworkers = eng.W
     shard = shard_dataset(train_set, max(rank - first, 0), nworkers, seed=args.seed)
+    # --batch-size is the micro-batch: a step draws all of its micro-batches at once
+    step_batch = args.batch_size * getattr(args, "accumulate_steps", 1)
     if getattr(args, "gpu_data", False):
         from ..data.gpu_loader import GpuLoader
         # the layout each engine's static input has: channels_last on the shadow engine, as the CPU batches otherwise
-        loader = GpuLoader(shard, args.batch_size, args.dataset, train=True, seed=args.seed + rank, device=dev,
+        loader = GpuLoader(shard, step_batch, args.dataset, train=True, seed=args.seed + rank, device=dev,
                            channels_last=kind == "shadow")
         test_loader = GpuLoader(test_set, args.test_batch_size, args.dataset, train=False, device=dev,
                                 channels_last=kind == "shadow")
     else:
-        loader = DataLoader(shard, batch_size=args.batch_size, shuffle=True, seed=args.seed + rank, drop_last=True,
+        loader = DataLoader(shard, batch_size=step_batch, shuffle=True, seed=args.seed + rank, drop_last=True,
                             pin_memory=True, prefetch=2)
         test_loader = torch.utils.data.DataLoader(test_set, batch_size=args.test_batch_size, shuffle=False)
     x0, y0 = loader.next_batch()
@@ -193,7 +203,7 @@ def run_p2p_training(args, device=None):
             comm = (ph.get("param_wait_us", 0.0) + max(ph.get("to_params_us", 0.0) - ph.get("to_push_us", 0.0), 0.0)) / 1e6
             comp = max(step_s - comm, 0.0) if kind == "fused" else max(ph.get("to_push_us", 0.0) / 1e6, 0.0)
             if eng.is_worker:
-                print(worker_line(rank, cur, loader.epochs_completed, (cur * args.batch_size) % n_data, n_data, loss,
+                print(worker_line(rank, cur, loader.epochs_completed, (cur * step_batch) % n_data, n_data, loss,
                                   step_s, comp, enc, comm, msg_mb, p1, p5))
             if eng.is_ps or (kind == "shadow" and eng.is_owner):
                 print(master_line(cur, ph.get("ps_work_us", 0.0) / 1e6, eng.lr, ph.get("ps_wait_push_us", 0.0) / 1e6))

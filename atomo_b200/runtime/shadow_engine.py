@@ -53,6 +53,13 @@ one central PS kernel at the end of the step):
   autograd's gradient buffer in place and keeps ``A - bf16(A)``; the encoders' epilogues add ``bf16(A) - g_hat``, the
   part of ``A`` this push did not carry.  Nothing is discarded, only delayed.  Each worker checkpoints its residual
   and warm-start state in ``model_step_<N>_worker<R>`` (``save_checkpoint``), so a resume continues bit for bit.
+* **Gradient accumulation** (``accumulate_steps=N``): a step runs ``N`` micro-batches of ``B / N`` samples and pushes
+  once.  For every micro-batch but the last, each group's hook adds the bf16 gradients into an fp32 accumulator on the
+  encode stream (``csrc/v2_accum.cu``) and releases autograd's buffers, so no bf16 add ever happens; the vectors'
+  ``vgrads`` are added and zeroed the same way.  Before the last micro-batch's encode a fold launch writes
+  ``bf16((sum g_j) / N (+ e))`` into its gradient buffers in place (with error feedback it takes the place of the apply
+  launch), so every code, ``code_stats`` and the residual work unchanged.  BN statistics take one update per
+  micro-batch.  ``N = 1`` launches exactly what it launched before.
 * Optimizers fused in the PS epilogue: momentum-SGD (``src/optim/sgd.py:57-90``), Adam / AMSGrad
   (``src/optim/adam.py:37-94``).
 
@@ -62,6 +69,7 @@ step-stamped flags in peer memory (``csrc/v2_common.cuh``); no NCCL call on the 
 """
 from __future__ import annotations
 
+import numbers
 import os
 import struct
 from typing import List, Optional
@@ -94,7 +102,10 @@ class ShadowEngine:
                  warm_start: bool = True, max_sweeps: int = 1, main_priority: int = 0, debug_jitter_us: float = 0.0,
                  side_priority: int = -1, resample_empty: bool = False, quantization_level: int = 4,
                  bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False,
-                 error_feedback: bool = False):
+                 error_feedback: bool = False, accumulate_steps: int = 1):
+        if isinstance(accumulate_steps, bool) or not isinstance(accumulate_steps, numbers.Integral) \
+                or accumulate_steps < 1:        # checked before any CUDA work
+            raise ValueError("accumulate_steps must be an integer >= 1 (got %r)" % (accumulate_steps,))
         self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
         if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign", "powersgd", "fp8",
                              "hadamard"):
@@ -180,6 +191,8 @@ class ShadowEngine:
         self.owner_index = self.owner_ranks.index(rank) if self.is_owner else -1
         self.worker_index = self.worker_ranks.index(rank) if self.is_worker else 0
         self.first_worker = self.worker_ranks[0]
+        # micro-batches per step; a dedicated PS rank runs no backward and ignores the setting
+        self.accum = int(accumulate_steps) if self.is_worker else 1
         self.systematic = sampling == "systematic"
         self.waterfill = prob_rule == "waterfill"
         self.random_sample = random_sample
@@ -366,11 +379,25 @@ class ShadowEngine:
         # error feedback: fp32 residual per weight element (wshadow's physical order) and the apply chunks per group
         self.residual = self.t_ef_chunks = None
         self.ef_range = []
-        if self.error_feedback and self.is_worker:
+        if (self.error_feedback or self.accum > 1) and self.is_worker:
             assert C.v2_ef_chunk_bytes() == struct.calcsize(P2.EF_CHUNK_FMT)
-            self.residual = z(pl.w_total)
+            if self.error_feedback:
+                self.residual = z(pl.w_total)
             chunks, self.ef_range = P2.ef_chunks(pl)
             self.t_ef_chunks = _dev_bytes(chunks, dev)
+        # gradient accumulation (accumulate_steps > 1, csrc/v2_accum.cu): fp32 sums of the micro-batches' weight and
+        # vector gradients (zero at every step boundary), the vector chunks per group, and one gradient-pointer table
+        # per micro-batch before the last (each micro-batch's gradients live at their own addresses; the last one
+        # uses t_gptr, which the encoders read)
+        self.acc = self.vacc = self.t_vec_chunks = self.t_aptr = self.host_aptr = None
+        self.vec_range = []
+        if self.accum > 1:
+            self.acc, self.vacc = z(pl.w_total), z(pl.v_total)
+            vchunks, self.vec_range = P2.vec_chunks(pl)
+            self.t_vec_chunks = _dev_bytes(vchunks, dev)
+            self.t_aptr = torch.zeros((self.accum - 1, n_w), dtype=torch.int64, device=dev)
+            self.host_aptr = np.zeros((self.accum - 1, n_w), dtype=np.int64)
+        self.inv_n = float(np.float32(1.0 / self.accum))
         self.pw_warm = P2.pw_warm_ranges(pl) if self.power else []     # Q_w inside gpart (checkpointed)
         self._fresh_worker_state()
         self.loss_buf = torch.zeros(3, dtype=torch.float32, device=dev)
@@ -383,21 +410,22 @@ class ShadowEngine:
         # with the fused BN, the convolutions' weight gradients run on a stream of their own, beside the backward
         # chain (ops/split_conv.py); the encode of a group waits for it.  Same priority as the backward: the main
         # stream is at the lowest priority by default, and the wgrad is as urgent as the rest of the backward.
-        self.s_wgrad, self.ev_wgrad, self.group_w_params, self.split_wgrad_layers = None, [], [], 0
+        self.s_wgrad, self.ev_wgrad, self.split_wgrad_layers = None, [], 0
+        self.group_w_params = [[p for p, q in zip(self.params, pl.params) if q.is_w and q.group == g]
+                               for g in range(self.G)]
         if self.fused_bn_layers and self.is_worker:
             from ..ops.split_conv import enable_split_wgrad
             self.s_wgrad = torch.cuda.Stream(device=dev, priority=main_priority)
             self.split_wgrad_layers = enable_split_wgrad(self.model, self.s_wgrad)
             if self.split_wgrad_layers:
                 self.ev_wgrad = [torch.cuda.Event() for _ in range(self.G)]
-                self.group_w_params = [[p for p, q in zip(self.params, pl.params) if q.is_w and q.group == g]
-                                       for g in range(self.G)]
             else:
                 self.s_wgrad = None
         self.ev_ready = [torch.cuda.Event() for _ in range(self.G)]
         self.ev_push = [torch.cuda.Event() for _ in range(self.G)]
         self.ev_enc_done, self.ev_ps_done = torch.cuda.Event(), torch.cuda.Event()
-        self._pending, self._fired, self._nlaunch = list(self.group_size), 0, 0
+        self.ev_acc_done = torch.cuda.Event()      # the adds of a micro-batch have read (and zeroed) vgrads
+        self._pending, self._fired, self._nlaunch, self._micro = list(self.group_size), 0, 0, 0
         self._capturing = False
         self._initial_sync()
 
@@ -583,7 +611,8 @@ class ShadowEngine:
 
         def hook(p):
             if q.is_w:
-                self.host_gptr[q.widx] = p.grad.data_ptr()
+                j = self._micro
+                (self.host_gptr if j == self.accum - 1 else self.host_aptr[j])[q.widx] = p.grad.data_ptr()
             g = q.group
             self._pending[g] -= 1
             if self._pending[g] == 0:
@@ -598,7 +627,15 @@ class ShadowEngine:
             if hi > lo:   # pageable source: staged synchronously, safe against the host table changing next step
                 self.t_gptr[lo:hi].copy_(torch.from_numpy(self.host_gptr[lo:hi].copy()))
         res = self.residual.data_ptr() if self.residual is not None else 0
-        if res:     # A = g + e into the gradient buffers (bf16) and the residual (its rounding remainder)
+        if self.acc is not None:
+            # the last micro-batch: A = (sum of the micro-batches) / N (+ e) into its gradient buffers (bf16), the
+            # rounding remainder into the residual, the vectors' mean into vgrads; the accumulators back to zero
+            (c0, nw), (v0, nv), cb = self.ef_range[g], self.vec_range[g], struct.calcsize(P2.EF_CHUNK_FMT)
+            C.v2_accum_fold(self.t_ef_chunks.data_ptr() + cb * c0, nw, self.t_vec_chunks.data_ptr() + cb * v0, nv,
+                            self.t_gptr.data_ptr(), self.acc.data_ptr(), self.vacc.data_ptr(), self.vgrads.data_ptr(),
+                            self.inv_n, res)
+            self._nlaunch += 1
+        elif res:     # A = g + e into the gradient buffers (bf16) and the residual (its rounding remainder)
             c0, ncs = self.ef_range[g]
             C.v2_ef_apply(self.t_ef_chunks.data_ptr(), c0, ncs, self.t_gptr.data_ptr(), res)
             self._nlaunch += 1
@@ -755,6 +792,9 @@ class ShadowEngine:
             reader.wait_event(self.ev_wgrad[g])
             for p in self.group_w_params[g]:
                 p.grad.record_stream(reader)
+        if self._micro < self.accum - 1:
+            self._launch_accum(g, cur)
+            return
         if not self.overlap:
             self._launch_encode(g)
             self._launch_code_stats(g)
@@ -780,19 +820,55 @@ class ShadowEngine:
                 if final:
                     self.ev_ps_done.record(self.s_ps)
 
-    def _forward_backward(self):
+    def _launch_accum(self, g: int, cur):
+        """Group ``g`` of a micro-batch before the last: add its gradients into the accumulators (on the encode
+        stream, or on ``cur`` without overlap), then release the gradient buffers, so that the next backward hands
+        over fresh ones instead of adding into them in bf16."""
+        j = self._micro
+        reader = self.s_enc if self.overlap else cur
+        if self.overlap:
+            self.ev_ready[g].record(cur)
+            self.s_enc.wait_event(self.ev_ready[g])
+        with torch.cuda.stream(reader):
+            lo, hi = self.w_range[g]
+            if not self._capturing and hi > lo:     # as in _launch_encode; after a capture prepare() fills the table
+                self.t_aptr[j, lo:hi].copy_(torch.from_numpy(self.host_aptr[j, lo:hi].copy()))
+            (c0, nw), (v0, nv), cb = self.ef_range[g], self.vec_range[g], struct.calcsize(P2.EF_CHUNK_FMT)
+            self.C.v2_accum_add(self.t_ef_chunks.data_ptr() + cb * c0, nw, self.t_vec_chunks.data_ptr() + cb * v0, nv,
+                                self.t_aptr[j].data_ptr(), self.acc.data_ptr(), self.vacc.data_ptr(),
+                                self.vgrads.data_ptr(), j == 0)
+            self._nlaunch += 1
+            if self._fired == self.G:
+                self.ev_acc_done.record(reader)
+        for p in self.group_w_params[g]:
+            p.grad.record_stream(reader)        # not reused before the add has read it
+            p.grad = None
+
+    def _forward_backward(self, j: int = 0):
+        """Forward and backward of micro-batch ``j`` (the whole static batch when ``accumulate_steps`` is 1); the
+        loss and precisions in ``loss_buf`` are means over the whole batch."""
+        n = self.accum
         x, y = self.static_x, self.static_y
+        if n > 1:
+            b = x.size(0) // n
+            x, y = x[j * b:(j + 1) * b], y[j * b:(j + 1) * b]
         with torch.autocast("cuda", dtype=torch.bfloat16):
             logits = self.model(x)
             loss = self.criterion(logits.float(), y)
+        if j > 0 and self.overlap:      # the previous micro-batch's adds read vgrads, which this backward rewrites
+            torch.cuda.current_stream(self.device).wait_event(self.ev_acc_done)
         loss.backward()
         with torch.no_grad():
             lg = logits.detach().float()
             k = min(5, lg.size(1))
             hit = lg.topk(k, 1).indices.eq(y.view(-1, 1))
-            self.loss_buf[0] = loss.detach()
-            self.loss_buf[1] = hit[:, :1].float().sum() * (100.0 / y.numel())
-            self.loss_buf[2] = hit.float().sum() * (100.0 / y.numel())
+            vals = (loss.detach() if n == 1 else loss.detach() / n, hit[:, :1].float().sum() * (100.0 / (y.numel() * n)),
+                    hit.float().sum() * (100.0 / (y.numel() * n)))
+            for i, v in enumerate(vals):
+                if j == 0:
+                    self.loss_buf[i] = v
+                else:
+                    self.loss_buf[i] += v
 
     def _step_body(self):
         C = self.C
@@ -804,14 +880,16 @@ class ShadowEngine:
             self.vgrads.zero_()
             for p in self.w_params:
                 p.grad = None
-            self._pending, self._fired = list(self.group_size), 0
             if self.s_wgrad is not None:
                 # fork the wgrad stream here, so that it is part of a graph capture before any group records on it;
                 # the encode's waits on the last group's event join it again
                 self.s_wgrad.wait_stream(torch.cuda.current_stream(self.device))
-            self._forward_backward()
-            self._nlaunch += 4 * self.fused_bn_layers
-            assert self._fired == self.G, "a backward group never fired (%d of %d)" % (self._fired, self.G)
+            for j in range(self.accum):     # only the last micro-batch codes, pushes and steps the PS
+                self._micro = j
+                self._pending, self._fired = list(self.group_size), 0
+                self._forward_backward(j)
+                self._nlaunch += 4 * self.fused_bn_layers
+                assert self._fired == self.G, "a backward group never fired (%d of %d)" % (self._fired, self.G)
             if self.overlap:
                 cur = torch.cuda.current_stream(self.device)
                 cur.wait_event(self.ev_enc_done)
@@ -826,6 +904,9 @@ class ShadowEngine:
 
     # ------------------------------------------------------------------------------------------------------
     def prepare(self, x_example: torch.Tensor, y_example: torch.Tensor, warmup: int = 3):
+        if x_example.size(0) % self.accum:
+            raise ValueError("accumulate_steps=%d needs a batch divisible by it (got %d samples)"
+                             % (self.accum, x_example.size(0)))
         self.static_x = torch.empty_like(x_example, device=self.device)
         if self.static_x.dim() == 4:
             self.static_x = self.static_x.contiguous(memory_format=torch.channels_last)
@@ -859,6 +940,8 @@ class ShadowEngine:
                 self._capturing = False
             # the gradient tensors allocated during capture live at fixed addresses of the graph's pool
             self.t_gptr.copy_(torch.from_numpy(self.host_gptr.copy()))
+            if self.t_aptr is not None:
+                self.t_aptr.copy_(torch.from_numpy(self.host_aptr.copy()))
             torch.cuda.synchronize(self.device)
         return self
 
@@ -968,6 +1051,7 @@ class ShadowEngine:
         (c) scratch, rewritten every step before it is read: the rest of ``gpart`` (Gram partials, ``P``,
             ``P_hat``, ``Q'``), ``vsel``, ``selcount``, ``sigma``, ``clip`` / ``clip_partials``, ``l1`` /
             ``l1_partials``, ``topk_sel``, ``topk_tiles``, ``pw_gram``, ``stats_partials``, ``vgrads``, ``wstage``,
+            the gradient-accumulation sums ``acc`` / ``vacc`` (zero at every step boundary) and pointer tables,
             the arena slots (step-stamped), the fused-BN statistics arena, ``loss_buf`` and the input staging; zero
             between launches by design: ``counters``, ``stats_counters``, ``topk_hist``; ``signals`` carries step
             stamps, and ``load_checkpoint`` raises the parameter flags to the resumed step.

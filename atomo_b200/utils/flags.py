@@ -108,4 +108,9 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "top-k, topk, sign and powersgd, the contractive codes, and with fp8 and hadamard at 4 or 8 "
                         "bits, whose variance is small), every push counted (no --num-aggregate below the worker "
                         "count).  Residuals (and PowerSGD's warm state) are not checkpointed: --resume starts them afresh")
+    p.add_argument("--accumulate-steps", type=int, default=1,
+                   help="p2p backend, bf16 engine: micro-batches per optimizer step.  Each worker runs N forward / "
+                        "backward passes of --batch-size samples, sums their gradients in fp32 and codes and pushes "
+                        "their mean once, so the global batch is workers x N x --batch-size and the pushes per sample "
+                        "fall N-fold.  The LR schedule, checkpoints and --eval-freq count optimizer steps")
     return p.parse_args(argv)

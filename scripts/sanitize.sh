@@ -17,8 +17,8 @@ for tool in $tools; do
   echo "== compute-sanitizer --tool $tool"
   limit=600; [ "$tool" = racecheck ] && limit=900
   timeout $limit compute-sanitizer --tool $tool --error-exitcode 1 \
-    python -m pytest tests/test_gpu_v2.py tests/test_gpu_kernels.py tests/test_gpu_hadamard.py -m gpu -q -x -p no:cacheprovider \
-    -k "(gram or topk or unbiased or ps_matches or qsvd or num_aggregate or full_rank or ps_update or qsgd or entrywise or bn or v2_hadamard or v2_ps_hadamard) and not graph and not engine and not multi" \
+    python -m pytest tests/test_gpu_v2.py tests/test_gpu_kernels.py tests/test_gpu_hadamard.py tests/test_gpu_accumulate.py -m gpu -q -x -p no:cacheprovider \
+    -k "(gram or topk or unbiased or ps_matches or qsvd or num_aggregate or full_rank or ps_update or qsgd or entrywise or bn or v2_hadamard or v2_ps_hadamard or fold_is_the_fp32_oracle) and not graph and not engine and not multi" \
     > gpurun_out/sanitizer_$tool.log 2>&1 || echo "$tool: exit $? (see gpurun_out/sanitizer_$tool.log)"
   tail -3 gpurun_out/sanitizer_$tool.log
 done
