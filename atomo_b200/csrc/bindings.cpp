@@ -345,6 +345,8 @@ void check_nhwc_bf16(const torch::Tensor& t, const char* name) {
   TORCH_CHECK(t.is_cuda() && t.scalar_type() == torch::kBFloat16, name, " must be a CUDA bf16 tensor");
   TORCH_CHECK(t.dim() == 4 && t.is_contiguous(at::MemoryFormat::ChannelsLast), name, " must be channels_last");
   TORCH_CHECK(t.size(1) % 8 == 0 && t.size(1) <= 2048, name, ": C must be a multiple of 8 (<= 2048)");
+  // the kernels move 8 channels as one 16-byte vector
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0, name, " must be 16-byte aligned");
 }
 
 // the ReLU mask of a fused BN layer: uint8, one byte (8 channel bits) per 8 channels of each row
@@ -385,6 +387,7 @@ void bn_backward(const torch::Tensor& dy, const torch::Tensor& x, c10::optional<
   check_nhwc_bf16(dy, "dy");
   check_nhwc_bf16(x, "x");
   check_nhwc_bf16(dx, "dx");
+  if (dres.has_value()) check_nhwc_bf16(*dres, "dres");
   if (mask.has_value()) check_relu_mask(*mask, x);
   c10::cuda::CUDAGuard guard(x.device());
   const long long R = x.numel() / x.size(1);

@@ -119,7 +119,8 @@ bn_apply_kernel(const uint4* __restrict__ x, const uint4* __restrict__ res, uint
   const float invR = 1.f / (float)R;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     const float mean = acc[c] * invR;
-    const float var = fmaxf(acc[C + c] * invR - mean * mean, 0.f);
+    const float v = acc[C + c] * invR - mean * mean;
+    const float var = v < 0.f ? 0.f : v;  // not fmaxf: fmaxf(NaN, 0) = 0 would give a non-finite channel finite stats
     const float invstd = rsqrtf(var + eps);
     const float sc = gamma[c] * invstd;
     tab[c] = sc;
@@ -151,19 +152,21 @@ bn_apply_kernel(const uint4* __restrict__ x, const uint4* __restrict__ res, uint
       for (int i = 0; i < 8; ++i) o[i] = fmaf(f[i], tab[cg * 8 + i], tab[C + cg * 8 + i]);
     }
     if (relu) {
+      // a NaN stays NaN, as in stock ReLU (fmaxf(NaN, 0) is 0); every other o gets exactly fmaxf(o, 0)
 #pragma unroll
-      for (int i = 0; i < 8; ++i) o[i] = fmaxf(o[i], 0.f);
+      for (int i = 0; i < 8; ++i) o[i] = o[i] != o[i] ? o[i] : fmaxf(o[i], 0.f);
     }
     const uint4 out = pack8(o);
     y[e] = out;
     if (relu) {
       // the bits come from the stored bf16 values (a positive fp32 o can round to bf16 zero), compared exactly as
-      // the backward compared y before it read the mask
+      // the backward compared y before it read the mask; a NaN output passes its gradient, as stock
+      // threshold_backward (y <= 0 ? 0 : dy) does
       float yv[8];
       unpack8(out, yv);
       unsigned m = 0;
 #pragma unroll
-      for (int i = 0; i < 8; ++i) m |= (yv[i] > 0.f ? 1u : 0u) << i;
+      for (int i = 0; i < 8; ++i) m |= (!(yv[i] <= 0.f) ? 1u : 0u) << i;
       mask[e] = (uint8_t)m;
     }
   }

@@ -77,6 +77,12 @@ class BNAct(nn.BatchNorm2d):
             return False
         if not x.is_contiguous(memory_format=torch.channels_last):
             return False
+        # an empty batch leaves the running statistics alone and one value per channel raises: stock does both
+        if x.numel() < 2 * x.size(1):
+            return False
+        # the kernels move 8 channels as one 16-byte vector
+        if x.data_ptr() % 16 != 0 or (residual is not None and residual.data_ptr() % 16 != 0):
+            return False
         if residual is not None and (residual.dtype != x.dtype or residual.shape != x.shape or
                                      not residual.is_contiguous(memory_format=torch.channels_last)):
             return False
