@@ -232,6 +232,22 @@ void atomo_v2_launch_code_stats(const void* units, const void* tiles, int tile0,
                                 int random_sample, int waterfill, double* partials, unsigned int* unit_counters,
                                 double* acc, cudaStream_t stream);
 void atomo_v2_launch_advance_step(void* ctrl, cudaStream_t stream);
+// v2_layerwise.cu (LARS / LAMB on the bf16 engine: phase 1 = the PS kernels' layer-wise instantiations, phase 2)
+int atomo_v2_layerwise_max_layers();
+void atomo_v2_launch_ps_layerwise(int ps, const void* units, const void* tiles, int tile0, int ntiles, int W,
+                                  int nranks, int group, int owner, float* master, float* mom, float* sq, float* vmom,
+                                  float* vsq, float* vparams_local, float* vparams_mc, float* const* vparams_peer,
+                                  const float* vgrads_mc, const float* const* vgrads_peer,
+                                  const void* const* stage_peer, const float* arenas, long long arena_floats, int* sig,
+                                  int* const* sig_peer, void* ctrl, unsigned int* group_counter, long long timeout,
+                                  long long* tstats, float inv_w, float* dir, void* part, int grid,
+                                  cudaStream_t stream);
+void atomo_v2_launch_layerwise(const void* units, const void* tiles, int tile0, int ntiles, const int* tile_layer,
+                               int nlayers, const void* part, const float* dir, int nranks, int group, int final_group,
+                               int owner, int n_owners, float* master, float* mom, void* wshadow_mc,
+                               void* const* wshadow_peer, double* xch, double* const* xch_peer, int* sig,
+                               int* const* sig_peer, void* ctrl, unsigned int* group_counter, long long timeout,
+                               long long* tstats, float* ratio_out, int grid, cudaStream_t stream);
 void atomo_v2_launch_bcast_bytes(const void* src, void* const* peer, void* mc, int nranks, int self, long long nbytes,
                                  cudaStream_t stream);
 // gemm_kernels.cu
@@ -873,6 +889,44 @@ void v2_accum_add(uint64_t wchunks, int nw, uint64_t vchunks, int nv, uint64_t g
 // the last micro-batch, before the group's encode on the same stream: A = (acc + g) * inv_n (+ e with a residual),
 // bf16(A) into the gradient buffers, A - bf16(A) into the residual, acc = 0; vgrads = (vacc + vgrads) * inv_n,
 // vacc = 0
+// LARS / LAMB phase 1: the code's PS kernel (`ps`: 0 spectral / dense, 1 QSGD / TernGrad, 2 entry-wise / top-k,
+// 3 sign, 4 fp8, 5 hadamard, 6 PowerSGD) with the layer-wise epilogue; `part` points at the launch's first tile
+void v2_ps_layerwise(int ps, uint64_t units, uint64_t tiles, int tile0, int ntiles, int W, int nranks, int group,
+                     int owner, uint64_t master, uint64_t mom, uint64_t sq, uint64_t vmom, uint64_t vsq,
+                     uint64_t vparams_local, uint64_t vparams_mc, uint64_t vparams_peer, uint64_t vgrads_mc,
+                     uint64_t vgrads_peer, uint64_t stage_peer, uint64_t arenas, int64_t arena_floats, uint64_t sig,
+                     uint64_t sig_peer, uint64_t ctrl, uint64_t group_counter, int64_t timeout, uint64_t tstats,
+                     double inv_w, uint64_t dir, uint64_t part, int grid, int max_level, int max_bucket) {
+  TORCH_CHECK(ps >= 0 && ps <= 6, "v2_ps_layerwise: unknown PS kernel");
+  TORCH_CHECK(W >= 1 && W <= 16, "too many workers for v2_ps_layerwise");
+  TORCH_CHECK(master != 0 && mom != 0 && dir != 0 && part != 0, "v2_ps_layerwise: master / mom / dir / part required");
+  if (ps == 1) check_qsgd_plan(max_level, max_bucket);
+  atomo_v2_launch_ps_layerwise(ps, P<const void>(units), P<const void>(tiles), tile0, ntiles, W, nranks, group, owner,
+                               P<float>(master), P<float>(mom), P<float>(sq), P<float>(vmom), P<float>(vsq),
+                               P<float>(vparams_local), P<float>(vparams_mc), P<float* const>(vparams_peer),
+                               P<const float>(vgrads_mc), P<const float* const>(vgrads_peer),
+                               P<const void* const>(stage_peer), P<const float>(arenas), arena_floats, P<int>(sig),
+                               P<int* const>(sig_peer), P<void>(ctrl), P<unsigned int>(group_counter), timeout,
+                               P<long long>(tstats), (float)inv_w, P<float>(dir), P<void>(part), grid, cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+// LARS / LAMB phase 2: norms across tiles and owners, trust ratios, the step and the bf16 broadcast of one group
+void v2_layerwise(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t tile_layer, int nlayers,
+                  uint64_t part, uint64_t dir, int nranks, int group, bool final_group, int owner, int n_owners,
+                  uint64_t master, uint64_t mom, uint64_t wshadow_mc, uint64_t wshadow_peer, uint64_t xch,
+                  uint64_t xch_peer, uint64_t sig, uint64_t sig_peer, uint64_t ctrl, uint64_t group_counter,
+                  int64_t timeout, uint64_t tstats, uint64_t ratio_out, int grid) {
+  TORCH_CHECK(nlayers >= 0 && nlayers <= atomo_v2_layerwise_max_layers(), "v2_layerwise: too many tensors in a group");
+  TORCH_CHECK(n_owners >= 1 && n_owners <= 16 && owner >= 0 && owner < n_owners, "v2_layerwise: bad owner");
+  TORCH_CHECK(n_owners == 1 || (xch != 0 && xch_peer != 0), "v2_layerwise: several owners need the exchange slots");
+  atomo_v2_launch_layerwise(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const int>(tile_layer), nlayers,
+                            P<const void>(part), P<const float>(dir), nranks, group, final_group ? 1 : 0, owner,
+                            n_owners, P<float>(master), P<float>(mom), P<void>(wshadow_mc), P<void* const>(wshadow_peer),
+                            P<double>(xch), P<double* const>(xch_peer), P<int>(sig), P<int* const>(sig_peer),
+                            P<void>(ctrl), P<unsigned int>(group_counter), timeout, P<long long>(tstats),
+                            P<float>(ratio_out), grid, cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
 void v2_accum_fold(uint64_t wchunks, int nw, uint64_t vchunks, int nv, uint64_t gptr, uint64_t acc, uint64_t vacc,
                    uint64_t vgrads, float inv_n, uint64_t residual) {
   TORCH_CHECK(nw >= 0 && nv >= 0, "v2_accum_fold: negative chunk count");
@@ -1069,6 +1123,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("v2_ef_chunk_bytes", &atomo_v2_ef_chunk_bytes);
   m.def("v2_accum_add", &v2_accum_add);
   m.def("v2_accum_fold", &v2_accum_fold);
+  m.def("v2_ps_layerwise", &v2_ps_layerwise);
+  m.def("v2_layerwise", &v2_layerwise);
+  m.def("v2_layerwise_max_layers", &atomo_v2_layerwise_max_layers);
   m.def("v2_ps_entry", &v2_ps_entry);
   m.def("v2_code_stats", &v2_code_stats);
   m.def("v2_stats_fields", &atomo_v2_stats_fields);

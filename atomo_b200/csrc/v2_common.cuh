@@ -71,7 +71,7 @@ struct Tile2 {
   int owner;
 };
 
-enum Opt : int { OPT_SGD = 0, OPT_ADAM = 1, OPT_AMSGRAD = 2 };
+enum Opt : int { OPT_SGD = 0, OPT_ADAM = 1, OPT_AMSGRAD = 2, OPT_LARS = 3, OPT_LAMB = 4 };
 
 struct Ctrl2 {
   int step;
@@ -83,21 +83,26 @@ struct Ctrl2 {
   float beta1, beta2, eps, pad0;
   int opt;
   int num_aggregate;   // 0 = wait for every worker; N = proceed after N pushes (backup workers)
-  int pad1, pad2;
+  float trust_coefficient;   // LARS: eta of the trust ratio (v2_layerwise.cu)
+  int pad2;
 };
 static_assert(sizeof(Ctrl2) == 72, "Ctrl2 layout must match ops/plan2.py CTRL2_FMT");
 
-enum Err2 : int { ERR2_NONE = 0, ERR2_WAIT_PUSH = 1, ERR2_WAIT_PARAM = 2, ERR2_SLOT_STEP = 4, ERR2_NONFINITE = 8 };
+enum Err2 : int {
+  ERR2_NONE = 0, ERR2_WAIT_PUSH = 1, ERR2_WAIT_PARAM = 2, ERR2_SLOT_STEP = 4, ERR2_NONFINITE = 8, ERR2_WAIT_NORMS = 16
+};
 
 constexpr int MAX_WORKERS = 16;
 constexpr int MAX_GROUPS = 8;
 constexpr int V2_MAX_COLS = TS_MAX_COLS;
 constexpr int V2_RCAP_MAX = RCAP_MAX;
 // signal region (ints): push flag of (group g, worker w) at g*MAX_WORKERS + w; param flag of owner o at 256 + o;
-// aggregation mask of (group g) at 320 + g (owner-local)
+// aggregation mask of (group g) at 320 + 2g (owner-local); layer-wise norms of (group g, owner o) published at
+// 352 + g*MAX_WORKERS + o (v2_layerwise.cu)
 constexpr int SIG_PUSH = 0;
 constexpr int SIG_PARAM = 256;
 constexpr int SIG_MASK = 320;
+constexpr int SIG_NORMS = 352;
 
 __device__ __forceinline__ float bf16_lo(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }

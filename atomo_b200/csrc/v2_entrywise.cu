@@ -74,7 +74,8 @@ __global__ void __launch_bounds__(EE_THREADS) v2_entry_encode_ef_kernel(const EE
 }
 
 // ---- PS: scatter-add + optimizer --------------------------------------------------------------------------
-__global__ void __launch_bounds__(EPS_THREADS) v2_ps_entry_kernel(const PsArgs2 a) {
+template <class A>
+__device__ __forceinline__ void ps_entry(const A& a) {
   __shared__ __align__(16) float OUT[ENTRY_TILE_ELEMS];   // summed entries of one tile, physical element order
   __shared__ int s_ok, s_bad;
   __shared__ unsigned int s_mask, s_use;
@@ -95,6 +96,7 @@ __global__ void __launch_bounds__(EPS_THREADS) v2_ps_entry_kernel(const PsArgs2 
   const int per_cta = (a.ntiles + gridDim.x - 1) / gridDim.x;
   const int t_begin = blockIdx.x * per_cta;
   const int t_end = min(a.ntiles, t_begin + per_cta);
+  lw_begin(a);
   for (int ti = t_begin; ok && ti < t_end; ++ti) {
     const Tile2 t = a.tiles[ti];
     const Unit2 u = a.units[t.unit];
@@ -147,11 +149,15 @@ __global__ void __launch_bounds__(EPS_THREADS) v2_ps_entry_kernel(const PsArgs2 
       update8(a, c, e0 + 8LL * v, g);
     }
     for (int i = (nvec << 3) + tid; i < t.b; i += blockDim.x) update1(a, c, e0 + i, OUT[i] * inv_w);
+    lw_tile_done(a, ti);
   }
 
   __syncthreads();
   if (tid == 0) ps_complete(a, ctrl, step, s_bad != 0, t_enter, t_ready);
 }
+
+__global__ void __launch_bounds__(EPS_THREADS) v2_ps_entry_kernel(const PsArgs2 a) { ps_entry(a); }
+__global__ void __launch_bounds__(EPS_THREADS, 1) v2_ps_entry_lw_kernel(const PsArgsLw a) { ps_entry(a); }
 
 extern "C" {
 
@@ -192,6 +198,11 @@ void atomo_v2_launch_ps_entry(const void* units, const void* tiles, int tile0, i
       ps_args(units, tiles, tile0, ntiles, W, nranks, group, final_group, owner, master, mom, sq, sqmax, vmom, vsq,
               vsqmax, wshadow_mc, wshadow_peer, vparams_local, vparams_mc, vparams_peer, vgrads_mc, vgrads_peer,
               nullptr, arenas, arena_floats, sig, sig_peer, ctrl, group_counter, timeout, tstats, inv_w));
+}
+
+void atomo_v2_launch_ps_entry_lw(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsLw& a = *static_cast<const PsArgsLw*>(args);
+  v2_ps_entry_lw_kernel<<<ps_grid(grid, a.ntiles), EPS_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

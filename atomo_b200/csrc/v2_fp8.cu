@@ -196,7 +196,8 @@ __global__ void __launch_bounds__(FE_THREADS) v2_fp8_encode_kernel(const PushArg
 __global__ void __launch_bounds__(FE_THREADS) v2_fp8_encode_ef_kernel(const PushArgs a) { fp8_encode<true>(a); }
 
 // ---- PS: decode + sum + optimizer --------------------------------------------------------------------------
-__global__ void __launch_bounds__(FPS_THREADS) v2_ps_fp8_kernel(const PsArgs2 a) {
+template <class A>
+__device__ __forceinline__ void ps_fp8(const A& a) {
   __shared__ int s_ok, s_bad;
   __shared__ unsigned int s_mask, s_use;
   __shared__ long long s_t_enter, s_t_ready;            // live across the whole launch: kept out of registers
@@ -212,6 +213,7 @@ __global__ void __launch_bounds__(FPS_THREADS) v2_ps_fp8_kernel(const PsArgs2 a)
   const OptC c = ps_opt_consts(ctrl, step);
   const float inv_w = all_workers ? a.inv_w : 1.f / (float)max(__popc(wmask), 1);
   const auto [t_begin, t_end] = ps_tile_range(a);
+  lw_begin(a);
   for (int ti = t_begin; ok && ti < t_end; ++ti) {
     const Tile2 t = a.tiles[ti];
     const Unit2 u = a.units[t.unit];
@@ -259,11 +261,15 @@ __global__ void __launch_bounds__(FPS_THREADS) v2_ps_fp8_kernel(const PsArgs2 a)
         for (int i = 0; i < 16 && i0 + i < t.b; ++i) update1(a, c, e0 + i0 + i, g[i >> 3][i & 7]);
       }
     }
+    lw_tile_done(a, ti);
   }
 
   __syncthreads();
   if (tid == 0) ps_complete(a, ctrl, step, s_bad != 0, s_t_enter, s_t_ready);
 }
+
+__global__ void __launch_bounds__(FPS_THREADS) v2_ps_fp8_kernel(const PsArgs2 a) { ps_fp8(a); }
+__global__ void __launch_bounds__(FPS_THREADS, 1) v2_ps_fp8_lw_kernel(const PsArgsLw a) { ps_fp8(a); }
 
 // ---- --code-stats ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(FE_THREADS) v2_fp8_code_stats_kernel(const ScaleStatArgs a) {
@@ -362,6 +368,11 @@ void atomo_v2_launch_fp8_code_stats(const void* units, const void* tiles, int ti
   a.arena_peer = arena_peer; a.n_owners = n_owners; a.arena_floats = arena_floats; a.worker = worker;
   a.partials = partials; a.unit_counters = unit_counters; a.acc = acc;
   v2_fp8_code_stats_kernel<<<ntiles, FE_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_fp8_lw(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsLw& a = *static_cast<const PsArgsLw*>(args);
+  v2_ps_fp8_lw_kernel<<<ps_grid(grid, a.ntiles), FPS_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

@@ -338,7 +338,8 @@ __global__ void __launch_bounds__(HD_THREADS, 1) v2_hadamard_encode_ef_kernel(co
 }
 
 // ---- PS: decode + sum in the rotated domain + one inverse transform + optimizer --------------------------------
-__global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_kernel(const PsArgs2 a) {
+template <class A>
+__device__ __forceinline__ void ps_hadamard(const A& a) {
   __shared__ __align__(16) float s_x[HD_TILE];
   __shared__ int s_ok, s_bad;
   __shared__ unsigned int s_mask, s_use;
@@ -356,6 +357,7 @@ __global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_kernel(const PsA
   const float inv_w = all_workers ? a.inv_w : 1.f / (float)max(__popc(wmask), 1);
   const unsigned long long seed = ctrl->seed;
   const auto [t_begin, t_end] = ps_tile_range(a);
+  lw_begin(a);
   for (int ti = t_begin; ok && ti < t_end; ++ti) {
     const Tile2 t = a.tiles[ti];
     const Unit2 u = a.units[t.unit];
@@ -398,6 +400,20 @@ __global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_kernel(const PsA
       const float xr = __fmul_rn(g[r], inv_d);
       g[r] = __fmul_rn(((neg >> r) & 1u) ? -xr : xr, inv_w);
     }
+    if constexpr (ps_layerwise<A>) {   // the epilogue below, then the reduction every thread of the CTA reaches
+      if (live && i0 < t.b) {
+        const long long ew = u.w_off + e0;
+        if (i0 + 16 <= t.b) {
+          update8(a, c, ew, *reinterpret_cast<const float(*)[8]>(g));
+          update8(a, c, ew + 8, *reinterpret_cast<const float(*)[8]>(g + 8));
+        } else {
+          for (int r = 0; r < 16; ++r)
+            if (i0 + r < t.b) update1(a, c, ew + r, g[r]);
+        }
+      }
+      lw_tile_done(a, ti);
+      continue;
+    }
     if (!live || i0 >= t.b) continue;
     const long long ew = u.w_off + e0;                   // % 16 == 0
     if (i0 + 16 <= t.b) {
@@ -413,6 +429,9 @@ __global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_kernel(const PsA
   __syncthreads();
   if (tid == 0) ps_complete(a, ctrl, step, s_bad != 0, s_t_enter, s_t_ready);
 }
+
+__global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_kernel(const PsArgs2 a) { ps_hadamard(a); }
+__global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_lw_kernel(const PsArgsLw a) { ps_hadamard(a); }
 
 // ---- --code-stats ------------------------------------------------------------------------------------------
 struct HStatArgs {
@@ -526,6 +545,11 @@ void atomo_v2_launch_hadamard_code_stats(const void* units, const void* tiles, i
   a.arena_peer = arena_peer; a.n_owners = n_owners; a.arena_floats = arena_floats; a.worker = worker;
   a.ctrl = (const Ctrl2*)ctrl; a.partials = partials; a.unit_counters = unit_counters; a.acc = acc;
   v2_hadamard_code_stats_kernel<<<ntiles, HD_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_hadamard_lw(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsLw& a = *static_cast<const PsArgsLw*>(args);
+  v2_ps_hadamard_lw_kernel<<<ps_grid(grid, a.ntiles), HD_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

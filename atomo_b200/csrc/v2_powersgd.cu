@@ -415,7 +415,8 @@ __global__ void __launch_bounds__(PW_THREADS) v2_powersgd_encode_ef_kernel(const
 }
 
 // ---- PS: reconstruct + sum + optimizer ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(PW_THREADS) v2_ps_powersgd_kernel(const PsArgs2 a) {
+template <class A>
+__device__ __forceinline__ void ps_powersgd(const A& a) {
   __shared__ float sph[MAX_WORKERS][PW_PS_ROWS][PW_MAXR];   // the counted workers' P_hat rows of one tile
   __shared__ int s_ok, s_bad;
   __shared__ unsigned int s_mask, s_use;
@@ -432,6 +433,7 @@ __global__ void __launch_bounds__(PW_THREADS) v2_ps_powersgd_kernel(const PsArgs
   const OptC c = ps_opt_consts(ctrl, step);
   const float inv_w = all_workers ? a.inv_w : 1.f / (float)max(__popc(wmask), 1);
   const auto [t_begin, t_end] = ps_tile_range(a);
+  lw_begin(a);
   for (int ti = t_begin; ok && ti < t_end; ++ti) {
     const Tile2 t = a.tiles[ti];
     const Unit2 u = a.units[t.unit];
@@ -441,6 +443,7 @@ __global__ void __launch_bounds__(PW_THREADS) v2_ps_powersgd_kernel(const PsArgs
     }
     if (u.kind == KIND_DENSE16) {
       ps_dense16_tile(a, c, u, t, wmask, inv_w);
+      lw_tile_done(a, ti);
       continue;
     }
     if (u.kind != KIND_POWER) continue;
@@ -513,11 +516,15 @@ __global__ void __launch_bounds__(PW_THREADS) v2_ps_powersgd_kernel(const PsArgs
         }
       }
     }
+    lw_tile_done(a, ti);
   }
 
   __syncthreads();
   if (tid == 0) ps_complete(a, ctrl, step, s_bad != 0, s_t_enter, s_t_ready);
 }
+
+__global__ void __launch_bounds__(PW_THREADS) v2_ps_powersgd_kernel(const PsArgs2 a) { ps_powersgd(a); }
+__global__ void __launch_bounds__(PW_THREADS, 1) v2_ps_powersgd_lw_kernel(const PsArgsLw a) { ps_powersgd(a); }
 
 // ---- --code-stats ------------------------------------------------------------------------------------------------
 struct PwStatArgs {
@@ -655,6 +662,11 @@ void atomo_v2_launch_powersgd_code_stats(const void* units, const void* tiles, i
   a.scratch = scratch; a.state = (const PwState*)state; a.partials = partials; a.unit_counters = unit_counters;
   a.acc = acc;
   v2_powersgd_code_stats_kernel<<<ntiles, PW_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_powersgd_lw(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsLw& a = *static_cast<const PsArgsLw*>(args);
+  v2_ps_powersgd_lw_kernel<<<ps_grid(grid, a.ntiles), PW_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

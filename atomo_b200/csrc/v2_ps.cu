@@ -29,7 +29,8 @@ constexpr int PS2_SMEM = (PS2_TILE_ELEMS + PS2_KC * V2_MAX_COLS + PS2_KC * PS2_U
 
 extern __shared__ __align__(16) float ps2_smem[];
 
-__global__ void __launch_bounds__(PS2_THREADS) v2_ps_kernel(const PsArgs2 a) {
+template <class A>
+__device__ __forceinline__ void ps_spectral(const A& a) {
   float* OUT = ps2_smem;                         // tile of the averaged gradient, physical element order
   float* SV = OUT + PS2_TILE_ELEMS;              // [PS2_KC][64]
   float* UT = SV + PS2_KC * V2_MAX_COLS;         // [PS2_KC][PS2_UP]  (transposed U chunk)
@@ -110,6 +111,7 @@ __global__ void __launch_bounds__(PS2_THREADS) v2_ps_kernel(const PsArgs2 a) {
   const int per_cta = (a.ntiles + gridDim.x - 1) / gridDim.x;
   const int t_begin = blockIdx.x * per_cta;
   const int t_end = min(a.ntiles, t_begin + per_cta);
+  lw_begin(a);
   for (int ti = t_begin; ok && ti < t_end; ++ti) {
     const Tile2 t = a.tiles[ti];
     const Unit2 u = a.units[t.unit];
@@ -147,6 +149,7 @@ __global__ void __launch_bounds__(PS2_THREADS) v2_ps_kernel(const PsArgs2 a) {
           if ((wmask >> w) & 1u) g += ld_cg_bf16(a.stage_peer[w] + s0 + i);
         update1(a, c, e0 + i, g * inv_w);
       }
+      lw_tile_done(a, ti);
       continue;
     }
 
@@ -289,12 +292,16 @@ __global__ void __launch_bounds__(PS2_THREADS) v2_ps_kernel(const PsArgs2 a) {
         update1(a, c, segbase + s * segstride + i, OUT[v]);
       }
     }
+    lw_tile_done(a, ti);
   }
 
   // ---- completion ------------------------------------------------------------------------------------
   __syncthreads();
   if (tid == 0) ps_complete(a, ctrl, step, s_bad != 0, t_enter, t_ready);
 }
+
+__global__ void __launch_bounds__(PS2_THREADS) v2_ps_kernel(const PsArgs2 a) { ps_spectral(a); }
+__global__ void __launch_bounds__(PS2_THREADS, 1) v2_ps_lw_kernel(const PsArgsLw a) { ps_spectral(a); }
 
 // worker side: block the stream until every owner has delivered its shard of the parameters of `step`
 __global__ void v2_wait_params_kernel(const int* sig, int n_owners, Ctrl2* ctrl, long long timeout, long long* tstats) {
@@ -357,6 +364,16 @@ void atomo_v2_launch_ps(const void* units, const void* tiles, int tile0, int nti
       ps_args(units, tiles, tile0, ntiles, W, nranks, group, final_group, owner, master, mom, sq, sqmax, vmom, vsq,
               vsqmax, wshadow_mc, wshadow_peer, vparams_local, vparams_mc, vparams_peer, vgrads_mc, vgrads_peer,
               stage_peer, arenas, arena_floats, sig, sig_peer, ctrl, group_counter, timeout, tstats, inv_w));
+}
+
+void atomo_v2_launch_ps_spectral_lw(const void* args, int grid, cudaStream_t stream) {
+  static bool attr = false;
+  if (!attr) {
+    cudaFuncSetAttribute(v2_ps_lw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PS2_SMEM);
+    attr = true;
+  }
+  const PsArgsLw& a = *static_cast<const PsArgsLw*>(args);
+  v2_ps_lw_kernel<<<ps_grid(grid, a.ntiles), PS2_THREADS, PS2_SMEM, stream>>>(a);
 }
 
 void atomo_v2_launch_wait_params(const int* sig, int n_owners, void* ctrl, long long timeout, long long* tstats,

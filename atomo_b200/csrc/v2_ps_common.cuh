@@ -4,6 +4,8 @@
 // packing of the launch arguments.  Every v2_ps*_kernel uses them (v2_ps.cu, v2_qsgd.cu, v2_entrywise.cu, v2_sign.cu,
 // v2_fp8.cu, v2_hadamard.cu, v2_powersgd.cu); v2_ps_kernel keeps its own copies where noted.
 #pragma once
+#include <type_traits>
+
 #include "v2_common.cuh"
 
 namespace atomo {
@@ -56,6 +58,92 @@ __device__ __forceinline__ void opt_update(float g, float& p, float& m, float& v
     if (c.opt == OPT_AMSGRAD) { vmax = fmaxf(vmax, v); vv = vmax; }
     const float denom = sqrtf(vv) / c.sbc2 + c.eps;
     p -= (c.lr / c.bc1) * (m / denom);
+  }
+}
+
+// ---- layer-wise optimizers (LARS / LAMB), phase 1 -----------------------------------------------------------------
+// A trust ratio needs whole-tensor norms before any element of the tensor moves, and no owner sees a whole tensor.
+// So every PS kernel has a layer-wise instantiation (its body is a template over the argument type): where the plain one
+// steps the optimizer and broadcasts, it writes the direction x (LARS: d = g + wd w; LAMB: u, after the Adam moments)
+// to `dir` and adds (w^2, x^2) to the thread's partial; the partials are reduced in a fixed order per PS tile into
+// `part`.  Weights are neither written nor broadcast: v2_layerwise.cu (phase 2) takes the norms across tiles and owners
+// and steps them.  Vector tiles are finished here: momentum-SGD (LARS) or Adam (LAMB), without weight decay.
+constexpr int LW_THREADS = 256;   // every PS kernel runs 256 threads
+
+struct PsArgsLw : PsArgs2 {
+  float* dir;      // direction, indexed like master (owner-local scratch)
+  float2* part;    // per PS tile of the launch: (sum w^2, sum x^2)
+};
+
+template <class A>
+constexpr bool ps_layerwise = std::is_same<A, PsArgsLw>::value;
+
+__shared__ float2 lw_acc[LW_THREADS];    // one partial per thread, reduced and zeroed at the end of every weight tile
+
+// the direction of one weight element and its partials (lw_acc of this thread)
+__device__ __forceinline__ float lw_direction(const PsArgsLw& a, const OptC& c, long long e, float g, float p,
+                                              float2& acc) {
+  float x;
+  if (c.opt == OPT_LARS) {
+    x = fmaf(c.wd, p, g);
+    acc.y = fmaf(g, g, acc.y);
+  } else {
+    float m = a.mom[e], v = a.sq[e];
+    m = fmaf(c.b1, m, (1.f - c.b1) * g);
+    v = fmaf(c.b2, v, (1.f - c.b2) * g * g);
+    a.mom[e] = m;
+    a.sq[e] = v;
+    x = fmaf(c.wd, p, (m / c.bc1) / (sqrtf(v) / c.sbc2 + c.eps));
+    acc.y = fmaf(x, x, acc.y);
+  }
+  acc.x = fmaf(p, p, acc.x);
+  return x;
+}
+
+__device__ __forceinline__ void update8(const PsArgsLw& a, const OptC& c, long long e, const float (&g)[8]) {
+  float2 acc = lw_acc[threadIdx.x];
+  const float4 p0 = *reinterpret_cast<const float4*>(a.master + e), p1 = *reinterpret_cast<const float4*>(a.master + e + 4);
+  const float p[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
+  float x[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) x[i] = lw_direction(a, c, e + i, g[i], p[i], acc);
+  *reinterpret_cast<float4*>(a.dir + e) = make_float4(x[0], x[1], x[2], x[3]);
+  *reinterpret_cast<float4*>(a.dir + e + 4) = make_float4(x[4], x[5], x[6], x[7]);
+  lw_acc[threadIdx.x] = acc;
+}
+
+__device__ __forceinline__ void update1(const PsArgsLw& a, const OptC& c, long long e, float g) {
+  float2 acc = lw_acc[threadIdx.x];
+  a.dir[e] = lw_direction(a, c, e, g, a.master[e], acc);
+  lw_acc[threadIdx.x] = acc;
+}
+
+// start of the launch: zero partials
+template <class A>
+__device__ __forceinline__ void lw_begin(const A&) {
+  if constexpr (ps_layerwise<A>) lw_acc[threadIdx.x] = make_float2(0.f, 0.f);
+}
+
+// end of weight tile ti (every thread of the CTA): the partials summed in a fixed order into part[ti], then zeroed
+template <class A>
+__device__ __forceinline__ void lw_tile_done(const A& a, int ti) {
+  if constexpr (ps_layerwise<A>) {
+    __shared__ float2 wsum[LW_THREADS / 32];
+    float2 v = lw_acc[threadIdx.x];
+    lw_acc[threadIdx.x] = make_float2(0.f, 0.f);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      v.x += __shfl_xor_sync(0xffffffffu, v.x, o);
+      v.y += __shfl_xor_sync(0xffffffffu, v.y, o);
+    }
+    __syncthreads();   // every lane's epilogue is done, and the previous tile's wsum has been read
+    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = v;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float2 s = wsum[0];
+      for (int w = 1; w < (int)(blockDim.x >> 5); ++w) { s.x += wsum[w].x; s.y += wsum[w].y; }
+      a.part[ti] = s;
+    }
   }
 }
 
@@ -293,9 +381,19 @@ __device__ __forceinline__ void ps_vec_tile(const PsArgs2& a, const OptC& c, con
   }
 }
 
+// layer-wise: vectors take momentum-SGD (LARS) or Adam (LAMB) without weight decay and trust ratio
+__device__ __forceinline__ void ps_vec_tile(const PsArgsLw& a, const OptC& c, const Unit2& u, const Tile2& t,
+                                            unsigned int wmask, bool all_workers, float inv_w) {
+  OptC cv = c;
+  cv.opt = c.opt == OPT_LARS ? OPT_SGD : OPT_ADAM;
+  cv.wd = 0.f;
+  ps_vec_tile(static_cast<const PsArgs2&>(a), cv, u, t, wmask, all_workers, inv_w);
+}
+
 // ---- bf16 weight tile that travels dense: the counted workers' staged copies summed in worker order, optimizer,
 // bf16 broadcast.  v2_ps_kernel keeps its own inline copy (calling this there changes its instruction schedule).
-__device__ __forceinline__ void ps_dense16_tile(const PsArgs2& a, const OptC& c, const Unit2& u, const Tile2& t,
+template <class A>
+__device__ __forceinline__ void ps_dense16_tile(const A& a, const OptC& c, const Unit2& u, const Tile2& t,
                                                 unsigned int wmask, float inv_w) {
   const int tid = threadIdx.x;
   const long long e0 = u.w_off + t.a;

@@ -266,7 +266,8 @@ __global__ void __launch_bounds__(QE_THREADS) v2_qsgd_stats_kernel(const QStatAr
 }
 
 // ---- PS: decode + sum + optimizer --------------------------------------------------------------------------
-__global__ void __launch_bounds__(QPS_THREADS) v2_ps_qsgd_kernel(const PsArgs2 a) {
+template <class A>
+__device__ __forceinline__ void ps_qsgd(const A& a) {
   __shared__ __align__(16) float OUT[QPS_TILE_ELEMS];   // summed decodes of one tile, physical element order
   __shared__ int s_ok, s_bad;
   __shared__ unsigned int s_mask, s_use;
@@ -283,6 +284,7 @@ __global__ void __launch_bounds__(QPS_THREADS) v2_ps_qsgd_kernel(const PsArgs2 a
   const OptC c = ps_opt_consts(ctrl, step);
   const float inv_w = all_workers ? a.inv_w : 1.f / (float)max(__popc(wmask), 1);
   const auto [t_begin, t_end] = ps_tile_range(a);
+  lw_begin(a);
   for (int ti = t_begin; ok && ti < t_end; ++ti) {
     const Tile2 t = a.tiles[ti];
     const Unit2 u = a.units[t.unit];
@@ -347,11 +349,15 @@ __global__ void __launch_bounds__(QPS_THREADS) v2_ps_qsgd_kernel(const PsArgs2 a
       update8(a, c, e0 + 8LL * v, g);
     }
     for (int i = (nvec << 3) + tid; i < t.b; i += blockDim.x) update1(a, c, e0 + i, OUT[i] * inv_w);
+    lw_tile_done(a, ti);
   }
 
   __syncthreads();
   if (tid == 0) ps_complete(a, ctrl, step, s_bad != 0, t_enter, t_ready);
 }
+
+__global__ void __launch_bounds__(QPS_THREADS) v2_ps_qsgd_kernel(const PsArgs2 a) { ps_qsgd(a); }
+__global__ void __launch_bounds__(QPS_THREADS, 1) v2_ps_qsgd_lw_kernel(const PsArgsLw a) { ps_qsgd(a); }
 
 extern "C" {
 
@@ -393,6 +399,11 @@ void atomo_v2_launch_ps_qsgd(const void* units, const void* tiles, int tile0, in
       ps_args(units, tiles, tile0, ntiles, W, nranks, group, final_group, owner, master, mom, sq, sqmax, vmom, vsq,
               vsqmax, wshadow_mc, wshadow_peer, vparams_local, vparams_mc, vparams_peer, vgrads_mc, vgrads_peer,
               nullptr, arenas, arena_floats, sig, sig_peer, ctrl, group_counter, timeout, tstats, inv_w));
+}
+
+void atomo_v2_launch_ps_qsgd_lw(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsLw& a = *static_cast<const PsArgsLw*>(args);
+  v2_ps_qsgd_lw_kernel<<<ps_grid(grid, a.ntiles), QPS_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

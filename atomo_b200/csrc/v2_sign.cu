@@ -129,7 +129,8 @@ __global__ void __launch_bounds__(SE_THREADS) v2_sign_encode_kernel(const PushAr
 __global__ void __launch_bounds__(SE_THREADS) v2_sign_encode_ef_kernel(const PushArgs a) { sign_encode<true>(a); }
 
 // ---- PS: decode + sum + optimizer --------------------------------------------------------------------------
-__global__ void __launch_bounds__(SPS_THREADS) v2_ps_sign_kernel(const PsArgs2 a) {
+template <class A>
+__device__ __forceinline__ void ps_sign(const A& a) {
   __shared__ __align__(16) float OUT[SPS_TILE_ELEMS];   // summed decodes of one tile, physical element order
   __shared__ int s_ok, s_bad;
   __shared__ unsigned int s_mask, s_use;
@@ -146,6 +147,7 @@ __global__ void __launch_bounds__(SPS_THREADS) v2_ps_sign_kernel(const PsArgs2 a
   const OptC c = ps_opt_consts(ctrl, step);
   const float inv_w = all_workers ? a.inv_w : 1.f / (float)max(__popc(wmask), 1);
   const auto [t_begin, t_end] = ps_tile_range(a);
+  lw_begin(a);
   for (int ti = t_begin; ok && ti < t_end; ++ti) {
     const Tile2 t = a.tiles[ti];
     const Unit2 u = a.units[t.unit];
@@ -197,11 +199,15 @@ __global__ void __launch_bounds__(SPS_THREADS) v2_ps_sign_kernel(const PsArgs2 a
       update8(a, c, e0 + 8LL * v, g);
     }
     for (int i = (nvec << 3) + tid; i < t.b; i += blockDim.x) update1(a, c, e0 + i, OUT[i] * inv_w);
+    lw_tile_done(a, ti);
   }
 
   __syncthreads();
   if (tid == 0) ps_complete(a, ctrl, step, s_bad != 0, s_t_enter, s_t_ready);
 }
+
+__global__ void __launch_bounds__(SPS_THREADS) v2_ps_sign_kernel(const PsArgs2 a) { ps_sign(a); }
+__global__ void __launch_bounds__(SPS_THREADS, 1) v2_ps_sign_lw_kernel(const PsArgsLw a) { ps_sign(a); }
 
 // ---- --code-stats ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(SE_THREADS) v2_sign_code_stats_kernel(const ScaleStatArgs a) {
@@ -292,6 +298,11 @@ void atomo_v2_launch_sign_code_stats(const void* units, const void* tiles, int t
   a.arena_peer = arena_peer; a.n_owners = n_owners; a.arena_floats = arena_floats; a.worker = worker;
   a.partials = partials; a.unit_counters = unit_counters; a.acc = acc;
   v2_sign_code_stats_kernel<<<ntiles, SE_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_sign_lw(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsLw& a = *static_cast<const PsArgsLw*>(args);
+  v2_ps_sign_lw_kernel<<<ps_grid(grid, a.ntiles), SPS_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

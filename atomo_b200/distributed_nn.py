@@ -37,6 +37,7 @@ def _kwargs(args, role: str) -> dict:
     if role == "master":
         kw.update({"num_aggregate": args.num_aggregate, "lr_shrinkage": args.lr_shrinkage,
                    "optimizer": args.optimizer, "weight_decay": args.weight_decay, "nesterov": args.nesterov,
+                   "trust_coefficient": getattr(args, "trust_coefficient", 0.001),
                    "resume": args.resume, "kill_stragglers": args.straggler_kill})
     else:
         kw["split_backward"] = args.straggler_kill

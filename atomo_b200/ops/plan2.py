@@ -81,7 +81,7 @@ UNIT_FMT = "<4q20i"           # 112 bytes, mirrors struct Unit2
 TILE_FMT = "<4i"              # unit, a, b, owner
 UNIT_BYTES = struct.calcsize(UNIT_FMT)
 TILE_BYTES = struct.calcsize(TILE_FMT)
-CTRL2_FMT = "<iiffffiiQffffiiii"   # mirrors struct Ctrl2 (72 bytes)
+CTRL2_FMT = "<iiffffiiQffffiifi"   # mirrors struct Ctrl2 (72 bytes)
 CTRL2_BYTES = struct.calcsize(CTRL2_FMT)
 
 
@@ -771,12 +771,28 @@ def plan_digest(plan: "Plan2") -> str:
     return hashlib.sha256(plan.units_bytes()).hexdigest()
 
 
-OPT_SGD, OPT_ADAM, OPT_AMSGRAD = 0, 1, 2
+OPT_SGD, OPT_ADAM, OPT_AMSGRAD, OPT_LARS, OPT_LAMB = 0, 1, 2, 3, 4
+LAYERWISE_OPTS = (OPT_LARS, OPT_LAMB)
 
 
 def pack_ctrl2(step: int = 1, lr: float = 0.01, momentum: float = 0.0, dampening: float = 0.0,
                weight_decay: float = 0.0, nesterov: bool = False, first_step: int = 1, seed: int = 1,
                beta1: float = 0.9, beta2: float = 0.999, eps: float = 1e-8, opt: int = OPT_SGD,
-               num_aggregate: int = 0) -> bytes:
+               num_aggregate: int = 0, trust_coefficient: float = 0.0) -> bytes:
     return struct.pack(CTRL2_FMT, step, 0, lr, momentum, dampening, weight_decay, int(nesterov), first_step,
-                       seed & 0xFFFFFFFFFFFFFFFF, beta1, beta2, eps, 0.0, int(opt), int(num_aggregate), 0, 0)
+                       seed & 0xFFFFFFFFFFFFFFFF, beta1, beta2, eps, 0.0, int(opt), int(num_aggregate),
+                       float(trust_coefficient), 0)
+
+
+def layerwise_tables(plan: "Plan2") -> Tuple[List[int], List[int]]:
+    """LARS / LAMB (csrc/v2_layerwise.cu): per PS tile of ``plan.ps_tiles``, the group-local index of its weight
+    tensor (-1 for a vector tile), and the number of weight tensors per group.  A tensor is one parameter, however many
+    units (column blocks) it is split into."""
+    local, per_group = {}, [0] * plan.n_groups
+    for q in plan.params:
+        if q.is_w:
+            local[q.index] = per_group[q.group]
+            per_group[q.group] += 1
+    tile_layer = [-1 if plan.units[ui].kind == KIND_VEC else local[plan.units[ui].param]
+                  for (ui, _a, _b, _o) in plan.ps_tiles]
+    return tile_layer, per_group

@@ -20,7 +20,7 @@ import torch
 
 from .. import codings
 from ..models import build_model
-from ..optim import SGD, Adam
+from ..optim import LAMB, LARS, SGD, Adam
 from ..parallel.transport import Transport, STOP_STEP
 from ..utils import checkpoint as ckpt
 from ..utils.logging import MetricsWriter, master_line
@@ -133,6 +133,14 @@ class SyncReplicasMaster_NN(NN_Trainer):
         bind_parameters(self.network, self.flat_params, self.layout)
         if self._optimizer_name == "adam":
             self.optimizer = Adam(self.network.parameters(), lr=self.lr)
+        elif self._optimizer_name == "lars":
+            self.optimizer = LARS(self.network.parameters(), lr=self.lr, momentum=self.momentum,
+                                  weight_decay=self._kwargs.get("weight_decay", 0.0),
+                                  trust_coefficient=self._kwargs.get("trust_coefficient", 0.001),
+                                  nesterov=self._kwargs.get("nesterov", False))
+        elif self._optimizer_name == "lamb":
+            self.optimizer = LAMB(self.network.parameters(), lr=self.lr,
+                                  weight_decay=self._kwargs.get("weight_decay", 0.0))
         else:
             self.optimizer = SGD(self.network.parameters(), lr=self.lr, momentum=self.momentum,
                                  weight_decay=self._kwargs.get("weight_decay", 0.0),

@@ -87,11 +87,16 @@ def _build_engine(args, model, rank, world):
             kw["error_feedback"] = True      # the engine refuses codes / --num-aggregate it cannot feed back
         if accum != 1:
             kw["accumulate_steps"] = accum      # the engine refuses a value below 1
+        if args.optimizer in ("lars", "lamb"):
+            kw["trust_coefficient"] = getattr(args, "trust_coefficient", 0.001)
         return ShadowEngine(model, rank, world, code=args.code, svd_rank=args.svd_rank, lr=args.lr,
                             momentum=args.momentum, weight_decay=args.weight_decay, nesterov=args.nesterov,
                             optimizer=args.optimizer, ps_mode=args.ps_mode, groups=args.groups, sampling=args.sampling,
                             prob_rule=args.prob_rule, seed=args.seed, num_aggregate=args.num_aggregate,
                             timeout_s=args.flag_timeout, **kw), "shadow"
+    if args.optimizer in ("lars", "lamb"):
+        raise SystemExit("--optimizer %s runs on the bf16 engine (--engine shadow, --dtype bf16); the fp32-flat engine "
+                         "has no layer-wise trust ratio" % args.optimizer)
     from .engine import FusedEngine
     if accum != 1:
         raise SystemExit("--accumulate-steps runs on the bf16 engine (--dtype bf16, --engine auto|shadow, --code "

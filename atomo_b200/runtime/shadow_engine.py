@@ -61,7 +61,10 @@ one central PS kernel at the end of the step):
   launch), so every code, ``code_stats`` and the residual work unchanged.  BN statistics take one update per
   micro-batch.  ``N = 1`` launches exactly what it launched before.
 * Optimizers fused in the PS epilogue: momentum-SGD (``src/optim/sgd.py:57-90``), Adam / AMSGrad
-  (``src/optim/adam.py:37-94``).
+  (``src/optim/adam.py:37-94``).  LARS and LAMB (``optimizer="lars" | "lamb"``, ``trust_coefficient``) need whole-tensor
+  norms first: the code's PS kernel runs its layer-wise instantiation (moments, direction, per-tile partials; vectors
+  finished), then ``csrc/v2_layerwise.cu`` takes the norms across tiles and owners, the trust ratios and the step of
+  the weights, and broadcasts them (``optim/lars.py`` / ``optim/lamb.py`` are the oracles).
 
 Per step and rank: ``wait_params`` -> forward -> backward [group hooks -> encode, project+push on stream E;
 PS launch of the group on stream P] -> join -> ``advance_step``.  All cross-GPU ordering is carried by
@@ -102,7 +105,18 @@ class ShadowEngine:
                  warm_start: bool = True, max_sweeps: int = 1, main_priority: int = 0, debug_jitter_us: float = 0.0,
                  side_priority: int = -1, resample_empty: bool = False, quantization_level: int = 4,
                  bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False,
-                 error_feedback: bool = False, accumulate_steps: int = 1):
+                 error_feedback: bool = False, accumulate_steps: int = 1, trust_coefficient: float = 0.001):
+        self.optimizer = optimizer.lower()
+        if self.optimizer not in ("sgd", "adam", "lars", "lamb"):      # checked before any CUDA work
+            raise ValueError("ShadowEngine optimizers: sgd | adam | lars | lamb (got %r)" % (optimizer,))
+        self.layerwise = self.optimizer in ("lars", "lamb")
+        if self.optimizer == "lars" and (nesterov or dampening != 0):
+            raise ValueError("lars takes plain momentum: nesterov=False and dampening=0")
+        if self.optimizer == "lars" and not trust_coefficient > 0:
+            raise ValueError("lars: trust_coefficient must be positive (got %r)" % (trust_coefficient,))
+        if self.optimizer == "lamb" and amsgrad:
+            raise ValueError("lamb has no AMSGrad variant (amsgrad=False)")
+        self.trust_coefficient = float(trust_coefficient)
         if isinstance(accumulate_steps, bool) or not isinstance(accumulate_steps, numbers.Integral) \
                 or accumulate_steps < 1:        # checked before any CUDA work
             raise ValueError("accumulate_steps must be an integer >= 1 (got %r)" % (accumulate_steps,))
@@ -205,7 +219,8 @@ class ShadowEngine:
         self.criterion = criterion or nn.CrossEntropyLoss()
         self.timeout_ticks = int(timeout_s * 1.5e9)
         self.step, self.lr = 1, lr
-        self.opt = {"sgd": P2.OPT_SGD, "adam": P2.OPT_AMSGRAD if amsgrad else P2.OPT_ADAM}[optimizer.lower()]
+        self.opt = {"sgd": P2.OPT_SGD, "adam": P2.OPT_AMSGRAD if amsgrad else P2.OPT_ADAM, "lars": P2.OPT_LARS,
+                    "lamb": P2.OPT_LAMB}[self.optimizer]
         self.launches_per_step = 0
 
         # ---- model: NHWC activations, fused BN ------------------------------------------------------------
@@ -223,8 +238,12 @@ class ShadowEngine:
         self.G = pl.n_groups
 
         # ---- symmetric heap ---------------------------------------------------------------------------------
+        # LARS / LAMB: per group, the per-tensor norms every owner exchanges ([2 step parities][owner][tensor][2] fp64)
+        self.lw_tile_layer, self.lw_layers = P2.layerwise_tables(pl) if self.layerwise else ([], [])
+        self.lw_xch_off = [2 * 2 * self.n_owners * sum(self.lw_layers[:g]) for g in range(self.G)]
+        xch_doubles = 2 * 2 * self.n_owners * sum(self.lw_layers)
         need = 4 * SIGNAL_INTS + 2 * pl.w_total + 8 * pl.v_total + 2 * pl.stage_total + \
-            4 * pl.arena_floats * self.W + (1 << 16)
+            4 * pl.arena_floats * self.W + 8 * xch_doubles + (1 << 16)
         self.heap = h = SymmetricHeap(need + (1 << 20), rank, world, dev.index, group=group, multicast=multicast,
                                       mode=heap_mode)
         h.alloc("signals", 4 * SIGNAL_INTS)
@@ -233,6 +252,8 @@ class ShadowEngine:
         h.alloc("vgrads", 4 * pl.v_total)
         h.alloc("wstage", 2 * pl.stage_total)
         h.alloc("arena", 4 * pl.arena_floats * self.W)
+        if self.layerwise:
+            h.alloc("lwx", 8 * max(xch_doubles, 2))
         self.signals = h.tensor("signals", torch.int32)
         self.wshadow = h.tensor("wshadow", torch.bfloat16)
         self.vparams = h.tensor("vparams")
@@ -292,7 +313,7 @@ class ShadowEngine:
 
         # ---- owner state ----------------------------------------------------------------------------------
         z = lambda n: torch.zeros(n, dtype=torch.float32, device=dev)
-        adam = self.opt != P2.OPT_SGD
+        adam = self.opt in (P2.OPT_ADAM, P2.OPT_AMSGRAD, P2.OPT_LAMB)
         if self.is_owner:
             self.mom, self.vmom = z(pl.w_total), z(pl.v_total)
             self.sq, self.vsq = (z(pl.w_total), z(pl.v_total)) if adam else (None, None)
@@ -350,7 +371,8 @@ class ShadowEngine:
         self.ctrl = _dev_bytes(P2.pack_ctrl2(step=1, lr=lr, momentum=momentum, dampening=dampening,
                                              weight_decay=weight_decay, nesterov=nesterov, first_step=1, seed=seed,
                                              beta1=betas[0], beta2=betas[1], eps=eps, opt=self.opt,
-                                             num_aggregate=num_aggregate), dev)
+                                             num_aggregate=num_aggregate,
+                                             trust_coefficient=self.trust_coefficient if self.layerwise else 0.0), dev)
         self.ctrl_i32, self.ctrl_f32 = self.ctrl.view(torch.int32), self.ctrl.view(torch.float32)
         n_w = max(len(self.w_params), 1)
         self.t_gptr = torch.zeros(n_w, dtype=torch.int64, device=dev)
@@ -367,6 +389,22 @@ class ShadowEngine:
         self.vgrads_mc = h.region_mc_ptr("vgrads")
         sm = torch.cuda.get_device_properties(dev).multi_processor_count
         self.ps_grid = ps_grid or 3 * sm
+        # LARS / LAMB (csrc/v2_layerwise.cu): the owner's direction per weight element (indexed like master), the
+        # (sum w^2, sum x^2) of every PS tile, the tensor of every PS tile, the exchange slots and the trust ratios
+        self.lw_dir = self.lw_part = self.t_lw_tile_layer = self.lw_ratio = self.lw_counter = None
+        self.t_lw_xch_peer = []
+        if self.layerwise:
+            if max(self.lw_layers, default=0) > C.v2_layerwise_max_layers():
+                raise ValueError("lars / lamb: at most %d weight tensors per backward group (use more groups)"
+                                 % C.v2_layerwise_max_layers())
+            self.lw_ratio = z(max(sum(self.lw_layers), 1))
+            self.lw_counter = torch.zeros(P2.MAX_GROUPS, dtype=torch.int32, device=dev)
+            if self.is_owner:
+                self.lw_dir = z(pl.w_total)
+                self.lw_part = z(2 * max(len(pl.ps_tiles), 1))
+                self.t_lw_tile_layer = torch.tensor(self.lw_tile_layer or [0], dtype=torch.int32, device=dev)
+            self.t_lw_xch_peer = [i64(h.region_ptr("lwx", r) + 8 * self.lw_xch_off[g] for r in range(world))
+                                  for g in range(self.G)]
         self.tstats = torch.zeros(32, dtype=torch.int64, device=dev)
         # --code-stats: per coded unit fp64 sums over steps (v2_stats.cu), the per-tile partials and unit counters
         self.code_stats_on = bool(code_stats)
@@ -726,6 +764,9 @@ class ShadowEngine:
         C, pl = self.C, self.plan
         t0, nt = pl.ps_range[g][self.owner_index]
         p = lambda t: t.data_ptr() if t is not None else 0
+        if self.layerwise:
+            self._launch_ps_layerwise(g, final, t0, nt)
+            return
         if self.quant:
             C.v2_ps_qsgd(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g, final,
                          self.owner_index, p(self.master), p(self.mom), p(self.sq), p(self.sqmax), p(self.vmom),
@@ -778,6 +819,48 @@ class ShadowEngine:
                 self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(), self.cnt_ps_group + 4 * g,
                 self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W, max(1, min(self.ps_grid, max(nt, 1))))
         self._nlaunch += 1
+
+    def _launch_ps_layerwise(self, g: int, final: bool, t0: int, nt: int):
+        """LARS / LAMB: phase 1 (the code's PS kernel with the layer-wise epilogue: moments, direction, tile
+        partials, vectors finished), then phase 2 (norms across tiles and owners, trust ratios, the step of the
+        weights and their bf16 broadcast; the last group publishes the parameters)."""
+        C, pl = self.C, self.plan
+        p = lambda t: t.data_ptr() if t is not None else 0
+        grid = max(1, min(self.ps_grid, max(nt, 1)))
+        ps = 1 if self.quant else 2 if self.entry else 3 if self.sign else 4 if self.fp8 else 5 if self.hadamard \
+            else 6 if self.power else 0
+        part = self.lw_part.data_ptr() + 8 * t0
+        C.v2_ps_layerwise(ps, self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g,
+                          self.owner_index, p(self.master), p(self.mom), p(self.sq), p(self.vmom), p(self.vsq),
+                          self.vparams.data_ptr(), self.vparams_mc, self.t_vparams_peer.data_ptr(), self.vgrads_mc,
+                          self.t_vgrads_peer.data_ptr(), self.t_stage_peer.data_ptr(), self.heap.region_ptr("arena"),
+                          pl.arena_floats, self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
+                          self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
+                          self.lw_dir.data_ptr(), part, grid, self.q_max_level, self.q_max_bucket)
+        C.v2_layerwise(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt,
+                       self.t_lw_tile_layer.data_ptr() + 4 * t0, self.lw_layers[g], part, self.lw_dir.data_ptr(),
+                       self.world, g, final, self.owner_index, self.n_owners, p(self.master), p(self.mom),
+                       self.wshadow_mc, self.t_wshadow_peer.data_ptr(),
+                       self.heap.region_ptr("lwx") + 8 * self.lw_xch_off[g], self.t_lw_xch_peer[g].data_ptr(),
+                       self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
+                       self.lw_counter.data_ptr() + 4 * g, self.timeout_ticks, self.tstats.data_ptr(),
+                       self.lw_ratio.data_ptr() + 4 * sum(self.lw_layers[:g]), grid)
+        self._nlaunch += 2
+
+    def trust_ratios(self) -> dict:
+        """LARS / LAMB: the trust ratio of every weight tensor in the last step (parameter name -> ratio), as this
+        owner's phase 2 computed it.  Reading it synchronises the device."""
+        if not self.layerwise:
+            raise RuntimeError("trust_ratios() needs ShadowEngine(..., optimizer='lars' | 'lamb')")
+        names = {id(p): n for n, p in self.model.named_parameters()}
+        r = self.lw_ratio.tolist()
+        base = [sum(self.lw_layers[:g]) for g in range(self.G)]
+        out, seen = {}, [0] * self.G
+        for p, q in zip(self.params, self.plan.params):
+            if q.is_w:
+                out[names.get(id(p), str(q.index))] = r[base[q.group] + seen[q.group]]
+                seen[q.group] += 1
+        return out
 
     def _launch_group(self, g: int):
         """Called from the autograd thread when the last gradient of group ``g`` exists: fork the encode stream
@@ -1048,7 +1131,8 @@ class ShadowEngine:
             carries over; ``R^{-1}``, the mask and the non-finite flag are rewritten by pass A before pass B reads
             them; its unit counters are zero between launches); the device's default CUDA generator (seed and
             offset), from which the model's dropout layers draw their masks (VGG's classifier).
-        (c) scratch, rewritten every step before it is read: the rest of ``gpart`` (Gram partials, ``P``,
+        (c) scratch, rewritten every step before it is read: LARS / LAMB's direction ``lw_dir``, tile partials
+            ``lw_part``, exchange slots and trust ratios; the rest of ``gpart`` (Gram partials, ``P``,
             ``P_hat``, ``Q'``), ``vsel``, ``selcount``, ``sigma``, ``clip`` / ``clip_partials``, ``l1`` /
             ``l1_partials``, ``topk_sel``, ``topk_tiles``, ``pw_gram``, ``stats_partials``, ``vgrads``, ``wstage``,
             the gradient-accumulation sums ``acc`` / ``vacc`` (zero at every step boundary) and pointer tables,
@@ -1067,7 +1151,8 @@ class ShadowEngine:
         if self.world > 1:
             dist.all_reduce(vm, group=self.group)
         adam_state = {}
-        if self.opt != P2.OPT_SGD:      # Adam / AMSGrad: second moments too (collective gathers, every rank takes part)
+        if self.opt != P2.OPT_SGD and self.opt != P2.OPT_LARS:      # Adam / AMSGrad / LAMB: second moments too
+            # (collective gathers, every rank takes part)
             names = [("sq", "vsq")] + ([("sqmax", "vsqmax")] if self.opt == P2.OPT_AMSGRAD else [])
             for wname, vname in names:
                 vt = (getattr(self, vname) if self.is_owner else torch.zeros_like(self.vparams)) * mv
@@ -1086,7 +1171,7 @@ class ShadowEngine:
         torch.save({k: v.cpu() for k, v in sd.items()}, tmp)
         os.replace(tmp, path)
         side = {"step": step, "lr": self.lr, "mom_w": mom.cpu(), "mom_v": vm.cpu(), "code": self.code,
-                "svd_rank": self.svd_rank, "engine": "shadow"}
+                "svd_rank": self.svd_rank, "engine": "shadow", "optimizer": self.optimizer}
         if self.quant or self.hadamard:
             side.update(quantization_level=self.quantization_level, bucket_size=self.bucket_size)
         if self.sign or self.fp8:
@@ -1150,6 +1235,12 @@ class ShadowEngine:
         from ..utils import checkpoint as ckpt
         self._barrier()
         path = ckpt.model_path(train_dir, step)
+        if os.path.exists(path + "_optim"):     # refused before any state changes
+            saved = torch.load(path + "_optim", map_location="cpu", weights_only=False).get("optimizer", "sgd or adam")
+            layerwise = ("lars", "lamb")
+            if (self.layerwise or saved in layerwise) and saved != self.optimizer:
+                raise ValueError("checkpoint %s was written by optimizer %s; this engine runs %s" % (path, saved,
+                                                                                                  self.optimizer))
         sd = torch.load(path, map_location="cpu", weights_only=False)
         byname = dict(self.model.named_parameters())
         byid = {id(p): q for p, q in zip(self.params, self.plan.params)}

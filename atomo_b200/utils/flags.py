@@ -66,7 +66,11 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                    "elements below 1, else an atom count (top-k sends floor of it)")
     p.add_argument("--sampling", type=str, default="bernoulli", choices=["bernoulli", "systematic"])
     p.add_argument("--prob-rule", type=str, default="reference", choices=["reference", "waterfill"])
-    p.add_argument("--optimizer", type=str, default="sgd", choices=["sgd", "adam"])
+    p.add_argument("--optimizer", type=str, default="sgd", choices=["sgd", "adam", "lars", "lamb"],
+                   help="lars / lamb: layer-wise trust ratios (LARS on momentum-SGD, LAMB on Adam) for large batches; "
+                        "p2p backend on the bf16 engine (--engine shadow), or the gloo / nccl role path")
+    p.add_argument("--trust-coefficient", type=float, default=0.001,
+                   help="--optimizer lars: eta of the trust ratio eta ||w|| / (||g|| + wd ||w||)")
     p.add_argument("--weight-decay", type=float, default=0.0)
     p.add_argument("--nesterov", type=bool_flag, default=False)
     p.add_argument("--resume", type=bool_flag, default=False)
