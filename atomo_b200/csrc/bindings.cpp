@@ -248,6 +248,20 @@ void atomo_v2_launch_layerwise(const void* units, const void* tiles, int tile0, 
                                void* const* wshadow_peer, double* xch, double* const* xch_peer, int* sig,
                                int* const* sig_peer, void* ctrl, unsigned int* group_counter, long long timeout,
                                long long* tstats, float* ratio_out, int grid, cudaStream_t stream);
+// v2_clip.cu (gradient-norm clipping on the bf16 engine: phase 1 = the PS kernels' gather instantiations, phase 2)
+void atomo_v2_launch_ps_gather(int ps, const void* units, const void* tiles, int tile0, int ntiles, int W, int nranks,
+                               int group, int owner, const float* vgrads_mc, const float* const* vgrads_peer,
+                               const void* const* stage_peer, const float* arenas, long long arena_floats, int* sig,
+                               int* const* sig_peer, void* ctrl, unsigned int* group_counter, long long timeout,
+                               long long* tstats, float inv_w, float* grad, float* vgrad, void* part, int grid,
+                               cudaStream_t stream);
+void atomo_v2_launch_clip(int layerwise, const void* units, const void* tiles, const int* owner_tiles, int ntiles,
+                          const void* gpart, const float* grad, const float* vgrad, int nranks, int owner, int n_owners,
+                          float* master, float* mom, float* sq, float* sqmax, float* vmom, float* vsq, float* vsqmax,
+                          void* wshadow_mc, void* const* wshadow_peer, float* vparams_local, float* vparams_mc,
+                          float* const* vparams_peer, float* dir, void* lwpart, double* xch, double* const* xch_peer,
+                          int* sig, int* const* sig_peer, void* ctrl, unsigned int* counter, long long timeout,
+                          long long* tstats, float* norm_out, int grid, cudaStream_t stream);
 void atomo_v2_launch_bcast_bytes(const void* src, void* const* peer, void* mc, int nranks, int self, long long nbytes,
                                  cudaStream_t stream);
 // gemm_kernels.cu
@@ -927,6 +941,49 @@ void v2_layerwise(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_
                             P<float>(ratio_out), grid, cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
+// gradient-norm clipping phase 1: the code's PS kernel (`ps` as v2_ps_layerwise) with the gather epilogue: mean
+// gradient into grad / vgrad, sum g^2 per PS tile; `part` points at the launch's first tile
+void v2_ps_gather(int ps, uint64_t units, uint64_t tiles, int tile0, int ntiles, int W, int nranks, int group,
+                  int owner, uint64_t vgrads_mc, uint64_t vgrads_peer, uint64_t stage_peer, uint64_t arenas,
+                  int64_t arena_floats, uint64_t sig, uint64_t sig_peer, uint64_t ctrl, uint64_t group_counter,
+                  int64_t timeout, uint64_t tstats, double inv_w, uint64_t grad, uint64_t vgrad, uint64_t part, int grid,
+                  int max_level, int max_bucket) {
+  TORCH_CHECK(ps >= 0 && ps <= 6, "v2_ps_gather: unknown PS kernel");
+  TORCH_CHECK(W >= 1 && W <= 16, "too many workers for v2_ps_gather");
+  TORCH_CHECK(grad != 0 && vgrad != 0 && part != 0, "v2_ps_gather: grad / vgrad / part required");
+  if (ps == 1) check_qsgd_plan(max_level, max_bucket);
+  atomo_v2_launch_ps_gather(ps, P<const void>(units), P<const void>(tiles), tile0, ntiles, W, nranks, group, owner,
+                            P<const float>(vgrads_mc), P<const float* const>(vgrads_peer),
+                            P<const void* const>(stage_peer), P<const float>(arenas), arena_floats, P<int>(sig),
+                            P<int* const>(sig_peer), P<void>(ctrl), P<unsigned int>(group_counter), timeout,
+                            P<long long>(tstats), (float)inv_w, P<float>(grad), P<float>(vgrad), P<void>(part), grid,
+                            cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+// gradient-norm clipping phase 2: the whole-model norm across tiles and owners, the clip coefficient, and the step of
+// every tile of the owner (with `layerwise`, LARS / LAMB's direction and tile partials instead; v2_layerwise follows)
+void v2_clip(bool layerwise, uint64_t units, uint64_t tiles, uint64_t owner_tiles, int ntiles, uint64_t gpart,
+             uint64_t grad, uint64_t vgrad, int nranks, int owner, int n_owners, uint64_t master, uint64_t mom,
+             uint64_t sq, uint64_t sqmax, uint64_t vmom, uint64_t vsq, uint64_t vsqmax, uint64_t wshadow_mc,
+             uint64_t wshadow_peer, uint64_t vparams_local, uint64_t vparams_mc, uint64_t vparams_peer, uint64_t dir,
+             uint64_t lwpart, uint64_t xch, uint64_t xch_peer, uint64_t sig, uint64_t sig_peer, uint64_t ctrl,
+             uint64_t counter, int64_t timeout, uint64_t tstats, uint64_t norm_out, int grid) {
+  TORCH_CHECK(ntiles >= 0 && (ntiles == 0 || owner_tiles != 0), "v2_clip: owner tile list required");
+  TORCH_CHECK(n_owners >= 1 && n_owners <= 16 && owner >= 0 && owner < n_owners, "v2_clip: bad owner");
+  TORCH_CHECK(n_owners == 1 || (xch != 0 && xch_peer != 0), "v2_clip: several owners need the exchange slots");
+  TORCH_CHECK(gpart != 0 && grad != 0 && vgrad != 0 && master != 0 && mom != 0 && counter != 0,
+              "v2_clip: gpart / grad / vgrad / master / mom / counter required");
+  TORCH_CHECK(!layerwise || (dir == grad && lwpart != 0), "v2_clip: LARS / LAMB take the direction in grad");
+  atomo_v2_launch_clip(layerwise ? 1 : 0, P<const void>(units), P<const void>(tiles), P<const int>(owner_tiles), ntiles,
+                       P<const void>(gpart), P<const float>(grad), P<const float>(vgrad), nranks, owner, n_owners,
+                       P<float>(master), P<float>(mom), P<float>(sq), P<float>(sqmax), P<float>(vmom), P<float>(vsq),
+                       P<float>(vsqmax), P<void>(wshadow_mc), P<void* const>(wshadow_peer), P<float>(vparams_local),
+                       P<float>(vparams_mc), P<float* const>(vparams_peer), P<float>(dir), P<void>(lwpart),
+                       P<double>(xch), P<double* const>(xch_peer), P<int>(sig), P<int* const>(sig_peer),
+                       P<void>(ctrl), P<unsigned int>(counter), timeout, P<long long>(tstats), P<float>(norm_out), grid,
+                       cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
 void v2_accum_fold(uint64_t wchunks, int nw, uint64_t vchunks, int nv, uint64_t gptr, uint64_t acc, uint64_t vacc,
                    uint64_t vgrads, float inv_n, uint64_t residual) {
   TORCH_CHECK(nw >= 0 && nv >= 0, "v2_accum_fold: negative chunk count");
@@ -1126,6 +1183,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("v2_ps_layerwise", &v2_ps_layerwise);
   m.def("v2_layerwise", &v2_layerwise);
   m.def("v2_layerwise_max_layers", &atomo_v2_layerwise_max_layers);
+  m.def("v2_ps_gather", &v2_ps_gather);
+  m.def("v2_clip", &v2_clip);
   m.def("v2_ps_entry", &v2_ps_entry);
   m.def("v2_code_stats", &v2_code_stats);
   m.def("v2_stats_fields", &atomo_v2_stats_fields);

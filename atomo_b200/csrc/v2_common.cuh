@@ -80,7 +80,8 @@ struct Ctrl2 {
   int nesterov;
   int first_step;
   unsigned long long seed;
-  float beta1, beta2, eps, pad0;
+  float beta1, beta2, eps;
+  float clip_grad_norm;   // max whole-model gradient norm; 0 = no clipping (v2_clip.cu)
   int opt;
   int num_aggregate;   // 0 = wait for every worker; N = proceed after N pushes (backup workers)
   float trust_coefficient;   // LARS: eta of the trust ratio (v2_layerwise.cu)
@@ -98,11 +99,14 @@ constexpr int V2_MAX_COLS = TS_MAX_COLS;
 constexpr int V2_RCAP_MAX = RCAP_MAX;
 // signal region (ints): push flag of (group g, worker w) at g*MAX_WORKERS + w; param flag of owner o at 256 + o;
 // aggregation mask of (group g) at 320 + 2g (owner-local); layer-wise norms of (group g, owner o) published at
-// 352 + g*MAX_WORKERS + o (v2_layerwise.cu)
+// 352 + g*MAX_WORKERS + o (v2_layerwise.cu); gradient-norm clipping: owner o's squared norm published at 480 + o
+// (v2_clip.cu)
 constexpr int SIG_PUSH = 0;
 constexpr int SIG_PARAM = 256;
 constexpr int SIG_MASK = 320;
 constexpr int SIG_NORMS = 352;
+constexpr int SIG_CLIP = SIG_NORMS + MAX_GROUPS * MAX_WORKERS;
+static_assert(SIG_CLIP + MAX_WORKERS <= 1024, "the signal region holds SIGNAL_INTS = 1024 ints (runtime/shadow_engine.py)");
 
 __device__ __forceinline__ float bf16_lo(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }

@@ -102,6 +102,7 @@ __device__ __forceinline__ void ps_entry(const A& a) {
     const Unit2 u = a.units[t.unit];
     if (u.kind == KIND_VEC) {
       ps_vec_tile(a, c, u, t, wmask, all_workers, inv_w);
+      clip_vec_done(a, ti);
       continue;
     }
     if (u.kind != KIND_ENTRY) continue;
@@ -158,6 +159,7 @@ __device__ __forceinline__ void ps_entry(const A& a) {
 
 __global__ void __launch_bounds__(EPS_THREADS) v2_ps_entry_kernel(const PsArgs2 a) { ps_entry(a); }
 __global__ void __launch_bounds__(EPS_THREADS, 1) v2_ps_entry_lw_kernel(const PsArgsLw a) { ps_entry(a); }
+__global__ void __launch_bounds__(EPS_THREADS, 1) v2_ps_entry_gather_kernel(const PsArgsGather a) { ps_entry(a); }
 
 extern "C" {
 
@@ -203,6 +205,11 @@ void atomo_v2_launch_ps_entry(const void* units, const void* tiles, int tile0, i
 void atomo_v2_launch_ps_entry_lw(const void* args, int grid, cudaStream_t stream) {
   const PsArgsLw& a = *static_cast<const PsArgsLw*>(args);
   v2_ps_entry_lw_kernel<<<ps_grid(grid, a.ntiles), EPS_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_entry_gather(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsGather& a = *static_cast<const PsArgsGather*>(args);
+  v2_ps_entry_gather_kernel<<<ps_grid(grid, a.ntiles), EPS_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

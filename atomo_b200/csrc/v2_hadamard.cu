@@ -363,6 +363,7 @@ __device__ __forceinline__ void ps_hadamard(const A& a) {
     const Unit2 u = a.units[t.unit];
     if (u.kind == KIND_VEC) {
       ps_vec_tile(a, c, u, t, wmask, all_workers, inv_w);
+      clip_vec_done(a, ti);
       continue;
     }
     if (u.kind != KIND_HADAMARD) continue;
@@ -400,7 +401,7 @@ __device__ __forceinline__ void ps_hadamard(const A& a) {
       const float xr = __fmul_rn(g[r], inv_d);
       g[r] = __fmul_rn(((neg >> r) & 1u) ? -xr : xr, inv_w);
     }
-    if constexpr (ps_layerwise<A>) {   // the epilogue below, then the reduction every thread of the CTA reaches
+    if constexpr (ps_tile_partials<A>) {   // the epilogue below, then the reduction every thread of the CTA reaches
       if (live && i0 < t.b) {
         const long long ew = u.w_off + e0;
         if (i0 + 16 <= t.b) {
@@ -432,6 +433,7 @@ __device__ __forceinline__ void ps_hadamard(const A& a) {
 
 __global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_kernel(const PsArgs2 a) { ps_hadamard(a); }
 __global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_lw_kernel(const PsArgsLw a) { ps_hadamard(a); }
+__global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_gather_kernel(const PsArgsGather a) { ps_hadamard(a); }
 
 // ---- --code-stats ------------------------------------------------------------------------------------------
 struct HStatArgs {
@@ -550,6 +552,11 @@ void atomo_v2_launch_hadamard_code_stats(const void* units, const void* tiles, i
 void atomo_v2_launch_ps_hadamard_lw(const void* args, int grid, cudaStream_t stream) {
   const PsArgsLw& a = *static_cast<const PsArgsLw*>(args);
   v2_ps_hadamard_lw_kernel<<<ps_grid(grid, a.ntiles), HD_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_hadamard_gather(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsGather& a = *static_cast<const PsArgsGather*>(args);
+  v2_ps_hadamard_gather_kernel<<<ps_grid(grid, a.ntiles), HD_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

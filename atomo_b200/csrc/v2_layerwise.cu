@@ -32,31 +32,6 @@ struct LwArgs : PsArgs2 {
   float* ratio_out;          // [nlayers] the group's trust ratios (diagnostics; written by CTA 0)
 };
 
-// The elements of PS tile t of unit u: nseg segments of seglen elements, segstride apart, from segbase (the tiles of
-// v2_ps_kernel's low-rank epilogue, of PowerSGD's row tiles, and of every code whose tiles are consecutive elements)
-struct LwSegs {
-  int nseg, seglen;
-  long long segbase, segstride;
-};
-
-__device__ __forceinline__ LwSegs lw_tile_segs(const Unit2& u, const Tile2& t) {
-  LwSegs s;
-  if (u.kind == KIND_SLAB) {
-    const int half = u.I >> 1;
-    s.nseg = 1; s.seglen = (t.b / half) * u.K * u.I; s.segbase = u.w_off + (long long)(t.a / half) * u.K * u.I;
-    s.segstride = 0;
-  } else if (u.kind == KIND_MAT && u.cs == 1) {
-    s.nseg = t.b; s.seglen = u.cols; s.segbase = u.w_off + (long long)t.a * u.rs; s.segstride = u.rs;
-  } else if (u.kind == KIND_MAT) {
-    s.nseg = u.cols; s.seglen = t.b; s.segbase = u.w_off + t.a; s.segstride = u.cs;
-  } else if (u.kind == KIND_POWER) {
-    s.nseg = 1; s.seglen = t.b * u.cols; s.segbase = u.w_off + (long long)t.a * u.cols; s.segstride = 0;
-  } else {
-    s.nseg = 1; s.seglen = t.b; s.segbase = u.w_off + t.a; s.segstride = 0;
-  }
-  return s;
-}
-
 __device__ __forceinline__ float lw_step(const OptC& c, float ratio, float x, float p, float& m) {
   if (c.opt == OPT_LARS) {
     m = c.first ? ratio * x : fmaf(c.mu, m, ratio * x);

@@ -439,6 +439,7 @@ __device__ __forceinline__ void ps_powersgd(const A& a) {
     const Unit2 u = a.units[t.unit];
     if (u.kind == KIND_VEC) {
       ps_vec_tile(a, c, u, t, wmask, all_workers, inv_w);
+      clip_vec_done(a, ti);
       continue;
     }
     if (u.kind == KIND_DENSE16) {
@@ -525,6 +526,7 @@ __device__ __forceinline__ void ps_powersgd(const A& a) {
 
 __global__ void __launch_bounds__(PW_THREADS) v2_ps_powersgd_kernel(const PsArgs2 a) { ps_powersgd(a); }
 __global__ void __launch_bounds__(PW_THREADS, 1) v2_ps_powersgd_lw_kernel(const PsArgsLw a) { ps_powersgd(a); }
+__global__ void __launch_bounds__(PW_THREADS, 1) v2_ps_powersgd_gather_kernel(const PsArgsGather a) { ps_powersgd(a); }
 
 // ---- --code-stats ------------------------------------------------------------------------------------------------
 struct PwStatArgs {
@@ -667,6 +669,11 @@ void atomo_v2_launch_powersgd_code_stats(const void* units, const void* tiles, i
 void atomo_v2_launch_ps_powersgd_lw(const void* args, int grid, cudaStream_t stream) {
   const PsArgsLw& a = *static_cast<const PsArgsLw*>(args);
   v2_ps_powersgd_lw_kernel<<<ps_grid(grid, a.ntiles), PW_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_powersgd_gather(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsGather& a = *static_cast<const PsArgsGather*>(args);
+  v2_ps_powersgd_gather_kernel<<<ps_grid(grid, a.ntiles), PW_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

@@ -78,6 +78,25 @@ struct PsArgsLw : PsArgs2 {
 template <class A>
 constexpr bool ps_layerwise = std::is_same<A, PsArgsLw>::value;
 
+// ---- gradient-norm clipping, phase 1 ("gather") ------------------------------------------------------------------
+// The clip coefficient needs the norm of the whole step's gradient, summed over every group and owner, before any
+// element moves.  So with clipping on, every PS kernel runs its gather instantiation: it stores the mean gradient g
+// (the value the plain instantiation hands to the optimizer) into owner-local fp32 scratch and reduces sum g^2 per PS
+// tile, vector tiles included, in a fixed order into part[ti].x.  It steps, broadcasts and publishes nothing:
+// v2_clip.cu (phase 2) takes the norm across tiles and owners and steps every tile of the owner.
+struct PsArgsGather : PsArgs2 {
+  float* grad;     // g, indexed like master (owner-local scratch)
+  float* vgrad;    // g of the vector tiles, indexed like vparams
+  float2* part;    // per PS tile of the launch: (sum g^2, 0)
+};
+
+template <class A>
+constexpr bool ps_gather = std::is_same<A, PsArgsGather>::value;
+
+// the instantiations that reduce a partial per PS tile into a.part (lw_begin / lw_tile_done)
+template <class A>
+constexpr bool ps_tile_partials = ps_layerwise<A> || ps_gather<A>;
+
 __shared__ float2 lw_acc[LW_THREADS];    // one partial per thread, reduced and zeroed at the end of every weight tile
 
 // the direction of one weight element and its partials (lw_acc of this thread)
@@ -118,16 +137,30 @@ __device__ __forceinline__ void update1(const PsArgsLw& a, const OptC& c, long l
   lw_acc[threadIdx.x] = acc;
 }
 
+__device__ __forceinline__ void update8(const PsArgsGather& a, const OptC&, long long e, const float (&g)[8]) {
+  float2 acc = lw_acc[threadIdx.x];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) acc.x = fmaf(g[i], g[i], acc.x);
+  *reinterpret_cast<float4*>(a.grad + e) = make_float4(g[0], g[1], g[2], g[3]);
+  *reinterpret_cast<float4*>(a.grad + e + 4) = make_float4(g[4], g[5], g[6], g[7]);
+  lw_acc[threadIdx.x] = acc;
+}
+
+__device__ __forceinline__ void update1(const PsArgsGather& a, const OptC&, long long e, float g) {
+  lw_acc[threadIdx.x].x = fmaf(g, g, lw_acc[threadIdx.x].x);
+  a.grad[e] = g;
+}
+
 // start of the launch: zero partials
 template <class A>
 __device__ __forceinline__ void lw_begin(const A&) {
-  if constexpr (ps_layerwise<A>) lw_acc[threadIdx.x] = make_float2(0.f, 0.f);
+  if constexpr (ps_tile_partials<A>) lw_acc[threadIdx.x] = make_float2(0.f, 0.f);
 }
 
-// end of weight tile ti (every thread of the CTA): the partials summed in a fixed order into part[ti], then zeroed
+// end of PS tile ti (every thread of the CTA): the partials summed in a fixed order into part[ti], then zeroed
 template <class A>
 __device__ __forceinline__ void lw_tile_done(const A& a, int ti) {
-  if constexpr (ps_layerwise<A>) {
+  if constexpr (ps_tile_partials<A>) {
     __shared__ float2 wsum[LW_THREADS / 32];
     float2 v = lw_acc[threadIdx.x];
     lw_acc[threadIdx.x] = make_float2(0.f, 0.f);
@@ -145,6 +178,31 @@ __device__ __forceinline__ void lw_tile_done(const A& a, int ti) {
       a.part[ti] = s;
     }
   }
+}
+
+// The elements of PS tile t of unit u: nseg segments of seglen elements, segstride apart, from segbase (the tiles of
+// v2_ps_kernel's low-rank epilogue, of PowerSGD's row tiles, and of every code whose tiles are consecutive elements)
+struct LwSegs {
+  int nseg, seglen;
+  long long segbase, segstride;
+};
+
+__device__ __forceinline__ LwSegs lw_tile_segs(const Unit2& u, const Tile2& t) {
+  LwSegs s;
+  if (u.kind == KIND_SLAB) {
+    const int half = u.I >> 1;
+    s.nseg = 1; s.seglen = (t.b / half) * u.K * u.I; s.segbase = u.w_off + (long long)(t.a / half) * u.K * u.I;
+    s.segstride = 0;
+  } else if (u.kind == KIND_MAT && u.cs == 1) {
+    s.nseg = t.b; s.seglen = u.cols; s.segbase = u.w_off + (long long)t.a * u.rs; s.segstride = u.rs;
+  } else if (u.kind == KIND_MAT) {
+    s.nseg = u.cols; s.seglen = t.b; s.segbase = u.w_off + t.a; s.segstride = u.cs;
+  } else if (u.kind == KIND_POWER) {
+    s.nseg = 1; s.seglen = t.b * u.cols; s.segbase = u.w_off + (long long)t.a * u.cols; s.segstride = 0;
+  } else {
+    s.nseg = 1; s.seglen = t.b; s.segbase = u.w_off + t.a; s.segstride = 0;
+  }
+  return s;
 }
 
 __device__ __forceinline__ uint4 ld_cg_u4(const void* p) {
@@ -388,6 +446,48 @@ __device__ __forceinline__ void ps_vec_tile(const PsArgsLw& a, const OptC& c, co
   cv.opt = c.opt == OPT_LARS ? OPT_SGD : OPT_ADAM;
   cv.wd = 0.f;
   ps_vec_tile(static_cast<const PsArgs2&>(a), cv, u, t, wmask, all_workers, inv_w);
+}
+
+// gather: the vector tile's mean gradient into vgrad, its squares into the thread's partial (the sums as ps_vec_tile)
+__device__ __forceinline__ void ps_vec_tile(const PsArgsGather& a, const OptC&, const Unit2& u, const Tile2& t,
+                                            unsigned int wmask, bool all_workers, float inv_w) {
+  const int tid = threadIdx.x;
+  const long long e0 = u.w_off + t.a;
+  const int nvec = t.b >> 2;
+  float acc = lw_acc[tid].x;
+  for (int v = tid; v < nvec; v += blockDim.x) {
+    const long long e = e0 + 4LL * v;
+    float4 g;
+    if (a.vgrads_mc != nullptr && all_workers) {
+      g = multimem_ld_reduce_f4(reinterpret_cast<const float4*>(a.vgrads_mc + e));
+    } else {
+      g = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int w = 0; w < a.W; ++w) {
+        if (!((wmask >> w) & 1u)) continue;
+        const float4 x = ld_cg_f4(reinterpret_cast<const float4*>(a.vgrads_peer[w] + e));
+        g.x += x.x; g.y += x.y; g.z += x.z; g.w += x.w;
+      }
+    }
+    g = make_float4(g.x * inv_w, g.y * inv_w, g.z * inv_w, g.w * inv_w);
+    acc = fmaf(g.x, g.x, acc); acc = fmaf(g.y, g.y, acc); acc = fmaf(g.z, g.z, acc); acc = fmaf(g.w, g.w, acc);
+    *reinterpret_cast<float4*>(a.vgrad + e) = g;
+  }
+  for (int i = (nvec << 2) + tid; i < t.b; i += blockDim.x) {
+    const long long e = e0 + i;
+    float g = 0.f;
+    for (int w = 0; w < a.W; ++w)
+      if ((wmask >> w) & 1u) g += ld_cg_f(a.vgrads_peer[w] + e);
+    g *= inv_w;
+    acc = fmaf(g, g, acc);
+    a.vgrad[e] = g;
+  }
+  lw_acc[tid].x = acc;
+}
+
+// end of vector tile ti: only the gather instantiation keeps a partial of it (every thread of the CTA)
+template <class A>
+__device__ __forceinline__ void clip_vec_done(const A& a, int ti) {
+  if constexpr (ps_gather<A>) lw_tile_done(a, ti);
 }
 
 // ---- bf16 weight tile that travels dense: the counted workers' staged copies summed in worker order, optimizer,

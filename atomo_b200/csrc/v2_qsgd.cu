@@ -290,6 +290,7 @@ __device__ __forceinline__ void ps_qsgd(const A& a) {
     const Unit2 u = a.units[t.unit];
     if (u.kind == KIND_VEC) {
       ps_vec_tile(a, c, u, t, wmask, all_workers, inv_w);
+      clip_vec_done(a, ti);
       continue;
     }
     if (u.kind != KIND_QSGD) continue;
@@ -358,6 +359,7 @@ __device__ __forceinline__ void ps_qsgd(const A& a) {
 
 __global__ void __launch_bounds__(QPS_THREADS) v2_ps_qsgd_kernel(const PsArgs2 a) { ps_qsgd(a); }
 __global__ void __launch_bounds__(QPS_THREADS, 1) v2_ps_qsgd_lw_kernel(const PsArgsLw a) { ps_qsgd(a); }
+__global__ void __launch_bounds__(QPS_THREADS, 1) v2_ps_qsgd_gather_kernel(const PsArgsGather a) { ps_qsgd(a); }
 
 extern "C" {
 
@@ -404,6 +406,11 @@ void atomo_v2_launch_ps_qsgd(const void* units, const void* tiles, int tile0, in
 void atomo_v2_launch_ps_qsgd_lw(const void* args, int grid, cudaStream_t stream) {
   const PsArgsLw& a = *static_cast<const PsArgsLw*>(args);
   v2_ps_qsgd_lw_kernel<<<ps_grid(grid, a.ntiles), QPS_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_qsgd_gather(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsGather& a = *static_cast<const PsArgsGather*>(args);
+  v2_ps_qsgd_gather_kernel<<<ps_grid(grid, a.ntiles), QPS_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

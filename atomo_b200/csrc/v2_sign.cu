@@ -153,6 +153,7 @@ __device__ __forceinline__ void ps_sign(const A& a) {
     const Unit2 u = a.units[t.unit];
     if (u.kind == KIND_VEC) {
       ps_vec_tile(a, c, u, t, wmask, all_workers, inv_w);
+      clip_vec_done(a, ti);
       continue;
     }
     if (u.kind != KIND_SIGN) continue;
@@ -208,6 +209,7 @@ __device__ __forceinline__ void ps_sign(const A& a) {
 
 __global__ void __launch_bounds__(SPS_THREADS) v2_ps_sign_kernel(const PsArgs2 a) { ps_sign(a); }
 __global__ void __launch_bounds__(SPS_THREADS, 1) v2_ps_sign_lw_kernel(const PsArgsLw a) { ps_sign(a); }
+__global__ void __launch_bounds__(SPS_THREADS, 1) v2_ps_sign_gather_kernel(const PsArgsGather a) { ps_sign(a); }
 
 // ---- --code-stats ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(SE_THREADS) v2_sign_code_stats_kernel(const ScaleStatArgs a) {
@@ -303,6 +305,11 @@ void atomo_v2_launch_sign_code_stats(const void* units, const void* tiles, int t
 void atomo_v2_launch_ps_sign_lw(const void* args, int grid, cudaStream_t stream) {
   const PsArgsLw& a = *static_cast<const PsArgsLw*>(args);
   v2_ps_sign_lw_kernel<<<ps_grid(grid, a.ntiles), SPS_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_sign_gather(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsGather& a = *static_cast<const PsArgsGather*>(args);
+  v2_ps_sign_gather_kernel<<<ps_grid(grid, a.ntiles), SPS_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

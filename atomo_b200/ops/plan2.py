@@ -778,9 +778,9 @@ LAYERWISE_OPTS = (OPT_LARS, OPT_LAMB)
 def pack_ctrl2(step: int = 1, lr: float = 0.01, momentum: float = 0.0, dampening: float = 0.0,
                weight_decay: float = 0.0, nesterov: bool = False, first_step: int = 1, seed: int = 1,
                beta1: float = 0.9, beta2: float = 0.999, eps: float = 1e-8, opt: int = OPT_SGD,
-               num_aggregate: int = 0, trust_coefficient: float = 0.0) -> bytes:
+               num_aggregate: int = 0, trust_coefficient: float = 0.0, clip_grad_norm: float = 0.0) -> bytes:
     return struct.pack(CTRL2_FMT, step, 0, lr, momentum, dampening, weight_decay, int(nesterov), first_step,
-                       seed & 0xFFFFFFFFFFFFFFFF, beta1, beta2, eps, 0.0, int(opt), int(num_aggregate),
+                       seed & 0xFFFFFFFFFFFFFFFF, beta1, beta2, eps, float(clip_grad_norm), int(opt), int(num_aggregate),
                        float(trust_coefficient), 0)
 
 
@@ -796,3 +796,10 @@ def layerwise_tables(plan: "Plan2") -> Tuple[List[int], List[int]]:
     tile_layer = [-1 if plan.units[ui].kind == KIND_VEC else local[plan.units[ui].param]
                   for (ui, _a, _b, _o) in plan.ps_tiles]
     return tile_layer, per_group
+
+
+def owner_ps_tiles(plan: "Plan2", owner: int) -> List[int]:
+    """Gradient-norm clipping (csrc/v2_clip.cu): the indices into ``plan.ps_tiles`` of every PS tile owner ``owner``
+    steps, group by group.  With several owners they are not contiguous: each group's tiles are sorted by owner."""
+    return [t for g in range(plan.n_groups) for t in range(plan.ps_range[g][owner][0],
+                                                             sum(plan.ps_range[g][owner]))]

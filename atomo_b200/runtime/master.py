@@ -23,6 +23,7 @@ from ..models import build_model
 from ..optim import LAMB, LARS, SGD, Adam
 from ..parallel.transport import Transport, STOP_STEP
 from ..utils import checkpoint as ckpt
+from ..utils.flags import check_clip_grad_norm
 from ..utils.logging import MetricsWriter, master_line
 from .flat import FlatLayout, bind_parameters
 from .nn_ops import NN_Trainer
@@ -92,6 +93,14 @@ class GradientAccumulator:
         self.gradient_aggregate_counter = [0] * len(self.layout)
 
 
+def clip_grad_norm(grads, max_norm: float):
+    """``torch.nn.utils.clip_grad_norm_`` on a list of gradients: scaled by ``min(1, max_norm / (||g|| + 1e-6))``, the
+    norm taken over all of them, in their own precision.  Returns the scaled gradients and ``(total, coef)``."""
+    total = torch.nn.utils.get_total_norm(grads)
+    coef = torch.clamp(max_norm / (total + 1e-6), max=1.0)
+    return [g * coef.to(g.device) for g in grads], (float(total), float(coef))
+
+
 class SyncReplicasMaster_NN(NN_Trainer):
     def __init__(self, comm: Transport, **kwargs):
         self.comm = comm
@@ -118,6 +127,8 @@ class SyncReplicasMaster_NN(NN_Trainer):
         self._quantization_level = kwargs.get("quantization_level", 4)
         self._bucket_size = kwargs.get("bucket_size", 512)
         self._optimizer_name = kwargs.get("optimizer", "sgd")
+        self._clip_grad_norm = check_clip_grad_norm(kwargs.get("clip_grad_norm", 0.0))
+        self.last_grad_norm = None      # (total, coef) of the last update with clipping on
         self._save_checkpoints = kwargs.get("save_checkpoints", True)
         self._resume = kwargs.get("resume", False)
         self._verbose = kwargs.get("verbose", True)
@@ -240,6 +251,8 @@ class SyncReplicasMaster_NN(NN_Trainer):
     def _model_update(self, n_used: Optional[int] = None):
         n = float(n_used or self._num_workers)
         grads = [g / n for g in self.grad_accumulator.gradient_aggregator]
+        if self._clip_grad_norm:
+            grads, self.last_grad_norm = clip_grad_norm(grads, self._clip_grad_norm)
         self.optimizer.step(grads=grads, cuda=self._enable_gpu)
 
     def _generate_model_path(self):

@@ -24,6 +24,8 @@ import torch
 import torch.distributed as dist
 import torch.nn.functional as F
 
+from ..utils.flags import check_clip_grad_norm
+
 
 class _HostEvent:
     """perf_counter stand-in for torch.cuda.Event when the loop runs on a CPU stand-in engine (tests)."""
@@ -39,6 +41,10 @@ def _build_engine(args, model, rank, world):
     engine = getattr(args, "engine", "auto")
     code = args.code.lower()
     accum = getattr(args, "accumulate_steps", 1)
+    try:
+        clip = check_clip_grad_norm(getattr(args, "clip_grad_norm", 0.0))
+    except ValueError as e:
+        raise SystemExit("--clip-grad-norm: %s" % e)
     if code == "topk" and (engine == "fused" or args.dtype != "bf16"):
         raise SystemExit("--code topk runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the fp32-flat "
                          "engine has no top-k selection")
@@ -89,11 +95,16 @@ def _build_engine(args, model, rank, world):
             kw["accumulate_steps"] = accum      # the engine refuses a value below 1
         if args.optimizer in ("lars", "lamb"):
             kw["trust_coefficient"] = getattr(args, "trust_coefficient", 0.001)
+        if clip:
+            kw["clip_grad_norm"] = clip
         return ShadowEngine(model, rank, world, code=args.code, svd_rank=args.svd_rank, lr=args.lr,
                             momentum=args.momentum, weight_decay=args.weight_decay, nesterov=args.nesterov,
                             optimizer=args.optimizer, ps_mode=args.ps_mode, groups=args.groups, sampling=args.sampling,
                             prob_rule=args.prob_rule, seed=args.seed, num_aggregate=args.num_aggregate,
                             timeout_s=args.flag_timeout, **kw), "shadow"
+    if clip:
+        raise SystemExit("--clip-grad-norm runs on the bf16 engine (--engine shadow, --dtype bf16); the fp32-flat engine "
+                         "steps each tensor as its push lands and never sees the whole-model norm")
     if args.optimizer in ("lars", "lamb"):
         raise SystemExit("--optimizer %s runs on the bf16 engine (--engine shadow, --dtype bf16); the fp32-flat engine "
                          "has no layer-wise trust ratio" % args.optimizer)
@@ -217,6 +228,8 @@ def run_p2p_training(args, device=None):
                 extra["code_stats"] = eng.code_stats(reset=True)
             if getattr(args, "error_feedback", False) and eng.is_worker:
                 extra["ef_norm"] = eng.error_feedback_norm()["model"]
+            if getattr(args, "clip_grad_norm", 0.0) and eng.is_owner:
+                extra["grad_norm"], extra["clip_coef"] = eng.grad_norm()
             metrics.write(step=cur, loss=loss, prec1=p1, prec5=p5, step_s=step_s, comp=comp, encode=enc, comm=comm,
                           msg_mb=msg_mb, lr=eng.lr, phase_us={k: round(float(v), 1) for k, v in ph.items()}, **extra)
             ev_a.record()

@@ -65,6 +65,10 @@ one central PS kernel at the end of the step):
   norms first: the code's PS kernel runs its layer-wise instantiation (moments, direction, per-tile partials; vectors
   finished), then ``csrc/v2_layerwise.cu`` takes the norms across tiles and owners, the trust ratios and the step of
   the weights, and broadcasts them (``optim/lars.py`` / ``optim/lamb.py`` are the oracles).
+* Gradient-norm clipping (``clip_grad_norm=MAX``, ``torch.nn.utils.clip_grad_norm_`` semantics): the code's PS kernel
+  runs its gather instantiation per group (mean gradient and sum g^2 per tile, nothing stepped), then one launch per
+  owner after the final group (``csrc/v2_clip.cu``) takes the whole-model norm across tiles and owners and steps every
+  tile of the owner on ``coef * g`` (LARS / LAMB: their phase 2 follows per group).  ``grad_norm()`` reports it.
 
 Per step and rank: ``wait_params`` -> forward -> backward [group hooks -> encode, project+push on stream E;
 PS launch of the group on stream P] -> join -> ``advance_step``.  All cross-GPU ordering is carried by
@@ -85,6 +89,7 @@ import torch.nn as nn
 from ..ops import plan2 as P2
 from ..ops._ext import load as load_ext
 from ..parallel.symm import SymmetricHeap
+from ..utils.flags import check_clip_grad_norm
 
 SIGNAL_INTS = 1024
 
@@ -105,7 +110,8 @@ class ShadowEngine:
                  warm_start: bool = True, max_sweeps: int = 1, main_priority: int = 0, debug_jitter_us: float = 0.0,
                  side_priority: int = -1, resample_empty: bool = False, quantization_level: int = 4,
                  bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False,
-                 error_feedback: bool = False, accumulate_steps: int = 1, trust_coefficient: float = 0.001):
+                 error_feedback: bool = False, accumulate_steps: int = 1, trust_coefficient: float = 0.001,
+                 clip_grad_norm: float = 0.0):
         self.optimizer = optimizer.lower()
         if self.optimizer not in ("sgd", "adam", "lars", "lamb"):      # checked before any CUDA work
             raise ValueError("ShadowEngine optimizers: sgd | adam | lars | lamb (got %r)" % (optimizer,))
@@ -120,6 +126,8 @@ class ShadowEngine:
         if isinstance(accumulate_steps, bool) or not isinstance(accumulate_steps, numbers.Integral) \
                 or accumulate_steps < 1:        # checked before any CUDA work
             raise ValueError("accumulate_steps must be an integer >= 1 (got %r)" % (accumulate_steps,))
+        self.clip_grad_norm = check_clip_grad_norm(clip_grad_norm)      # checked before any CUDA work
+        self.clip_on = self.clip_grad_norm > 0
         self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
         if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign", "powersgd", "fp8",
                              "hadamard"):
@@ -242,8 +250,10 @@ class ShadowEngine:
         self.lw_tile_layer, self.lw_layers = P2.layerwise_tables(pl) if self.layerwise else ([], [])
         self.lw_xch_off = [2 * 2 * self.n_owners * sum(self.lw_layers[:g]) for g in range(self.G)]
         xch_doubles = 2 * 2 * self.n_owners * sum(self.lw_layers)
+        # gradient-norm clipping: every owner's sum of g^2 ([2 step parities][owner] fp64)
+        clip_doubles = 2 * self.n_owners if self.clip_on else 0
         need = 4 * SIGNAL_INTS + 2 * pl.w_total + 8 * pl.v_total + 2 * pl.stage_total + \
-            4 * pl.arena_floats * self.W + 8 * xch_doubles + (1 << 16)
+            4 * pl.arena_floats * self.W + 8 * xch_doubles + 8 * clip_doubles + (1 << 16)
         self.heap = h = SymmetricHeap(need + (1 << 20), rank, world, dev.index, group=group, multicast=multicast,
                                       mode=heap_mode)
         h.alloc("signals", 4 * SIGNAL_INTS)
@@ -254,6 +264,8 @@ class ShadowEngine:
         h.alloc("arena", 4 * pl.arena_floats * self.W)
         if self.layerwise:
             h.alloc("lwx", 8 * max(xch_doubles, 2))
+        if self.clip_on:
+            h.alloc("clipx", 8 * clip_doubles)
         self.signals = h.tensor("signals", torch.int32)
         self.wshadow = h.tensor("wshadow", torch.bfloat16)
         self.vparams = h.tensor("vparams")
@@ -372,7 +384,8 @@ class ShadowEngine:
                                              weight_decay=weight_decay, nesterov=nesterov, first_step=1, seed=seed,
                                              beta1=betas[0], beta2=betas[1], eps=eps, opt=self.opt,
                                              num_aggregate=num_aggregate,
-                                             trust_coefficient=self.trust_coefficient if self.layerwise else 0.0), dev)
+                                             trust_coefficient=self.trust_coefficient if self.layerwise else 0.0,
+                                             clip_grad_norm=self.clip_grad_norm), dev)
         self.ctrl_i32, self.ctrl_f32 = self.ctrl.view(torch.int32), self.ctrl.view(torch.float32)
         n_w = max(len(self.w_params), 1)
         self.t_gptr = torch.zeros(n_w, dtype=torch.int64, device=dev)
@@ -405,6 +418,21 @@ class ShadowEngine:
                 self.t_lw_tile_layer = torch.tensor(self.lw_tile_layer or [0], dtype=torch.int32, device=dev)
             self.t_lw_xch_peer = [i64(h.region_ptr("lwx", r) + 8 * self.lw_xch_off[g] for r in range(world))
                                   for g in range(self.G)]
+        # gradient-norm clipping (csrc/v2_clip.cu): the owner's mean gradient per element (LARS / LAMB: in lw_dir, which
+        # phase 2 overwrites with the direction) and per vector element, sum g^2 of every PS tile, the owner's PS tiles
+        # of every group, a completion counter, the exchange slots and the last (total, coef)
+        self.clip_grad = self.clip_vgrad = self.clip_part = self.t_clip_tiles = self.clip_counter = None
+        self.clip_norm, self.clip_tiles, self.t_clip_xch_peer = None, [], None
+        if self.clip_on:
+            self.clip_norm = z(2)
+            if self.is_owner:
+                self.clip_grad = self.lw_dir if self.layerwise else z(pl.w_total)
+                self.clip_vgrad = z(pl.v_total)
+                self.clip_part = z(2 * max(len(pl.ps_tiles), 1))
+                self.clip_tiles = P2.owner_ps_tiles(pl, self.owner_index)
+                self.t_clip_tiles = torch.tensor(self.clip_tiles or [0], dtype=torch.int32, device=dev)
+                self.clip_counter = torch.zeros(1, dtype=torch.int32, device=dev)
+            self.t_clip_xch_peer = i64(h.region_ptr("clipx", r) for r in range(world))
         self.tstats = torch.zeros(32, dtype=torch.int64, device=dev)
         # --code-stats: per coded unit fp64 sums over steps (v2_stats.cu), the per-tile partials and unit counters
         self.code_stats_on = bool(code_stats)
@@ -764,6 +792,9 @@ class ShadowEngine:
         C, pl = self.C, self.plan
         t0, nt = pl.ps_range[g][self.owner_index]
         p = lambda t: t.data_ptr() if t is not None else 0
+        if self.clip_on:
+            self._launch_ps_clip(g, final, t0, nt)
+            return
         if self.layerwise:
             self._launch_ps_layerwise(g, final, t0, nt)
             return
@@ -827,16 +858,24 @@ class ShadowEngine:
         C, pl = self.C, self.plan
         p = lambda t: t.data_ptr() if t is not None else 0
         grid = max(1, min(self.ps_grid, max(nt, 1)))
-        ps = 1 if self.quant else 2 if self.entry else 3 if self.sign else 4 if self.fp8 else 5 if self.hadamard \
-            else 6 if self.power else 0
         part = self.lw_part.data_ptr() + 8 * t0
-        C.v2_ps_layerwise(ps, self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g,
+        C.v2_ps_layerwise(self._ps_kind(), self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g,
                           self.owner_index, p(self.master), p(self.mom), p(self.sq), p(self.vmom), p(self.vsq),
                           self.vparams.data_ptr(), self.vparams_mc, self.t_vparams_peer.data_ptr(), self.vgrads_mc,
                           self.t_vgrads_peer.data_ptr(), self.t_stage_peer.data_ptr(), self.heap.region_ptr("arena"),
                           pl.arena_floats, self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
                           self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
                           self.lw_dir.data_ptr(), part, grid, self.q_max_level, self.q_max_bucket)
+        self._nlaunch += 1
+        self._launch_layerwise(g, final)
+
+    def _launch_layerwise(self, g: int, final: bool):
+        """LARS / LAMB phase 2 of group ``g`` (csrc/v2_layerwise.cu), on the direction and tile partials phase 1 (or
+        the clip launch) left."""
+        C = self.C
+        p = lambda t: t.data_ptr() if t is not None else 0
+        t0, nt = self.plan.ps_range[g][self.owner_index]
+        part = self.lw_part.data_ptr() + 8 * t0
         C.v2_layerwise(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt,
                        self.t_lw_tile_layer.data_ptr() + 4 * t0, self.lw_layers[g], part, self.lw_dir.data_ptr(),
                        self.world, g, final, self.owner_index, self.n_owners, p(self.master), p(self.mom),
@@ -844,8 +883,54 @@ class ShadowEngine:
                        self.heap.region_ptr("lwx") + 8 * self.lw_xch_off[g], self.t_lw_xch_peer[g].data_ptr(),
                        self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
                        self.lw_counter.data_ptr() + 4 * g, self.timeout_ticks, self.tstats.data_ptr(),
-                       self.lw_ratio.data_ptr() + 4 * sum(self.lw_layers[:g]), grid)
-        self._nlaunch += 2
+                       self.lw_ratio.data_ptr() + 4 * sum(self.lw_layers[:g]), max(1, min(self.ps_grid, max(nt, 1))))
+        self._nlaunch += 1
+
+    def _ps_kind(self) -> int:
+        """The PS kernel of the code, as the phase-1 launches (v2_ps_layerwise, v2_ps_gather) select it."""
+        return 1 if self.quant else 2 if self.entry else 3 if self.sign else 4 if self.fp8 else 5 if self.hadamard \
+            else 6 if self.power else 0
+
+    def _launch_ps_clip(self, g: int, final: bool, t0: int, nt: int):
+        """Gradient-norm clipping: phase 1 of every group (the code's PS kernel with the gather epilogue: mean gradient
+        and sum g^2 per tile, nothing stepped); after the final group, phase 2 (the whole-model norm across tiles and
+        owners, the coefficient, and the step of every tile of this owner on coef * g), and for LARS / LAMB their
+        phase 2 per group, unchanged (the last one publishes the parameters)."""
+        C, pl = self.C, self.plan
+        p = lambda t: t.data_ptr() if t is not None else 0
+        C.v2_ps_gather(self._ps_kind(), self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W,
+                       self.world, g, self.owner_index, self.vgrads_mc, self.t_vgrads_peer.data_ptr(),
+                       self.t_stage_peer.data_ptr(), self.heap.region_ptr("arena"), pl.arena_floats,
+                       self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
+                       self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
+                       self.clip_grad.data_ptr(), self.clip_vgrad.data_ptr(), self.clip_part.data_ptr() + 8 * t0,
+                       max(1, min(self.ps_grid, max(nt, 1))), self.q_max_level, self.q_max_bucket)
+        self._nlaunch += 1
+        if not final:
+            return
+        n = len(self.clip_tiles)
+        C.v2_clip(self.layerwise, self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), self.t_clip_tiles.data_ptr(), n,
+                  self.clip_part.data_ptr(), self.clip_grad.data_ptr(), self.clip_vgrad.data_ptr(), self.world,
+                  self.owner_index, self.n_owners, p(self.master), p(self.mom), p(self.sq), p(self.sqmax),
+                  p(self.vmom), p(self.vsq), p(self.vsqmax), self.wshadow_mc, self.t_wshadow_peer.data_ptr(),
+                  self.vparams.data_ptr(), self.vparams_mc, self.t_vparams_peer.data_ptr(), p(self.lw_dir),
+                  p(self.lw_part), self.heap.region_ptr("clipx"), self.t_clip_xch_peer.data_ptr(),
+                  self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
+                  self.clip_counter.data_ptr(), self.timeout_ticks, self.tstats.data_ptr(), self.clip_norm.data_ptr(),
+                  max(1, min(self.ps_grid, max(n, 1))))
+        self._nlaunch += 1
+        if self.layerwise:
+            for gg in range(self.G):
+                self._launch_layerwise(gg, gg == self.G - 1)
+
+    def grad_norm(self) -> tuple:
+        """Gradient-norm clipping: ``(total, coef)`` of the last step, the whole-model norm of the mean gradient the
+        owners received and the factor they stepped with, as this owner's clip launch computed them (zeros on a rank
+        that owns no PS tiles).  Reading it synchronises the device."""
+        if not self.clip_on:
+            raise RuntimeError("grad_norm() needs ShadowEngine(..., clip_grad_norm=MAX) with MAX > 0")
+        total, coef = self.clip_norm.tolist()
+        return total, coef
 
     def trust_ratios(self) -> dict:
         """LARS / LAMB: the trust ratio of every weight tensor in the last step (parameter name -> ratio), as this
@@ -1132,7 +1217,8 @@ class ShadowEngine:
             them; its unit counters are zero between launches); the device's default CUDA generator (seed and
             offset), from which the model's dropout layers draw their masks (VGG's classifier).
         (c) scratch, rewritten every step before it is read: LARS / LAMB's direction ``lw_dir``, tile partials
-            ``lw_part``, exchange slots and trust ratios; the rest of ``gpart`` (Gram partials, ``P``,
+            ``lw_part``, exchange slots and trust ratios; gradient-norm clipping's ``clip_grad``, ``clip_vgrad``,
+            ``clip_part``, exchange slots and ``clip_norm``; the rest of ``gpart`` (Gram partials, ``P``,
             ``P_hat``, ``Q'``), ``vsel``, ``selcount``, ``sigma``, ``clip`` / ``clip_partials``, ``l1`` /
             ``l1_partials``, ``topk_sel``, ``topk_tiles``, ``pw_gram``, ``stats_partials``, ``vgrads``, ``wstage``,
             the gradient-accumulation sums ``acc`` / ``vacc`` (zero at every step boundary) and pointer tables,

@@ -4,6 +4,8 @@ kept with its default) plus the H100-specific additions."""
 from __future__ import annotations
 
 import argparse
+import math
+import numbers
 
 
 def bool_flag(v) -> bool:
@@ -71,6 +73,10 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "p2p backend on the bf16 engine (--engine shadow), or the gloo / nccl role path")
     p.add_argument("--trust-coefficient", type=float, default=0.001,
                    help="--optimizer lars: eta of the trust ratio eta ||w|| / (||g|| + wd ||w||)")
+    p.add_argument("--clip-grad-norm", type=float, default=0.0,
+                   help="clip the averaged gradient to this whole-model L2 norm before the optimizer, as "
+                        "torch.nn.utils.clip_grad_norm_ (0 = off); p2p backend on the bf16 engine (--engine shadow), or "
+                        "the gloo / nccl role path")
     p.add_argument("--weight-decay", type=float, default=0.0)
     p.add_argument("--nesterov", type=bool_flag, default=False)
     p.add_argument("--resume", type=bool_flag, default=False)
@@ -118,3 +124,10 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "their mean once, so the global batch is workers x N x --batch-size and the pushes per sample "
                         "fall N-fold.  The LR schedule, checkpoints and --eval-freq count optimizer steps")
     return p.parse_args(argv)
+
+
+def check_clip_grad_norm(value) -> float:
+    """--clip-grad-norm / clip_grad_norm=: 0 (off) or a finite positive norm; anything else raises ValueError."""
+    if isinstance(value, bool) or not isinstance(value, numbers.Real) or not (value == 0 or 0 < value < math.inf):
+        raise ValueError("clip_grad_norm must be 0 (off) or a finite norm > 0 (got %r)" % (value,))
+    return float(value)
