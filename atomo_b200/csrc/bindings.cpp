@@ -135,7 +135,7 @@ void atomo_v2_launch_topk_encode(const void* units, const void* tiles, int tile0
                                  const int* sel, const int* tile_counts, float* const* arena_peer,
                                  int* const* sig_peer, int n_owners, long long arena_floats, int worker, int group,
                                  const void* ctrl, unsigned int* group_counter, long long* tstats, int final_group,
-                                 float* residual, cudaStream_t stream);
+                                 float* residual, float* mom, cudaStream_t stream);
 void atomo_v2_launch_topk_code_stats(const void* units, const void* tiles, int tile0, int ntiles,
                                      const long long* gptr, const int* sel, const int* tile_counts,
                                      float* const* arena_peer, int n_owners, long long arena_floats, int worker,
@@ -218,6 +218,10 @@ int atomo_v2_ef_chunk_bytes();
 void atomo_v2_launch_ef_apply(const void* chunks, int chunk0, int nchunks, const long long* gptr, float* residual,
                               cudaStream_t stream);
 // v2_accum.cu (gradient accumulation of the bf16 engine)
+// v2_momentum.cu (top-k momentum correction of the bf16 engine)
+void atomo_v2_launch_mc_apply(const void* wchunks, int nw, const void* vchunks, int nv, const long long* gptr,
+                              const void* wshadow, float* mom, float* residual, float* vgrads, const float* vparams,
+                              float* vmom, float m, float wd, int nesterov, cudaStream_t stream);
 void atomo_v2_launch_accum_add(const void* wchunks, int nw, const void* vchunks, int nv, const long long* gptr,
                                float* acc, float* vacc, float* vgrads, int first, cudaStream_t stream);
 void atomo_v2_launch_accum_fold(const void* wchunks, int nw, const void* vchunks, int nv, const long long* gptr,
@@ -694,14 +698,16 @@ void v2_topk_select(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint6
 void v2_topk_encode(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t sel,
                     uint64_t tile_counts, uint64_t arena_peer, uint64_t sig_peer, int n_owners, int64_t arena_floats,
                     int worker, int group, uint64_t ctrl, uint64_t group_counter, uint64_t tstats, bool final_group,
-                    uint64_t residual) {
+                    uint64_t residual, uint64_t mom) {
   TORCH_CHECK(sel != 0 && tile_counts != 0, "v2_topk_encode: needs the selection of v2_topk_select");
+  TORCH_CHECK(mom == 0 || residual != 0, "v2_topk_encode: momentum-factor masking (mom) needs the error-feedback "
+              "residual");
   TORCH_CHECK(worker >= 0 && worker < 16, "v2_topk_encode: worker index must be in [0, 16)");
   atomo_v2_launch_topk_encode(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
                               P<const int>(sel), P<const int>(tile_counts), P<float* const>(arena_peer),
                               P<int* const>(sig_peer), n_owners, arena_floats, worker, group, P<const void>(ctrl),
                               P<unsigned int>(group_counter), P<long long>(tstats), final_group ? 1 : 0,
-                              P<float>(residual), cur_stream());
+                              P<float>(residual), P<float>(mom), cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 void v2_topk_code_stats(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t sel,
@@ -886,6 +892,23 @@ void v2_powersgd_code_stats(uint64_t units, uint64_t tiles, int tile0, int ntile
 void v2_ef_apply(uint64_t chunks, int chunk0, int nchunks, uint64_t gptr, uint64_t residual) {
   TORCH_CHECK(chunks != 0 && gptr != 0 && residual != 0, "v2_ef_apply: chunks / gptr / residual required");
   atomo_v2_launch_ef_apply(P<const void>(chunks), chunk0, nchunks, P<const long long>(gptr), P<float>(residual),
+                           cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+// momentum correction (top-k with error feedback): the worker's momentum u = m u + (g + wd w) and A = (nesterov ?
+// d + m u : u) + e over the weight chunks [0, nw) of `wchunks`, bf16(A) into the gradient buffers and A - bf16(A) into
+// the residual; the vectors' u and direction over the vector chunks [0, nv) of `vchunks`, the direction into vgrads.
+// It takes the place of v2_ef_apply for the group, on the encode stream
+void v2_mc_apply(uint64_t wchunks, int nw, uint64_t vchunks, int nv, uint64_t gptr, uint64_t wshadow, uint64_t mom,
+                 uint64_t residual, uint64_t vgrads, uint64_t vparams, uint64_t vmom, float momentum,
+                 float weight_decay, bool nesterov) {
+  TORCH_CHECK(nw >= 0 && nv >= 0, "v2_mc_apply: negative chunk count");
+  TORCH_CHECK((nw == 0 || (wchunks != 0 && gptr != 0 && wshadow != 0 && mom != 0 && residual != 0)) &&
+              (nv == 0 || (vchunks != 0 && vgrads != 0 && vparams != 0 && vmom != 0)),
+              "v2_mc_apply: chunks / gptr / wshadow / momentum / residual / vector buffers required");
+  atomo_v2_launch_mc_apply(P<const void>(wchunks), nw, P<const void>(vchunks), nv, P<const long long>(gptr),
+                           P<const void>(wshadow), P<float>(mom), P<float>(residual), P<float>(vgrads),
+                           P<const float>(vparams), P<float>(vmom), momentum, weight_decay, nesterov ? 1 : 0,
                            cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
@@ -1148,7 +1171,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("v2_topk_encode", &v2_topk_encode, py::arg("units"), py::arg("tiles"), py::arg("tile0"), py::arg("ntiles"),
         py::arg("gptr"), py::arg("sel"), py::arg("tile_counts"), py::arg("arena_peer"), py::arg("sig_peer"),
         py::arg("n_owners"), py::arg("arena_floats"), py::arg("worker"), py::arg("group"), py::arg("ctrl"),
-        py::arg("group_counter"), py::arg("tstats"), py::arg("final_group"), py::arg("residual") = 0);
+        py::arg("group_counter"), py::arg("tstats"), py::arg("final_group"), py::arg("residual") = 0,
+        py::arg("mom") = 0);
   m.def("v2_topk_code_stats", &v2_topk_code_stats);
   m.def("v2_topk_sizes", []() {
     return py::make_tuple(atomo_v2_topk_state_ints(), atomo_v2_topk_hist_bins(), atomo_v2_topk_tile_bins());
@@ -1178,6 +1202,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("v2_powersgd_code_stats", &v2_powersgd_code_stats);
   m.def("v2_ef_apply", &v2_ef_apply);
   m.def("v2_ef_chunk_bytes", &atomo_v2_ef_chunk_bytes);
+  m.def("v2_mc_apply", &v2_mc_apply);
   m.def("v2_accum_add", &v2_accum_add);
   m.def("v2_accum_fold", &v2_accum_fold);
   m.def("v2_ps_layerwise", &v2_ps_layerwise);

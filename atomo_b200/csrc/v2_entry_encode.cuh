@@ -81,8 +81,10 @@ __device__ __forceinline__ float entry_residual(uint32_t bits, uint32_t kept, ui
   return kept ? (exact ? 0.f : x - copysignf(scale, x)) : x;
 }
 
-template <int KEEP, bool EF, class Args>
-__device__ __forceinline__ void entry_encode(const Args& a) {
+// MASK (top-k momentum correction, v2_momentum.cu): also store 0 into the worker's momentum `mom` (indexed like the
+// residual) at every kept entry; entries not kept keep theirs.
+template <int KEEP, bool EF, bool MASK = false, class Args>
+__device__ __forceinline__ void entry_encode(const Args& a, float* mom = nullptr) {
   __shared__ __align__(16) uint32_t ent[ENTRY_TILE_ELEMS];
   __shared__ int wsum[EE_WARPS];
   const Tile2 t = a.tiles[blockIdx.x];
@@ -141,6 +143,12 @@ __device__ __forceinline__ void entry_encode(const Args& a) {
     } else {
       for (int i = 0; i < n; ++i) ep[i] += entry_residual(bf16_bits(h, i), (keep >> i) & 1u, (exact >> i) & 1u, scale);
     }
+  }
+  if constexpr (MASK) {
+    float* mp = mom + u.w_off + e0;                          // kept entries are sparse: scalar stores
+#pragma unroll
+    for (int i = 0; i < EE_PER_THREAD; ++i)
+      if ((keep >> i) & 1u) mp[i] = 0.f;
   }
 
   // ---- compaction in element order: warp scan of the per-thread counts, then the warp totals -------------------

@@ -14,7 +14,8 @@
 //   v2_topk_encode_kernel   entry_encode (v2_entry_encode.cuh) with the top-k keep policy: |g| > T, or |g| == T with a
 //                           tie rank (T counts of the unit's earlier tiles + in-tile prefix) below need_ties; every
 //                           kept entry carries the exact flag, the header's scale is 0.  The owners decode with
-//                           v2_ps_entry_kernel unchanged.  v2_topk_encode_ef_kernel adds the error-feedback epilogue.
+//                           v2_ps_entry_kernel unchanged.  v2_topk_encode_ef_kernel adds the error-feedback epilogue,
+//                           v2_topk_encode_mc_kernel also momentum-factor masking (momentum correction, v2_momentum.cu).
 //   v2_topk_code_stats_kernel  --code-stats of top-k units, in the layout of v2_code_stats_kernel (v2_stats.cu).
 #include "v2_entry_encode.cuh"
 
@@ -209,6 +210,10 @@ __global__ void __launch_bounds__(EE_THREADS) v2_topk_encode_kernel(const TEncAr
 __global__ void __launch_bounds__(EE_THREADS) v2_topk_encode_ef_kernel(const TEncArgs a) {
   entry_encode<KEEP_TOPK, true>(a);
 }
+// momentum correction: the error-feedback encode, and the worker's momentum zeroed at every kept entry
+__global__ void __launch_bounds__(EE_THREADS) v2_topk_encode_mc_kernel(const TEncArgs a, float* mom) {
+  entry_encode<KEEP_TOPK, true, true>(a, mom);
+}
 
 // ---- --code-stats for top-k units ----------------------------------------------------------------------------
 // The partials / accumulator layout of every --code-stats kernel (STAT_PART / STAT_ACC, v2_common.cuh).  gsq = ||bf16(g)||^2; mse = the dropped energy, the entries below T plus the
@@ -317,7 +322,7 @@ void atomo_v2_launch_topk_encode(const void* units, const void* tiles, int tile0
                                  const int* sel, const int* tile_counts, float* const* arena_peer,
                                  int* const* sig_peer, int n_owners, long long arena_floats, int worker, int group,
                                  const void* ctrl, unsigned int* group_counter, long long* tstats, int final_group,
-                                 float* residual, cudaStream_t stream) {
+                                 float* residual, float* mom, cudaStream_t stream) {
   if (ntiles <= 0) return;
   TEncArgs a;
   a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.gptr = gptr; a.l1 = nullptr;
@@ -325,7 +330,8 @@ void atomo_v2_launch_topk_encode(const void* units, const void* tiles, int tile0
   a.worker = worker; a.group = group; a.ctrl = (const Ctrl2*)ctrl; a.group_counter = group_counter;
   a.ext_uniforms = nullptr; a.tstats = tstats; a.final_group = final_group; a.residual = residual;
   a.sel = sel; a.tile_counts = tile_counts;
-  if (residual != nullptr) v2_topk_encode_ef_kernel<<<ntiles, EE_THREADS, 0, stream>>>(a);
+  if (mom != nullptr) v2_topk_encode_mc_kernel<<<ntiles, EE_THREADS, 0, stream>>>(a, mom);
+  else if (residual != nullptr) v2_topk_encode_ef_kernel<<<ntiles, EE_THREADS, 0, stream>>>(a);
   else v2_topk_encode_kernel<<<ntiles, EE_THREADS, 0, stream>>>(a);
 }
 

@@ -69,6 +69,9 @@ def run_rank(args) -> None:
     if getattr(args, "error_feedback", False):
         raise SystemExit("--error-feedback keeps its residuals in the --backend p2p bf16 engine; the %s backend's "
                          "PyTorch coders do not (run without --error-feedback)" % backend)
+    if getattr(args, "momentum_correction", False):
+        raise SystemExit("--momentum-correction keeps each worker's momentum in the --backend p2p bf16 engine; the %s "
+                         "backend's workers keep none (run without --momentum-correction)" % backend)
     if getattr(args, "accumulate_steps", 1) != 1:
         raise SystemExit("--accumulate-steps runs on the --backend p2p bf16 engine; the %s backend's workers push "
                          "after every backward (run without --accumulate-steps)" % backend)

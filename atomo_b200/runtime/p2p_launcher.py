@@ -97,6 +97,8 @@ def _build_engine(args, model, rank, world):
             kw["trust_coefficient"] = getattr(args, "trust_coefficient", 0.001)
         if clip:
             kw["clip_grad_norm"] = clip
+        if getattr(args, "momentum_correction", False):
+            kw["momentum_correction"] = True    # the engine refuses codes / optimizers it cannot correct
         return ShadowEngine(model, rank, world, code=args.code, svd_rank=args.svd_rank, lr=args.lr,
                             momentum=args.momentum, weight_decay=args.weight_decay, nesterov=args.nesterov,
                             optimizer=args.optimizer, ps_mode=args.ps_mode, groups=args.groups, sampling=args.sampling,
@@ -116,6 +118,9 @@ def _build_engine(args, model, rank, world):
     if getattr(args, "error_feedback", False):
         raise SystemExit("--error-feedback runs on the bf16 engine (--dtype bf16, --engine auto|shadow); the fp32-flat "
                          "engine keeps no residual (run without --error-feedback)")
+    if getattr(args, "momentum_correction", False):
+        raise SystemExit("--momentum-correction runs on the bf16 engine (--dtype bf16, --engine auto|shadow, --code "
+                         "topk --error-feedback 1); the fp32-flat engine keeps no worker momentum")
     if getattr(args, "code_stats", False):
         raise SystemExit("--code-stats reads the statistics of the bf16 engine (--dtype bf16, --engine auto|shadow); "
                          "the fp32-flat engine does not compute them (run without --code-stats)")
@@ -228,6 +233,8 @@ def run_p2p_training(args, device=None):
                 extra["code_stats"] = eng.code_stats(reset=True)
             if getattr(args, "error_feedback", False) and eng.is_worker:
                 extra["ef_norm"] = eng.error_feedback_norm()["model"]
+            if getattr(args, "momentum_correction", False) and eng.is_worker:
+                extra["mom_norm"] = eng.momentum_correction_norm()["model"]
             if getattr(args, "clip_grad_norm", 0.0) and eng.is_owner:
                 extra["grad_norm"], extra["clip_coef"] = eng.grad_norm()
             metrics.write(step=cur, loss=loss, prec1=p1, prec5=p5, step_s=step_s, comp=comp, encode=enc, comm=comm,

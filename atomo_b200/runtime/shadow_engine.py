@@ -60,6 +60,13 @@ one central PS kernel at the end of the step):
   ``bf16((sum g_j) / N (+ e))`` into its gradient buffers in place (with error feedback it takes the place of the apply
   launch), so every code, ``code_stats`` and the residual work unchanged.  BN statistics take one update per
   micro-batch.  ``N = 1`` launches exactly what it launched before.
+* **Momentum correction** (``momentum_correction=True``; top-k with error feedback and SGD only): Deep Gradient
+  Compression's momentum on the workers, before the gradient is sparsified.  Each worker keeps an fp32 momentum ``u``
+  per weight and vector element; per group, an apply launch (``csrc/v2_momentum.cu``, in place of the error-feedback
+  apply) forms ``u = m u + g + wd w`` (``w`` the worker's bf16 weight) and codes ``A = u + e`` (Nesterov: ``d + m u +
+  e``), and the top-k encode zeroes ``u`` at every entry it sent (momentum-factor masking).  Vectors travel exactly:
+  ``vgrads`` becomes their momentum direction, unmasked.  The PS runs plain SGD on what it receives.  Unlike
+  ``torch.optim.SGD``, weight decay uses the bf16 weight the worker trained with, not the owner's fp32 master.
 * Optimizers fused in the PS epilogue: momentum-SGD (``src/optim/sgd.py:57-90``), Adam / AMSGrad
   (``src/optim/adam.py:37-94``).  LARS and LAMB (``optimizer="lars" | "lamb"``, ``trust_coefficient``) need whole-tensor
   norms first: the code's PS kernel runs its layer-wise instantiation (moments, direction, per-tile partials; vectors
@@ -76,6 +83,7 @@ step-stamped flags in peer memory (``csrc/v2_common.cuh``); no NCCL call on the 
 """
 from __future__ import annotations
 
+import math
 import numbers
 import os
 import struct
@@ -111,7 +119,7 @@ class ShadowEngine:
                  side_priority: int = -1, resample_empty: bool = False, quantization_level: int = 4,
                  bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False,
                  error_feedback: bool = False, accumulate_steps: int = 1, trust_coefficient: float = 0.001,
-                 clip_grad_norm: float = 0.0):
+                 clip_grad_norm: float = 0.0, momentum_correction: bool = False):
         self.optimizer = optimizer.lower()
         if self.optimizer not in ("sgd", "adam", "lars", "lamb"):      # checked before any CUDA work
             raise ValueError("ShadowEngine optimizers: sgd | adam | lars | lamb (got %r)" % (optimizer,))
@@ -180,6 +188,24 @@ class ShadowEngine:
             if not (P2.HADAMARD_MIN_BUCKET <= hb <= P2.HADAMARD_MAX_BUCKET and hb & (hb - 1) == 0):
                 raise ValueError("hadamard: bucket_size must be a power of two in [%d, %d] (got %r)"
                                  % (P2.HADAMARD_MIN_BUCKET, P2.HADAMARD_MAX_BUCKET, bucket_size))
+        self.momentum_correction = bool(momentum_correction)
+        if self.momentum_correction:        # checked before any CUDA work
+            if self.code != "topk" or not self.error_feedback:
+                raise ValueError("momentum_correction needs code='topk' with error_feedback=True: masking the momentum "
+                                 "of the entries sent has no meaning for the other codes (got code=%r, "
+                                 "error_feedback=%r)" % (self.code, self.error_feedback))
+            if self.optimizer != "sgd":
+                raise ValueError("momentum_correction moves momentum-SGD to the workers: optimizer='sgd' only "
+                                 "(got %r)" % (optimizer,))
+            if dampening != 0:
+                raise ValueError("momentum_correction takes dampening=0 (got %r)" % (dampening,))
+            if isinstance(momentum, bool) or not isinstance(momentum, numbers.Real) or not 0 <= momentum < math.inf:
+                raise ValueError("momentum_correction needs a finite momentum >= 0 (got %r)" % (momentum,))
+            if self.clip_on:
+                raise ValueError("momentum_correction cannot be combined with clip_grad_norm: the workers' momentum "
+                                 "would run on the unclipped gradient")
+            if accumulate_steps != 1:
+                raise ValueError("momentum_correction cannot be combined with accumulate_steps > 1")
         self.C = load_ext()
         C = self.C
         assert C.v2_unit_bytes() == P2.UNIT_BYTES and C.v2_ctrl_bytes() == P2.CTRL2_BYTES
@@ -380,6 +406,10 @@ class ShadowEngine:
         self.counters = torch.zeros(nc + 2 * P2.MAX_GROUPS + 8, dtype=torch.int32, device=dev)
         self.cnt_enc_group = self.counters.data_ptr() + 4 * nc
         self.cnt_ps_group = self.cnt_enc_group + 4 * P2.MAX_GROUPS
+        # momentum correction: momentum, weight decay and Nesterov act on the workers (v2_mc_apply), the PS runs plain SGD
+        self.mc_momentum, self.mc_weight_decay, self.mc_nesterov = float(momentum), float(weight_decay), bool(nesterov)
+        if self.momentum_correction:
+            momentum, dampening, weight_decay, nesterov = 0.0, 0.0, 0.0, False
         self.ctrl = _dev_bytes(P2.pack_ctrl2(step=1, lr=lr, momentum=momentum, dampening=dampening,
                                              weight_decay=weight_decay, nesterov=nesterov, first_step=1, seed=seed,
                                              beta1=betas[0], beta2=betas[1], eps=eps, opt=self.opt,
@@ -457,13 +487,19 @@ class ShadowEngine:
         # uses t_gptr, which the encoders read)
         self.acc = self.vacc = self.t_vec_chunks = self.t_aptr = self.host_aptr = None
         self.vec_range = []
-        if self.accum > 1:
-            self.acc, self.vacc = z(pl.w_total), z(pl.v_total)
+        if self.accum > 1 or (self.momentum_correction and self.is_worker):
             vchunks, self.vec_range = P2.vec_chunks(pl)
             self.t_vec_chunks = _dev_bytes(vchunks, dev)
+        if self.accum > 1:
+            self.acc, self.vacc = z(pl.w_total), z(pl.v_total)
             self.t_aptr = torch.zeros((self.accum - 1, n_w), dtype=torch.int64, device=dev)
             self.host_aptr = np.zeros((self.accum - 1, n_w), dtype=np.int64)
         self.inv_n = float(np.float32(1.0 / self.accum))
+        # momentum correction (csrc/v2_momentum.cu): the worker's fp32 momentum per weight element (wshadow's physical
+        # order, the residual's offsets) and per vector element (vgrads' order)
+        self.mc_mom = self.mc_vmom = None
+        if self.momentum_correction and self.is_worker:
+            self.mc_mom, self.mc_vmom = z(pl.w_total), z(pl.v_total)
         self.pw_warm = P2.pw_warm_ranges(pl) if self.power else []     # Q_w inside gpart (checkpointed)
         self._fresh_worker_state()
         self.loss_buf = torch.zeros(3, dtype=torch.float32, device=dev)
@@ -501,6 +537,9 @@ class ShadowEngine:
         PowerSGD's first draw of ``Q_w`` (Philox keyed by seed, unit, column) with a cleared unit state."""
         if self.residual is not None:
             self.residual.zero_()
+        if self.mc_mom is not None:
+            self.mc_mom.zero_()
+            self.mc_vmom.zero_()
         if self.vprev is not None:
             self.vprev.zero_()
             for u in self.plan.units:
@@ -626,6 +665,18 @@ class ShadowEngine:
         sq = torch.stack([self.residual[q.off:q.off + q.numel].double().square().sum() for _, q in ws]).tolist()
         return {"model": float(sum(sq)) ** 0.5, "tensors": {n: v ** 0.5 for (n, _), v in zip(ws, sq)}}
 
+    def momentum_correction_norm(self) -> dict:
+        """``||u||`` of this worker's momentum (``momentum_correction=True``): per parameter tensor (weights and
+        vectors) and for the whole model.  Reading it synchronises the device."""
+        if self.mc_mom is None:
+            raise RuntimeError("momentum_correction_norm() needs ShadowEngine(..., momentum_correction=True) on a "
+                               "worker")
+        names = {id(p): n for n, p in self.model.named_parameters()}
+        ts = [(names.get(id(p), str(q.index)), (self.mc_mom if q.is_w else self.mc_vmom)[q.off:q.off + q.numel])
+              for p, q in zip(self.params, self.plan.params)]
+        sq = torch.stack([t.double().square().sum() for _, t in ts]).tolist()
+        return {"model": float(sum(sq)) ** 0.5, "tensors": {n: v ** 0.5 for (n, _), v in zip(ts, sq)}}
+
     def _launch_code_stats(self, g: int):
         """Estimator statistics of group ``g``: after its push on the same stream (the gradient, this step's sigma /
         selcount / L1 / clip and this worker's slot headers and norms are live until the next encode)."""
@@ -701,6 +752,15 @@ class ShadowEngine:
                             self.t_gptr.data_ptr(), self.acc.data_ptr(), self.vacc.data_ptr(), self.vgrads.data_ptr(),
                             self.inv_n, res)
             self._nlaunch += 1
+        elif self.mc_mom is not None:
+            # momentum correction: u = m u + g (+ wd w), A = u (Nesterov: d + m u) + e into the gradient buffers
+            # (bf16) and the residual; the vectors' direction into vgrads
+            (c0, nw), (v0, nv), cb = self.ef_range[g], self.vec_range[g], struct.calcsize(P2.EF_CHUNK_FMT)
+            C.v2_mc_apply(self.t_ef_chunks.data_ptr() + cb * c0, nw, self.t_vec_chunks.data_ptr() + cb * v0, nv,
+                          self.t_gptr.data_ptr(), self.wshadow.data_ptr(), self.mc_mom.data_ptr(), res,
+                          self.vgrads.data_ptr(), self.vparams.data_ptr(), self.mc_vmom.data_ptr(), self.mc_momentum,
+                          self.mc_weight_decay, self.mc_nesterov)
+            self._nlaunch += 1
         elif res:     # A = g + e into the gradient buffers (bf16) and the residual (its rounding remainder)
             c0, ncs = self.ef_range[g]
             C.v2_ef_apply(self.t_ef_chunks.data_ptr(), c0, ncs, self.t_gptr.data_ptr(), res)
@@ -750,7 +810,7 @@ class ShadowEngine:
                              self.topk_sel.data_ptr(), self.topk_tiles.data_ptr(), self.t_arena_peer.data_ptr(),
                              self.t_sig_owner.data_ptr(), self.n_owners, pl.arena_floats, self.worker_index, g,
                              self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g, self.tstats.data_ptr(),
-                             self._fired == self.G, res)
+                             self._fired == self.G, res, self.mc_mom.data_ptr() if self.mc_mom is not None else 0)
             self._nlaunch += 3
             return
         if nt > 0 and self.entry:
@@ -1210,7 +1270,8 @@ class ShadowEngine:
             ``sq`` / ``vsq`` and for AMSGrad ``sqmax`` / ``vsqmax``, the BN running statistics, and the step and LR
             of ``ctrl``.
         (b) per-worker state, in ``model_step_<N>_worker<R>`` (:meth:`_worker_tensors`, physical order):
-            ``residual`` (``error_feedback``, fp32 per weight element); ``vprev`` (svd / qsvd with ``warm_start``,
+            ``residual`` (``error_feedback``, fp32 per weight element); ``mom`` / ``vmom_w``
+            (``momentum_correction``, the worker's fp32 momentum per weight / vector element); ``vprev`` (svd / qsvd with ``warm_start``,
             the previous step's Jacobi basis per coded unit); PowerSGD's warm ``Q_w`` (only those ranges of
             ``gpart``, ``ops/plan2.py`` ``pw_warm_ranges``) and ``pw_state`` (160 bytes per unit: the draw counter
             carries over; ``R^{-1}``, the mask and the non-finite flag are rewritten by pass A before pass B reads
@@ -1264,6 +1325,8 @@ class ShadowEngine:
             side.update(bucket_size=self.bucket_size)
         if self.entry:
             side.update(entry_budget=self.entry_budget)
+        if self.momentum_correction:
+            side.update(momentum_correction=True)
         side.update(adam_state)
         torch.save(side, path + "_optim.tmp")
         os.replace(path + "_optim.tmp", path + "_optim")
@@ -1271,9 +1334,11 @@ class ShadowEngine:
 
     def _worker_config(self) -> dict:
         """What this worker's state depends on: a worker file is applied only where every field matches."""
-        return {"code": self.code, "plan": P2.plan_digest(self.plan), "error_feedback": self.error_feedback,
-                "warm_start": self.warm_start, "world": self.world, "ps_mode": self.ps_mode,
-                "worker": self.worker_index}
+        cfg = {"code": self.code, "plan": P2.plan_digest(self.plan), "error_feedback": self.error_feedback,
+               "warm_start": self.warm_start, "world": self.world, "ps_mode": self.ps_mode, "worker": self.worker_index}
+        if self.momentum_correction:
+            cfg["momentum_correction"] = True
+        return cfg
 
     def _worker_tensors(self) -> dict:
         """Class (b) of :meth:`save_checkpoint`: this worker's tensors that carry over between steps.  ``pw_qw`` is a
@@ -1282,6 +1347,8 @@ class ShadowEngine:
         out = {}
         if self.residual is not None:
             out["residual"] = self.residual
+        if self.mc_mom is not None:
+            out["mom"], out["vmom_w"] = self.mc_mom, self.mc_vmom
         if self.vprev is not None:
             out["vprev"] = self.vprev
         if self.power:
@@ -1322,11 +1389,15 @@ class ShadowEngine:
         self._barrier()
         path = ckpt.model_path(train_dir, step)
         if os.path.exists(path + "_optim"):     # refused before any state changes
-            saved = torch.load(path + "_optim", map_location="cpu", weights_only=False).get("optimizer", "sgd or adam")
+            side = torch.load(path + "_optim", map_location="cpu", weights_only=False)
+            saved = side.get("optimizer", "sgd or adam")
             layerwise = ("lars", "lamb")
             if (self.layerwise or saved in layerwise) and saved != self.optimizer:
                 raise ValueError("checkpoint %s was written by optimizer %s; this engine runs %s" % (path, saved,
                                                                                                   self.optimizer))
+            if bool(side.get("momentum_correction", False)) != self.momentum_correction:
+                raise ValueError("checkpoint %s was written with momentum_correction=%s; this engine runs %s"
+                                 % (path, bool(side.get("momentum_correction", False)), self.momentum_correction))
         sd = torch.load(path, map_location="cpu", weights_only=False)
         byname = dict(self.model.named_parameters())
         byid = {id(p): q for p, q in zip(self.params, self.plan.params)}

@@ -118,6 +118,12 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "top-k, topk, sign and powersgd, the contractive codes, and with fp8 and hadamard at 4 or 8 "
                         "bits, whose variance is small), every push counted (no --num-aggregate below the worker "
                         "count).  Residuals (and PowerSGD's warm state) are not checkpointed: --resume starts them afresh")
+    p.add_argument("--momentum-correction", type=bool_flag, default=False,
+                   help="p2p backend, bf16 engine, --code topk --error-feedback 1 --optimizer sgd: Deep Gradient "
+                        "Compression's momentum correction.  Every worker applies --momentum, --nesterov and "
+                        "--weight-decay to its own gradient before top-k (weight decay on its bf16 weights) and zeroes "
+                        "the momentum of the entries it sent; the parameter server runs plain SGD.  Not with "
+                        "--accumulate-steps > 1 or --clip-grad-norm")
     p.add_argument("--accumulate-steps", type=int, default=1,
                    help="p2p backend, bf16 engine: micro-batches per optimizer step.  Each worker runs N forward / "
                         "backward passes of --batch-size samples, sums their gradients in fp32 and codes and pushes "
