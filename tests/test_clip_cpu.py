@@ -18,15 +18,14 @@ from atomo_b200.runtime import master as M
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args, check_clip_grad_norm
 
+from shadow_harness import fit_args, forbid_cuda
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BAD = [-1.0, float("nan"), float("inf"), -float("inf"), True, "1.0"]
 
 
 def _args(tmp_path, *extra):
-    return add_fit_args(argparse.ArgumentParser(), [
-        "--network", "LeNet", "--dataset", "MNIST", "--synthetic", "1", "--train-len", "512", "--test-len", "128",
-        "--batch-size", "32", "--test-batch-size", "64", "--lr", "0.05", "--code", "svd", "--svd-rank", "3",
-        "--log-interval", "1", "--eval-freq", "100", "--train-dir", str(tmp_path) + "/", *extra])
+    return fit_args(tmp_path, "--code", "svd", "--svd-rank", "3", *extra)
 
 
 def test_flag_parses_and_defaults_to_off():
@@ -44,10 +43,7 @@ def test_bad_values_are_refused(bad):
 @pytest.mark.parametrize("bad", BAD[:4])
 def test_engine_refuses_before_cuda_work(bad, monkeypatch):
     from atomo_b200.runtime import shadow_engine as S
-
-    def no_cuda(*a, **k):
-        raise AssertionError("refused only after CUDA work started")
-    monkeypatch.setattr(S, "load_ext", no_cuda)
+    forbid_cuda(monkeypatch)
     with pytest.raises(ValueError, match="clip_grad_norm"):
         S.ShadowEngine(None, 0, 1, clip_grad_norm=bad)
 

@@ -10,6 +10,8 @@ import torch
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
 
+from shadow_harness import fit_args, forbid_cuda
+
 
 def test_code_stats_flag_parses():
     assert add_fit_args(argparse.ArgumentParser(), []).code_stats is False
@@ -20,19 +22,13 @@ def test_code_stats_flag_parses():
 @pytest.mark.parametrize("kw,match", [(dict(code="qsvd"), "QSVD"), (dict(code="svd", resample_empty=True), "resample")])
 def test_shadow_engine_refuses_settings_without_a_closed_form(kw, match, monkeypatch):
     from atomo_b200.runtime import shadow_engine as S
-
-    def no_cuda(*a, **k):
-        raise AssertionError("refused only after CUDA work started")
-    monkeypatch.setattr(S, "load_ext", no_cuda)
+    forbid_cuda(monkeypatch)
     with pytest.raises(ValueError, match=match):
         S.ShadowEngine(torch.nn.Linear(4, 4), code_stats=True, **kw)
 
 
 def _args(tmp_path, *extra):
-    return add_fit_args(argparse.ArgumentParser(), [
-        "--network", "LeNet", "--dataset", "MNIST", "--synthetic", "1", "--train-len", "512", "--test-len", "128",
-        "--batch-size", "32", "--test-batch-size", "64", "--lr", "0.05", "--code", "svd", "--svd-rank", "3",
-        "--log-interval", "1", "--eval-freq", "100", "--train-dir", str(tmp_path) + "/", *extra])
+    return fit_args(tmp_path, "--code", "svd", "--svd-rank", "3", *extra)
 
 
 def test_fused_engine_and_qsvd_refuse_the_flag(tmp_path):

@@ -17,6 +17,8 @@ import torch
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
 
+from shadow_harness import fit_args, forbid_cuda
+
 FLT_MIN = float(np.finfo(np.float32).tiny)
 
 
@@ -29,10 +31,7 @@ def test_accumulate_flag_parses():
 @pytest.mark.parametrize("n", [0, -1, 1.5, True])
 def test_engine_refuses_bad_accumulate_steps(n, monkeypatch):
     from atomo_b200.runtime import shadow_engine as S
-
-    def no_cuda(*a, **k):
-        raise AssertionError("refused only after CUDA work started")
-    monkeypatch.setattr(S, "load_ext", no_cuda)
+    forbid_cuda(monkeypatch)
     with pytest.raises(ValueError, match="accumulate_steps"):
         S.ShadowEngine(None, 0, 1, accumulate_steps=n)
 
@@ -46,10 +45,7 @@ def test_prepare_refuses_an_indivisible_batch():
 
 
 def _args(tmp_path, *extra):
-    return add_fit_args(argparse.ArgumentParser(), [
-        "--network", "LeNet", "--dataset", "MNIST", "--synthetic", "1", "--train-len", "512", "--test-len", "128",
-        "--batch-size", "32", "--test-batch-size", "64", "--lr", "0.05", "--code", "svd", "--svd-rank", "3",
-        "--log-interval", "1", "--eval-freq", "100", "--train-dir", str(tmp_path) + "/", *extra])
+    return fit_args(tmp_path, "--code", "svd", "--svd-rank", "3", *extra)
 
 
 def test_fused_engine_and_fp32_refuse_the_flag(tmp_path):

@@ -10,9 +10,10 @@ import os
 import numpy as np
 import pytest
 import torch
-import torch.nn as nn
 
 from atomo_b200.ops import plan2 as P
+
+from shadow_harness import Linear
 
 pytestmark = pytest.mark.gpu
 
@@ -33,19 +34,6 @@ def _grads(seed=0):
             x.zero_()
         out.append(x.bfloat16().float().cuda())     # bf16-representable: the engine's gradient is exactly this
     return out
-
-
-class Linear(nn.Module):
-    """loss = sum_p <p, G_p>: the gradient of every parameter is G_p whatever the weights are."""
-
-    def __init__(self, grads):
-        super().__init__()
-        self.ps = nn.ParameterList([nn.Parameter(torch.zeros(g.shape)) for g in grads])
-        self.gs = grads
-
-    def forward(self, x):
-        s = sum((p.float() * g).sum() for p, g in zip(self.ps, self.gs))
-        return s.reshape(1, 1).expand(x.shape[0], 2)
 
 
 def _engine(code, grads, lr=0.0, **kw):

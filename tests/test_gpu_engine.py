@@ -4,15 +4,9 @@ import os
 import pytest
 import torch
 
+from shadow_harness import batch
+
 pytestmark = pytest.mark.gpu
-
-
-def _batch(net, n=32, seed=0):
-    from atomo_b200.models import input_shape
-    from atomo_b200.data import SyntheticImageDataset
-    ds = SyntheticImageDataset(input_shape(net), 10, 4096, seed=seed)
-    x, y = ds.materialize(n)
-    return x.pin_memory(), y.pin_memory()
 
 
 @pytest.mark.parametrize("code,net,graph", [("svd", "LeNet", False), ("svd", "ResNet18", True), ("sgd", "LeNet", True),
@@ -26,7 +20,7 @@ def test_single_gpu_engine_trains(code, net, graph):
     model = build_model(net, 10)
     eng = FusedEngine(model, 0, 1, code=code, svd_rank=3, lr=0.05, momentum=0.9, use_graph=graph,
                       entry_budget=0.25, seed=3)
-    x, y = _batch(net, 64)
+    x, y = batch(net, 64)
     eng.prepare(x, y, warmup=2)
     first = None
     for i in range(30):
@@ -53,7 +47,7 @@ def test_dense_engine_matches_plain_sgd():
     ref = copy.deepcopy(model).cuda()
     opt = torch.optim.SGD(ref.parameters(), lr=0.05, momentum=0.9)
     eng = FusedEngine(model, 0, 1, code="sgd", lr=0.05, momentum=0.9, use_graph=False)
-    x, y = _batch("LeNet", 32)
+    x, y = batch("LeNet", 32)
     eng.prepare(x, y, warmup=0)
     xc, yc = x.cuda(), y.cuda()
     for _ in range(5):
@@ -79,7 +73,7 @@ def _two_rank_worker(rank, world, code, port, out):
     model = build_model("LeNet", 10)
     eng = FusedEngine(model, rank, world, code=code, svd_rank=3, lr=0.05, momentum=0.9, use_graph=True, seed=5,
                       entry_budget=0.25)
-    x, y = _batch("LeNet", 32, seed=rank)
+    x, y = batch("LeNet", 32, seed=rank)
     eng.prepare(x, y, warmup=2)
     losses = []
     for _ in range(20):
@@ -184,7 +178,7 @@ def test_subspace_engine_trains(net):
     torch.cuda.set_device(0)
     eng = FusedEngine(build_model(net, 10), 0, 1, code="svd", svd_rank=3, lr=0.02, momentum=0.9, use_graph=True,
                       subspace=True)
-    x, y = _batch(net, 64)
+    x, y = batch(net, 64)
     eng.prepare(x, y, warmup=2)
     first = float(eng.train_step(x, y)[0])
     for _ in range(40):

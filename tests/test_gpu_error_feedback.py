@@ -8,10 +8,11 @@ import math
 
 import pytest
 import torch
-import torch.nn as nn
 
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
+
+from shadow_harness import Loopback, ef_grads, fit_args, forbid_cuda
 
 
 # ---------------------------------------------------------------------------------------------------- CPU
@@ -29,10 +30,7 @@ def test_error_feedback_flag_parses():
 def test_shadow_engine_refuses_codes_without_feedback(kw, match, monkeypatch):
     """Checked before any CUDA work, so a bad setting fails the same way on every machine."""
     from atomo_b200.runtime import shadow_engine as S
-
-    def no_cuda(*a, **k):
-        raise AssertionError("refused only after CUDA work started")
-    monkeypatch.setattr(S, "load_ext", no_cuda)
+    forbid_cuda(monkeypatch)
     kw = dict(kw)
     world = kw.pop("world", 1)
     with pytest.raises(ValueError, match=match):
@@ -40,10 +38,7 @@ def test_shadow_engine_refuses_codes_without_feedback(kw, match, monkeypatch):
 
 
 def _args(tmp_path, *extra):
-    return add_fit_args(argparse.ArgumentParser(), [
-        "--network", "LeNet", "--dataset", "MNIST", "--synthetic", "1", "--train-len", "512", "--test-len", "128",
-        "--batch-size", "32", "--test-batch-size", "64", "--lr", "0.05", "--code", "svd", "--svd-rank", "3",
-        "--log-interval", "1", "--eval-freq", "100", "--train-dir", str(tmp_path) + "/", *extra])
+    return fit_args(tmp_path, "--code", "svd", "--svd-rank", "3", *extra)
 
 
 def test_fused_engine_refuses_the_flag(tmp_path):
@@ -62,72 +57,10 @@ def test_role_backends_refuse_the_flag(monkeypatch, tmp_path):
 
 
 # ---------------------------------------------------------------------------------------------------- GPU harness
-# stem (MAT units), 3x3 convs (SLAB units; one a multiple of 4096 elements, one not), fc layers (MAT blocks), a tensor
-# smaller than an absolute budget, a vector
-SHAPES = [(64, 3, 3, 3), (64, 32, 3, 3), (128, 64, 3, 3), (10, 512), (300, 200), (7, 20), (32, 16, 3, 3), (64,)]
-
 CODES = [("svd", dict(svd_rank=3)), ("svd", dict(svd_rank=1, random_sample=False)),
          ("svd", dict(svd_rank=2, random_sample=False)), ("entrywise", dict(entry_budget=0.05)),
          ("entrywise", dict(entry_budget=0.01)), ("qsgd", dict(quantization_level=2)),
          ("qsgd", dict(quantization_level=4, bucket_size=128))]
-
-
-def _grads(seed=0):
-    g = torch.Generator().manual_seed(seed)
-    return [(torch.randn(s, generator=g) * (0.01 * (1 + i))).bfloat16().float().cuda() for i, s in enumerate(SHAPES)]
-
-
-class Linear(nn.Module):
-    """loss = sum_p <p, G_p>: the gradient of every parameter is G_p whatever the weights are."""
-
-    def __init__(self, grads):
-        super().__init__()
-        self.ps = nn.ParameterList([nn.Parameter(torch.zeros(g.shape)) for g in grads])
-        self.gs = grads
-
-    def forward(self, x):
-        s = sum((p.float() * g).sum() for p, g in zip(self.ps, self.gs))
-        return s.reshape(1, 1).expand(x.shape[0], 2)
-
-
-class Loopback:
-    """One rank that is the only worker and the only owner, fed a fixed gradient.  With lr = 1, no momentum and the
-    fp32 master zeroed before every step, the master after the step is minus what the owner reconstructed from this
-    worker's slot: g_hat."""
-
-    def __init__(self, code, grads, ef=True, **kw):
-        from atomo_b200.runtime.shadow_engine import ShadowEngine
-        torch.cuda.set_device(0)
-        self.eng = ShadowEngine(Linear(grads), 0, 1, code=code, lr=1.0, momentum=0.0, use_graph=False, overlap=False,
-                                warm_start=False, criterion=lambda lg, y: lg[0, 0], error_feedback=ef, seed=5, **kw)
-        self.x, self.y = torch.zeros(4, 2), torch.zeros(4, dtype=torch.long)
-        self.eng.prepare(self.x, self.y, warmup=0)
-        self.eng.heap.tensor("arena").zero_()      # slot words no push writes compare equal across engines
-        pl = self.eng.plan
-        self.w = [q for q in pl.params if q.is_w]
-        g = torch.zeros(pl.w_total, dtype=torch.float64, device="cuda")
-        for q in self.w:
-            t = grads[q.index].double()
-            g[q.off:q.off + q.numel] = (t.permute(0, 2, 3, 1) if t.dim() == 4 else t).reshape(-1)
-        self.g = g
-        self.mask = torch.zeros(pl.w_total, dtype=torch.bool, device="cuda")
-        for q in self.w:
-            self.mask[q.off:q.off + q.numel] = True
-
-    def residual(self):
-        r = self.eng.residual
-        return r.double().clone() if r is not None else torch.zeros_like(self.g)
-
-    def step(self):
-        """(g_hat, residual after the step), fp64, physical order (zero outside the weight tensors)."""
-        self.eng.master.zero_()
-        self.eng.train_step(self.x, self.y)
-        torch.cuda.synchronize()
-        assert self.eng.error_code() == 0
-        return (-self.eng.master.double()) * self.mask, self.residual() * self.mask
-
-    def close(self):
-        self.eng.close()
 
 
 # ---------------------------------------------------------------------------------------------------- GPU: kernels
@@ -135,7 +68,7 @@ class Loopback:
 @pytest.mark.parametrize("code,kw", CODES)
 def test_per_step_identity(code, kw):
     """g + e_old == g_hat + e_new for every weight element, step after step: what is not pushed stays owed."""
-    h = Loopback(code, _grads(1), **kw)
+    h = Loopback(code, ef_grads(1), **kw)
     try:
         g = h.g
         e_old = h.residual()
@@ -161,7 +94,7 @@ def test_telescoping_topk_rank1():
     """A fixed gradient for T = 200 steps: the pushed sum misses T g by exactly the final residual (the sum
     telescopes), which stays bounded; without error feedback the same top-k code misses by T ||g - g_hat||."""
     T = 200
-    grads = _grads(2)
+    grads = ef_grads(2)
     sums, norms = {}, {}
     for ef in (True, False):
         h = Loopback("svd", grads, ef=ef, svd_rank=1, random_sample=False)
@@ -194,7 +127,7 @@ def test_off_means_off(code, kw):
     first step pushes the same bits with the option on as with it off (arena, gradient buffers, reconstructed master)."""
     out = {}
     for ef in (False, True):
-        h = Loopback(code, _grads(3), ef=ef, **kw)
+        h = Loopback(code, ef_grads(3), ef=ef, **kw)
         try:
             ghat, _ = h.step()
             arena = h.eng.heap.tensor("arena").clone()
@@ -256,7 +189,7 @@ def test_loss_falls_on_a_fixed_batch():
                                      ("qsgd", dict(quantization_level=2))])
 def test_code_stats_describe_the_coded_input(code, kw):
     """With error feedback the encoders read bf16(g + e): --code-stats' gsq is ||bf16(A)||^2."""
-    h = Loopback(code, _grads(4), code_stats=True, **kw)
+    h = Loopback(code, ef_grads(4), code_stats=True, **kw)
     try:
         h.step()                        # e != 0 from here on
         h.eng.code_stats(reset=True)

@@ -16,6 +16,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from shadow_harness import ext
+
 pytestmark = pytest.mark.gpu
 
 # The statistics bound: every kernel sum is a chain of at most ~300 dependent fp32 adds for the shapes here (worst
@@ -54,11 +56,6 @@ GEOMETRY = [
     (2040, "4cap-1", False, True, 0.1, 1e-5), (2048, "4cap+1", False, False, 0.01, 1e-5),
     (1032, "7", False, False, 0.01, 1e-5),
 ]
-
-
-def _ext():
-    from atomo_b200.ops._ext import load
-    return load()
 
 
 def _rows(t):
@@ -119,7 +116,7 @@ def _inputs(R, C, res, exact, gen):
 
 def _run_binding(inp, relu, rm, rv, eps, momentum):
     """both kernel chains through the binding on [R][C] rows viewed as (1, C, R, 1); rm / rv are updated in place"""
-    K = _ext()
+    K = ext()
     x = _nchw(inp["x"], 1, inp["x"].size(0), 1)
     res = None if inp["res"] is None else _nchw(inp["res"], 1, x.size(2), 1)
     dy = _nchw(inp["dy"], 1, x.size(2), 1)
@@ -382,7 +379,7 @@ def test_fused_bn_misaligned_view_falls_back_to_stock():
     assert bn._can_fuse(x, None) is False
     assert bn._can_fuse(xa, r) is False
 
-    K = _ext()
+    K = ext()
     f32 = lambda k: torch.empty(k, device="cuda")
     y = torch.empty_like(xa)
     with pytest.raises(RuntimeError, match="16-byte aligned"):

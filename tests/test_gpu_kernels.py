@@ -4,88 +4,9 @@ import math
 import pytest
 import torch
 
+from shadow_harness import Harness, ext
+
 pytestmark = pytest.mark.gpu
-
-
-def _ext():
-    from atomo_b200.ops._ext import load
-    return load()
-
-
-class Harness:
-    """One rank that is both worker 0 and the PS (world == 1): peer pointers are local."""
-
-    def __init__(self, shapes, code="svd", rank=3, systematic=False, lr=0.1, momentum=0.0, wd=0.0, nesterov=False,
-                 seed=7):
-        from atomo_b200.ops import plan as P
-        from atomo_b200.runtime.flat import FlatLayout
-        self.C, self.P = _ext(), P
-        dev = torch.device("cuda", 0)
-        self.dev = dev
-        self.layout = FlatLayout(shapes)
-        self.plan = P.build_plan(shapes, code, rank, systematic, offsets=self.layout.offsets)
-        pl = self.plan
-        total = pl.total_elems
-        u8 = lambda b: torch.frombuffer(bytearray(b if len(b) else b"\0" * 16), dtype=torch.uint8).to(dev)
-        self.t_layers = u8(pl.layers_bytes())
-        self.t_enc = u8(P.Plan.tiles_bytes(pl.enc_tiles))
-        self.t_ps = u8(P.Plan.tiles_bytes(pl.ps_tiles))
-        self.t_dense = u8(P.Plan.tiles_bytes(pl.dense_tiles))
-        self.t_ts = torch.tensor(pl.ts_layers or [0], dtype=torch.int32, device=dev)
-        n_ts = max(len(pl.ts_layers), 1)
-        self.gpart = torch.zeros(pl.gpart_floats, device=dev)
-        self.vsel = torch.zeros(n_ts * P.TS_MAX_COLS * P.RCAP_MAX, device=dev)
-        self.selcount = torch.zeros(n_ts, dtype=torch.int32, device=dev)
-        self.sigma = torch.zeros(n_ts * P.TS_MAX_COLS, device=dev)
-        self.arena = torch.zeros(pl.arena_floats, device=dev)
-        self.flags = torch.zeros(1024, dtype=torch.int32, device=dev)
-        self.params = torch.randn(total, device=dev)
-        self.grads = torch.zeros(total, device=dev)
-        self.mom = torch.zeros(total, device=dev)
-        self.ctrl = u8(P.pack_ctrl(step=1, lr=lr, momentum=momentum, weight_decay=wd, nesterov=nesterov, seed=seed))
-        self.t_params_peer = torch.tensor([self.params.data_ptr()], dtype=torch.int64, device=dev)
-        self.t_grads_peer = torch.tensor([self.grads.data_ptr()], dtype=torch.int64, device=dev)
-        self.t_flag_peer = torch.tensor([self.flags.data_ptr() + 4 * 64], dtype=torch.int64, device=dev)
-        self.rank_budget = rank
-        self.systematic = systematic
-
-    def set_step(self, step):
-        self.ctrl.view(torch.int32)[0] = step
-
-    def grad_views(self):
-        return self.layout.views(self.grads)
-
-    def encode(self, random_sample=True, waterfill=False, uniforms=None, rank=None):
-        C, pl = self.C, self.plan
-        C.gram(self.grads, self.t_layers, self.t_enc, len(pl.enc_tiles), self.gpart)
-        C.eig_sample(self.t_layers, self.t_ts, self.gpart, self.vsel, self.selcount, self.sigma,
-                     self.arena.data_ptr(), pl.arena_floats, self.ctrl, uniforms,
-                     self.rank_budget if rank is None else rank, random_sample, waterfill, self.systematic, 0, 1024)
-        C.project_push(self.grads, self.t_layers, self.t_enc, len(pl.enc_tiles), self.vsel, self.selcount,
-                       self.arena.data_ptr(), pl.arena_floats, self.flags.data_ptr(), self.ctrl, 0, True)
-
-    def ps_update(self):
-        C, pl = self.C, self.plan
-        C.ps_update(self.t_layers, self.t_ps, len(pl.ps_tiles), 1, 1, 1, self.params, self.mom, self.t_params_peer,
-                    0, self.t_grads_peer, 0, self.arena.data_ptr(), pl.arena_floats, self.flags.data_ptr(),
-                    self.t_flag_peer, self.ctrl, int(5e9), 1.0, min(len(pl.ps_tiles), 296))
-
-    def slot(self, layer):
-        P = self.P
-        base = self.arena[layer.slot_off:]
-        hdr = base[:4].view(torch.int32)
-        count = int(hdr[0])
-        rc, n = layer.rcap, layer.cols
-        s = base[4:4 + rc][:count]
-        V = base[4 + rc:4 + rc + rc * n].view(rc, n)[:count]
-        uo = P.slot_u_off(rc, n)
-        U = base[uo:uo + layer.rows * rc].view(layer.rows, rc)[:, :count]
-        return count, s, V, U
-
-    def tall(self, layer, flat):
-        """tall (rows x cols) view of a layer inside a flat buffer"""
-        t = flat[layer.off:layer.off + layer.numel]
-        return torch.as_strided(t, (layer.rows, layer.cols), (layer.row_stride, layer.col_stride))
 
 
 SHAPES = [(64, 32, 3, 3), (50, 20, 5, 5), (10, 512), (128, 64, 1, 1), (64,), (300, 200), (33, 7, 3, 3), (10,)]
@@ -206,7 +127,7 @@ def test_ps_update_lowrank_and_dense_matches_reference(momentum, nesterov, wd):
 
 def test_qsgd_kernel_matches_oracle_bits():
     from atomo_b200 import codings
-    C = _ext()
+    C = ext()
     dev = torch.device("cuda", 0)
     for scheme, q, bucket in (("qsgd", 4, 512), ("qsgd", 2, 256), ("terngrad", 4, 512), ("qsgd", 8, 1024)):
         torch.manual_seed(q)
@@ -246,7 +167,7 @@ def test_qsgd_kernel_matches_oracle_bits():
 
 def test_entrywise_kernel_matches_oracle():
     from atomo_b200.ops import plan as P
-    C = _ext()
+    C = ext()
     dev = torch.device("cuda", 0)
     shapes = [(64, 50), (1000,), (33, 7, 3, 3)]
     h = Harness(shapes, code="sgd")
@@ -291,7 +212,7 @@ def test_entrywise_kernel_matches_oracle():
 def test_wgmma_skinny_gemm_matches_fp32_matmul():
     """Grouped tf32 wgmma GEMM vs torch fp32 matmul for every operand layout the subspace route uses."""
     import struct
-    C = _ext()
+    C = ext()
     dev = torch.device("cuda", 0)
     torch.manual_seed(0)
     ctrl = torch.frombuffer(bytearray(__import__("atomo_b200.ops.plan", fromlist=["x"]).pack_ctrl()), dtype=torch.uint8).to(dev)

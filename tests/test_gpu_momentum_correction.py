@@ -21,6 +21,8 @@ from atomo_b200.optim import momentum_correction as MC
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
 
+from shadow_harness import fit_args, forbid_cuda
+
 
 # ---------------------------------------------------------------------------------------------------- CPU
 def test_flag_parses():
@@ -43,19 +45,9 @@ BASE = dict(code="topk", error_feedback=True, momentum=0.9)
     (dict(accumulate_steps=2), "accumulate_steps")])
 def test_engine_refuses_before_cuda(kw, match, monkeypatch):
     from atomo_b200.runtime import shadow_engine as S
-
-    def no_cuda(*a, **k):
-        raise AssertionError("refused only after CUDA work started")
-    monkeypatch.setattr(S, "load_ext", no_cuda)
+    forbid_cuda(monkeypatch)
     with pytest.raises(ValueError, match=match):
         S.ShadowEngine(None, 0, 1, momentum_correction=True, **dict(BASE, **kw))
-
-
-def _args(tmp_path, *extra):
-    return add_fit_args(argparse.ArgumentParser(), [
-        "--network", "LeNet", "--dataset", "MNIST", "--synthetic", "1", "--train-len", "512", "--test-len", "128",
-        "--batch-size", "32", "--test-batch-size", "64", "--lr", "0.05", "--log-interval", "1", "--eval-freq", "100",
-        "--train-dir", str(tmp_path) + "/", *extra])
 
 
 def test_launcher_passes_the_kwarg_only_when_on(tmp_path, monkeypatch):
@@ -67,18 +59,18 @@ def test_launcher_passes_the_kwarg_only_when_on(tmp_path, monkeypatch):
             seen.append(kw)
     monkeypatch.setattr(S, "ShadowEngine", Fake)
     topk = ("--code", "topk", "--dtype", "bf16", "--entry-budget", "0.01", "--error-feedback", "1")
-    L._build_engine(_args(tmp_path, *topk), nn.Linear(4, 4), 0, 1)
+    L._build_engine(fit_args(tmp_path, *topk), nn.Linear(4, 4), 0, 1)
     assert "momentum_correction" not in seen[-1]
-    L._build_engine(_args(tmp_path, *topk, "--momentum-correction", "0"), nn.Linear(4, 4), 0, 1)
+    L._build_engine(fit_args(tmp_path, *topk, "--momentum-correction", "0"), nn.Linear(4, 4), 0, 1)
     assert "momentum_correction" not in seen[-1]
-    L._build_engine(_args(tmp_path, *topk, "--momentum-correction", "1", "--momentum", "0.9"), nn.Linear(4, 4), 0, 1)
+    L._build_engine(fit_args(tmp_path, *topk, "--momentum-correction", "1", "--momentum", "0.9"), nn.Linear(4, 4), 0, 1)
     assert seen[-1]["momentum_correction"] is True and seen[-1]["momentum"] == 0.9
 
 
 def test_fp32_flat_engine_refuses_the_flag(tmp_path):
     for extra in (("--dtype", "fp32"), ("--dtype", "bf16", "--engine", "fused")):
         with pytest.raises(SystemExit, match="--momentum-correction"):
-            L._build_engine(_args(tmp_path, "--code", "svd", "--momentum-correction", "1", *extra), nn.Linear(4, 4),
+            L._build_engine(fit_args(tmp_path, "--code", "svd", "--momentum-correction", "1", *extra), nn.Linear(4, 4),
                             0, 1)
 
 
@@ -87,7 +79,7 @@ def test_gloo_refuses_the_flag(monkeypatch, tmp_path):
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
     with pytest.raises(SystemExit, match="--momentum-correction"):
-        distributed_nn.run_rank(_args(tmp_path, "--code", "svd", "--momentum-correction", "1", "--backend", "gloo"))
+        distributed_nn.run_rank(fit_args(tmp_path, "--code", "svd", "--momentum-correction", "1", "--backend", "gloo"))
 
 
 def _f32(rng, n, scale):

@@ -5,6 +5,7 @@ and ``--code-stats`` (GPU loopback harness); and the engine end to end (GPU).
 The kernels sum in fp32 in a fixed order that differs from the oracle's fp64 products, so factors are compared within
 ``TOL`` of the largest magnitude of the compared array; repeated encodes are compared bit for bit."""
 import argparse
+import functools
 import hashlib
 import json
 import math
@@ -18,6 +19,9 @@ from atomo_b200.codings import powersgd as PS
 from atomo_b200.ops import plan2 as P
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
+
+from shadow_harness import (LoopbackPS, Loopback, ef_grads, fit_args, flat, forbid_cuda, opt_ref, physical, run_mp,
+                            train)
 
 TOL = 2e-4
 NET_SHAPES = [(64, 3, 3, 3), (64,), (64,), (128, 64, 3, 3), (128,), (256, 128, 3, 3), (512, 256, 1, 1), (300, 200),
@@ -201,10 +205,7 @@ def test_plan2_other_codes_unchanged_by_the_new_code():
 @pytest.mark.parametrize("r", [0, 5])
 def test_shadow_engine_powersgd_refuses_before_cuda(r, monkeypatch):
     from atomo_b200.runtime import shadow_engine as S
-
-    def no_cuda(*a, **k):
-        raise AssertionError("refused only after CUDA work started")
-    monkeypatch.setattr(S, "load_ext", no_cuda)
+    forbid_cuda(monkeypatch)
     with pytest.raises(ValueError, match="svd_rank"):
         S.ShadowEngine(None, 0, 1, code="powersgd", svd_rank=r)
     with pytest.raises(ValueError, match="num_aggregate"):     # the error-feedback rule applies unchanged
@@ -212,13 +213,6 @@ def test_shadow_engine_powersgd_refuses_before_cuda(r, monkeypatch):
 
 
 # ---------------------------------------------------------------------------------------------------- CPU: launcher
-def _args(tmp_path, *extra):
-    return add_fit_args(argparse.ArgumentParser(), [
-        "--network", "LeNet", "--dataset", "MNIST", "--synthetic", "1", "--train-len", "512", "--test-len", "128",
-        "--batch-size", "32", "--test-batch-size", "64", "--lr", "0.05", "--log-interval", "1", "--eval-freq", "100",
-        "--train-dir", str(tmp_path) + "/", *extra])
-
-
 def test_launcher_routes_powersgd(tmp_path, monkeypatch):
     from atomo_b200.runtime import shadow_engine as S
     seen = []
@@ -229,7 +223,7 @@ def test_launcher_routes_powersgd(tmp_path, monkeypatch):
     monkeypatch.setattr(S, "ShadowEngine", Fake)
     model = torch.nn.Linear(4, 4)
     for engine in ("auto", "shadow"):
-        _, kind = L._build_engine(_args(tmp_path, "--code", "powersgd", "--dtype", "bf16", "--engine", engine,
+        _, kind = L._build_engine(fit_args(tmp_path, "--code", "powersgd", "--dtype", "bf16", "--engine", engine,
                                         "--svd-rank", "2", "--error-feedback", "1", "--code-stats", "1"),
                                   model, 0, 1)
         assert kind == "shadow" and seen[-1]["code"] == "powersgd" and seen[-1]["svd_rank"] == 2
@@ -238,7 +232,7 @@ def test_launcher_routes_powersgd(tmp_path, monkeypatch):
     for extra in (("--dtype", "fp32", "--svd-rank", "2"), ("--dtype", "bf16", "--engine", "fused", "--svd-rank", "2"),
                   ("--dtype", "bf16"), ("--dtype", "bf16", "--svd-rank", "5")):
         with pytest.raises(SystemExit, match="powersgd"):
-            L._build_engine(_args(tmp_path, "--code", "powersgd", *extra), model, 0, 1)
+            L._build_engine(fit_args(tmp_path, "--code", "powersgd", *extra), model, 0, 1)
     assert len(seen) == n
 
 
@@ -248,138 +242,70 @@ def test_role_paths_refuse_powersgd(monkeypatch, tmp_path):
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
     with pytest.raises(SystemExit, match="p2p bf16 engine"):
-        distributed_nn.run_rank(_args(tmp_path, "--code", "powersgd", "--svd-rank", "2", "--backend", "gloo"))
+        distributed_nn.run_rank(fit_args(tmp_path, "--code", "powersgd", "--svd-rank", "2", "--backend", "gloo"))
     with pytest.raises(ValueError, match="p2p bf16 engine"):
         build_coder({"code": "powersgd", "svd_rank": 2}, worker_side=True)
 
 
 # ---------------------------------------------------------------------------------------------------- GPU harness
-def _ext():
-    from atomo_b200.ops._ext import load
-    return load()
+class HP(LoopbackPS):
+    """PowerSGD, with per-worker warm state and staging copies; owners are virtual too."""
 
-
-class HP:
-    """Loopback harness: one rank that is worker 0..W-1 (virtual) and the only owner."""
+    PS = "v2_ps_powersgd"
 
     def __init__(self, shapes, r=2, W=1, lr=0.1, momentum=0.0, wd=0.0, nesterov=False, opt=0, seed=7,
                  num_aggregate=0, n_owners=1):
-        self.C = _ext()
-        dev = self.dev = torch.device("cuda", 0)
-        self.W, self.r, self.seed, self.n_owners = W, r, seed, n_owners
-        self.plan = pl = P.build_plan2(shapes, "powersgd", r, n_owners=n_owners, n_groups=1)
-        u8 = lambda b: torch.frombuffer(bytearray(b), dtype=torch.uint8).to(dev)
-        self.t_units = u8(pl.units_bytes())
-        self.t_enc = u8(P.Plan2.tiles_bytes(pl.enc_tiles))
-        self.t_pw = u8(P.Plan2.tiles_bytes(pl.pw_tiles))
-        self.t_ps = u8(P.Plan2.tiles_bytes(pl.ps_tiles))
-        nc = self.nc = max(pl.n_coded, 1)
-        z = lambda n, dt=torch.float32: torch.zeros(n, dtype=dt, device=dev)
-        self.counters = z(nc + 32 + 8 * n_owners, torch.int32)
+        super().__init__(shapes, "powersgd", W, lr, momentum, wd, nesterov, opt, seed, num_aggregate,
+                         n_owners=n_owners, stage=True, rank=r)
+        self.r = r
+        pl, z, nc = self.plan, self.zeros, self.nc
+        self.t_pw = torch.frombuffer(bytearray(P.Plan2.tiles_bytes(pl.pw_tiles)), dtype=torch.uint8).to(self.dev)
         self.spart = z(5 * max(len(pl.enc_tiles), 1), torch.float64)
         self.acc = z(7 * nc, torch.float64)
-        # one arena and one signal region per owner (owners are virtual too: one GPU)
-        self.arenas = [z(pl.arena_floats * W) for _ in range(n_owners)]
-        self.sigs = [z(1024, torch.int32) for _ in range(n_owners)]
-        for o in range(n_owners):
-            self.sigs[o][256:256 + n_owners] = 1
-        self.arena, self.signals = self.arenas[0], self.sigs[0]
-        self.ctrl = u8(P.pack_ctrl2(step=1, lr=lr, momentum=momentum, weight_decay=wd, nesterov=nesterov, seed=seed,
-                                    opt=opt, num_aggregate=num_aggregate))
-        # per virtual worker: warm state + factors, Gram partials, unit state, staging copy
+        # per virtual worker: warm state + factors, Gram partials, unit state
         self.scratch = [z(pl.gpart_floats) for _ in range(W)]
         self.gram = [z(P.PW_GRAM * max(len(pl.enc_tiles), 1), torch.float64) for _ in range(W)]
         self.state = [z(nc * self.C.v2_powersgd_state_bytes(), torch.uint8) for _ in range(W)]
-        self.stage = [z(pl.stage_total, torch.bfloat16) for _ in range(W)]
         for w in range(W):
             self.C.v2_powersgd_init(self.t_units.data_ptr(), len(pl.units), self.scratch[w].data_ptr(),
                                     self.ctrl.data_ptr())
-        g = torch.Generator(device="cuda").manual_seed(seed)
-        self.master = torch.randn(pl.w_total, device=dev, generator=g)
-        self.wshadow = self.master.to(torch.bfloat16)
-        self.vparams = torch.randn(pl.v_total, device=dev, generator=g)
-        self.mom, self.vmom = z(pl.w_total), z(pl.v_total)
-        self.sq, self.vsq, self.sqmax, self.vsqmax = z(pl.w_total), z(pl.v_total), z(pl.w_total), z(pl.v_total)
-        self.vgrads = [z(pl.v_total) for _ in range(W)]
-        self.wgrads = [None] * W
-        i64 = lambda xs: torch.tensor(list(xs), dtype=torch.int64, device=dev)
-        self.t_arena_peer = i64([t.data_ptr() for t in self.arenas])
-        self.t_sig_peer = i64([t.data_ptr() for t in self.sigs])
-        self.t_wshadow_peer = i64([self.wshadow.data_ptr()])
-        self.t_vparams_peer = i64([self.vparams.data_ptr()])
-        self.t_vgrads_peer = i64([t.data_ptr() for t in self.vgrads])
-        self.t_stage_peer = i64([t.data_ptr() for t in self.stage])
-        self.tstats = z(32, torch.int64)
         torch.cuda.synchronize()
 
-    def set_step(self, step):
-        self.ctrl.view(torch.int32)[0] = step
+    def tensor(self, q, x, g, special=False):
+        if special and q.index == ZERO:
+            x.zero_()
+        elif special and q.index == RANK1:     # powers of two times bf16 values: exactly rank 1 in bf16
+            u = 2.0 ** torch.randint(-2, 3, (q.shape[0],), device=self.dev, generator=g).float()
+            v = torch.randn(q.numel // q.shape[0], device=self.dev, generator=g).bfloat16().float()
+            x = (u[:, None] * v[None, :])
+            x = x.view(q.shape[0], q.shape[2], q.shape[3], q.shape[1]).permute(0, 3, 1, 2) \
+                if len(q.shape) == 4 else x.view(q.shape)
+        elif special and q.index == INF:
+            x = physical(x)
+            flat(x)[1234] = float("inf")
+        return x
 
     def fill(self, w, seed, special=False):
         """Random bf16 gradients of virtual worker w ({param index: fp32 [O][C] matrix in physical order, or the
         fp32 vector}); with ``special`` the ZERO / RANK1 / INF tensors of ORACLE_SHAPES get their content."""
-        pl, dev = self.plan, self.dev
-        g = torch.Generator(device="cuda").manual_seed(seed)
-        grads, phys = [], {}
-        for q in pl.params:
-            if q.is_w:
-                x = torch.randn(q.shape, device=dev, generator=g)
-                if special and q.index == ZERO:
-                    x.zero_()
-                elif special and q.index == RANK1:     # powers of two times bf16 values: exactly rank 1 in bf16
-                    u = 2.0 ** torch.randint(-2, 3, (q.shape[0],), device=dev, generator=g).float()
-                    v = torch.randn(q.numel // q.shape[0], device=dev, generator=g).bfloat16().float()
-                    x = (u[:, None] * v[None, :])
-                    x = x.view(q.shape[0], q.shape[2], q.shape[3], q.shape[1]).permute(0, 3, 1, 2) \
-                        if len(q.shape) == 4 else x.view(q.shape)
-                x = x.to(torch.bfloat16)
-                t = x.contiguous(memory_format=torch.channels_last) if x.dim() == 4 else x.contiguous()
-                if special and q.index == INF:
-                    (t.permute(0, 2, 3, 1) if t.dim() == 4 else t).view(-1)[1234] = float("inf")
-                grads.append(t)
-                phys[q.index] = (t.permute(0, 2, 3, 1) if t.dim() == 4 else t).reshape(q.shape[0], -1).float()
-            else:
-                v = torch.randn(q.numel, device=dev, generator=g)
-                self.vgrads[w][q.off:q.off + q.numel] = v
-                phys[q.index] = v
-        self.wgrads[w] = grads
-        return phys
+        phys = super().fill(w, seed, special=special)
+        return {i: v.reshape(self.plan.params[i].shape[0], -1) if self.plan.params[i].is_w else v
+                for i, v in phys.items()}
 
     def encode(self, w, residual=0, stats=False):
         C, pl = self.C, self.plan
-        gptr = torch.tensor([t.data_ptr() for t in self.wgrads[w]], dtype=torch.int64, device=self.dev)
-        self._gptr = gptr
+        gptr = self.gptr(w)
         t0, nt = pl.enc_range[0]
         p0, npw = pl.pw_range[0]
         C.v2_powersgd_encode(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, self.t_pw.data_ptr(), p0, npw,
-                             gptr.data_ptr(), self.scratch[w].data_ptr(), self.gram[w].data_ptr(),
+                             gptr, self.scratch[w].data_ptr(), self.gram[w].data_ptr(),
                              self.state[w].data_ptr(), self.stage[w].data_ptr(), self.t_arena_peer.data_ptr(),
                              self.t_sig_peer.data_ptr(), self.n_owners, pl.arena_floats, w, 0, self.ctrl.data_ptr(),
-                             self.counters.data_ptr() + 4 * (self.nc + 8), 0, False, residual)
+                             self.counter(), 0, False, residual)
         if stats:
-            C.v2_powersgd_code_stats(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr.data_ptr(),
+            C.v2_powersgd_code_stats(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr,
                                      self.scratch[w].data_ptr(), self.state[w].data_ptr(), self.spart.data_ptr(),
                                      self.counters.data_ptr(), self.acc.data_ptr())
-        torch.cuda.synchronize()
-
-    def ps(self, grid=64):
-        for o in range(self.n_owners):
-            self.ps_owner(o, grid)
-
-    def ps_owner(self, o, grid=64):
-        """The PS launch of owner o: its tiles, its arena and its signal region."""
-        C, pl = self.C, self.plan
-        t0, nt = pl.ps_range[0][o]
-        sig = torch.tensor([self.sigs[o].data_ptr()], dtype=torch.int64, device=self.dev)
-        self._sig = sig
-        C.v2_ps_powersgd(self.t_units.data_ptr(), self.t_ps.data_ptr(), t0, nt, self.W, 1, 0, True, o,
-                         self.master.data_ptr(), self.mom.data_ptr(), self.sq.data_ptr(), self.sqmax.data_ptr(),
-                         self.vmom.data_ptr(), self.vsq.data_ptr(), self.vsqmax.data_ptr(), 0,
-                         self.t_wshadow_peer.data_ptr(), self.vparams.data_ptr(), 0, self.t_vparams_peer.data_ptr(), 0,
-                         self.t_vgrads_peer.data_ptr(), self.t_stage_peer.data_ptr(), self.arenas[o].data_ptr(),
-                         pl.arena_floats, self.sigs[o].data_ptr(), sig.data_ptr(), self.ctrl.data_ptr(),
-                         self.counters.data_ptr() + 4 * (self.nc + 16 + 8 * o), int(5e9), self.tstats.data_ptr(),
-                         1.0 / self.W, grid)
         torch.cuda.synchronize()
 
     def slot(self, u, w, owner=None):
@@ -400,13 +326,6 @@ class HP:
     def draw(self, u, w):
         st = self.state[w].view(-1, self.C.v2_powersgd_state_bytes())[u.ts_index]
         return int(st[128:].view(torch.int32)[2])
-
-    def used(self):
-        mw = torch.zeros(self.plan.w_total, dtype=torch.bool, device=self.dev)
-        mv = torch.zeros(self.plan.v_total, dtype=torch.bool, device=self.dev)
-        for q in self.plan.params:
-            (mw if q.is_w else mv)[q.off:q.off + q.numel] = True
-        return mw, mv
 
 
 def _close(a, b, what):
@@ -518,7 +437,6 @@ def test_v2_ps_powersgd_mean_matches_the_oracle(W, r):
 @pytest.mark.parametrize("momentum,nesterov,wd,opt", [(0.0, False, 0.0, 0), (0.9, True, 1e-3, 0), (0.0, False, 0.0, 1),
                                                       (0.0, False, 1e-3, 2)])
 def test_v2_ps_powersgd_optimizer_epilogues(momentum, nesterov, wd, opt):
-    from test_gpu_shadow_qsgd import _opt_ref
     W, lr = 2, 0.05
     h = HP(NET_SHAPES, 2, W=W, lr=lr, momentum=momentum, wd=wd, nesterov=nesterov, opt=opt)
     used, vused = h.used()
@@ -531,9 +449,9 @@ def test_v2_ps_powersgd_optimizer_epilogues(momentum, nesterov, wd, opt):
             h.encode(w)
         gw = (_oracle_sum(h, phys, qws) / W).float().to(h.dev)
         gv = sum(h.vgrads) / W
-        rp, _ = _opt_ref(h.master.clone(), gw, h.mom.clone(), h.sq.clone(), h.sqmax.clone(), step, lr, momentum,
+        rp, _ = opt_ref(h.master.clone(), gw, h.mom.clone(), h.sq.clone(), h.sqmax.clone(), step, lr, momentum,
                          nesterov, wd, opt)
-        rv, _ = _opt_ref(h.vparams.clone(), gv, h.vmom.clone(), h.vsq.clone(), h.vsqmax.clone(), step, lr, momentum,
+        rv, _ = opt_ref(h.vparams.clone(), gv, h.vmom.clone(), h.vsq.clone(), h.vsqmax.clone(), step, lr, momentum,
                          nesterov, wd, opt)
         h.ps()
         assert int(h.ctrl.view(torch.int32)[1]) == 0
@@ -638,17 +556,10 @@ def test_v2_powersgd_code_stats_match_fp64(r):
 
 
 # ---------------------------------------------------------------------------------------------------- GPU: feedback
-def _grads(seed=0):
-    from test_gpu_error_feedback import SHAPES
-    g = torch.Generator().manual_seed(seed)
-    return [(torch.randn(s, generator=g) * (0.01 * (1 + i))).bfloat16().float().cuda() for i, s in enumerate(SHAPES)]
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("r", [1, 2, 4])
 def test_error_feedback_identity_and_contraction(r):
-    from test_gpu_error_feedback import Loopback
-    h = Loopback("powersgd", _grads(1), svd_rank=r)
+    h = Loopback("powersgd", ef_grads(1), svd_rank=r)
     try:
         g, e_old = h.g, h.residual()
         for _ in range(4):
@@ -669,8 +580,7 @@ def test_error_feedback_identity_and_contraction(r):
 def test_error_feedback_residual_stays_bounded():
     """A fixed gradient for 200 steps: every step contracts (||e_{t+1}|| <= rho ||g + e_t||, rho < 1), so ||e|| stays
     below rho / (1 - rho) ||g||; the pushed sum misses 200 g by exactly the final residual."""
-    from test_gpu_error_feedback import Loopback
-    h = Loopback("powersgd", _grads(2), svd_rank=2)
+    h = Loopback("powersgd", ef_grads(2), svd_rank=2)
     try:
         s = torch.zeros_like(h.g)
         e = h.residual()
@@ -690,8 +600,7 @@ def test_error_feedback_residual_stays_bounded():
 
 @pytest.mark.gpu
 def test_code_stats_bytes_follow_the_plan():
-    from test_gpu_error_feedback import Loopback
-    h = Loopback("powersgd", _grads(4), svd_rank=2, code_stats=True)
+    h = Loopback("powersgd", ef_grads(4), svd_rank=2, code_stats=True)
     try:
         h.step()
         st = h.eng.code_stats()
@@ -709,26 +618,7 @@ def test_code_stats_bytes_follow_the_plan():
 
 
 # ---------------------------------------------------------------------------------------------------- GPU: engine
-def _train(net, graph, ef, steps=6, r=2, lr=0.05, seed=3):
-    from atomo_b200.data import SyntheticImageDataset
-    from atomo_b200.models import build_model, input_shape
-    from atomo_b200.runtime.shadow_engine import ShadowEngine
-    torch.manual_seed(0)
-    torch.cuda.set_device(0)
-    x, y = SyntheticImageDataset(input_shape(net), 10, 4096, seed=0).materialize(32)
-    eng = ShadowEngine(build_model(net, 10), 0, 1, code="powersgd", svd_rank=r, lr=lr, momentum=0.9,
-                       use_graph=graph, overlap=graph, seed=seed, error_feedback=ef)
-    eng.prepare(x.pin_memory(), y.pin_memory(), warmup=2)
-    losses, norms = [], []
-    for _ in range(steps):
-        losses.append(float(eng.train_step(x, y)[0]))
-        if ef:
-            norms.append(eng.error_feedback_norm()["model"])
-    torch.cuda.synchronize()
-    assert eng.error_code() == 0
-    m = eng.gather_fp32("master").clone()
-    eng.close()
-    return m, losses, norms
+_train = functools.partial(train, code="powersgd", svd_rank=2)
 
 
 @pytest.mark.gpu
@@ -806,8 +696,7 @@ def test_shadow_engine_powersgd_multi_gpu_replicas_identical():
     n = torch.cuda.device_count()
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
-    from test_gpu_v2 import _run_mp
     world = 2 if n < 8 else (8 if os.environ.get("ATOMO_TEST_WORLD8") else 2)
-    res = _run_mp(world, {"code": "powersgd", "ps_mode": "sharded", "net": "VGG11"}, 29812)
+    res = run_mp(world, {"code": "powersgd", "ps_mode": "sharded", "net": "VGG11"}, 29812)
     for rank, err, same, l0, l1, mode, mc, _ in res:
         assert err == 0 and same, res

@@ -10,6 +10,8 @@ import torch
 
 from atomo_b200.ops import plan2 as P
 
+from shadow_harness import LoopbackPS, batch, opt_ref, run_mp
+
 NET_SHAPES = [(64, 3, 3, 3), (64,), (64,), (128, 64, 3, 3), (128,), (256, 128, 3, 3), (512, 256, 1, 1), (300, 200),
               (10, 512), (10,)]
 ORACLE_SHAPES = [(64, 3, 3, 3), (64, 32, 3, 3), (10, 512), (300, 200), (7, 20), (5, 300), (64,)]
@@ -152,99 +154,39 @@ def test_p2p_launcher_engine_shadow_refuses_entrywise_and_fp32(monkeypatch):
 
 
 # ---------------------------------------------------------------------------------------------------- GPU harness
-def _ext():
-    from atomo_b200.ops._ext import load
-    return load()
+class HQ(LoopbackPS):
+    """QSGD / TernGrad; ``fill`` scales the gradients by ``scale``."""
 
-
-class HQ:
-    """Loopback harness: one rank that is worker 0..W-1 (virtual) and the only owner."""
+    PS = "v2_ps_qsgd"
 
     def __init__(self, shapes, code="qsgd", q=4, bucket=512, W=1, lr=0.1, momentum=0.0, wd=0.0, nesterov=False,
                  opt=0, seed=7, num_aggregate=0):
-        self.C = _ext()
-        dev = self.dev = torch.device("cuda", 0)
-        self.W, self.code = W, code
-        self.plan = pl = P.build_plan2(shapes, code, n_owners=1, n_groups=1, quantization_level=q, bucket_size=bucket)
-        u8 = lambda b: torch.frombuffer(bytearray(b), dtype=torch.uint8).to(dev)
-        self.t_units = u8(pl.units_bytes())
-        self.t_enc = u8(P.Plan2.tiles_bytes(pl.enc_tiles))
-        self.t_ps = u8(P.Plan2.tiles_bytes(pl.ps_tiles))
-        nc = max(pl.n_coded, 1)
-        z = lambda n, dt=torch.float32: torch.zeros(n, dtype=dt, device=dev)
-        self.clip = z(nc)
-        self.partials = z(2 * len(pl.enc_tiles), torch.float64)
-        self.counters = z(nc + 32, torch.int32)
-        self.arena = z(pl.arena_floats * W)
-        self.signals = z(1024, torch.int32)
-        self.signals[256] = 1
-        self.ctrl = u8(P.pack_ctrl2(step=1, lr=lr, momentum=momentum, weight_decay=wd, nesterov=nesterov, seed=seed,
-                                    opt=opt, num_aggregate=num_aggregate))
-        g = torch.Generator(device="cuda").manual_seed(seed)
-        self.master = torch.randn(pl.w_total, device=dev, generator=g)
-        self.wshadow = self.master.to(torch.bfloat16)
-        self.vparams = torch.randn(pl.v_total, device=dev, generator=g)
-        self.mom, self.vmom = z(pl.w_total), z(pl.v_total)
-        self.sq, self.vsq, self.sqmax, self.vsqmax = z(pl.w_total), z(pl.v_total), z(pl.w_total), z(pl.v_total)
-        self.vgrads = [z(pl.v_total) for _ in range(W)]
-        self.wgrads = [None] * W
-        i64 = lambda xs: torch.tensor(list(xs), dtype=torch.int64, device=dev)
-        self.t_arena_peer = i64([self.arena.data_ptr()])
-        self.t_sig_peer = i64([self.signals.data_ptr()])
-        self.t_wshadow_peer = i64([self.wshadow.data_ptr()])
-        self.t_vparams_peer = i64([self.vparams.data_ptr()])
-        self.t_vgrads_peer = i64([t.data_ptr() for t in self.vgrads])
-        self.tstats = z(32, torch.int64)
+        super().__init__(shapes, code, W, lr, momentum, wd, nesterov, opt, seed, num_aggregate, quantization_level=q,
+                         bucket_size=bucket)
+        self.code = code
+        pl = self.plan
+        self.clip = self.zeros(self.nc)
+        self.partials = self.zeros(2 * len(pl.enc_tiles), torch.float64)
         self.maxq = max(u.I for u in pl.units if u.kind == P.KIND_QSGD)
         self.maxb = max(u.K for u in pl.units if u.kind == P.KIND_QSGD)
+        self.ps_tail = (self.maxq, self.maxb)
 
-    def set_step(self, step):
-        self.ctrl.view(torch.int32)[0] = step
-
-    def fill(self, w, seed, scale=1.0):
-        """Random bf16 gradients of virtual worker w; returns {param index: fp32 physical-order flat tensor}."""
-        pl, dev = self.plan, self.dev
-        g = torch.Generator(device="cuda").manual_seed(seed)
-        grads, phys = [], {}
-        for q in pl.params:
-            if q.is_w:
-                x = (torch.randn(q.shape, device=dev, generator=g) * scale).to(torch.bfloat16)
-                t = x.contiguous(memory_format=torch.channels_last) if x.dim() == 4 else x.contiguous()
-                grads.append(t)
-                phys[q.index] = (t.permute(0, 2, 3, 1) if t.dim() == 4 else t).reshape(-1).float()
-            else:
-                v = torch.randn(q.numel, device=dev, generator=g)
-                self.vgrads[w][q.off:q.off + q.numel] = v
-                phys[q.index] = v
-        self.wgrads[w] = grads
-        return phys
+    def tensor(self, q, x, g, scale=1.0):
+        return x * scale
 
     def encode(self, w, uniforms=None):
         C, pl = self.C, self.plan
-        gptr = torch.tensor([t.data_ptr() for t in self.wgrads[w]], dtype=torch.int64, device=self.dev)
-        self._gptr = gptr
+        gptr = self.gptr(w)
         t0, nt = pl.enc_range[0]
         tern = self.code == "terngrad"
         if tern:
-            C.v2_qsgd_stats(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr.data_ptr(),
-                            self.partials.data_ptr(), self.counters.data_ptr(), self.clip.data_ptr(), 0, 0)
-        C.v2_qsgd_encode(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr.data_ptr(),
+            C.v2_qsgd_stats(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr, self.partials.data_ptr(),
+                            self.counters.data_ptr(), self.clip.data_ptr(), 0, 0)
+        C.v2_qsgd_encode(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr,
                          self.clip.data_ptr() if tern else 0, self.t_arena_peer.data_ptr(), self.t_sig_peer.data_ptr(),
-                         1, pl.arena_floats, w, 0, self.ctrl.data_ptr(),
-                         self.counters.data_ptr() + 4 * (pl.n_coded + 8), uniforms.data_ptr() if uniforms is not None
-                         else 0, 0, False, not tern, self.maxq, self.maxb, tern)
-        torch.cuda.synchronize()
-
-    def ps(self, grid=64):
-        C, pl = self.C, self.plan
-        t0, nt = pl.ps_range[0][0]
-        C.v2_ps_qsgd(self.t_units.data_ptr(), self.t_ps.data_ptr(), t0, nt, self.W, 1, 0, True, 0,
-                     self.master.data_ptr(), self.mom.data_ptr(), self.sq.data_ptr(), self.sqmax.data_ptr(),
-                     self.vmom.data_ptr(), self.vsq.data_ptr(), self.vsqmax.data_ptr(), 0,
-                     self.t_wshadow_peer.data_ptr(), self.vparams.data_ptr(), 0, self.t_vparams_peer.data_ptr(), 0,
-                     self.t_vgrads_peer.data_ptr(), self.arena.data_ptr(), pl.arena_floats, self.signals.data_ptr(),
-                     self.t_sig_peer.data_ptr(), self.ctrl.data_ptr(), self.counters.data_ptr() + 4 * (pl.n_coded + 16),
-                     int(5e9), self.tstats.data_ptr(), 1.0 / self.W, grid, self.maxq, self.maxb)
+                         1, pl.arena_floats, w, 0, self.ctrl.data_ptr(), self.counter(),
+                         uniforms.data_ptr() if uniforms is not None else 0, 0, False, not tern, self.maxq, self.maxb,
+                         tern)
         torch.cuda.synchronize()
 
     def slot(self, u, w):
@@ -329,23 +271,6 @@ def test_v2_qsgd_philox_rounding_is_unbiased(code):
 
 
 # ---------------------------------------------------------------------------------------------------- GPU: PS
-def _opt_ref(p, g, m, s2, s2m, step, lr, momentum, nesterov, wd, opt):
-    g = g + wd * p
-    if opt == 0:
-        if momentum:
-            m = g.clone() if step == 1 else momentum * m + g
-            d = g + momentum * m if nesterov else m
-        else:
-            d = g
-        return p - lr * d, m
-    b1, b2, eps = 0.9, 0.999, 1e-8
-    m = b1 * m + (1 - b1) * g
-    s2 = b2 * s2 + (1 - b2) * g * g
-    vv = torch.maximum(s2m, s2) if opt == 2 else s2
-    denom = vv.sqrt() / (1 - b2 ** step) ** 0.5 + eps
-    return p - lr / (1 - b1 ** step) * m / denom, m
-
-
 def _decoded_sum(h, workers, coder):
     """sum over `workers` (in worker order, fp32) of the codings.qsgd decodes of the words actually in the arena,
     physical order.  Decoded on the CPU: there ``norms / s`` is an IEEE division, as in the PS kernel (on CUDA, torch
@@ -411,9 +336,9 @@ def test_v2_ps_qsgd_matches_reference(code, momentum, nesterov, wd, opt):
             h.encode(w)
         gw = _decoded_sum(h, range(W), coder) / W
         gv = sum(h.vgrads) / W
-        rp, rm = _opt_ref(h.master.clone(), gw, h.mom.clone(), h.sq.clone(), h.sqmax.clone(), step, lr, momentum,
+        rp, rm = opt_ref(h.master.clone(), gw, h.mom.clone(), h.sq.clone(), h.sqmax.clone(), step, lr, momentum,
                           nesterov, wd, opt)
-        rv, _ = _opt_ref(h.vparams.clone(), gv, h.vmom.clone(), h.vsq.clone(), h.vsqmax.clone(), step, lr, momentum,
+        rv, _ = opt_ref(h.vparams.clone(), gv, h.vmom.clone(), h.vsq.clone(), h.vsqmax.clone(), step, lr, momentum,
                          nesterov, wd, opt)
         h.ps()
         assert int(h.ctrl.view(torch.int32)[1]) == 0
@@ -461,13 +386,6 @@ def test_v2_ps_qsgd_num_aggregate_and_stale_slots(code):
 
 
 # ---------------------------------------------------------------------------------------------------- GPU: engine
-def _batch(net, n=32, seed=0):
-    from atomo_b200.data import SyntheticImageDataset
-    from atomo_b200.models import input_shape
-    x, y = SyntheticImageDataset(input_shape(net), 10, 4096, seed=seed).materialize(n)
-    return x.pin_memory(), y.pin_memory()
-
-
 def _engine(net, code, graph, overlap, seed=3):
     from atomo_b200.models import build_model
     from atomo_b200.runtime.shadow_engine import ShadowEngine
@@ -484,7 +402,7 @@ def _engine(net, code, graph, overlap, seed=3):
 def test_shadow_engine_qsgd_trains_single_gpu(net, code, graph, overlap, tmp_path, monkeypatch):
     monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)      # bitwise-reproducible backward
     monkeypatch.setattr(torch.backends.cudnn, "benchmark", False)
-    x, y = _batch(net, 64)
+    x, y = batch(net, 64)
     masters = []
     for rep in range(2):
         eng = _engine(net, code, graph, overlap)
@@ -535,10 +453,9 @@ def test_shadow_engine_qsgd_multi_gpu_replicas_identical(code, ps_mode):
     n = torch.cuda.device_count()
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
-    from test_gpu_v2 import _run_mp
     world = 2 if n < 8 else (8 if os.environ.get("ATOMO_TEST_WORLD8") else 2)
     port = 29600 + 7 * ["sharded", "colocated"].index(ps_mode) + (3 if code == "terngrad" else 0)
-    res = _run_mp(world, {"code": code, "ps_mode": ps_mode, "net": "VGG11"}, port)
+    res = run_mp(world, {"code": code, "ps_mode": ps_mode, "net": "VGG11"}, port)
     for rank, err, same, l0, l1, mode, mc, _ in res:
         assert err == 0 and same, res
     assert all(r[4] < r[3] for r in res), res
@@ -550,9 +467,8 @@ def test_shadow_engine_qsgd_protocol_survives_random_delays():
     n = torch.cuda.device_count()
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
-    from test_gpu_v2 import _run_mp
     world = 2 if n < 8 else (8 if os.environ.get("ATOMO_TEST_WORLD8") else 2)
-    res = _run_mp(world, {"code": "qsgd", "ps_mode": "sharded", "graph": False, "steps": 8, "warmup": 0,
+    res = run_mp(world, {"code": "qsgd", "ps_mode": "sharded", "graph": False, "steps": 8, "warmup": 0,
                           "jitter_us": 300.0}, 29650)
     for r in res:
         assert r[1] == 0 and r[2], res

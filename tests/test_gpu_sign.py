@@ -2,6 +2,7 @@
 refusals and the launcher routing (CPU); the encode against the oracle bit for bit, the PS, error feedback and
 ``--code-stats`` (GPU loopback harness); and the engine end to end (GPU)."""
 import argparse
+import functools
 import hashlib
 import json
 import math
@@ -14,6 +15,9 @@ import torch
 from atomo_b200.ops import plan2 as P
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
+
+from shadow_harness import (LoopbackPS, Loopback, ef_grads, fit_args, flat, forbid_cuda, opt_ref, physical, run_mp,
+                            train)
 
 NET_SHAPES = [(64, 3, 3, 3), (64,), (64,), (128, 64, 3, 3), (128,), (256, 128, 3, 3), (512, 256, 1, 1), (300, 200),
               (10, 512), (7, 20), (10,)]
@@ -163,10 +167,7 @@ def test_plan2_other_codes_unchanged_by_the_new_code():
 @pytest.mark.parametrize("bucket", [0, 32, 100, 4160])
 def test_shadow_engine_sign_refuses_before_cuda(bucket, monkeypatch):
     from atomo_b200.runtime import shadow_engine as S
-
-    def no_cuda(*a, **k):
-        raise AssertionError("refused only after CUDA work started")
-    monkeypatch.setattr(S, "load_ext", no_cuda)
+    forbid_cuda(monkeypatch)
     with pytest.raises(ValueError, match="multiple of 64"):
         S.ShadowEngine(None, 0, 1, code="sign", bucket_size=bucket)
     with pytest.raises(ValueError, match="num_aggregate"):     # the error-feedback rule applies unchanged
@@ -174,13 +175,6 @@ def test_shadow_engine_sign_refuses_before_cuda(bucket, monkeypatch):
 
 
 # ---------------------------------------------------------------------------------------------------- CPU: launcher
-def _args(tmp_path, *extra):
-    return add_fit_args(argparse.ArgumentParser(), [
-        "--network", "LeNet", "--dataset", "MNIST", "--synthetic", "1", "--train-len", "512", "--test-len", "128",
-        "--batch-size", "32", "--test-batch-size", "64", "--lr", "0.05", "--log-interval", "1", "--eval-freq", "100",
-        "--train-dir", str(tmp_path) + "/", *extra])
-
-
 def test_launcher_routes_sign(tmp_path, monkeypatch):
     from atomo_b200.runtime import shadow_engine as S
     seen = []
@@ -191,7 +185,7 @@ def test_launcher_routes_sign(tmp_path, monkeypatch):
     monkeypatch.setattr(S, "ShadowEngine", Fake)
     model = torch.nn.Linear(4, 4)
     for engine in ("auto", "shadow"):
-        _, kind = L._build_engine(_args(tmp_path, "--code", "sign", "--dtype", "bf16", "--engine", engine,
+        _, kind = L._build_engine(fit_args(tmp_path, "--code", "sign", "--dtype", "bf16", "--engine", engine,
                                         "--bucket-size", "256", "--error-feedback", "1", "--code-stats", "1"),
                                   model, 0, 1)
         assert kind == "shadow" and seen[-1]["code"] == "sign" and seen[-1]["bucket_size"] == 256
@@ -199,7 +193,7 @@ def test_launcher_routes_sign(tmp_path, monkeypatch):
     n = len(seen)
     for extra in (("--dtype", "fp32"), ("--dtype", "bf16", "--engine", "fused")):
         with pytest.raises(SystemExit, match="sign"):
-            L._build_engine(_args(tmp_path, "--code", "sign", *extra), model, 0, 1)
+            L._build_engine(fit_args(tmp_path, "--code", "sign", *extra), model, 0, 1)
     assert len(seen) == n
 
 
@@ -209,110 +203,47 @@ def test_role_paths_refuse_sign(monkeypatch, tmp_path):
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
     with pytest.raises(SystemExit, match="p2p bf16 engine"):
-        distributed_nn.run_rank(_args(tmp_path, "--code", "sign", "--backend", "gloo"))
+        distributed_nn.run_rank(fit_args(tmp_path, "--code", "sign", "--backend", "gloo"))
     with pytest.raises(ValueError, match="p2p bf16 engine"):
         build_coder({"code": "sign", "bucket_size": 512}, worker_side=True)
 
 
 # ---------------------------------------------------------------------------------------------------- GPU harness
-def _ext():
-    from atomo_b200.ops._ext import load
-    return load()
+class HS(LoopbackPS):
+    """Scaled sign; with ``special``, ``fill`` gives the ZERO / SIGNED_ZERO / INF tensors of ORACLE_SHAPES their
+    content."""
 
-
-class HS:
-    """Loopback harness (the QSGD tests' style): one rank that is worker 0..W-1 (virtual) and the only owner."""
+    PS = "v2_ps_sign"
 
     def __init__(self, shapes, bucket=512, W=1, lr=0.1, momentum=0.0, wd=0.0, nesterov=False, opt=0, seed=7,
                  num_aggregate=0):
-        self.C = _ext()
-        dev = self.dev = torch.device("cuda", 0)
-        self.W, self.bucket = W, bucket
-        self.plan = pl = P.build_plan2(shapes, "sign", n_owners=1, n_groups=1, bucket_size=bucket)
-        u8 = lambda b: torch.frombuffer(bytearray(b), dtype=torch.uint8).to(dev)
-        self.t_units = u8(pl.units_bytes())
-        self.t_enc = u8(P.Plan2.tiles_bytes(pl.enc_tiles))
-        self.t_ps = u8(P.Plan2.tiles_bytes(pl.ps_tiles))
-        nc = self.nc = max(pl.n_coded, 1)
-        z = lambda n, dt=torch.float32: torch.zeros(n, dtype=dt, device=dev)
-        self.counters = z(nc + 32, torch.int32)
-        self.spart = z(5 * max(len(pl.enc_tiles), 1), torch.float64)
-        self.acc = z(7 * nc, torch.float64)
-        self.arena = z(pl.arena_floats * W)
-        self.signals = z(1024, torch.int32)
-        self.signals[256] = 1
-        self.ctrl = u8(P.pack_ctrl2(step=1, lr=lr, momentum=momentum, weight_decay=wd, nesterov=nesterov, seed=seed,
-                                    opt=opt, num_aggregate=num_aggregate))
-        g = torch.Generator(device="cuda").manual_seed(seed)
-        self.master = torch.randn(pl.w_total, device=dev, generator=g)
-        self.wshadow = self.master.to(torch.bfloat16)
-        self.vparams = torch.randn(pl.v_total, device=dev, generator=g)
-        self.mom, self.vmom = z(pl.w_total), z(pl.v_total)
-        self.sq, self.vsq, self.sqmax, self.vsqmax = z(pl.w_total), z(pl.v_total), z(pl.w_total), z(pl.v_total)
-        self.vgrads = [z(pl.v_total) for _ in range(W)]
-        self.wgrads = [None] * W
-        i64 = lambda xs: torch.tensor(list(xs), dtype=torch.int64, device=dev)
-        self.t_arena_peer = i64([self.arena.data_ptr()])
-        self.t_sig_peer = i64([self.signals.data_ptr()])
-        self.t_wshadow_peer = i64([self.wshadow.data_ptr()])
-        self.t_vparams_peer = i64([self.vparams.data_ptr()])
-        self.t_vgrads_peer = i64([t.data_ptr() for t in self.vgrads])
-        self.tstats = z(32, torch.int64)
+        super().__init__(shapes, "sign", W, lr, momentum, wd, nesterov, opt, seed, num_aggregate, bucket_size=bucket)
+        self.bucket = bucket
+        self.spart = self.zeros(5 * max(len(self.plan.enc_tiles), 1), torch.float64)
+        self.acc = self.zeros(7 * self.nc, torch.float64)
 
-    def set_step(self, step):
-        self.ctrl.view(torch.int32)[0] = step
-
-    def fill(self, w, seed, special=False):
-        """Random bf16 gradients of virtual worker w ({param index: fp32 physical-order flat tensor}); with
-        ``special`` the ZERO / SIGNED_ZERO / INF tensors of ORACLE_SHAPES get their content."""
-        pl, dev = self.plan, self.dev
-        g = torch.Generator(device="cuda").manual_seed(seed)
-        grads, phys = [], {}
-        for q in pl.params:
-            if q.is_w:
-                x = torch.randn(q.shape, device=dev, generator=g)
-                if special and q.index == ZERO:
-                    x.zero_()
-                elif special and q.index == SIGNED_ZERO:
-                    r = torch.rand(q.shape, device=dev, generator=g)
-                    x = torch.where(r < 0.3, torch.zeros_like(x), torch.where(r < 0.6, -torch.zeros_like(x), x))
-                x = x.to(torch.bfloat16)
-                t = x.contiguous(memory_format=torch.channels_last) if x.dim() == 4 else x.contiguous()
-                if special and q.index == INF:
-                    (t.permute(0, 2, 3, 1) if t.dim() == 4 else t).view(-1)[1234] = float("inf")
-                grads.append(t)
-                phys[q.index] = (t.permute(0, 2, 3, 1) if t.dim() == 4 else t).reshape(-1).float()
-            else:
-                v = torch.randn(q.numel, device=dev, generator=g)
-                self.vgrads[w][q.off:q.off + q.numel] = v
-                phys[q.index] = v
-        self.wgrads[w] = grads
-        return phys
+    def tensor(self, q, x, g, special=False):
+        if special and q.index == ZERO:
+            x.zero_()
+        elif special and q.index == SIGNED_ZERO:
+            r = torch.rand(q.shape, device=self.dev, generator=g)
+            x = torch.where(r < 0.3, torch.zeros_like(x), torch.where(r < 0.6, -torch.zeros_like(x), x))
+        if special and q.index == INF:
+            x = physical(x)
+            flat(x)[1234] = float("inf")
+        return x
 
     def encode(self, w, residual=0, stats=False):
         C, pl = self.C, self.plan
-        gptr = torch.tensor([t.data_ptr() for t in self.wgrads[w]], dtype=torch.int64, device=self.dev)
-        self._gptr = gptr
+        gptr = self.gptr(w)
         t0, nt = pl.enc_range[0]
-        C.v2_sign_encode(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr.data_ptr(),
+        C.v2_sign_encode(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr,
                          self.t_arena_peer.data_ptr(), self.t_sig_peer.data_ptr(), 1, pl.arena_floats, w, 0,
-                         self.ctrl.data_ptr(), self.counters.data_ptr() + 4 * (self.nc + 8), 0, False, residual)
+                         self.ctrl.data_ptr(), self.counter(), 0, False, residual)
         if stats:
-            C.v2_sign_code_stats(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr.data_ptr(),
+            C.v2_sign_code_stats(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr,
                                  self.t_arena_peer.data_ptr(), 1, pl.arena_floats, w, self.spart.data_ptr(),
                                  self.counters.data_ptr(), self.acc.data_ptr())
-        torch.cuda.synchronize()
-
-    def ps(self, grid=64):
-        C, pl = self.C, self.plan
-        t0, nt = pl.ps_range[0][0]
-        C.v2_ps_sign(self.t_units.data_ptr(), self.t_ps.data_ptr(), t0, nt, self.W, 1, 0, True, 0,
-                     self.master.data_ptr(), self.mom.data_ptr(), self.sq.data_ptr(), self.sqmax.data_ptr(),
-                     self.vmom.data_ptr(), self.vsq.data_ptr(), self.vsqmax.data_ptr(), 0,
-                     self.t_wshadow_peer.data_ptr(), self.vparams.data_ptr(), 0, self.t_vparams_peer.data_ptr(), 0,
-                     self.t_vgrads_peer.data_ptr(), self.arena.data_ptr(), pl.arena_floats, self.signals.data_ptr(),
-                     self.t_sig_peer.data_ptr(), self.ctrl.data_ptr(), self.counters.data_ptr() + 4 * (self.nc + 16),
-                     int(5e9), self.tstats.data_ptr(), 1.0 / self.W, grid)
         torch.cuda.synchronize()
 
     def slot(self, u, w):
@@ -323,13 +254,6 @@ class HS:
         scales = base[so:so + u.rows].clone()
         words = base[wo:wo + 2 * u.rows * u.cols].view(torch.int64).view(u.rows, u.cols).clone()
         return stamps, scales, words
-
-    def used(self):
-        mw = torch.zeros(self.plan.w_total, dtype=torch.bool, device=self.dev)
-        mv = torch.zeros(self.plan.v_total, dtype=torch.bool, device=self.dev)
-        for q in self.plan.params:
-            (mw if q.is_w else mv)[q.off:q.off + q.numel] = True
-        return mw, mv
 
 
 def _decoded_sum(h, phys_by_worker):
@@ -394,7 +318,6 @@ def test_v2_ps_sign_decoded_mean_is_bitwise_the_oracles(W, bucket):
 @pytest.mark.parametrize("momentum,nesterov,wd,opt", [(0.0, False, 0.0, 0), (0.9, True, 1e-3, 0), (0.9, False, 0.0, 0),
                                                       (0.0, False, 0.0, 1), (0.0, False, 1e-3, 2)])
 def test_v2_ps_sign_matches_reference(momentum, nesterov, wd, opt):
-    from test_gpu_shadow_qsgd import _opt_ref
     W, lr = 3, 0.05
     h = HS(NET_SHAPES, 512, W=W, lr=lr, momentum=momentum, wd=wd, nesterov=nesterov, opt=opt)
     used, vused = h.used()
@@ -406,9 +329,9 @@ def test_v2_ps_sign_matches_reference(momentum, nesterov, wd, opt):
             h.encode(w)
         gw = _decoded_sum(h, phys).to(h.dev) / W
         gv = sum(h.vgrads) / W
-        rp, _ = _opt_ref(h.master.clone(), gw, h.mom.clone(), h.sq.clone(), h.sqmax.clone(), step, lr, momentum,
+        rp, _ = opt_ref(h.master.clone(), gw, h.mom.clone(), h.sq.clone(), h.sqmax.clone(), step, lr, momentum,
                          nesterov, wd, opt)
-        rv, _ = _opt_ref(h.vparams.clone(), gv, h.vmom.clone(), h.vsq.clone(), h.vsqmax.clone(), step, lr, momentum,
+        rv, _ = opt_ref(h.vparams.clone(), gv, h.vmom.clone(), h.vsq.clone(), h.vsqmax.clone(), step, lr, momentum,
                          nesterov, wd, opt)
         h.ps()
         assert int(h.ctrl.view(torch.int32)[1]) == 0
@@ -471,17 +394,10 @@ def test_v2_sign_code_stats_match_fp64(bucket):
 
 
 # ---------------------------------------------------------------------------------------------------- GPU: feedback
-def _grads(seed=0):
-    from test_gpu_error_feedback import SHAPES
-    g = torch.Generator().manual_seed(seed)
-    return [(torch.randn(s, generator=g) * (0.01 * (1 + i))).bfloat16().float().cuda() for i, s in enumerate(SHAPES)]
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("bucket", BUCKETS)
 def test_error_feedback_identity_and_contraction(bucket):
-    from test_gpu_error_feedback import Loopback
-    h = Loopback("sign", _grads(1), bucket_size=bucket)
+    h = Loopback("sign", ef_grads(1), bucket_size=bucket)
     try:
         g, e_old = h.g, h.residual()
         for _ in range(4):
@@ -502,8 +418,7 @@ def test_error_feedback_identity_and_contraction(bucket):
 def test_error_feedback_residual_stays_bounded():
     """A fixed gradient for 200 steps: every step contracts (||e_{t+1}|| <= rho ||g + e_t||, rho < 1), so ||e|| stays
     below rho / (1 - rho) ||g||; the pushed sum misses 200 g by exactly the final residual."""
-    from test_gpu_error_feedback import Loopback
-    h = Loopback("sign", _grads(2), bucket_size=512)
+    h = Loopback("sign", ef_grads(2), bucket_size=512)
     try:
         s = torch.zeros_like(h.g)
         e = h.residual()
@@ -523,8 +438,7 @@ def test_error_feedback_residual_stays_bounded():
 
 @pytest.mark.gpu
 def test_code_stats_bytes_follow_the_plan():
-    from test_gpu_error_feedback import Loopback
-    h = Loopback("sign", _grads(4), bucket_size=256, code_stats=True)
+    h = Loopback("sign", ef_grads(4), bucket_size=256, code_stats=True)
     try:
         h.step()
         st = h.eng.code_stats()
@@ -542,26 +456,7 @@ def test_code_stats_bytes_follow_the_plan():
 
 
 # ---------------------------------------------------------------------------------------------------- GPU: engine
-def _train(net, graph, ef, steps=6, bucket=512, lr=0.05, seed=3):
-    from atomo_b200.data import SyntheticImageDataset
-    from atomo_b200.models import build_model, input_shape
-    from atomo_b200.runtime.shadow_engine import ShadowEngine
-    torch.manual_seed(0)
-    torch.cuda.set_device(0)
-    x, y = SyntheticImageDataset(input_shape(net), 10, 4096, seed=0).materialize(32)
-    eng = ShadowEngine(build_model(net, 10), 0, 1, code="sign", bucket_size=bucket, lr=lr, momentum=0.9,
-                       use_graph=graph, overlap=graph, seed=seed, error_feedback=ef)
-    eng.prepare(x.pin_memory(), y.pin_memory(), warmup=2)
-    losses, norms = [], []
-    for _ in range(steps):
-        losses.append(float(eng.train_step(x, y)[0]))
-        if ef:
-            norms.append(eng.error_feedback_norm()["model"])
-    torch.cuda.synchronize()
-    assert eng.error_code() == 0
-    m = eng.gather_fp32("master").clone()
-    eng.close()
-    return m, losses, norms
+_train = functools.partial(train, code="sign", bucket_size=512)
 
 
 @pytest.mark.gpu
@@ -639,8 +534,7 @@ def test_shadow_engine_sign_multi_gpu_replicas_identical():
     n = torch.cuda.device_count()
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
-    from test_gpu_v2 import _run_mp
     world = 2 if n < 8 else (8 if os.environ.get("ATOMO_TEST_WORLD8") else 2)
-    res = _run_mp(world, {"code": "sign", "ps_mode": "sharded", "net": "VGG11"}, 29810)
+    res = run_mp(world, {"code": "sign", "ps_mode": "sharded", "net": "VGG11"}, 29810)
     for rank, err, same, l0, l1, mode, mc, _ in res:
         assert err == 0 and same, res

@@ -19,8 +19,7 @@ import torch
 
 from atomo_b200.codings.sampling import atom_probabilities
 
-from test_gpu_kernels import Harness
-from test_gpu_v2 import H2
+from shadow_harness import H2, MODELS, Harness, model_shapes
 
 gpu = pytest.mark.gpu
 ERR2_NONFINITE = 8
@@ -200,14 +199,6 @@ def _read_basis(h, rule, uniforms=None):
     assert torch.equal(h.vprev, first), "the Jacobi basis of a fixed gradient must be deterministic"
 
 
-def _model_shapes(net, dataset=""):
-    from atomo_b200.models import build_model
-    return [tuple(p.shape) for p in build_model(net, 10, dataset).parameters()]
-
-
-MODELS = {"ResNet18": ("ResNet18", ""), "VGG11": ("VGG11", ""), "ResNet50-ImageNet": ("ResNet50", "ImageNet")}
-
-
 # ------------------------------------------------------------------------------------------------- items 1, 2, 5
 def _spectrum_bound(h, u, A):
     """Bound on |sigma_out_k^2 - sigma_k^2| (sigma_k: fp64 singular values of the bf16 unit matrix).
@@ -256,7 +247,7 @@ def test_encode_selects_orders_and_scales_like_the_oracle(model, rank):
     the reference rule and water-filling, the slot holds exactly S in the kernel's order with s = sigma / p, and the
     decoded atoms are A v v^T / p; the sorted spectrum is within the fp32 Gram bound (_spectrum_bound)."""
     net, ds = MODELS[model]
-    shapes = _model_shapes(net, ds)
+    shapes = model_shapes(net, ds)
     rng = np.random.default_rng(rank)
     h = H2(shapes, rank=rank, warm=True, max_sweeps=0)
     logical = h.fill(0, 11 + rank)
@@ -279,7 +270,7 @@ def test_encode_selects_orders_and_scales_like_the_oracle(model, rank):
 def test_encode_budget_zero_rule(model):
     """budget <= 0 (rank 0): p = sigma / sigma_max, the top atom always sent."""
     net, ds = MODELS[model]
-    h = H2(_model_shapes(net, ds), rank=0, warm=True, max_sweeps=0)
+    h = H2(model_shapes(net, ds), rank=0, warm=True, max_sweeps=0)
     logical = h.fill(0, 5)
     _read_basis(h, "reference")
     orc = _oracles(h, logical, "reference")
@@ -303,7 +294,7 @@ def test_redraws_follow_philox(warm):
     """A first draw over the slot capacity, or an empty one with resample_empty, is redrawn from Philox(seed;
     atom, attempt, unit, (worker << 24) ^ step).  warm=True is the production setting (warm start, one sweep): the
     basis is then approximate but orthonormal, and the same checks hold on it."""
-    shapes = _model_shapes("ResNet18")
+    shapes = model_shapes("ResNet18")
     h = H2(shapes, rank=3, warm=True, max_sweeps=1 if warm else 0)
     logical = h.fill(0, 21)
     step = 2
@@ -378,7 +369,7 @@ def _systematic_x(p_sorted):
 @pytest.mark.parametrize("rule", ["reference", "waterfill"])
 def test_systematic_and_topk_selection(rule):
     from atomo_b200.codings.sampling import sample_atoms
-    shapes = _model_shapes("ResNet18")
+    shapes = model_shapes("ResNet18")
     h = H2(shapes, rank=3, warm=True, max_sweeps=0, systematic=True)
     logical = h.fill(0, 31)
     _read_basis(h, rule)

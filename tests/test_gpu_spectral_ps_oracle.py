@@ -22,8 +22,7 @@ import torch
 
 from atomo_b200.ops import plan2 as P
 
-from test_gpu_spectral_oracle import MODELS, _model_shapes
-from test_gpu_v2 import H2
+from shadow_harness import H2, MODELS, model_shapes
 
 gpu = pytest.mark.gpu
 SIG_PUSH, SIG_PARAM, SIG_MASK = 0, 256, 320
@@ -455,7 +454,7 @@ def test_scatter_inverts_unit_matrix(model):
     """oracle_scatter puts every coded unit's matrix (H2.unit_matrix of a logical gradient) back where the physical
     channels-last weight holds it; with the DENSE16 units this covers every weight element exactly once."""
     net, ds = MODELS[model]
-    shapes = _model_shapes(net, ds)
+    shapes = model_shapes(net, ds)
     pl = P.build_plan2(shapes, "svd", 3, n_groups=5)
     g = torch.Generator().manual_seed(3)
     logical, phys = {}, torch.zeros(pl.w_total, dtype=torch.float64)
@@ -579,7 +578,7 @@ def test_ps_equals_oracle_bitwise_on_models(model, rank):
     CTAs and one CTA give the same bits."""
     net, ds = MODELS[model]
     W = 16 if rank < 8 else 8
-    h, _ = _harness(_model_shapes(net, ds), rank, W)
+    h, _ = _harness(model_shapes(net, ds), rank, W)
     d = Design(h.plan, W, 1, True, seed=rank, shift=rank)
     _run_exact(h, d, seed=rank)
 
@@ -597,7 +596,7 @@ def test_ps_equals_oracle_bitwise_on_odd_shapes(W, rank):
 @pytest.mark.parametrize("shapes", ["ResNet18", "odd"])
 def test_qsvd_ps_equals_oracle_bitwise(shapes):
     """int8 U with row scales whose de-quantization factor fp32(scale * fp32(1/127)) is a power of two."""
-    sh = _model_shapes("ResNet18") if shapes == "ResNet18" else ODD_SHAPES
+    sh = model_shapes("ResNet18") if shapes == "ResNet18" else ODD_SHAPES
     h, _ = _harness(sh, 3, 8, code="qsvd")
     assert all(u.ubits == 8 for u in _coded(h.plan))
     _run_exact(h, Design(h.plan, 8, 1, True, seed=5, shift=2), seed=5)
@@ -609,7 +608,7 @@ def test_gather_stores_the_oracle_mean_and_tile_sums(shapes):
     """The gather instantiation (clipping phase 1, as ShadowEngine._launch_ps_clip launches it): the stored mean
     gradient is the oracle's bit for bit; part[tile].x is sum g^2 of the tile within gamma_{N + 12} sum g^2 (N
     products of one thread's chain at most, then 5 shuffle and 7 warp additions)."""
-    sh = _model_shapes("ResNet18") if shapes == "ResNet18" else ODD_SHAPES
+    sh = model_shapes("ResNet18") if shapes == "ResNet18" else ODD_SHAPES
     W = 16
     h, _ = _harness(sh, 3, W)
     pl, C = h.plan, h.C

@@ -2,6 +2,7 @@
 the refusals and the launcher routing (CPU); the selection and encode kernels against the oracle bit for bit, the PS
 average, error feedback and ``--code-stats`` (GPU loopback harness); and the engine end to end (GPU)."""
 import argparse
+import functools
 import json
 import math
 import os
@@ -12,6 +13,8 @@ import torch
 from atomo_b200.ops import plan2 as P
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
+
+from shadow_harness import HE, Loopback, ef_grads, fit_args, flat, forbid_cuda, run_mp, train
 
 NET_SHAPES = [(64, 3, 3, 3), (64,), (64,), (128, 64, 3, 3), (128,), (256, 128, 3, 3), (512, 256, 1, 1), (300, 200),
               (10, 512), (7, 20), (10,)]
@@ -116,10 +119,7 @@ def test_plan2_other_codes_unchanged_by_the_new_code():
                                 {"entry_budget": -2.0}])
 def test_shadow_engine_topk_refuses_before_cuda(kw, monkeypatch):
     from atomo_b200.runtime import shadow_engine as S
-
-    def no_cuda(*a, **k):
-        raise AssertionError("refused only after CUDA work started")
-    monkeypatch.setattr(S, "load_ext", no_cuda)
+    forbid_cuda(monkeypatch)
     with pytest.raises(ValueError):
         S.ShadowEngine(None, 0, 1, code="topk", **kw)
     with pytest.raises(ValueError, match="num_aggregate"):     # the error-feedback rule applies unchanged
@@ -127,13 +127,6 @@ def test_shadow_engine_topk_refuses_before_cuda(kw, monkeypatch):
 
 
 # ---------------------------------------------------------------------------------------------------- CPU: launcher
-def _args(tmp_path, *extra):
-    return add_fit_args(argparse.ArgumentParser(), [
-        "--network", "LeNet", "--dataset", "MNIST", "--synthetic", "1", "--train-len", "512", "--test-len", "128",
-        "--batch-size", "32", "--test-batch-size", "64", "--lr", "0.05", "--log-interval", "1", "--eval-freq", "100",
-        "--train-dir", str(tmp_path) + "/", *extra])
-
-
 def test_flag_parse():
     a = add_fit_args(argparse.ArgumentParser(), ["--code", "topk", "--entry-budget", "0.01", "--error-feedback", "1"])
     assert a.code == "topk" and a.entry_budget == 0.01 and a.error_feedback is True
@@ -149,21 +142,21 @@ def test_launcher_routes_topk(tmp_path, monkeypatch):
     monkeypatch.setattr(S, "ShadowEngine", Fake)
     model = torch.nn.Linear(4, 4)
     for engine in ("auto", "shadow"):
-        eng, kind = L._build_engine(_args(tmp_path, "--code", "topk", "--dtype", "bf16", "--engine", engine,
+        eng, kind = L._build_engine(fit_args(tmp_path, "--code", "topk", "--dtype", "bf16", "--engine", engine,
                                           "--entry-budget", "0.01", "--error-feedback", "1"), model, 0, 1)
         assert kind == "shadow" and seen[-1]["code"] == "topk" and seen[-1]["entry_budget"] == 0.01
         assert seen[-1]["error_feedback"] is True
     n = len(seen)
     from atomo_b200.runtime import engine as E
     monkeypatch.setattr(E, "FusedEngine", lambda *a, **kw: None)
-    _, kind = L._build_engine(_args(tmp_path, "--code", "entrywise", "--dtype", "bf16", "--engine", "auto"), model, 0, 1)
+    _, kind = L._build_engine(fit_args(tmp_path, "--code", "entrywise", "--dtype", "bf16", "--engine", "auto"), model, 0, 1)
     assert kind == "fused" and len(seen) == n       # --engine auto keeps entrywise on the fp32-flat engine
     for extra in (("--dtype", "fp32"), ("--dtype", "bf16", "--engine", "fused")):
         with pytest.raises(SystemExit, match="topk"):
-            L._build_engine(_args(tmp_path, "--code", "topk", *extra), model, 0, 1)
+            L._build_engine(fit_args(tmp_path, "--code", "topk", *extra), model, 0, 1)
     assert len(seen) == n
     with pytest.raises(SystemExit, match="bf16"):           # --engine shadow still needs bf16 weights
-        L._build_engine(_args(tmp_path, "--code", "qsgd", "--dtype", "fp32", "--engine", "shadow"), model, 0, 1)
+        L._build_engine(fit_args(tmp_path, "--code", "qsgd", "--dtype", "fp32", "--engine", "shadow"), model, 0, 1)
     assert len(seen) == n
 
 
@@ -173,24 +166,20 @@ def test_role_paths_refuse_topk(monkeypatch, tmp_path):
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
     with pytest.raises(SystemExit, match="p2p bf16 engine"):
-        distributed_nn.run_rank(_args(tmp_path, "--code", "topk", "--backend", "gloo"))
+        distributed_nn.run_rank(fit_args(tmp_path, "--code", "topk", "--backend", "gloo"))
     with pytest.raises(ValueError, match="p2p bf16 engine"):
         build_coder({"code": "topk", "entry_budget": 0.05}, worker_side=True)
 
 
 # ---------------------------------------------------------------------------------------------------- GPU harness
-from test_gpu_shadow_entrywise import HE  # noqa: E402
-
-
 class HT(HE):
-    """The loopback harness of the entry-wise tests (one owner, W virtual workers) on a top-k plan."""
+    """The entry-wise harness on a top-k plan."""
+
+    CODE = "topk"
 
     def __init__(self, shapes, budget=0.05, W=1, **kw):
         super().__init__(shapes, budget, W=W, **kw)
-        pl = self.plan = P.build_plan2(shapes, "topk", n_owners=1, n_groups=1, entry_budget=budget)
-        u8 = lambda b: torch.frombuffer(bytearray(b), dtype=torch.uint8).to(self.dev)
-        self.t_units = u8(pl.units_bytes())
-        nc = max(pl.n_coded, 1)
+        pl, nc = self.plan, self.nc
         i32 = lambda n: torch.zeros(n, dtype=torch.int32, device=self.dev)
         self.sel, self.hist, self.tcounts = i32(8 * nc), i32(256 * nc), i32(128 * max(len(pl.enc_tiles), 1))
         self.acc = torch.zeros(7 * nc, dtype=torch.float64, device=self.dev)
@@ -204,24 +193,23 @@ class HT(HE):
                 if q.index == TIES:
                     t.copy_((t.float() * 2).round() / 8)        # 7-ish distinct magnitudes: ties across tiles
                 else:
-                    (t.permute(0, 2, 3, 1) if t.dim() == 4 else t).view(-1)[1234] = float("inf")
-                phys[q.index] = (t.permute(0, 2, 3, 1) if t.dim() == 4 else t).reshape(-1).float()
+                    flat(t)[1234] = float("inf")
+                phys[q.index] = flat(t).float()
         return phys
 
     def encode(self, w, residual=0, stats=False):
         C, pl = self.C, self.plan
-        gptr = torch.tensor([t.data_ptr() for t in self.wgrads[w]], dtype=torch.int64, device=self.dev)
-        self._gptr = gptr
+        gptr = self.gptr(w)
         t0, nt = pl.enc_range[0]
-        C.v2_topk_select(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr.data_ptr(),
+        C.v2_topk_select(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr,
                          self.hist.data_ptr(), self.tcounts.data_ptr(), self.counters.data_ptr(),
                          self.sel.data_ptr(), 0, 0)
-        C.v2_topk_encode(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr.data_ptr(), self.sel.data_ptr(),
+        C.v2_topk_encode(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr, self.sel.data_ptr(),
                          self.tcounts.data_ptr(), self.t_arena_peer.data_ptr(), self.t_sig_peer.data_ptr(), 1,
-                         pl.arena_floats, w, 0, self.ctrl.data_ptr(), self.counters.data_ptr() + 4 * (pl.n_coded + 8),
+                         pl.arena_floats, w, 0, self.ctrl.data_ptr(), self.counter(),
                          0, False, residual)
         if stats:
-            C.v2_topk_code_stats(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr.data_ptr(),
+            C.v2_topk_code_stats(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr,
                                  self.sel.data_ptr(), self.tcounts.data_ptr(), self.t_arena_peer.data_ptr(), 1,
                                  pl.arena_floats, w, self.spart.data_ptr(), self.counters.data_ptr(),
                                  self.acc.data_ptr())
@@ -336,17 +324,10 @@ def test_v2_topk_code_stats_match_fp64():
 
 
 # ---------------------------------------------------------------------------------------------------- GPU: feedback
-def _grads(seed=0):
-    from test_gpu_error_feedback import SHAPES
-    g = torch.Generator().manual_seed(seed)
-    return [(torch.randn(s, generator=g) * (0.01 * (1 + i))).bfloat16().float().cuda() for i, s in enumerate(SHAPES)]
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("budget", [0.01, 0.05])
 def test_error_feedback_identity_and_contraction(budget):
-    from test_gpu_error_feedback import Loopback
-    h = Loopback("topk", _grads(1), entry_budget=budget)
+    h = Loopback("topk", ef_grads(1), entry_budget=budget)
     try:
         g, e_old = h.g, h.residual()
         for _ in range(4):
@@ -368,8 +349,7 @@ def test_error_feedback_identity_and_contraction(budget):
 @pytest.mark.gpu
 def test_error_feedback_residual_stays_bounded():
     """A fixed gradient for 200 steps: e stays below the contraction bound sqrt(1-d) / (1 - sqrt(1-d)) ||g||."""
-    from test_gpu_error_feedback import Loopback
-    h = Loopback("topk", _grads(2), entry_budget=0.05)
+    h = Loopback("topk", ef_grads(2), entry_budget=0.05)
     try:
         s = torch.zeros_like(h.g)
         for _ in range(200):
@@ -384,26 +364,7 @@ def test_error_feedback_residual_stays_bounded():
 
 
 # ---------------------------------------------------------------------------------------------------- GPU: engine
-def _train(net, graph, ef, steps=6, budget=0.01, lr=0.05, seed=3):
-    from atomo_b200.data import SyntheticImageDataset
-    from atomo_b200.models import build_model, input_shape
-    from atomo_b200.runtime.shadow_engine import ShadowEngine
-    torch.manual_seed(0)
-    torch.cuda.set_device(0)
-    x, y = SyntheticImageDataset(input_shape(net), 10, 4096, seed=0).materialize(32)
-    eng = ShadowEngine(build_model(net, 10), 0, 1, code="topk", entry_budget=budget, lr=lr, momentum=0.9,
-                       use_graph=graph, overlap=graph, seed=seed, error_feedback=ef)
-    eng.prepare(x.pin_memory(), y.pin_memory(), warmup=2)
-    losses, norms = [], []
-    for _ in range(steps):
-        losses.append(float(eng.train_step(x, y)[0]))
-        if ef:
-            norms.append(eng.error_feedback_norm()["model"])
-    torch.cuda.synchronize()
-    assert eng.error_code() == 0
-    m = eng.gather_fp32("master").clone()
-    eng.close()
-    return m, losses, norms
+_train = functools.partial(train, code="topk", entry_budget=0.01)
 
 
 @pytest.mark.gpu
@@ -485,8 +446,7 @@ def test_shadow_engine_topk_multi_gpu_replicas_identical():
     n = torch.cuda.device_count()
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
-    from test_gpu_v2 import _run_mp
     world = 2 if n < 8 else (8 if os.environ.get("ATOMO_TEST_WORLD8") else 2)
-    res = _run_mp(world, {"code": "topk", "ps_mode": "sharded", "net": "VGG11"}, 29790)
+    res = run_mp(world, {"code": "topk", "ps_mode": "sharded", "net": "VGG11"}, 29790)
     for rank, err, same, l0, l1, mode, mc, _ in res:
         assert err == 0 and same, res

@@ -4,160 +4,12 @@ import os
 import pytest
 import torch
 
+from shadow_harness import H2, batch, run_mp
+
 pytestmark = pytest.mark.gpu
 
 SHAPES = [(64, 32, 3, 3), (32, 64, 3, 3), (48, 16, 5, 5), (10, 512), (128, 64, 1, 1), (64,), (512, 256, 1, 1),
           (64, 3, 3, 3), (300, 200), (10,)]
-
-
-def _ext():
-    from atomo_b200.ops._ext import load
-    return load()
-
-
-class H2:
-    """Loopback harness: one rank that is worker 0..W-1 (virtual) and the only owner."""
-
-    def __init__(self, shapes, code="svd", rank=3, W=1, lr=0.1, momentum=0.0, wd=0.0, nesterov=False, opt=0, seed=7,
-                 systematic=False, groups=1, warm=False, max_sweeps=0):
-        from atomo_b200.ops import plan2 as P
-        self.C, self.P = _ext(), P
-        dev = self.dev = torch.device("cuda", 0)
-        self.W = W
-        self.plan = pl = P.build_plan2(shapes, code, rank, systematic, n_owners=1, n_groups=groups)
-        u8 = lambda b: torch.frombuffer(bytearray(b), dtype=torch.uint8).to(dev)
-        self.t_units = u8(pl.units_bytes())
-        self.t_enc = u8(P.Plan2.tiles_bytes(pl.enc_tiles))
-        self.t_ps = u8(P.Plan2.tiles_bytes(pl.ps_tiles))
-        nc = max(pl.n_coded, 1)
-        z = lambda n, dt=torch.float32: torch.zeros(n, dtype=dt, device=dev)
-        self.gpart, self.vsel, self.sigma = z(pl.gpart_floats), z(nc * 64 * 32), z(nc * 64)
-        self.selcount = z(nc, torch.int32)
-        self.counters = z(nc + 32, torch.int32)
-        self.arena = z(pl.arena_floats * W)
-        self.signals = z(1024, torch.int32)
-        self.signals[256] = 1
-        self.ctrl = u8(P.pack_ctrl2(step=1, lr=lr, momentum=momentum, weight_decay=wd, nesterov=nesterov, seed=seed, opt=opt))
-        g = torch.Generator(device="cuda").manual_seed(seed)
-        self.master = torch.randn(pl.w_total, device=dev, generator=g)
-        self.wshadow = self.master.to(torch.bfloat16)
-        self.vparams = torch.randn(pl.v_total, device=dev, generator=g)
-        self.mom, self.vmom = z(pl.w_total), z(pl.v_total)
-        self.sq, self.vsq, self.sqmax, self.vsqmax = z(pl.w_total), z(pl.v_total), z(pl.w_total), z(pl.v_total)
-        self.stage = [z(pl.stage_total, torch.bfloat16) for _ in range(W)]
-        self.vgrads = [z(pl.v_total) for _ in range(W)]
-        self.wgrads = []          # per worker: list of bf16 grad tensors (physical layout), one per W param
-        i64 = lambda xs: torch.tensor(list(xs), dtype=torch.int64, device=dev)
-        self.t_arena_peer = i64([self.arena.data_ptr()])
-        self.t_sig_peer = i64([self.signals.data_ptr()])
-        self.t_wshadow_peer = i64([self.wshadow.data_ptr()])
-        self.t_vparams_peer = i64([self.vparams.data_ptr()])
-        self.t_vgrads_peer = i64([t.data_ptr() for t in self.vgrads])
-        self.t_stage_peer = i64([t.data_ptr() for t in self.stage])
-        self.tstats = z(32, torch.int64)
-        self.max_sweeps = max_sweeps
-        self.vprev = None
-        if warm:
-            self.vprev = z(nc * 64 * 64)
-            for u in pl.units:
-                if u.coded:
-                    self.vprev[u.ts_index * 4096:u.ts_index * 4096 + u.cols * u.cols] = torch.eye(u.cols, device=dev).reshape(-1)
-
-    def fill(self, w, seed, lowrank=True):
-        """Random gradients for virtual worker w; returns {param index: fp32 tensor in the logical layout}."""
-        pl, dev = self.plan, self.dev
-        g = torch.Generator(device="cuda").manual_seed(seed)
-        grads, logical = [], {}
-        for q in pl.params:
-            if q.is_w:
-                x = torch.randn(q.shape, device=dev, generator=g)
-                if lowrank and len(q.shape) >= 2:
-                    m = x.reshape(q.shape[0], -1)
-                    k = min(m.shape)
-                    a = torch.randn(m.shape[0], k, device=dev, generator=g) * torch.logspace(0, -1.5, k, device=dev)
-                    x = (a @ torch.linalg.qr(torch.randn(m.shape[1], k, device=dev, generator=g)).Q.T).reshape(q.shape)
-                xb = x.to(torch.bfloat16)
-                phys = xb.contiguous(memory_format=torch.channels_last) if xb.dim() == 4 else xb.contiguous()
-                grads.append(phys)
-                logical[q.index] = phys.float()
-            else:
-                v = torch.randn(q.numel, device=dev, generator=g)
-                self.vgrads[w][q.off:q.off + q.numel] = v
-                logical[q.index] = v
-        while len(self.wgrads) <= w:
-            self.wgrads.append(None)
-        self.wgrads[w] = grads
-        return logical
-
-    def encode(self, w, random_sample=True, waterfill=False, systematic=False, uniforms=None, resample_empty=False):
-        C, pl = self.C, self.plan
-        gptr = torch.tensor([t.data_ptr() for t in self.wgrads[w]] or [0], dtype=torch.int64, device=self.dev)
-        self._gptr = gptr
-        for g in range(pl.n_groups):
-            t0, nt = pl.enc_range[g]
-            C.v2_encode(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr.data_ptr(), self.gpart.data_ptr(),
-                        self.counters.data_ptr(), self.vsel.data_ptr(), self.selcount.data_ptr(), self.sigma.data_ptr(),
-                        self.t_arena_peer.data_ptr(), 1, pl.arena_floats, self.stage[w].data_ptr(), self.ctrl.data_ptr(),
-                        uniforms.data_ptr() if uniforms is not None else 0,
-                        self.vprev.data_ptr() if self.vprev is not None else 0, self.max_sweeps, random_sample,
-                        waterfill, systematic, w, resample_empty, 0, 0, g)
-            C.v2_project(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr.data_ptr(), self.vsel.data_ptr(),
-                         self.selcount.data_ptr(), self.t_arena_peer.data_ptr(), self.t_sig_peer.data_ptr(), 1,
-                         pl.arena_floats, w, g, self.ctrl.data_ptr(), self.counters.data_ptr() + 4 * (pl.n_coded + g), 0, 0,
-                         False, False)
-        torch.cuda.synchronize()
-
-    def ps(self, grid=64):
-        C, pl = self.C, self.plan
-        for g in range(pl.n_groups):
-            t0, nt = pl.ps_range[g][0]
-            C.v2_ps(self.t_units.data_ptr(), self.t_ps.data_ptr(), t0, nt, self.W, 1, g, g == pl.n_groups - 1, 0,
-                    self.master.data_ptr(), self.mom.data_ptr(), self.sq.data_ptr(), self.sqmax.data_ptr(),
-                    self.vmom.data_ptr(), self.vsq.data_ptr(), self.vsqmax.data_ptr(), 0, self.t_wshadow_peer.data_ptr(),
-                    self.vparams.data_ptr(), 0, self.t_vparams_peer.data_ptr(), 0, self.t_vgrads_peer.data_ptr(),
-                    self.t_stage_peer.data_ptr(), self.arena.data_ptr(), pl.arena_floats, self.signals.data_ptr(),
-                    self.t_sig_peer.data_ptr(), self.ctrl.data_ptr(),
-                    self.counters.data_ptr() + 4 * (pl.n_coded + 8 + g), int(5e9), self.tstats.data_ptr(), 1.0 / self.W,
-                    grid)
-        torch.cuda.synchronize()
-
-    # ---- references ---------------------------------------------------------------------------------------
-    def unit_matrix(self, u, logical):
-        """fp32 tall matrix of a coded unit, in the kernel's row/column convention."""
-        q = self.plan.params[u.param]
-        t = logical[q.index]
-        if u.kind == self.P.KIND_SLAB:
-            o, i, kh, kw = q.shape
-            return t.contiguous().reshape(o * i // 2, 2 * kh * kw)       # the reference's matricization
-        m = t.reshape(q.shape[0], -1)
-        tall = m if m.shape[0] >= m.shape[1] else m.t()
-        c0 = u.g_off // u.cs if u.cs > 1 else u.g_off
-        return tall[:, c0:c0 + u.cols]
-
-    def slot(self, u, w):
-        base = self.arena[w * self.plan.arena_floats + u.slot_off:]
-        hdr = base[:4].view(torch.int32)
-        count = int(hdr[0])
-        s = base[4:4 + u.rcap][:count]
-        V = base[4 + u.rcap:4 + u.rcap + u.rcap * u.cols].view(u.rcap, u.cols)[:count]
-        uo = self.P.slot_u_off(u.rcap, u.cols)
-        if u.ubits == 8:      # QSVD: int8 U with one fp32 scale per row
-            q = base[uo:uo + u.rows * u.rcap // 4].view(torch.int8).view(u.rows, u.rcap)[:, :count].float()
-            so = self.P.slot_scale_off(u.rows, u.cols, u.rcap)
-            U = q * (base[so:so + u.rows] / 127.0).unsqueeze(1)
-        else:
-            U = base[uo:uo + u.rows * u.rcap].view(u.rows, u.rcap)[:, :count]
-        return count, s, V, U, int(hdr[1])
-
-    def write_unit(self, u, flat, mat):
-        """Scatter a tall unit matrix into a flat fp32 array indexed like wshadow (physical order)."""
-        q = self.plan.params[u.param]
-        if u.kind == self.P.KIND_SLAB:
-            o, i, kh, kw = q.shape
-            logical = mat.reshape(o, i, kh, kw)
-            flat[q.off:q.off + q.numel] = logical.permute(0, 2, 3, 1).reshape(-1)
-        else:
-            torch.as_strided(flat, (u.rows, u.cols), (u.rs, u.cs), u.w_off).copy_(mat)
 
 
 def test_v2_gram_matches_torch():
@@ -433,13 +285,6 @@ def test_v2_ps_num_aggregate_uses_only_the_workers_that_pushed():
     assert torch.allclose(h.vparams[vused], (v0 - lr * est_v / 2)[vused], rtol=3e-4, atol=3e-5)
 
 
-def _batch(net, n=32, seed=0):
-    from atomo_b200.models import input_shape
-    from atomo_b200.data import SyntheticImageDataset
-    x, y = SyntheticImageDataset(input_shape(net), 10, 4096, seed=seed).materialize(n)
-    return x.pin_memory(), y.pin_memory()
-
-
 @pytest.mark.parametrize("code,graph,overlap", [("svd", False, False), ("svd", True, True), ("sgd", True, True)])
 def test_shadow_engine_trains_single_gpu(code, graph, overlap):
     from atomo_b200.models import build_model
@@ -448,7 +293,7 @@ def test_shadow_engine_trains_single_gpu(code, graph, overlap):
     torch.cuda.set_device(0)
     eng = ShadowEngine(build_model("ResNet18", 10), 0, 1, code=code, svd_rank=3, lr=0.05, momentum=0.9, use_graph=graph,
                        overlap=overlap, seed=3)
-    x, y = _batch("ResNet18", 64)
+    x, y = batch("ResNet18", 64)
     eng.prepare(x, y, warmup=2)
     first = None
     for _ in range(25):
@@ -476,7 +321,7 @@ def test_shadow_engine_dense_code_applies_exactly_its_gradients():
     torch.manual_seed(1)
     torch.cuda.set_device(0)
     eng = ShadowEngine(build_model("VGG11", 10), 0, 1, code="sgd", lr=0.05, momentum=0.9, use_graph=False, overlap=True)
-    x, y = _batch("VGG11", 32)
+    x, y = batch("VGG11", 32)
     eng.prepare(x, y, warmup=0)
     pl = eng.plan
     master = eng.gather_fp32("master").clone()
@@ -507,7 +352,7 @@ def test_shadow_engine_checkpoint_roundtrip(tmp_path):
     from atomo_b200.runtime.shadow_engine import ShadowEngine
     torch.cuda.set_device(0)
     d = str(tmp_path) + "/"
-    x, y = _batch("ResNet18", 32)
+    x, y = batch("ResNet18", 32)
 
     def make():
         torch.manual_seed(0)
@@ -535,73 +380,6 @@ def test_shadow_engine_checkpoint_roundtrip(tmp_path):
 
 
 # ---------------------------------------------------------------------------------------------------- multi GPU
-def _mp_worker(rank, world, port, cfg, out):
-    import torch.distributed as dist
-    from atomo_b200.models import build_model
-    from atomo_b200.runtime.shadow_engine import ShadowEngine
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
-                      LOCAL_RANK=str(rank))
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
-    torch.manual_seed(0)
-    net = cfg.get("net", "ResNet18")
-    eng = ShadowEngine(build_model(net, 10), rank, world, code=cfg["code"], svd_rank=3, lr=0.05, momentum=0.9,
-                       use_graph=cfg.get("graph", True), seed=5, ps_mode=cfg["ps_mode"], timeout_s=20.0,
-                       debug_jitter_us=cfg.get("jitter_us", 0.0))
-    x, y = _batch(net, 32, seed=rank)
-    eng.prepare(x, y, warmup=cfg.get("warmup", 2))
-    losses = []
-    ref = None
-    if cfg.get("check_dense"):
-        ref = {"master": eng.gather_fp32("master").clone(), "v": eng.vparams.clone()}
-        ref["mom"], ref["vmom"] = torch.zeros_like(ref["master"]), torch.zeros_like(ref["v"])
-    ok_dense = True
-    for it in range(cfg.get("steps", 12)):
-        losses.append(float(eng.train_step(x, y)[0]))
-        if ref is not None:
-            torch.cuda.synchronize()
-            g = torch.zeros_like(ref["master"])
-            for p, q in zip(eng.params, eng.plan.params):
-                if q.is_w and eng.is_worker:
-                    t = p.grad.float()
-                    g[q.off:q.off + q.numel] = t.permute(0, 2, 3, 1).reshape(-1) if t.dim() == 4 else t.reshape(-1)
-            gv = eng.vgrads.clone() if eng.is_worker else torch.zeros_like(eng.vgrads)
-            dist.all_reduce(g); dist.all_reduce(gv)
-            g /= eng.W; gv /= eng.W
-            first = eng.step - 1 == 1
-            ref["mom"] = g.clone() if first else 0.9 * ref["mom"] + g
-            ref["vmom"] = gv.clone() if first else 0.9 * ref["vmom"] + gv
-            ref["master"] -= 0.05 * ref["mom"]
-            ref["v"] -= 0.05 * ref["vmom"]
-            got = eng.gather_fp32("master")
-            ok_dense = ok_dense and bool(torch.allclose(got, ref["master"], rtol=2e-4, atol=2e-5)) and \
-                bool(torch.allclose(eng.vparams, ref["v"], rtol=2e-4, atol=2e-5))
-    torch.cuda.synchronize()
-    dist.barrier()           # every owner's last PS launch (peer / multicast stores into OUR copy) has completed
-    torch.cuda.synchronize()
-    ws = [torch.zeros_like(eng.wshadow) for _ in range(world)]
-    dist.all_gather(ws, eng.wshadow.clone())
-    vs = [torch.zeros_like(eng.vparams) for _ in range(world)]
-    dist.all_gather(vs, eng.vparams.clone())
-    same = all(torch.equal(ws[0], t) for t in ws) and all(torch.equal(vs[0], t) for t in vs)
-    out.put((rank, eng.error_code(), same, losses[0], losses[-1], eng.heap.mode, eng.heap.has_multicast, ok_dense))
-    eng.close()
-    dist.destroy_process_group()
-
-
-def _run_mp(world, cfg, port):
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    out = ctx.Queue()
-    procs = [ctx.Process(target=_mp_worker, args=(r, world, port, cfg, out)) for r in range(world)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(300)
-        assert p.exitcode == 0
-    return sorted(out.get() for _ in range(world))
-
-
 @pytest.mark.multigpu
 @pytest.mark.parametrize("code,ps_mode", [("svd", "sharded"), ("svd", "colocated"), ("sgd", "sharded"),
                                           ("svd", "dedicated")])
@@ -611,7 +389,7 @@ def test_shadow_engine_multi_gpu_replicas_identical(code, ps_mode):
         pytest.skip("needs >= 2 GPUs")
     world = 2 if n < 8 else (8 if os.environ.get("ATOMO_TEST_WORLD8") else 2)
     port = 29700 + 7 * ["sharded", "colocated", "dedicated"].index(ps_mode) + (3 if code == "sgd" else 0)
-    res = _run_mp(world, {"code": code, "ps_mode": ps_mode}, port)
+    res = run_mp(world, {"code": code, "ps_mode": ps_mode}, port)
     for rank, err, same, l0, l1, mode, mc, _ in res:
         assert err == 0 and same, res
     trained = [r for r in res if not (ps_mode == "dedicated" and r[0] == 0)]
@@ -628,11 +406,11 @@ def test_shadow_engine_protocol_survives_random_delays(ps_mode):
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
     world = 2 if n < 8 else (8 if os.environ.get("ATOMO_TEST_WORLD8") else 2)
-    res = _run_mp(world, {"code": "sgd", "ps_mode": ps_mode, "graph": False, "check_dense": True, "steps": 6,
+    res = run_mp(world, {"code": "sgd", "ps_mode": ps_mode, "graph": False, "check_dense": True, "steps": 6,
                           "net": "VGG11", "warmup": 0, "jitter_us": 300.0}, 29870 + (3 if ps_mode == "sharded" else 0))
     for r in res:
         assert r[1] == 0 and r[2] and r[7], res
-    res = _run_mp(world, {"code": "svd", "ps_mode": ps_mode, "graph": False, "steps": 8, "jitter_us": 300.0},
+    res = run_mp(world, {"code": "svd", "ps_mode": ps_mode, "graph": False, "steps": 8, "jitter_us": 300.0},
                   29890 + (3 if ps_mode == "sharded" else 0))
     for r in res:
         assert r[1] == 0 and r[2], res
@@ -646,7 +424,7 @@ def test_shadow_engine_multi_gpu_dense_equals_mean_gradient_sgd(ps_mode):
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
     world = 2 if n < 8 else (8 if os.environ.get("ATOMO_TEST_WORLD8") else 2)
-    res = _run_mp(world, {"code": "sgd", "ps_mode": ps_mode, "graph": False, "check_dense": True, "steps": 4,
+    res = run_mp(world, {"code": "sgd", "ps_mode": ps_mode, "graph": False, "check_dense": True, "steps": 4,
                           "net": "VGG11", "warmup": 0}, 29950 + (7 if ps_mode == "sharded" else 0))
     for r in res:
         assert r[1] == 0 and r[2] and r[7], res

@@ -17,6 +17,8 @@ from atomo_b200.optim import LAMB, LARS
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
 
+from shadow_harness import fit_args, forbid_cuda
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -120,19 +122,13 @@ def test_optimizers_refuse_what_they_do_not_define():
                                       (dict(optimizer="rmsprop"), "optimizers")])
 def test_engine_refuses_before_cuda_work(kw, match, monkeypatch):
     from atomo_b200.runtime import shadow_engine as S
-
-    def no_cuda(*a, **k):
-        raise AssertionError("refused only after CUDA work started")
-    monkeypatch.setattr(S, "load_ext", no_cuda)
+    forbid_cuda(monkeypatch)
     with pytest.raises(ValueError, match=match):
         S.ShadowEngine(None, 0, 1, **kw)
 
 
 def _args(tmp_path, *extra):
-    return add_fit_args(argparse.ArgumentParser(), [
-        "--network", "LeNet", "--dataset", "MNIST", "--synthetic", "1", "--train-len", "512", "--test-len", "128",
-        "--batch-size", "32", "--test-batch-size", "64", "--lr", "0.05", "--code", "svd", "--svd-rank", "3",
-        "--log-interval", "1", "--eval-freq", "100", "--train-dir", str(tmp_path) + "/", *extra])
+    return fit_args(tmp_path, "--code", "svd", "--svd-rank", "3", *extra)
 
 
 def test_flags_parse():
