@@ -268,6 +268,9 @@ void atomo_v2_launch_clip(int layerwise, const void* units, const void* tiles, c
                           long long* tstats, float* norm_out, int grid, cudaStream_t stream);
 void atomo_v2_launch_bcast_bytes(const void* src, void* const* peer, void* mc, int nranks, int self, long long nbytes,
                                  cudaStream_t stream);
+// v2_ema.cu (exponential moving average of the weights on the bf16 engine)
+void atomo_v2_launch_ema(const void* units, const void* tiles, int tile0, int ntiles, const float* master,
+                         const float* vparams, float* ema, float* vema, float w, int grid, cudaStream_t stream);
 // gemm_kernels.cu
 int atomo_gemm_tile_bytes();
 int atomo_gemm_smem_bytes();
@@ -1007,6 +1010,18 @@ void v2_clip(bool layerwise, uint64_t units, uint64_t tiles, uint64_t owner_tile
                        cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
+// exponential moving average of the weights (ema_decay): e <- e + w (p - e) over the PS tiles [tile0, tile0 + ntiles)
+// of one group and owner, master into ema and vparams into vema; on the PS stream, after the launch that writes the
+// group's final master values
+void v2_ema(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t master, uint64_t vparams, uint64_t ema,
+            uint64_t vema, float w, int grid) {
+  TORCH_CHECK(ntiles >= 0 && tile0 >= 0, "v2_ema: bad tile range");
+  TORCH_CHECK(ntiles == 0 || (units != 0 && tiles != 0 && master != 0 && vparams != 0 && ema != 0 && vema != 0),
+              "v2_ema: units / tiles / master / vparams / ema / vema required");
+  atomo_v2_launch_ema(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const float>(master),
+                      P<const float>(vparams), P<float>(ema), P<float>(vema), w, grid, cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
 void v2_accum_fold(uint64_t wchunks, int nw, uint64_t vchunks, int nv, uint64_t gptr, uint64_t acc, uint64_t vacc,
                    uint64_t vgrads, float inv_n, uint64_t residual) {
   TORCH_CHECK(nw >= 0 && nv >= 0, "v2_accum_fold: negative chunk count");
@@ -1210,6 +1225,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("v2_layerwise_max_layers", &atomo_v2_layerwise_max_layers);
   m.def("v2_ps_gather", &v2_ps_gather);
   m.def("v2_clip", &v2_clip);
+  m.def("v2_ema", &v2_ema);
   m.def("v2_ps_entry", &v2_ps_entry);
   m.def("v2_code_stats", &v2_code_stats);
   m.def("v2_stats_fields", &atomo_v2_stats_fields);

@@ -39,6 +39,7 @@ def _kwargs(args, role: str) -> dict:
                    "optimizer": args.optimizer, "weight_decay": args.weight_decay, "nesterov": args.nesterov,
                    "trust_coefficient": getattr(args, "trust_coefficient", 0.001),
                    "clip_grad_norm": getattr(args, "clip_grad_norm", 0.0),
+                   "ema_decay": getattr(args, "ema_decay", 0.0),
                    "resume": args.resume, "kill_stragglers": args.straggler_kill})
     else:
         kw["split_backward"] = args.straggler_kill

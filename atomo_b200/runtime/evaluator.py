@@ -5,7 +5,8 @@ poll ``<model_dir>model_step_<N>``; when it exists rebuild the net,
 ``load_state_dict(torch.load)``, report NLL + top-1/top-5 on the test set,
 ``N += eval_freq``; else sleep.  Works for every ``--network`` (the reference's
 only works for LeNet, SURVEY.md 2.9) and can stop (``max_evals`` / ``timeout``)
-instead of looping forever.
+instead of looping forever.  ``ema=True`` polls ``model_step_<N>_ema`` instead, the averaged weights that
+``--ema-decay`` writes beside each model file.
 """
 from __future__ import annotations
 
@@ -32,13 +33,14 @@ class DistributedEvaluator(NN_Trainer):
         self.num_classes = kwargs.get("num_classes", 10)
         self.device = torch.device(kwargs.get("device", "cpu"))
         self._poll_s = float(kwargs.get("poll_seconds", 10.0))
+        self._suffix = "_ema" if kwargs.get("ema", False) else ""
         self._next_step_to_fetch = self._eval_freq
         self.results = []
 
     def evaluate(self, validation_loader, max_evals: Optional[int] = None, timeout: Optional[float] = None):
         t0 = time.time()
         while True:
-            path = ckpt.model_path(self._model_dir, self._next_step_to_fetch)
+            path = ckpt.model_path(self._model_dir, self._next_step_to_fetch) + self._suffix
             if os.path.isfile(path):
                 self._load_model(path)
                 print("Evaluator evaluating results on step {}".format(self._next_step_to_fetch))

@@ -13,9 +13,11 @@ checkpointing every ``eval_freq`` steps is enabled; every ``--code`` builds.
 """
 from __future__ import annotations
 
+import os
 import time
 from typing import Optional
 
+import numpy as np
 import torch
 
 from .. import codings
@@ -23,7 +25,7 @@ from ..models import build_model
 from ..optim import LAMB, LARS, SGD, Adam
 from ..parallel.transport import Transport, STOP_STEP
 from ..utils import checkpoint as ckpt
-from ..utils.flags import check_clip_grad_norm
+from ..utils.flags import check_clip_grad_norm, check_ema_decay
 from ..utils.logging import MetricsWriter, master_line
 from .flat import FlatLayout, bind_parameters
 from .nn_ops import NN_Trainer
@@ -102,6 +104,8 @@ def clip_grad_norm(grads, max_norm: float):
 
 
 class SyncReplicasMaster_NN(NN_Trainer):
+    ema = None      # --ema-decay: the fp32 average of flat_params (build_model), None when off
+
     def __init__(self, comm: Transport, **kwargs):
         self.comm = comm
         self.world_size = comm.world_size
@@ -129,6 +133,9 @@ class SyncReplicasMaster_NN(NN_Trainer):
         self._optimizer_name = kwargs.get("optimizer", "sgd")
         self._clip_grad_norm = check_clip_grad_norm(kwargs.get("clip_grad_norm", 0.0))
         self.last_grad_norm = None      # (total, coef) of the last update with clipping on
+        # --ema-decay: an fp32 average of flat_params after every optimizer step, e <- e + w (p - e), w = fp32(1 - d)
+        self._ema_decay = check_ema_decay(kwargs.get("ema_decay", 0.0))
+        self._ema_w = float(np.float32(1.0 - self._ema_decay))
         self._save_checkpoints = kwargs.get("save_checkpoints", True)
         self._resume = kwargs.get("resume", False)
         self._verbose = kwargs.get("verbose", True)
@@ -159,17 +166,40 @@ class SyncReplicasMaster_NN(NN_Trainer):
         agg_dtype = torch.float64 if self.device.type == "cpu" else torch.float32
         self.grad_accumulator = GradientAccumulator(self.layout, self.device, agg_dtype)
         self._model_shapes = [tuple(p.shape) for p in self.network.parameters()]
-        if self._resume:
-            last = ckpt.latest_step(self._train_dir)
+        last = ckpt.latest_step(self._train_dir) if self._resume else None
+        if last is not None:
+            ckpt.load_model(self._train_dir, last, self.network, map_location=self.device)
+            side = ckpt.load_sidecar(self._train_dir, last, self.optimizer, map_location=self.device)
+            self.cur_step = last + 1
+            if side and side.get("lr") is not None:
+                self.lr = side["lr"]
+                self.optimizer.set_lr(self.lr)
+                self.shrink_counter = side.get("shrink_counter", 0)
+        if self._ema_decay:
+            self.ema = self.flat_params.clone()     # the initial (or loaded) weights
             if last is not None:
-                ckpt.load_model(self._train_dir, last, self.network, map_location=self.device)
-                side = ckpt.load_sidecar(self._train_dir, last, self.optimizer, map_location=self.device)
-                self.cur_step = last + 1
-                if side and side.get("lr") is not None:
-                    self.lr = side["lr"]
-                    self.optimizer.set_lr(self.lr)
-                    self.shrink_counter = side.get("shrink_counter", 0)
+                self._load_ema(ckpt.model_path(self._train_dir, last) + "_ema")
         return self
+
+    def _ema_views(self) -> dict:
+        """Parameter name -> its view of ``ema``."""
+        return {n: v for (n, _), v in zip(self.network.named_parameters(), self.layout.views(self.ema))}
+
+    def _load_ema(self, path: str):
+        if not os.path.exists(path):
+            print("%s missing: the weight average starts at the loaded weights" % path, flush=True)
+            return
+        sd = torch.load(path, map_location=self.device, weights_only=False)
+        with torch.no_grad():
+            for name, v in self._ema_views().items():
+                v.copy_(sd[name])
+
+    def _update_ema(self):
+        """e <- e + w (p - e) over flat_params, each operation rounded to fp32 (the bf16 engine's csrc/v2_ema.cu)."""
+        w = torch.tensor(self._ema_w, dtype=torch.float32, device=self.device)
+        d = torch.sub(self.flat_params, self.ema)
+        d.mul_(w)
+        self.ema.add_(d)
 
     # ------------------------------------------------------------------
     def train(self):
@@ -254,11 +284,20 @@ class SyncReplicasMaster_NN(NN_Trainer):
         if self._clip_grad_norm:
             grads, self.last_grad_norm = clip_grad_norm(grads, self._clip_grad_norm)
         self.optimizer.step(grads=grads, cuda=self._enable_gpu)
+        if self.ema is not None:
+            self._update_ema()
 
     def _generate_model_path(self):
         return ckpt.model_path(self._train_dir, self.cur_step)
 
     def _save_model(self, file_path=None):
         ckpt.save_model(self._train_dir, self.cur_step, self.network)
+        if self.ema is not None:
+            # the averaged weights with the live BN running statistics (from the first worker, _take_aux_buffers)
+            sd = self.network.state_dict()
+            sd.update({n: v.clone() for n, v in self._ema_views().items()})
+            path = ckpt.model_path(self._train_dir, self.cur_step) + "_ema"
+            torch.save(sd, path + ".tmp")
+            os.replace(path + ".tmp", path)
         ckpt.save_sidecar(self._train_dir, self.cur_step, self.optimizer, lr=self.lr,
                           extra={"shrink_counter": self.shrink_counter})

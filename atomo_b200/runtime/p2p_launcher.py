@@ -13,7 +13,8 @@ the overlapped, sharded
 entrywise``, which the launcher keeps on ``FusedEngine``; ``--engine fused`` always picks ``FusedEngine``.  ``--code
 topk``, ``--code sign``, ``--code powersgd``, ``--code fp8`` and ``--code hadamard`` (bits ``--quantization-level`` in
 {2, 4, 8}, a power-of-two ``--bucket-size``) exist only on ``ShadowEngine``, and so does ``--accumulate-steps N``
-(``N`` micro-batches of ``--batch-size`` per step: both loaders build batches of ``N * --batch-size``).
+(``N`` micro-batches of ``--batch-size`` per step: both loaders build batches of ``N * --batch-size``), and so does
+``--ema-decay D``: every ``--eval-freq`` step then also evaluates the averaged weights.
 """
 from __future__ import annotations
 
@@ -24,7 +25,7 @@ import torch
 import torch.distributed as dist
 import torch.nn.functional as F
 
-from ..utils.flags import check_clip_grad_norm
+from ..utils.flags import check_clip_grad_norm, check_ema_decay
 
 
 class _HostEvent:
@@ -45,6 +46,10 @@ def _build_engine(args, model, rank, world):
         clip = check_clip_grad_norm(getattr(args, "clip_grad_norm", 0.0))
     except ValueError as e:
         raise SystemExit("--clip-grad-norm: %s" % e)
+    try:
+        ema = check_ema_decay(getattr(args, "ema_decay", 0.0))
+    except ValueError as e:
+        raise SystemExit("--ema-decay: %s" % e)
     if code == "topk" and (engine == "fused" or args.dtype != "bf16"):
         raise SystemExit("--code topk runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the fp32-flat "
                          "engine has no top-k selection")
@@ -99,6 +104,8 @@ def _build_engine(args, model, rank, world):
             kw["clip_grad_norm"] = clip
         if getattr(args, "momentum_correction", False):
             kw["momentum_correction"] = True    # the engine refuses codes / optimizers it cannot correct
+        if ema:
+            kw["ema_decay"] = ema
         return ShadowEngine(model, rank, world, code=args.code, svd_rank=args.svd_rank, lr=args.lr,
                             momentum=args.momentum, weight_decay=args.weight_decay, nesterov=args.nesterov,
                             optimizer=args.optimizer, ps_mode=args.ps_mode, groups=args.groups, sampling=args.sampling,
@@ -107,6 +114,9 @@ def _build_engine(args, model, rank, world):
     if clip:
         raise SystemExit("--clip-grad-norm runs on the bf16 engine (--engine shadow, --dtype bf16); the fp32-flat engine "
                          "steps each tensor as its push lands and never sees the whole-model norm")
+    if ema:
+        raise SystemExit("--ema-decay runs on the bf16 engine (--engine shadow, --dtype bf16); the fp32-flat engine "
+                         "keeps no weight average")
     if args.optimizer in ("lars", "lamb"):
         raise SystemExit("--optimizer %s runs on the bf16 engine (--engine shadow, --dtype bf16); the fp32-flat engine "
                          "has no layer-wise trust ratio" % args.optimizer)
@@ -141,7 +151,7 @@ def run_p2p_training(args, device=None):
     from ..data import DataLoader, build_datasets, shard_dataset
     from ..models import build_model
     from ..utils import checkpoint as ckpt
-    from ..utils.logging import MetricsWriter, master_line, test_line, worker_line
+    from ..utils.logging import MetricsWriter, ema_test_line, master_line, test_line, worker_line
     from .nn_ops import accuracy
 
     rank = int(os.environ.get("RANK", "0"))
@@ -206,6 +216,30 @@ def run_p2p_training(args, device=None):
         if world > 1:
             dist.barrier()
 
+    def evaluate(net):
+        """(loss, prec1, prec5) of `net` on the test set, as the engine's forward runs it."""
+        net.eval()
+        tl, a1, a5, nbt, cnt = 0.0, 0.0, 0.0, 0, 0
+        with torch.no_grad():
+            for i, (dx, dy) in enumerate(test_loader):
+                if args.eval_batches and i >= args.eval_batches:
+                    break
+                dx, dy = dx.to(dev), dy.to(dev)
+                if kind == "shadow":
+                    dx = dx.contiguous(memory_format=torch.channels_last)
+                    with torch.autocast("cuda", dtype=torch.bfloat16):
+                        out = net(dx).float()
+                else:
+                    out = net(dx)
+                tl += F.cross_entropy(out, dy, reduction="sum").item()
+                b1, b5 = accuracy(out, dy, (1, 5))
+                a1 += b1.item(); a5 += b5.item(); nbt += 1; cnt += len(dy)
+        return tl / max(cnt, 1), a1 / max(nbt, 1), a5 / max(nbt, 1)
+
+    # --ema-decay: one evaluation copy of the model, loaded with the averaged weights at every evaluation
+    ema_on = bool(getattr(args, "ema_decay", 0.0))
+    ema_model = None
+
     while eng.step <= args.max_steps:
         x, y = loader.next_batch()
         stats = eng.train_step(x, y)
@@ -247,25 +281,16 @@ def run_p2p_training(args, device=None):
             # every rank calls it: a rank that TRAINS writes the evaluator's file (real BN running statistics; the
             # reference's PS checkpoints carry untrained ones, SURVEY 2.9), the PS side writes the optimizer sidecar
             eng.save_checkpoint(args.train_dir, cur)
+            ema_sd = eng.ema_state_dict() if ema_on else None       # collective
             if eng.is_worker and rank == first:
-                eng.model.eval()
-                tl, a1, a5, nbt, cnt = 0.0, 0.0, 0.0, 0, 0
-                with torch.no_grad():
-                    for i, (dx, dy) in enumerate(test_loader):
-                        if args.eval_batches and i >= args.eval_batches:
-                            break
-                        dx, dy = dx.to(dev), dy.to(dev)
-                        if kind == "shadow":
-                            dx = dx.contiguous(memory_format=torch.channels_last)
-                            with torch.autocast("cuda", dtype=torch.bfloat16):
-                                out = eng.model(dx).float()
-                        else:
-                            out = eng.model(dx)
-                        tl += F.cross_entropy(out, dy, reduction="sum").item()
-                        b1, b5 = accuracy(out, dy, (1, 5))
-                        a1 += b1.item(); a5 += b5.item(); nbt += 1; cnt += len(dy)
-                print(test_line(cur, tl / max(cnt, 1), a1 / max(nbt, 1), a5 / max(nbt, 1)))
+                print(test_line(cur, *evaluate(eng.model)))
                 eng.model.train()
+                if ema_sd is not None:
+                    if ema_model is None:
+                        ema_model = build_model(args.network, num_classes, args.dataset).to(dev)
+                        ema_model = ema_model.to(memory_format=torch.channels_last)
+                    ema_model.load_state_dict(ema_sd)
+                    print(ema_test_line(cur, *evaluate(ema_model)))
             collective_barrier()
         if (eng.step - 1) % freq == 0:          # shrinkage (master:232-234), actually applied to the optimizer
             eng.set_lr(base_lr * args.lr_shrinkage ** ((eng.step - 1) // freq))

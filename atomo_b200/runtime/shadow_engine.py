@@ -76,6 +76,12 @@ one central PS kernel at the end of the step):
   runs its gather instantiation per group (mean gradient and sum g^2 per tile, nothing stepped), then one launch per
   owner after the final group (``csrc/v2_clip.cu``) takes the whole-model norm across tiles and owners and steps every
   tile of the owner on ``coef * g`` (LARS / LAMB: their phase 2 follows per group).  ``grad_norm()`` reports it.
+* Exponential moving average of the weights (``ema_decay=d``, ``0 < d < 1``): every owner keeps an fp32 average of
+  every value it holds, ``ema`` indexed like ``master`` and ``vema`` like ``vparams``, starting at the initial
+  weights.  Per group, one launch on the PS stream right after the launch that writes the group's final master values
+  (``csrc/v2_ema.cu``; with clipping that is the end of the step) forms ``e <- e + w (p - e)`` with ``w = fp32(1 - d)``,
+  each operation rounded to fp32.  ``ema_state_dict()`` gathers the averaged model; BN running statistics are not
+  averaged: it carries the live ones.  Checkpoints add ``model_step_<N>_ema``.
 
 Per step and rank: ``wait_params`` -> forward -> backward [group hooks -> encode, project+push on stream E;
 PS launch of the group on stream P] -> join -> ``advance_step``.  All cross-GPU ordering is carried by
@@ -97,7 +103,7 @@ import torch.nn as nn
 from ..ops import plan2 as P2
 from ..ops._ext import load as load_ext
 from ..parallel.symm import SymmetricHeap
-from ..utils.flags import check_clip_grad_norm
+from ..utils.flags import check_clip_grad_norm, check_ema_decay
 
 SIGNAL_INTS = 1024
 
@@ -119,7 +125,7 @@ class ShadowEngine:
                  side_priority: int = -1, resample_empty: bool = False, quantization_level: int = 4,
                  bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False,
                  error_feedback: bool = False, accumulate_steps: int = 1, trust_coefficient: float = 0.001,
-                 clip_grad_norm: float = 0.0, momentum_correction: bool = False):
+                 clip_grad_norm: float = 0.0, momentum_correction: bool = False, ema_decay: float = 0.0):
         self.optimizer = optimizer.lower()
         if self.optimizer not in ("sgd", "adam", "lars", "lamb"):      # checked before any CUDA work
             raise ValueError("ShadowEngine optimizers: sgd | adam | lars | lamb (got %r)" % (optimizer,))
@@ -136,6 +142,8 @@ class ShadowEngine:
             raise ValueError("accumulate_steps must be an integer >= 1 (got %r)" % (accumulate_steps,))
         self.clip_grad_norm = check_clip_grad_norm(clip_grad_norm)      # checked before any CUDA work
         self.clip_on = self.clip_grad_norm > 0
+        self.ema_decay = check_ema_decay(ema_decay)      # checked before any CUDA work
+        self.ema_w = float(np.float32(1.0 - self.ema_decay))    # the average's step weight, rounded once
         self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
         if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign", "powersgd", "fp8",
                              "hadamard"):
@@ -358,6 +366,11 @@ class ShadowEngine:
             self.sqmax, self.vsqmax = (z(pl.w_total), z(pl.v_total)) if self.opt == P2.OPT_AMSGRAD else (None, None)
         else:
             self.master = None
+        # exponential moving average of the weights (csrc/v2_ema.cu): the owner's fp32 average of master and vparams,
+        # starting at the initial weights every rank now holds
+        self.ema = self.vema = None
+        if self.ema_decay and self.is_owner:
+            self.ema, self.vema = self.master.clone(), self.vparams.clone()
 
         # ---- device tables ---------------------------------------------------------------------------------
         self.t_units = _dev_bytes(pl.units_bytes(), dev)
@@ -849,15 +862,19 @@ class ShadowEngine:
         self._nlaunch += 1
 
     def _launch_ps(self, g: int, final: bool):
-        C, pl = self.C, self.plan
-        t0, nt = pl.ps_range[g][self.owner_index]
-        p = lambda t: t.data_ptr() if t is not None else 0
+        t0, nt = self.plan.ps_range[g][self.owner_index]
         if self.clip_on:
             self._launch_ps_clip(g, final, t0, nt)
-            return
-        if self.layerwise:
+        elif self.layerwise:
             self._launch_ps_layerwise(g, final, t0, nt)
-            return
+        else:
+            self._launch_ps_code(g, final, t0, nt)
+            self._launch_ema(g)
+
+    def _launch_ps_code(self, g: int, final: bool, t0: int, nt: int):
+        """The code's PS kernel for group ``g``: decode, optimizer step, broadcast of the new parameters."""
+        C, pl = self.C, self.plan
+        p = lambda t: t.data_ptr() if t is not None else 0
         if self.quant:
             C.v2_ps_qsgd(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g, final,
                          self.owner_index, p(self.master), p(self.mom), p(self.sq), p(self.sqmax), p(self.vmom),
@@ -945,6 +962,18 @@ class ShadowEngine:
                        self.lw_counter.data_ptr() + 4 * g, self.timeout_ticks, self.tstats.data_ptr(),
                        self.lw_ratio.data_ptr() + 4 * sum(self.lw_layers[:g]), max(1, min(self.ps_grid, max(nt, 1))))
         self._nlaunch += 1
+        self._launch_ema(g)
+
+    def _launch_ema(self, g: int):
+        """The average of group ``g`` (``ema_decay``, csrc/v2_ema.cu): ``e <- e + w (p - e)`` over this owner's PS tiles
+        of the group, on the stream of the launch that wrote their final master values, right after it."""
+        t0, nt = self.plan.ps_range[g][self.owner_index]
+        if self.ema is None or nt == 0:
+            return
+        self.C.v2_ema(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.master.data_ptr(),
+                      self.vparams.data_ptr(), self.ema.data_ptr(), self.vema.data_ptr(), self.ema_w,
+                      max(1, min(self.ps_grid, nt)))
+        self._nlaunch += 1
 
     def _ps_kind(self) -> int:
         """The PS kernel of the code, as the phase-1 launches (v2_ps_layerwise, v2_ps_gather) select it."""
@@ -979,9 +1008,11 @@ class ShadowEngine:
                   self.clip_counter.data_ptr(), self.timeout_ticks, self.tstats.data_ptr(), self.clip_norm.data_ptr(),
                   max(1, min(self.ps_grid, max(n, 1))))
         self._nlaunch += 1
-        if self.layerwise:
-            for gg in range(self.G):
+        for gg in range(self.G):
+            if self.layerwise:
                 self._launch_layerwise(gg, gg == self.G - 1)
+            else:
+                self._launch_ema(gg)
 
     def grad_norm(self) -> tuple:
         """Gradient-norm clipping: ``(total, coef)`` of the last step, the whole-model norm of the mean gradient the
@@ -1227,12 +1258,14 @@ class ShadowEngine:
         return mw, mv
 
     def gather_fp32(self, what: str = "master") -> torch.Tensor:
-        """Full fp32 array (weight indexing) assembled from the owners' shards: 'master' | 'mom' | 'sq' | 'sqmax'."""
+        """Full fp32 array assembled from the owners' shards: 'master' | 'mom' | 'sq' | 'sqmax' | 'ema' (weight
+        indexing) or 'vema' (vector indexing, ``vparams``')."""
         src = {"master": self.master, "mom": getattr(self, "mom", None), "sq": getattr(self, "sq", None),
-               "sqmax": getattr(self, "sqmax", None)}[what]
+               "sqmax": getattr(self, "sqmax", None), "ema": self.ema, "vema": self.vema}[what]
         torch.cuda.synchronize(self.device)
-        mw, _ = self._owned_mask()
-        out = (src * mw) if (self.is_owner and src is not None) else torch.zeros_like(mw)
+        mw, mv = self._owned_mask()
+        m = mv if what == "vema" else mw
+        out = (src * m) if (self.is_owner and src is not None) else torch.zeros_like(m)
         if self.world > 1:
             dist.all_reduce(out, group=self.group)
         return out
@@ -1241,7 +1274,19 @@ class ShadowEngine:
         """state_dict in the standard (OIHW, fp32) layout — the evaluator's ``model_step_<N>`` contract.  Weights
         come from the fp32 master copies on the owners; BN running statistics from THIS rank's model (call it on
         a rank that trains: the reference's PS checkpoints carried untrained BN statistics, SURVEY 2.9)."""
-        full = self.gather_fp32("master")
+        return self._state_dict(self.gather_fp32("master"))
+
+    def ema_state_dict(self) -> dict:
+        """Collective.  The averaged model (``ema_decay``) in the layout of :meth:`fp32_state_dict`: weights and BN /
+        bias vectors from the owners' fp32 averages, BN running statistics from THIS rank's live model (they are not
+        averaged, as ``torch.optim.swa_utils.AveragedModel(use_buffers=False)``)."""
+        if not self.ema_decay:
+            raise RuntimeError("ema_state_dict() needs ShadowEngine(..., ema_decay=d) with 0 < d < 1")
+        return self._state_dict(self.gather_fp32("ema"), self.gather_fp32("vema"))
+
+    def _state_dict(self, full: torch.Tensor, vfull: Optional[torch.Tensor] = None) -> dict:
+        """This rank's model state_dict (fp32) with the weights taken from ``full`` (weight indexing, physical order)
+        and, when given, the vectors from ``vfull`` (``vparams``' indexing)."""
         sd = {}
         byid = {id(p): q for p, q in zip(self.params, self.plan.params)}
         for name, t in self.model.state_dict().items():
@@ -1255,12 +1300,15 @@ class ShadowEngine:
                     sd[name] = flat.view(o, kh, kw, i).permute(0, 3, 1, 2).contiguous()
                 else:
                     sd[name] = flat.view(q.shape).clone()
+            elif vfull is not None:
+                sd[name] = vfull[q.off:q.off + q.numel].view(q.shape).clone()
         return sd
 
     def save_checkpoint(self, train_dir: str, step: Optional[int] = None) -> Optional[str]:
         """Collective.  Every training rank ``R`` writes ``model_step_<N>_worker<R>`` (its own state, below); after a
-        barrier the first training rank writes ``model_step_<N>`` (fp32, trained BN statistics) and the ``_optim``
-        sidecar.  So when the model file exists, its worker files exist too.  After ``load_checkpoint`` on the same
+        barrier the first training rank writes ``model_step_<N>`` (fp32, trained BN statistics), the ``_optim``
+        sidecar and, with ``ema_decay``, ``model_step_<N>_ema`` (:meth:`ema_state_dict`, the evaluator's layout).  So
+        when the model file exists, its worker files exist too.  After ``load_checkpoint`` on the same
         configuration, training continues bit for bit as if it had never stopped.
 
         Every device buffer the engine keeps across steps is in one of these classes:
@@ -1268,7 +1316,7 @@ class ShadowEngine:
         (a) owner state and BN buffers, in ``model_step_<N>`` / ``_optim``: ``master`` (``wshadow`` is rebuilt from
             it as ``bf16(master)``, what the PS epilogue publishes), ``vparams``, ``mom`` / ``vmom``, for Adam
             ``sq`` / ``vsq`` and for AMSGrad ``sqmax`` / ``vsqmax``, the BN running statistics, and the step and LR
-            of ``ctrl``.
+            of ``ctrl``; with ``ema_decay`` the averages ``ema`` / ``vema``, in ``model_step_<N>_ema``.
         (b) per-worker state, in ``model_step_<N>_worker<R>`` (:meth:`_worker_tensors`, physical order):
             ``residual`` (``error_feedback``, fp32 per weight element); ``mom`` / ``vmom_w``
             (``momentum_correction``, the worker's fp32 momentum per weight / vector element); ``vprev`` (svd / qsvd with ``warm_start``,
@@ -1291,6 +1339,7 @@ class ShadowEngine:
         from ..utils import checkpoint as ckpt
         step = (self.step - 1) if step is None else step
         sd = self.fp32_state_dict()
+        ema_sd = self.ema_state_dict() if self.ema_decay else None
         mom = self.gather_fp32("mom")
         vmom = self.vmom if self.is_owner else torch.zeros_like(self.vparams)
         _, mv = self._owned_mask()
@@ -1317,6 +1366,9 @@ class ShadowEngine:
         tmp = path + ".tmp"
         torch.save({k: v.cpu() for k, v in sd.items()}, tmp)
         os.replace(tmp, path)
+        if ema_sd is not None:
+            torch.save({k: v.cpu() for k, v in ema_sd.items()}, path + "_ema.tmp")
+            os.replace(path + "_ema.tmp", path + "_ema")
         side = {"step": step, "lr": self.lr, "mom_w": mom.cpu(), "mom_v": vm.cpu(), "code": self.code,
                 "svd_rank": self.svd_rank, "engine": "shadow", "optimizer": self.optimizer}
         if self.quant or self.hadamard:
@@ -1384,7 +1436,9 @@ class ShadowEngine:
 
     def load_checkpoint(self, train_dir: str, step: int) -> None:
         """Collective: every rank reads the same files (shared directory) and jumps to ``step + 1``.  Each training
-        rank also restores its own worker file (:meth:`_load_worker_state`)."""
+        rank also restores its own worker file (:meth:`_load_worker_state`).  With ``ema_decay`` the owners restore
+        the average from ``model_step_<N>_ema``; without that file it starts at the loaded weights (one line says
+        so).  Without ``ema_decay`` the file is ignored."""
         from ..utils import checkpoint as ckpt
         self._barrier()
         path = ckpt.model_path(train_dir, step)
@@ -1428,6 +1482,8 @@ class ShadowEngine:
                         getattr(self, vname).copy_(side[vname[1:] + "_v"].to(self.device))
                 if side.get("lr") is not None:
                     self.set_lr(float(side["lr"]))
+            if self.ema_decay:
+                self._load_ema(path + "_ema", byname, byid)
             if self.is_worker:
                 self._load_worker_state(train_dir, step)
         self.step = step + 1
@@ -1435,6 +1491,28 @@ class ShadowEngine:
         self._barrier()
         self.signals[256:256 + self.n_owners] = self.step
         self._barrier()
+
+    def _load_ema(self, path: str, byname: dict, byid: dict) -> None:
+        """The owners' averages from ``path`` (weights permuted to the physical order, as ``master``), or from the
+        loaded master and vectors when the file is missing."""
+        if not os.path.exists(path):
+            if self.is_owner:
+                self.ema.copy_(self.master)
+                self.vema.copy_(self.vparams)
+            if self.rank == self.first_worker:
+                print("%s missing: the weight average starts at the loaded weights" % path, flush=True)
+            return
+        if not self.is_owner:
+            return
+        for name, t in torch.load(path, map_location="cpu", weights_only=False).items():
+            if name in byname:
+                q = byid[id(byname[name])]
+                src = t.to(self.device, torch.float32)
+                if q.is_w:
+                    phys = src.permute(0, 2, 3, 1).contiguous().reshape(-1) if src.dim() == 4 else src.reshape(-1)
+                    self.ema[q.off:q.off + q.numel].copy_(phys)
+                else:
+                    self.vema[q.off:q.off + q.numel].copy_(src.reshape(-1))
 
     def close(self):
         torch.cuda.synchronize(self.device)

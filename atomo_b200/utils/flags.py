@@ -77,6 +77,12 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                    help="clip the averaged gradient to this whole-model L2 norm before the optimizer, as "
                         "torch.nn.utils.clip_grad_norm_ (0 = off); p2p backend on the bf16 engine (--engine shadow), or "
                         "the gloo / nccl role path")
+    p.add_argument("--ema-decay", type=float, default=0.0,
+                   help="keep an exponential moving average of the weights, e <- e + (1 - D) (p - e) after every "
+                        "optimizer step, in fp32 on the parameter server (0 = off, else 0 < D < 1).  Checkpoints add "
+                        "model_step_<N>_ema and every --eval-freq evaluation also tests the averaged model, with the "
+                        "live BN running statistics; p2p backend on the bf16 engine (--engine shadow), or the gloo / "
+                        "nccl role path")
     p.add_argument("--weight-decay", type=float, default=0.0)
     p.add_argument("--nesterov", type=bool_flag, default=False)
     p.add_argument("--resume", type=bool_flag, default=False)
@@ -136,4 +142,11 @@ def check_clip_grad_norm(value) -> float:
     """--clip-grad-norm / clip_grad_norm=: 0 (off) or a finite positive norm; anything else raises ValueError."""
     if isinstance(value, bool) or not isinstance(value, numbers.Real) or not (value == 0 or 0 < value < math.inf):
         raise ValueError("clip_grad_norm must be 0 (off) or a finite norm > 0 (got %r)" % (value,))
+    return float(value)
+
+
+def check_ema_decay(value) -> float:
+    """--ema-decay / ema_decay=: 0 (off) or a finite decay with 0 < d < 1; anything else raises ValueError."""
+    if isinstance(value, bool) or not isinstance(value, numbers.Real) or not (value == 0 or 0 < value < 1):
+        raise ValueError("ema_decay must be 0 (off) or a decay with 0 < d < 1 (got %r)" % (value,))
     return float(value)

@@ -7,6 +7,7 @@ WORKER_FMT = ("Worker: {}, Step: {}, Epoch: {} [{}/{} ({:.0f}%)], Loss: {:.4f}, 
               "Comp: {:.4f}, Encode: {: .4f}, Comm: {: .4f}, Msg(MB): {: .4f}, Prec@1: {: .4f}, Prec@5: {: .4f}")
 MASTER_FMT = "Master: Step: {}, Decode Cost: {}, Cur lr {}, Gather: {}"
 TEST_FMT = "Test set: Step: {}, Average loss: {:.4f}, Prec@1: {} Prec@5: {}"
+EMA_TEST_FMT = "Test set (EMA): Step: {}, Average loss: {:.4f}, Prec@1: {} Prec@5: {}"   # the weight average
 
 
 def worker_line(rank, step, epoch, seen, total, loss, time_cost, comp, encode, comm, msg_mb, prec1, prec5):
@@ -21,6 +22,10 @@ def master_line(step, decode_cost, lr, gather):
 
 def test_line(step, loss, prec1, prec5):
     return TEST_FMT.format(step, loss, prec1, prec5)
+
+
+def ema_test_line(step, loss, prec1, prec5):
+    return EMA_TEST_FMT.format(step, loss, prec1, prec5)
 
 
 class MetricsWriter:
