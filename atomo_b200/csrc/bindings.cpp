@@ -271,6 +271,9 @@ void atomo_v2_launch_bcast_bytes(const void* src, void* const* peer, void* mc, i
 // v2_ema.cu (exponential moving average of the weights on the bf16 engine)
 void atomo_v2_launch_ema(const void* units, const void* tiles, int tile0, int ntiles, const float* master,
                          const float* vparams, float* ema, float* vema, float w, int grid, cudaStream_t stream);
+// v2_ema.cu (AdamW's decoupled weight decay on the bf16 engine)
+void atomo_v2_launch_decay(const void* units, const void* tiles, int tile0, int ntiles, float* master,
+                           const void* ctrl, int grid, cudaStream_t stream);
 // gemm_kernels.cu
 int atomo_gemm_tile_bytes();
 int atomo_gemm_smem_bytes();
@@ -1022,6 +1025,17 @@ void v2_ema(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t mast
                       P<const float>(vparams), P<float>(ema), P<float>(vema), w, grid, cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
+// AdamW's decoupled weight decay: master <- master * Ctrl2::decay_factor over the weight elements of the PS tiles
+// [tile0, tile0 + ntiles) of one group and owner (vector tiles untouched); on the PS stream, before the launch that
+// steps those tiles
+void v2_decay(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t master, uint64_t ctrl, int grid) {
+  TORCH_CHECK(ntiles >= 0 && tile0 >= 0, "v2_decay: bad tile range");
+  TORCH_CHECK(ntiles == 0 || (units != 0 && tiles != 0 && master != 0 && ctrl != 0),
+              "v2_decay: units / tiles / master / ctrl required");
+  atomo_v2_launch_decay(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<float>(master),
+                        P<const void>(ctrl), grid, cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
 void v2_accum_fold(uint64_t wchunks, int nw, uint64_t vchunks, int nv, uint64_t gptr, uint64_t acc, uint64_t vacc,
                    uint64_t vgrads, float inv_n, uint64_t residual) {
   TORCH_CHECK(nw >= 0 && nv >= 0, "v2_accum_fold: negative chunk count");
@@ -1226,6 +1240,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("v2_ps_gather", &v2_ps_gather);
   m.def("v2_clip", &v2_clip);
   m.def("v2_ema", &v2_ema);
+  m.def("v2_decay", &v2_decay);
   m.def("v2_ps_entry", &v2_ps_entry);
   m.def("v2_code_stats", &v2_code_stats);
   m.def("v2_stats_fields", &atomo_v2_stats_fields);

@@ -85,7 +85,7 @@ struct Ctrl2 {
   int opt;
   int num_aggregate;   // 0 = wait for every worker; N = proceed after N pushes (backup workers)
   float trust_coefficient;   // LARS: eta of the trust ratio (v2_layerwise.cu)
-  int pad2;
+  float decay_factor;   // AdamW: fp32(1 - lr wd), the decoupled decay of master (v2_ema.cu v2_decay_kernel); 0 = unused
 };
 static_assert(sizeof(Ctrl2) == 72, "Ctrl2 layout must match ops/plan2.py CTRL2_FMT");
 

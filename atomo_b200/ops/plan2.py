@@ -81,7 +81,7 @@ UNIT_FMT = "<4q20i"           # 112 bytes, mirrors struct Unit2
 TILE_FMT = "<4i"              # unit, a, b, owner
 UNIT_BYTES = struct.calcsize(UNIT_FMT)
 TILE_BYTES = struct.calcsize(TILE_FMT)
-CTRL2_FMT = "<iiffffiiQffffiifi"   # mirrors struct Ctrl2 (72 bytes)
+CTRL2_FMT = "<iiffffiiQffffiiff"   # mirrors struct Ctrl2 (72 bytes); the last word is decay_factor (AdamW)
 CTRL2_BYTES = struct.calcsize(CTRL2_FMT)
 
 
@@ -778,10 +778,13 @@ LAYERWISE_OPTS = (OPT_LARS, OPT_LAMB)
 def pack_ctrl2(step: int = 1, lr: float = 0.01, momentum: float = 0.0, dampening: float = 0.0,
                weight_decay: float = 0.0, nesterov: bool = False, first_step: int = 1, seed: int = 1,
                beta1: float = 0.9, beta2: float = 0.999, eps: float = 1e-8, opt: int = OPT_SGD,
-               num_aggregate: int = 0, trust_coefficient: float = 0.0, clip_grad_norm: float = 0.0) -> bytes:
+               num_aggregate: int = 0, trust_coefficient: float = 0.0, clip_grad_norm: float = 0.0,
+               decay_factor: float = 0.0) -> bytes:
+    """Ctrl2's bytes.  ``decay_factor`` (offset 68) is AdamW's fp32(1 - lr wd), which only the decoupled-decay pass
+    reads (csrc/v2_ema.cu); 0 when that pass does not run."""
     return struct.pack(CTRL2_FMT, step, 0, lr, momentum, dampening, weight_decay, int(nesterov), first_step,
                        seed & 0xFFFFFFFFFFFFFFFF, beta1, beta2, eps, float(clip_grad_norm), int(opt), int(num_aggregate),
-                       float(trust_coefficient), 0)
+                       float(trust_coefficient), float(decay_factor))
 
 
 def layerwise_tables(plan: "Plan2") -> Tuple[List[int], List[int]]:

@@ -22,7 +22,7 @@ import torch
 
 from .. import codings
 from ..models import build_model
-from ..optim import LAMB, LARS, SGD, Adam
+from ..optim import LAMB, LARS, SGD, Adam, AdamW
 from ..parallel.transport import Transport, STOP_STEP
 from ..utils import checkpoint as ckpt
 from ..utils.flags import check_clip_grad_norm, check_ema_decay
@@ -156,6 +156,9 @@ class SyncReplicasMaster_NN(NN_Trainer):
                                   weight_decay=self._kwargs.get("weight_decay", 0.0),
                                   trust_coefficient=self._kwargs.get("trust_coefficient", 0.001),
                                   nesterov=self._kwargs.get("nesterov", False))
+        elif self._optimizer_name == "adamw":
+            self.optimizer = AdamW(self.network.parameters(), lr=self.lr,
+                                   weight_decay=self._kwargs.get("weight_decay", 0.0))
         elif self._optimizer_name == "lamb":
             self.optimizer = LAMB(self.network.parameters(), lr=self.lr,
                                   weight_decay=self._kwargs.get("weight_decay", 0.0))

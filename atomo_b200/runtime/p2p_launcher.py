@@ -120,6 +120,9 @@ def _build_engine(args, model, rank, world):
     if args.optimizer in ("lars", "lamb"):
         raise SystemExit("--optimizer %s runs on the bf16 engine (--engine shadow, --dtype bf16); the fp32-flat engine "
                          "has no layer-wise trust ratio" % args.optimizer)
+    if args.optimizer == "adamw":
+        raise SystemExit("--optimizer adamw runs on the bf16 engine (--engine shadow, --dtype bf16); the fp32-flat "
+                         "engine fuses momentum-SGD only and has no decoupled weight decay")
     from .engine import FusedEngine
     if accum != 1:
         raise SystemExit("--accumulate-steps runs on the bf16 engine (--dtype bf16, --engine auto|shadow, --code "

@@ -82,6 +82,12 @@ one central PS kernel at the end of the step):
   (``csrc/v2_ema.cu``; with clipping that is the end of the step) forms ``e <- e + w (p - e)`` with ``w = fp32(1 - d)``,
   each operation rounded to fp32.  ``ema_state_dict()`` gathers the averaged model; BN running statistics are not
   averaged: it carries the live ones.  Checkpoints add ``model_step_<N>_ema``.
+* AdamW (``optimizer="adamw"``, ``torch.optim.AdamW`` with two parameter groups): per group, one launch on the PS
+  stream right before the launch that steps the group's tiles (the PS launch; with clipping, the clip launch) scales
+  the owner's weight elements of ``master`` by ``f = fp32(1 - lr * wd)`` (``csrc/v2_ema.cu``), read from
+  ``Ctrl2.decay_factor``, which ``set_lr`` rewrites.  The PS kernels then run Adam (AMSGrad with ``amsgrad=True``)
+  with weight decay 0.  1-D parameters (BN, biases) take no decay.  With ``weight_decay=0`` it is ``adam``, bit for
+  bit, and launches nothing new.
 
 Per step and rank: ``wait_params`` -> forward -> backward [group hooks -> encode, project+push on stream E;
 PS launch of the group on stream P] -> join -> ``advance_step``.  All cross-GPU ordering is carried by
@@ -127,8 +133,16 @@ class ShadowEngine:
                  error_feedback: bool = False, accumulate_steps: int = 1, trust_coefficient: float = 0.001,
                  clip_grad_norm: float = 0.0, momentum_correction: bool = False, ema_decay: float = 0.0):
         self.optimizer = optimizer.lower()
-        if self.optimizer not in ("sgd", "adam", "lars", "lamb"):      # checked before any CUDA work
-            raise ValueError("ShadowEngine optimizers: sgd | adam | lars | lamb (got %r)" % (optimizer,))
+        if self.optimizer not in ("sgd", "adam", "adamw", "lars", "lamb"):      # checked before any CUDA work
+            raise ValueError("ShadowEngine optimizers: sgd | adam | adamw | lars | lamb (got %r)" % (optimizer,))
+        # AdamW: the PS kernels run Adam with weight_decay 0; the decoupled decay of the weights is its own pass
+        self.adamw_wd = 0.0
+        if self.optimizer == "adamw":      # checked before any CUDA work
+            if isinstance(weight_decay, bool) or not isinstance(weight_decay, numbers.Real) \
+                    or not 0 <= weight_decay < math.inf:
+                raise ValueError("adamw: weight_decay must be finite and >= 0 (got %r)" % (weight_decay,))
+            self.adamw_wd, weight_decay = float(weight_decay), 0.0
+        self.decay_on = self.adamw_wd > 0     # with weight_decay 0 AdamW is Adam: nothing new is launched
         self.layerwise = self.optimizer in ("lars", "lamb")
         if self.optimizer == "lars" and (nesterov or dampening != 0):
             raise ValueError("lars takes plain momentum: nesterov=False and dampening=0")
@@ -261,7 +275,8 @@ class ShadowEngine:
         self.criterion = criterion or nn.CrossEntropyLoss()
         self.timeout_ticks = int(timeout_s * 1.5e9)
         self.step, self.lr = 1, lr
-        self.opt = {"sgd": P2.OPT_SGD, "adam": P2.OPT_AMSGRAD if amsgrad else P2.OPT_ADAM, "lars": P2.OPT_LARS,
+        adam_opt = P2.OPT_AMSGRAD if amsgrad else P2.OPT_ADAM
+        self.opt = {"sgd": P2.OPT_SGD, "adam": adam_opt, "adamw": adam_opt, "lars": P2.OPT_LARS,
                     "lamb": P2.OPT_LAMB}[self.optimizer]
         self.launches_per_step = 0
 
@@ -428,7 +443,8 @@ class ShadowEngine:
                                              beta1=betas[0], beta2=betas[1], eps=eps, opt=self.opt,
                                              num_aggregate=num_aggregate,
                                              trust_coefficient=self.trust_coefficient if self.layerwise else 0.0,
-                                             clip_grad_norm=self.clip_grad_norm), dev)
+                                             clip_grad_norm=self.clip_grad_norm,
+                                             decay_factor=self.decay_factor(lr) if self.decay_on else 0.0), dev)
         self.ctrl_i32, self.ctrl_f32 = self.ctrl.view(torch.int32), self.ctrl.view(torch.float32)
         n_w = max(len(self.w_params), 1)
         self.t_gptr = torch.zeros(n_w, dtype=torch.int64, device=dev)
@@ -578,6 +594,13 @@ class ShadowEngine:
     def set_lr(self, lr: float):
         self.lr = lr
         self.ctrl_f32[2] = lr
+        if self.decay_on:
+            self.ctrl_f32[17] = self.decay_factor(lr)      # Ctrl2::decay_factor, read by every decay launch
+
+    def decay_factor(self, lr: float) -> float:
+        """AdamW: the factor of the decoupled weight decay at learning rate ``lr``, ``1 - lr * wd`` in double (as
+        torch.optim.AdamW computes it in Python) rounded to fp32 once."""
+        return float(np.float32(1.0 - float(lr) * self.adamw_wd))
 
     def error_code(self) -> int:
         return int(self.ctrl_i32[1].item())
@@ -868,6 +891,7 @@ class ShadowEngine:
         elif self.layerwise:
             self._launch_ps_layerwise(g, final, t0, nt)
         else:
+            self._launch_decay(g)
             self._launch_ps_code(g, final, t0, nt)
             self._launch_ema(g)
 
@@ -964,6 +988,17 @@ class ShadowEngine:
         self._nlaunch += 1
         self._launch_ema(g)
 
+    def _launch_decay(self, g: int):
+        """AdamW's decoupled weight decay of group ``g`` (csrc/v2_ema.cu): ``p <- p * f`` over the weight elements of
+        this owner's PS tiles of the group, ``f`` from ``Ctrl2.decay_factor``, on the stream of the launch that steps
+        those tiles, right before it."""
+        t0, nt = self.plan.ps_range[g][self.owner_index]
+        if not self.decay_on or nt == 0:
+            return
+        self.C.v2_decay(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.master.data_ptr(),
+                        self.ctrl.data_ptr(), max(1, min(self.ps_grid, nt)))
+        self._nlaunch += 1
+
     def _launch_ema(self, g: int):
         """The average of group ``g`` (``ema_decay``, csrc/v2_ema.cu): ``e <- e + w (p - e)`` over this owner's PS tiles
         of the group, on the stream of the launch that wrote their final master values, right after it."""
@@ -997,6 +1032,8 @@ class ShadowEngine:
         self._nlaunch += 1
         if not final:
             return
+        for gg in range(self.G):        # AdamW: every group's decay before the clip launch steps its tiles
+            self._launch_decay(gg)
         n = len(self.clip_tiles)
         C.v2_clip(self.layerwise, self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), self.t_clip_tiles.data_ptr(), n,
                   self.clip_part.data_ptr(), self.clip_grad.data_ptr(), self.clip_vgrad.data_ptr(), self.world,

@@ -68,9 +68,11 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                    "elements below 1, else an atom count (top-k sends floor of it)")
     p.add_argument("--sampling", type=str, default="bernoulli", choices=["bernoulli", "systematic"])
     p.add_argument("--prob-rule", type=str, default="reference", choices=["reference", "waterfill"])
-    p.add_argument("--optimizer", type=str, default="sgd", choices=["sgd", "adam", "lars", "lamb"],
+    p.add_argument("--optimizer", type=str, default="sgd", choices=["sgd", "adam", "adamw", "lars", "lamb"],
                    help="lars / lamb: layer-wise trust ratios (LARS on momentum-SGD, LAMB on Adam) for large batches; "
-                        "p2p backend on the bf16 engine (--engine shadow), or the gloo / nccl role path")
+                        "adamw: Adam with decoupled weight decay (torch.optim.AdamW), every weight (2 or more "
+                        "dimensions) scaled by 1 - lr * --weight-decay before the Adam step, BN / bias vectors not "
+                        "decayed; p2p backend on the bf16 engine (--engine shadow), or the gloo / nccl role path")
     p.add_argument("--trust-coefficient", type=float, default=0.001,
                    help="--optimizer lars: eta of the trust ratio eta ||w|| / (||g|| + wd ||w||)")
     p.add_argument("--clip-grad-norm", type=float, default=0.0,
