@@ -157,6 +157,21 @@ void atomo_v2_launch_sign_code_stats(const void* units, const void* tiles, int t
                                      const long long* gptr, float* const* arena_peer, int n_owners,
                                      long long arena_floats, int worker, double* partials, unsigned int* unit_counters,
                                      double* acc, cudaStream_t stream);
+// v2_signum.cu (Signum with majority vote on the bf16 engine)
+void atomo_v2_launch_signum_encode(const void* units, const void* tiles, int tile0, int ntiles, const long long* gptr,
+                                   const void* vchunks, int nv, float* vgrads, float* mom, float* vmom, float beta,
+                                   float* const* arena_peer, int* const* sig_peer, int n_owners,
+                                   long long arena_floats, int worker, int group, const void* ctrl,
+                                   unsigned int* group_counter, long long* tstats, int final_group,
+                                   const float* ext_uniforms, cudaStream_t stream);
+void atomo_v2_launch_ps_signum(const void* units, const void* tiles, int tile0, int ntiles, int W, int nranks,
+                               int group, int final_group, int owner, float* master, float* mom, float* sq,
+                               float* sqmax, float* vmom, float* vsq, float* vsqmax, void* wshadow_mc,
+                               void* const* wshadow_peer, float* vparams_local, float* vparams_mc,
+                               float* const* vparams_peer, const float* vgrads_mc, const float* const* vgrads_peer,
+                               const float* arenas, long long arena_floats, int* sig, int* const* sig_peer, void* ctrl,
+                               unsigned int* group_counter, long long timeout, long long* tstats, float inv_w, int grid,
+                               const float* vext, long long vext_stride, cudaStream_t stream);
 // v2_fp8.cu (fp8 units of the bf16 engine)
 void atomo_v2_launch_fp8_encode(const void* units, const void* tiles, int tile0, int ntiles, const long long* gptr,
                                 float* const* arena_peer, int* const* sig_peer, int n_owners, long long arena_floats,
@@ -756,6 +771,48 @@ void v2_ps_sign(uint64_t units, uint64_t tiles, int tile0, int ntiles, int W, in
                           cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
+// Signum: worker momentum, sign bits and the push of one group's weight tiles, plus its vector chunks' momentum (the
+// encode is the group's only launch; it raises the push flag).  mom == 0 (beta == 0): the sign of the gradient itself,
+// and no vector chunks.
+void v2_signum_encode(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t vchunks, int nv,
+                      uint64_t vgrads, uint64_t mom, uint64_t vmom, double beta, uint64_t arena_peer, uint64_t sig_peer,
+                      int n_owners, int64_t arena_floats, int worker, int group, uint64_t ctrl, uint64_t group_counter,
+                      uint64_t tstats, bool final_group, uint64_t ext_uniforms) {
+  TORCH_CHECK(worker >= 0 && worker < 16, "v2_signum_encode: worker index must be in [0, 16)");
+  TORCH_CHECK(ntiles >= 0 && nv >= 0 && tile0 >= 0, "v2_signum_encode: bad tile / chunk range");
+  TORCH_CHECK(beta >= 0.0 && beta < 1.0, "v2_signum_encode: beta must be in [0, 1)");
+  TORCH_CHECK(ntiles == 0 || (units != 0 && tiles != 0 && gptr != 0 && arena_peer != 0 && sig_peer != 0 && ctrl != 0),
+              "v2_signum_encode: units / tiles / gptr / arena / signal tables required");
+  TORCH_CHECK(ntiles == 0 || (mom != 0) == (beta > 0.0), "v2_signum_encode: a momentum buffer exactly when beta > 0");
+  TORCH_CHECK(nv == 0 || (beta > 0.0 && vchunks != 0 && vgrads != 0 && vmom != 0),
+              "v2_signum_encode: vector chunks need beta > 0 and vgrads / vmom");
+  atomo_v2_launch_signum_encode(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
+                                P<const void>(vchunks), nv, P<float>(vgrads), P<float>(mom), P<float>(vmom),
+                                (float)beta, P<float* const>(arena_peer), P<int* const>(sig_peer), n_owners,
+                                arena_floats, worker, group, P<const void>(ctrl), P<unsigned int>(group_counter),
+                                P<long long>(tstats), final_group ? 1 : 0, P<const float>(ext_uniforms), cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+// Signum PS: the arguments of v2_ps_sign, then the tests' vector coin uniforms ([worker][vparams index], 0 = Philox)
+void v2_ps_signum(uint64_t units, uint64_t tiles, int tile0, int ntiles, int W, int nranks, int group,
+                  bool final_group, int owner, uint64_t master, uint64_t mom, uint64_t sq, uint64_t sqmax,
+                  uint64_t vmom, uint64_t vsq, uint64_t vsqmax, uint64_t wshadow_mc, uint64_t wshadow_peer,
+                  uint64_t vparams_local, uint64_t vparams_mc, uint64_t vparams_peer, uint64_t vgrads_mc,
+                  uint64_t vgrads_peer, uint64_t arenas, int64_t arena_floats, uint64_t sig, uint64_t sig_peer,
+                  uint64_t ctrl, uint64_t group_counter, int64_t timeout, uint64_t tstats, double inv_w, int grid,
+                  uint64_t vext, int64_t vext_stride) {
+  TORCH_CHECK(W >= 1 && W <= 16, "too many workers for v2_ps_signum");
+  TORCH_CHECK(ntiles >= 0 && tile0 >= 0, "v2_ps_signum: bad tile range");
+  atomo_v2_launch_ps_signum(P<const void>(units), P<const void>(tiles), tile0, ntiles, W, nranks, group,
+                            final_group ? 1 : 0, owner, P<float>(master), P<float>(mom), P<float>(sq),
+                            P<float>(sqmax), P<float>(vmom), P<float>(vsq), P<float>(vsqmax), P<void>(wshadow_mc),
+                            P<void* const>(wshadow_peer), P<float>(vparams_local), P<float>(vparams_mc),
+                            P<float* const>(vparams_peer), P<const float>(vgrads_mc),
+                            P<const float* const>(vgrads_peer), P<const float>(arenas), arena_floats, P<int>(sig),
+                            P<int* const>(sig_peer), P<void>(ctrl), P<unsigned int>(group_counter), timeout,
+                            P<long long>(tstats), (float)inv_w, grid, P<const float>(vext), vext_stride, cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
 void v2_sign_code_stats(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t arena_peer,
                         int n_owners, int64_t arena_floats, int worker, uint64_t partials, uint64_t counters,
                         uint64_t acc) {
@@ -1212,6 +1269,19 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("final_group"), py::arg("residual") = 0);
   m.def("v2_ps_sign", &v2_ps_sign);
   m.def("v2_sign_code_stats", &v2_sign_code_stats);
+  m.def("v2_signum_encode", &v2_signum_encode, py::arg("units"), py::arg("tiles"), py::arg("tile0"), py::arg("ntiles"),
+        py::arg("gptr"), py::arg("vchunks"), py::arg("nv"), py::arg("vgrads"), py::arg("mom"), py::arg("vmom"),
+        py::arg("beta"), py::arg("arena_peer"), py::arg("sig_peer"), py::arg("n_owners"), py::arg("arena_floats"),
+        py::arg("worker"), py::arg("group"), py::arg("ctrl"), py::arg("group_counter"), py::arg("tstats"),
+        py::arg("final_group"), py::arg("ext_uniforms") = 0);
+  m.def("v2_ps_signum", &v2_ps_signum, py::arg("units"), py::arg("tiles"), py::arg("tile0"), py::arg("ntiles"),
+        py::arg("W"), py::arg("nranks"), py::arg("group"), py::arg("final_group"), py::arg("owner"),
+        py::arg("master"), py::arg("mom"), py::arg("sq"), py::arg("sqmax"), py::arg("vmom"), py::arg("vsq"),
+        py::arg("vsqmax"), py::arg("wshadow_mc"), py::arg("wshadow_peer"), py::arg("vparams_local"),
+        py::arg("vparams_mc"), py::arg("vparams_peer"), py::arg("vgrads_mc"), py::arg("vgrads_peer"),
+        py::arg("arenas"), py::arg("arena_floats"), py::arg("sig"), py::arg("sig_peer"), py::arg("ctrl"),
+        py::arg("group_counter"), py::arg("timeout"), py::arg("tstats"), py::arg("inv_w"), py::arg("grid"),
+        py::arg("vext") = 0, py::arg("vext_stride") = 0);
   m.def("v2_fp8_encode", &v2_fp8_encode, py::arg("units"), py::arg("tiles"), py::arg("tile0"), py::arg("ntiles"),
         py::arg("gptr"), py::arg("arena_peer"), py::arg("sig_peer"), py::arg("n_owners"), py::arg("arena_floats"),
         py::arg("worker"), py::arg("group"), py::arg("ctrl"), py::arg("group_counter"), py::arg("tstats"),

@@ -10,7 +10,7 @@ namespace v2 {
 
 enum Kind : int {
   KIND_SLAB = 1, KIND_MAT = 2, KIND_DENSE16 = 3, KIND_VEC = 4, KIND_QSGD = 5, KIND_ENTRY = 6, KIND_SIGN = 7,
-  KIND_POWER = 8, KIND_FP8 = 9, KIND_HADAMARD = 10
+  KIND_POWER = 8, KIND_FP8 = 9, KIND_HADAMARD = 10, KIND_SIGNUM = 11
 };
 
 // One coding unit: a conv gradient in [O][K][I] (channels_last) layout ("SLAB": row (o,ri), column (b,k) of the
@@ -25,6 +25,11 @@ enum Kind : int {
 // Scaled-sign units ("SIGN", v2_sign.cu: one per >= 2-D weight) use the QSGD fields and slot with one bit per element:
 // K = bucket, rows = buckets, cols = L = ceil(bucket / 64) uint64 words per bucket, cs = buckets per PS tile,
 // ps_rows = elements per PS tile, ts_index = index among the sign units; the slot's norms are the fp32 scales.
+//
+// Signum units ("SIGNUM", v2_signum.cu: one per >= 2-D weight) have the fields and slot of the sign units with one
+// bucket per PS tile (K = min(4096, numel), cs = 1, ps_rows = K, cols = ceil(K / 64)); the norm of bucket j is the tile's
+// status word (0, or NaN when the worker's momentum in the tile is not finite), and a tile's last word holds only the
+// bits of its real elements.
 //
 // FP8 units ("FP8", v2_fp8.cu) have the fields and slot of the sign units with one e4m3 byte per element:
 // cols = ceil(bucket / 8) uint64 words per bucket, the bytes in element order; the norms are the fp32 scales 2^-k.

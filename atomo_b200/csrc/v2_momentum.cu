@@ -19,17 +19,12 @@
 // geometry and 16-byte accesses of v2_ef_apply_kernel: 2 + 4 + 4 bytes read and 2 + 4 + 4 written per weight element,
 // plus 2 read for w when wd > 0.
 #include "v2_common.cuh"
+#include "v2_momentum.cuh"
 
 namespace atomo {
 namespace v2 {
 
 constexpr int MC_THREADS = 256;
-
-// u <- m u + d, returns the direction s; d already carries weight decay
-__device__ __forceinline__ float mc_step(float d, float& u, float m, bool nesterov) {
-  u = __fadd_rn(__fmul_rn(m, u), d);
-  return nesterov ? __fadd_rn(d, __fmul_rn(m, u)) : u;
-}
 
 // Blocks [0, nw) take the group's weight chunks, the rest its vector chunks (v2_accum_add_kernel's split).
 __global__ void __launch_bounds__(MC_THREADS) v2_mc_apply_kernel(const EfChunk* wchunks, int nw, const EfChunk* vchunks,

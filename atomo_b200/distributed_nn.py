@@ -90,6 +90,10 @@ def run_rank(args) -> None:
         raise SystemExit("--code sign runs on the --backend p2p bf16 engine (--dtype bf16), which keeps the "
                          "error-feedback residual; scaled sign without it is biased, and the %s backend's coders keep "
                          "none" % backend)
+    if args.code.lower() == "signum":
+        raise SystemExit("--code signum runs on the --backend p2p bf16 engine (--dtype bf16), which keeps each "
+                         "worker's momentum and takes the owners' majority vote; the %s backend's coders keep neither"
+                         % backend)
     if args.code.lower() == "topk":
         raise SystemExit("--code topk runs on the --backend p2p bf16 engine (--dtype bf16), which keeps the "
                          "error-feedback residual; top-k without it is biased, and the %s backend's coders keep none"

@@ -27,6 +27,9 @@ What changes against ``ops/plan.py`` (the fp32-flat plan of round 1):
   owners decode, sum and step the optimizer in one launch per group.
 * **Scaled sign** (``code="sign"``): every >= 2-D weight is one ``SIGN`` unit whose buckets are sent as one bit per
   element and one fp32 scale, in the slot and tile geometry of the quantizing codes.
+* **Signum** (``code="signum"``): every >= 2-D weight is one ``SIGNUM`` unit, the geometry of a sign unit with one
+  4096-element bucket per PS tile; the workers push the sign of their momentum, one bit per element and no scale, and
+  the owners step by the majority vote.
 * **FP8** (``code="fp8"``): every >= 2-D weight is one ``FP8`` unit whose buckets are sent as one e4m3 byte per
   element (stochastically rounded) and one power-of-two fp32 scale, in the geometry of the sign units.
 * **Randomized Hadamard** (``code="hadamard"``): every >= 2-D weight is one ``HADAMARD`` unit whose power-of-two
@@ -52,6 +55,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 KIND_SLAB, KIND_MAT, KIND_DENSE16, KIND_VEC, KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_POWER, KIND_FP8 = \
     1, 2, 3, 4, 5, 6, 7, 8, 9
 KIND_HADAMARD = 10
+KIND_SIGNUM = 11
 RCAP_MAX = 32
 MAX_COLS = 64
 BLOCK_COLS = 32               # column-block width of MAT units (Jacobi cost ~ cols^3 sits in the encode launch)
@@ -67,6 +71,7 @@ QSGD_TILE_ELEMS = 4096        # a QSGD PS / encode tile holds max(1, 4096 // buc
 QSGD_MAX_BUCKET = 1024        # one warp quantizes one bucket, staged in shared memory
 QSGD_MAX_LEVEL = 14           # (sign + 1) << q | level must fit 16 bits
 SIGN_MIN_BUCKET, SIGN_MAX_BUCKET = 64, 4096   # scaled sign and fp8: whole 64-bit words, at most one tile
+SIGNUM_TILE_ELEMS = 4096      # Signum: one bucket per PS / encode tile, 16 elements per thread of the kernels
 ENTRY_TILE_ELEMS = 4096       # entry-wise PS / encode tile: the element offset of an entry fits 12 bits
 TOPK_STATE_INTS, TOPK_HI_BINS, TOPK_LO_BINS = 8, 256, 128   # top-k selection state / histograms (csrc/v2_common.cuh)
 HADAMARD_BITS = (2, 4, 8)    # randomized Hadamard: whole codes per 64-bit word
@@ -289,7 +294,7 @@ class Plan2:
     arena_floats: int
     gpart_floats: int
     n_coded: int            # units with per-unit device state (coded SLAB / MAT units, or the QSGD / ENTRY / SIGN / FP8 /
-    #                         HADAMARD units)
+    #                         HADAMARD / SIGNUM units)
     rank: int
     code: str
     pw_tiles: List[Tuple[int, int, int, int]] = field(default_factory=list)   # PowerSGD pass B: (unit, col0, ncols, j)
@@ -312,6 +317,12 @@ class Plan2:
         ``scales``; for fp8 units ``codings.fp8``'s ``bytes`` and ``scales``)."""
         return sum(8 * u.rows * u.cols + 4 * u.rows for u in self.units if u.kind in (KIND_QSGD, KIND_SIGN, KIND_FP8))
 
+    def signum_bytes(self) -> int:
+        """Bytes of sign bits a worker pushes per step: ``ceil(numel / 64)`` uint64 words per weight tensor (a tile's
+        last word holds only its real elements).  The 4-byte status word and step stamp per PS tile are not counted,
+        and the fp32 vectors are ``dense_bytes``'."""
+        return sum(8 * ((u.numel + 63) // 64) for u in self.units if u.kind == KIND_SIGNUM)
+
     def powersgd_bytes(self) -> int:
         """Bytes of PowerSGD factors a worker pushes per step: ``4 r (O + C)`` per coded tensor, ``P_hat`` and ``Q'``
         sent once to the tensor's single owner, for any number of owners.  The 4-byte step stamps per PS tile are not
@@ -333,7 +344,8 @@ class Plan2:
         """Bytes actually stored per worker and step for the expected number of atoms (U is written in groups
         of 4 atoms); for the quantizing codes the words and norms of the QSGD units; for entry-wise ATOMO the
         entries and tile headers."""
-        tot = float(self.qsgd_bytes()) + self.entry_bytes() + float(self.powersgd_bytes()) + float(self.hadamard_bytes())
+        tot = float(self.qsgd_bytes()) + self.entry_bytes() + float(self.powersgd_bytes()) + \
+            float(self.hadamard_bytes()) + float(self.signum_bytes())
         for u in self.units:
             if u.coded:
                 atoms = min(u.budget if u.budget > 0 else u.cols, u.cols)
@@ -344,7 +356,7 @@ class Plan2:
     def dense_bytes(self) -> int:
         return sum((2 if u.kind == KIND_DENSE16 else 4) * u.numel for u in self.units
                    if not u.coded and u.kind not in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_POWER, KIND_FP8,
-                                                     KIND_HADAMARD))
+                                                     KIND_HADAMARD, KIND_SIGNUM))
 
 
 def default_groups(shapes: Sequence[Sequence[int]], n_groups: int) -> List[int]:
@@ -393,7 +405,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 block_cols: int = BLOCK_COLS, min_coded_numel: int = 256, quantization_level: int = 4,
                 bucket_size: int = 512, entry_budget: float = 0.05) -> Plan2:
     """Plan of the bf16 engine for ``code`` in ``svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign |
-    powersgd | fp8 | hadamard``.
+    signum | powersgd | fp8 | hadamard``.
 
     ``qsgd`` / ``terngrad``: every >= 2-D weight (the 3-channel stem and the fc layers included) is exactly one
     ``KIND_QSGD`` unit; there are no ``DENSE16`` units.  1-D parameters stay ``KIND_VEC`` (fp32, summed by
@@ -434,6 +446,12 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
     in ``[64, 4096]``) and ``L = ceil(bucket / 64)`` words per bucket: one bit per element (``codings/sign.py``) in
     place of the quantized codes and one fp32 scale per bucket in place of the norm.  ``Unit2`` fields: ``K`` = bucket,
     ``rows`` = buckets, ``cols`` = L, ``cs`` = buckets per tile, ``ps_rows`` = elements per tile, ``I`` = ``rs`` = 0.
+
+    ``signum``: the units, tiles, owners and slots of ``sign`` (kind ``KIND_SIGNUM``) with one bucket per PS tile,
+    ``bucket = min(SIGNUM_TILE_ELEMS, numel)`` whatever ``bucket_size`` says: ``K`` = ``ps_rows`` = bucket, ``cs`` = 1,
+    ``cols`` = ``ceil(bucket / 64)``.  Bit ``i`` of word ``j`` of a tile is its element ``64 j + i``; only the words of
+    real elements are written (:meth:`Plan2.signum_bytes`).  The norm of bucket ``j`` is tile ``j``'s status word, not
+    a scale (``csrc/v2_signum.cu``).
 
     ``fp8``: the units, buckets, tiles, owners and slots of ``sign`` (kind ``KIND_FP8``) with ``cols`` =
     ``ceil(bucket / 8)`` uint64 words per bucket: one e4m3 byte per element in element order, bucket ``j`` starting at
@@ -539,6 +557,11 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             add(Unit2(0, KIND_SIGN, p.index, p.widx, p.off, 0, rows=(p.numel + bucket - 1) // bucket,
                       cols=(bucket + 63) // 64, K=bucket, cs=bpt, numel=p.numel, group=p.group, ps_rows=bpt * bucket))
             continue
+        if code == "signum":
+            bucket = min(SIGNUM_TILE_ELEMS, p.numel)
+            add(Unit2(0, KIND_SIGNUM, p.index, p.widx, p.off, 0, rows=(p.numel + bucket - 1) // bucket,
+                      cols=(bucket + 63) // 64, K=bucket, cs=1, numel=p.numel, group=p.group, ps_rows=bucket))
+            continue
         if fp8:
             bucket = min(sbsz, p.numel)
             bpt = max(1, QSGD_TILE_ELEMS // bucket)
@@ -635,7 +658,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
             elif u.kind == KIND_DENSE16:
                 for e0 in range(0, u.numel, 8192):     # staging copy tiles
                     enc_tiles.append((u.index, e0, min(8192, u.numel - e0), 0))
-            elif u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_FP8, KIND_HADAMARD):   # encode = PS tiles
+            elif u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_FP8, KIND_HADAMARD, KIND_SIGNUM):   # encode = PS tiles
                 for j, e0 in enumerate(range(0, u.numel, u.ps_rows)):
                     enc_tiles.append((u.index, e0, min(u.ps_rows, u.numel - e0), j))
             elif u.kind == KIND_POWER:
@@ -644,7 +667,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 for j, c0 in enumerate(range(0, u.cols, PW_COL_BLOCK)):
                     pw_tiles.append((u.index, c0, min(PW_COL_BLOCK, u.cols - c0), j))
             u.n_enc = len(enc_tiles) - u.enc_tile0
-            if u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_FP8, KIND_HADAMARD):
+            if u.kind in (KIND_QSGD, KIND_ENTRY, KIND_SIGN, KIND_FP8, KIND_HADAMARD, KIND_SIGNUM):
                 u.ts_index = n_coded
                 n_coded += 1
                 u.ps_tile0 = len(ps_by_group[g])
@@ -653,7 +676,7 @@ def build_plan2(shapes: Sequence[Sequence[int]], code: str = "svd", rank: int = 
                 u.n_ps = len(ps_by_group[g]) - u.ps_tile0
                 u.own0 = u.ps_tile0 % n_owners
                 u.slot_off = slot_off
-                if u.kind in (KIND_QSGD, KIND_SIGN, KIND_FP8):
+                if u.kind in (KIND_QSGD, KIND_SIGN, KIND_FP8, KIND_SIGNUM):
                     slot_off += qsgd_slot_floats(u.n_ps, u.rows, u.cols)
                 elif u.kind == KIND_HADAMARD:
                     slot_off += hadamard_slot_floats(u.n_ps, u.rows, u.cols)

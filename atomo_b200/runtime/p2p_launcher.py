@@ -56,6 +56,9 @@ def _build_engine(args, model, rank, world):
     if code == "sign" and (engine == "fused" or args.dtype != "bf16"):
         raise SystemExit("--code sign runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the fp32-flat "
                          "engine has no scaled-sign code")
+    if code == "signum" and (engine == "fused" or args.dtype != "bf16"):
+        raise SystemExit("--code signum runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the "
+                         "fp32-flat engine has no worker momentum or majority vote")
     if code == "fp8" and (engine == "fused" or args.dtype != "bf16"):
         raise SystemExit("--code fp8 runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the fp32-flat "
                          "engine has no fp8 code")
@@ -70,14 +73,14 @@ def _build_engine(args, model, rank, world):
                          % args.svd_rank)
     if engine == "auto":
         shadow = args.dtype == "bf16" and code in ("svd", "qsvd", "sgd", "dense", "lossless", "topk", "sign",
-                                                   "powersgd", "fp8", "hadamard")
+                                                   "signum", "powersgd", "fp8", "hadamard")
     elif engine == "shadow":
         if args.dtype != "bf16":
             raise SystemExit("--engine shadow trains bf16 weights: it needs --dtype bf16 (fp32 runs on --engine fused)")
-        if code not in ("svd", "qsvd", "sgd", "dense", "lossless", "qsgd", "terngrad", "topk", "sign", "powersgd",
-                        "fp8", "hadamard"):
-            raise SystemExit("--engine shadow runs --code svd|qsvd|sgd|qsgd|terngrad|topk|sign|powersgd|fp8|hadamard; "
-                             "--code %s runs on --engine fused" % args.code)
+        if code not in ("svd", "qsvd", "sgd", "dense", "lossless", "qsgd", "terngrad", "topk", "sign", "signum",
+                        "powersgd", "fp8", "hadamard"):
+            raise SystemExit("--engine shadow runs --code svd|qsvd|sgd|qsgd|terngrad|topk|sign|signum|powersgd|fp8|"
+                             "hadamard; --code %s runs on --engine fused" % args.code)
         shadow = True
     else:
         shadow = False
@@ -270,7 +273,8 @@ def run_p2p_training(args, device=None):
                 extra["code_stats"] = eng.code_stats(reset=True)
             if getattr(args, "error_feedback", False) and eng.is_worker:
                 extra["ef_norm"] = eng.error_feedback_norm()["model"]
-            if getattr(args, "momentum_correction", False) and eng.is_worker:
+            if (getattr(args, "momentum_correction", False) or getattr(eng, "mc_mom", None) is not None) \
+                    and eng.is_worker:
                 extra["mom_norm"] = eng.momentum_correction_norm()["model"]
             if getattr(args, "clip_grad_norm", 0.0) and eng.is_owner:
                 extra["grad_norm"], extra["clip_coef"] = eng.grad_norm()

@@ -34,6 +34,14 @@ one central PS kernel at the end of the step):
   fp32 scale ``||b||_1 / |b|`` in the slots and tiles of QSGD (``csrc/v2_sign.cu``, one encode launch per group); the
   owners decode ``+-scale``, sum in worker order and step the optimizer.  Deterministic, dense and biased on its own:
   the contractive code of EF-SignSGD for ``error_feedback=True``.
+* **Signum with majority vote** (``code="signum"``, ``momentum`` = beta in ``[0, 1)``; SGD only): each worker keeps an
+  fp32 momentum ``u <- beta u + g`` per weight and vector element (no buffer with ``beta == 0``: ``u = g``) and pushes
+  ``sign(u)``, one bit per element and no scale, in the slots of sign with one 4096-element bucket per tile
+  (``csrc/v2_signum.cu``, one encode launch per group that also forms the vectors' momentum in ``vgrads``).  A zero
+  takes a fair Philox coin.  The owners count the 1 bits of the counted workers per element and step
+  ``p <- p - lr * vote``, ``vote`` in {-1, 0, +1} (NaN when a counted worker's tile is not finite); vectors are voted on
+  the sign of each worker's ``vgrads``.  Weight decay is decoupled and owner-side, the pass of AdamW before the PS
+  launch.  The momentum lives in momentum correction's buffers and checkpoint keys.
 * **PowerSGD** (``code="powersgd"``, ``svd_rank`` = r in ``[1, 4]``): every weight matrix (``[O][C]`` in its physical
   layout) is pushed as a rank-``r`` pair from one power step warm-started by the previous step's right factor
   (``csrc/v2_powersgd.cu``, two encode launches per group); the owners reconstruct ``P_hat Q'^T`` in worker order and
@@ -135,12 +143,15 @@ class ShadowEngine:
         self.optimizer = optimizer.lower()
         if self.optimizer not in ("sgd", "adam", "adamw", "lars", "lamb"):      # checked before any CUDA work
             raise ValueError("ShadowEngine optimizers: sgd | adam | adamw | lars | lamb (got %r)" % (optimizer,))
-        # AdamW: the PS kernels run Adam with weight_decay 0; the decoupled decay of the weights is its own pass
+        self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
+        self.signum = self.code == "signum"
+        # AdamW and Signum: the PS kernels run with weight_decay 0; the decoupled decay of the weights is its own pass
         self.adamw_wd = 0.0
-        if self.optimizer == "adamw":      # checked before any CUDA work
+        if self.optimizer == "adamw" or self.signum:      # checked before any CUDA work
             if isinstance(weight_decay, bool) or not isinstance(weight_decay, numbers.Real) \
                     or not 0 <= weight_decay < math.inf:
-                raise ValueError("adamw: weight_decay must be finite and >= 0 (got %r)" % (weight_decay,))
+                raise ValueError("%s: weight_decay must be finite and >= 0 (got %r)"
+                                 % ("signum" if self.signum else "adamw", weight_decay))
             self.adamw_wd, weight_decay = float(weight_decay), 0.0
         self.decay_on = self.adamw_wd > 0     # with weight_decay 0 AdamW is Adam: nothing new is launched
         self.layerwise = self.optimizer in ("lars", "lamb")
@@ -158,11 +169,29 @@ class ShadowEngine:
         self.clip_on = self.clip_grad_norm > 0
         self.ema_decay = check_ema_decay(ema_decay)      # checked before any CUDA work
         self.ema_w = float(np.float32(1.0 - self.ema_decay))    # the average's step weight, rounded once
-        self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
-        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign", "powersgd", "fp8",
-                             "hadamard"):
-            raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign | powersgd "
-                             "| fp8 | hadamard")
+        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign", "signum",
+                             "powersgd", "fp8", "hadamard"):
+            raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign | signum "
+                             "| powersgd | fp8 | hadamard")
+        if self.signum:     # checked before any CUDA work
+            if self.optimizer != "sgd":
+                raise ValueError("signum steps the owners by the vote of the workers' momentum signs: optimizer='sgd' "
+                                 "only (got %r)" % (optimizer,))
+            if nesterov:
+                raise ValueError("signum takes heavy-ball momentum on the workers: nesterov=False")
+            if dampening != 0:
+                raise ValueError("signum takes dampening=0 (got %r)" % (dampening,))
+            if isinstance(momentum, bool) or not isinstance(momentum, numbers.Real) or not 0 <= momentum < 1:
+                raise ValueError("signum: momentum (the workers' beta) must be in [0, 1) (got %r)" % (momentum,))
+            if error_feedback:
+                raise ValueError("signum sends sign(momentum) without a residual: error_feedback=False (use "
+                                 "code='sign' for EF-SignSGD)")
+            if code_stats:
+                raise ValueError("code_stats has no estimator model for a majority vote (signum)")
+            if check_clip_grad_norm(clip_grad_norm) > 0:
+                raise ValueError("signum cannot be combined with clip_grad_norm: every step has length lr per element")
+            if momentum_correction:
+                raise ValueError("signum keeps its own worker momentum: momentum_correction=False")
         self.power = self.code == "powersgd"
         if self.power and not 1 <= int(svd_rank) <= P2.POWER_MAX_RANK:      # checked before any CUDA work
             raise ValueError("powersgd: svd_rank must be in [1, %d] (got %r)" % (P2.POWER_MAX_RANK, svd_rank))
@@ -401,7 +430,7 @@ class ShadowEngine:
         self.max_sweeps = int(max_sweeps) if warm_start else 0
         self.vprev = None
         if warm_start and not self.quant and not self.entry and not self.sign and not self.power and not self.fp8 \
-                and not self.hadamard:
+                and not self.hadamard and not self.signum:
             self.vprev = z(nc * P2.MAX_COLS * P2.MAX_COLS)      # set by _fresh_worker_state()
         # QSGD: largest level / bucket of the plan (checked by the bindings), TernGrad clip per unit + its partials
         qunits = [u for u in pl.units if u.kind == P2.KIND_QSGD]
@@ -436,7 +465,7 @@ class ShadowEngine:
         self.cnt_ps_group = self.cnt_enc_group + 4 * P2.MAX_GROUPS
         # momentum correction: momentum, weight decay and Nesterov act on the workers (v2_mc_apply), the PS runs plain SGD
         self.mc_momentum, self.mc_weight_decay, self.mc_nesterov = float(momentum), float(weight_decay), bool(nesterov)
-        if self.momentum_correction:
+        if self.momentum_correction or self.signum:
             momentum, dampening, weight_decay, nesterov = 0.0, 0.0, 0.0, False
         self.ctrl = _dev_bytes(P2.pack_ctrl2(step=1, lr=lr, momentum=momentum, dampening=dampening,
                                              weight_decay=weight_decay, nesterov=nesterov, first_step=1, seed=seed,
@@ -516,7 +545,7 @@ class ShadowEngine:
         # uses t_gptr, which the encoders read)
         self.acc = self.vacc = self.t_vec_chunks = self.t_aptr = self.host_aptr = None
         self.vec_range = []
-        if self.accum > 1 or (self.momentum_correction and self.is_worker):
+        if self.accum > 1 or ((self.momentum_correction or self.signum) and self.is_worker):
             vchunks, self.vec_range = P2.vec_chunks(pl)
             self.t_vec_chunks = _dev_bytes(vchunks, dev)
         if self.accum > 1:
@@ -524,10 +553,11 @@ class ShadowEngine:
             self.t_aptr = torch.zeros((self.accum - 1, n_w), dtype=torch.int64, device=dev)
             self.host_aptr = np.zeros((self.accum - 1, n_w), dtype=np.int64)
         self.inv_n = float(np.float32(1.0 / self.accum))
-        # momentum correction (csrc/v2_momentum.cu): the worker's fp32 momentum per weight element (wshadow's physical
-        # order, the residual's offsets) and per vector element (vgrads' order)
+        # momentum correction (csrc/v2_momentum.cu) and Signum with beta > 0 (csrc/v2_signum.cu): the worker's fp32
+        # momentum per weight element (wshadow's physical order, the residual's offsets) and per vector element (vgrads'
+        # order)
         self.mc_mom = self.mc_vmom = None
-        if self.momentum_correction and self.is_worker:
+        if (self.momentum_correction or (self.signum and self.mc_momentum > 0)) and self.is_worker:
             self.mc_mom, self.mc_vmom = z(pl.w_total), z(pl.v_total)
         self.pw_warm = P2.pw_warm_ranges(pl) if self.power else []     # Q_w inside gpart (checkpointed)
         self._fresh_worker_state()
@@ -598,8 +628,8 @@ class ShadowEngine:
             self.ctrl_f32[17] = self.decay_factor(lr)      # Ctrl2::decay_factor, read by every decay launch
 
     def decay_factor(self, lr: float) -> float:
-        """AdamW: the factor of the decoupled weight decay at learning rate ``lr``, ``1 - lr * wd`` in double (as
-        torch.optim.AdamW computes it in Python) rounded to fp32 once."""
+        """AdamW and Signum: the factor of the decoupled weight decay at learning rate ``lr``, ``1 - lr * wd`` in double
+        (as torch.optim.AdamW computes it in Python) rounded to fp32 once."""
         return float(np.float32(1.0 - float(lr) * self.adamw_wd))
 
     def error_code(self) -> int:
@@ -702,11 +732,12 @@ class ShadowEngine:
         return {"model": float(sum(sq)) ** 0.5, "tensors": {n: v ** 0.5 for (n, _), v in zip(ws, sq)}}
 
     def momentum_correction_norm(self) -> dict:
-        """``||u||`` of this worker's momentum (``momentum_correction=True``): per parameter tensor (weights and
-        vectors) and for the whole model.  Reading it synchronises the device."""
+        """``||u||`` of this worker's momentum (``momentum_correction=True``, or ``code="signum"`` with
+        ``momentum > 0``): per parameter tensor (weights and vectors) and for the whole model.  Reading it synchronises
+        the device."""
         if self.mc_mom is None:
-            raise RuntimeError("momentum_correction_norm() needs ShadowEngine(..., momentum_correction=True) on a "
-                               "worker")
+            raise RuntimeError("momentum_correction_norm() needs ShadowEngine(..., momentum_correction=True) or "
+                               "code='signum' with momentum > 0, on a worker")
         names = {id(p): n for n, p in self.model.named_parameters()}
         ts = [(names.get(id(p), str(q.index)), (self.mc_mom if q.is_w else self.mc_vmom)[q.off:q.off + q.numel])
               for p, q in zip(self.params, self.plan.params)]
@@ -788,7 +819,7 @@ class ShadowEngine:
                             self.t_gptr.data_ptr(), self.acc.data_ptr(), self.vacc.data_ptr(), self.vgrads.data_ptr(),
                             self.inv_n, res)
             self._nlaunch += 1
-        elif self.mc_mom is not None:
+        elif self.momentum_correction:
             # momentum correction: u = m u + g (+ wd w), A = u (Nesterov: d + m u) + e into the gradient buffers
             # (bf16) and the residual; the vectors' direction into vgrads
             (c0, nw), (v0, nv), cb = self.ef_range[g], self.vec_range[g], struct.calcsize(P2.EF_CHUNK_FMT)
@@ -814,6 +845,21 @@ class ShadowEngine:
                              self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g, 0, self.tstats.data_ptr(),
                              self._fired == self.G, self.clip is None, self.q_max_level, self.q_max_bucket,
                              self.code == "terngrad", res)
+            self._nlaunch += 1
+            return
+        if self.signum and (nt > 0 or self.mc_vmom is not None):
+            # worker momentum of the weights and (beta > 0) of the vectors, sign bits pushed into the owners' arenas; the
+            # encode raises the push flag
+            (v0, nv), cb = self.vec_range[g], struct.calcsize(P2.EF_CHUNK_FMT)
+            if self.mc_vmom is None:
+                nv = 0
+            p = lambda t: t.data_ptr() if t is not None else 0
+            C.v2_signum_encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
+                               self.t_vec_chunks.data_ptr() + cb * v0, nv, self.vgrads.data_ptr(), p(self.mc_mom),
+                               p(self.mc_vmom), self.mc_momentum, self.t_arena_peer.data_ptr(),
+                               self.t_sig_owner.data_ptr(), self.n_owners, pl.arena_floats, self.worker_index, g,
+                               self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g, self.tstats.data_ptr(),
+                               self._fired == self.G)
             self._nlaunch += 1
             return
         if self.power:
@@ -930,6 +976,17 @@ class ShadowEngine:
                self.heap.region_ptr("arena"), pl.arena_floats, self.signals.data_ptr(), self.t_sig_all.data_ptr(),
                self.ctrl.data_ptr(), self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(),
                1.0 / self.W, max(1, min(self.ps_grid, max(nt, 1))))
+            self._nlaunch += 1
+            return
+        if self.signum:
+            C.v2_ps_signum(self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world, g, final,
+                           self.owner_index, p(self.master), p(self.mom), p(self.sq), p(self.sqmax), p(self.vmom),
+                           p(self.vsq), p(self.vsqmax), self.wshadow_mc, self.t_wshadow_peer.data_ptr(),
+                           self.vparams.data_ptr(), self.vparams_mc, self.t_vparams_peer.data_ptr(), self.vgrads_mc,
+                           self.t_vgrads_peer.data_ptr(), self.heap.region_ptr("arena"), pl.arena_floats,
+                           self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
+                           self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
+                           max(1, min(self.ps_grid, max(nt, 1))))
             self._nlaunch += 1
             return
         if self.entry:
@@ -1282,7 +1339,7 @@ class ShadowEngine:
             if u.kind == P2.KIND_VEC:
                 mv[u.w_off + a:u.w_off + a + b] = 1
             elif u.kind in (P2.KIND_DENSE16, P2.KIND_QSGD, P2.KIND_ENTRY, P2.KIND_SIGN, P2.KIND_FP8,
-                            P2.KIND_HADAMARD):                                           # (first, count)
+                            P2.KIND_HADAMARD, P2.KIND_SIGNUM):                                           # (first, count)
                 mw[u.w_off + a:u.w_off + a + b] = 1
             elif u.kind == P2.KIND_POWER:                                                # (first row, rows)
                 mw[u.w_off + a * u.cols:u.w_off + (a + b) * u.cols] = 1
@@ -1416,6 +1473,8 @@ class ShadowEngine:
             side.update(entry_budget=self.entry_budget)
         if self.momentum_correction:
             side.update(momentum_correction=True)
+        if self.signum:
+            side.update(signum_momentum=self.mc_momentum, weight_decay=self.adamw_wd)
         side.update(adam_state)
         torch.save(side, path + "_optim.tmp")
         os.replace(path + "_optim.tmp", path + "_optim")
@@ -1427,6 +1486,8 @@ class ShadowEngine:
                "warm_start": self.warm_start, "world": self.world, "ps_mode": self.ps_mode, "worker": self.worker_index}
         if self.momentum_correction:
             cfg["momentum_correction"] = True
+        if self.signum:
+            cfg["signum_momentum"] = self.mc_momentum
         return cfg
 
     def _worker_tensors(self) -> dict:

@@ -36,7 +36,11 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "largest entries per tensor, sent exactly; --backend p2p --dtype bf16 only, meant for "
                         "--error-feedback 1) | sign (scaled sign: one bit per element and one fp32 scale "
                         "||b||_1/|b| per --bucket-size bucket, a multiple of 64 in [64, 4096]; --backend p2p --dtype "
-                        "bf16 only, meant for --error-feedback 1) | powersgd (rank --svd-rank in [1, 4] factors of every "
+                        "bf16 only, meant for --error-feedback 1) | signum (Signum with majority vote: each worker "
+                        "keeps a momentum with beta = --momentum in [0, 1) and sends its sign, one bit per element and "
+                        "no scale; the owners step by lr times the vote; --backend p2p --dtype bf16 only, SGD without "
+                        "--nesterov, --error-feedback, --clip-grad-norm or --code-stats; --weight-decay is decoupled, "
+                        "on the owners) | powersgd (rank --svd-rank in [1, 4] factors of every "
                         "weight matrix from one warm-started power step; --backend p2p --dtype bf16 only, meant for "
                         "--error-feedback 1) | fp8 (one e4m3 byte per element, stochastically rounded and so "
                         "unbiased, and one power-of-two fp32 scale per --bucket-size bucket, a multiple of 64 in "
