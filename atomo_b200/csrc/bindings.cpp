@@ -283,6 +283,14 @@ void atomo_v2_launch_clip(int layerwise, const void* units, const void* tiles, c
                           long long* tstats, float* norm_out, int grid, cudaStream_t stream);
 void atomo_v2_launch_bcast_bytes(const void* src, void* const* peer, void* mc, int nranks, int self, long long nbytes,
                                  cudaStream_t stream);
+// v2_lion.cu (Lion on the bf16 engine: the PS kernels' Lion instantiations)
+void atomo_v2_launch_ps_lion(int ps, const void* units, const void* tiles, int tile0, int ntiles, int W, int nranks,
+                             int group, int final_group, int owner, float* master, float* mom, float* vmom,
+                             void* wshadow_mc, void* const* wshadow_peer, float* vparams_local, float* vparams_mc,
+                             float* const* vparams_peer, const float* vgrads_mc, const float* const* vgrads_peer,
+                             const void* const* stage_peer, const float* arenas, long long arena_floats, int* sig,
+                             int* const* sig_peer, void* ctrl, unsigned int* group_counter, long long timeout,
+                             long long* tstats, float inv_w, int grid, cudaStream_t stream);
 // v2_ema.cu (exponential moving average of the weights on the bf16 engine)
 void atomo_v2_launch_ema(const void* units, const void* tiles, int tile0, int ntiles, const float* master,
                          const float* vparams, float* ema, float* vema, float w, int grid, cudaStream_t stream);
@@ -1046,6 +1054,28 @@ void v2_ps_gather(int ps, uint64_t units, uint64_t tiles, int tile0, int ntiles,
                             cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
+// Lion: the code's PS kernel (`ps` as v2_ps_layerwise) with the Lion epilogue on master / mom and vparams / vmom,
+// the broadcast and the completion of the plain launch (the final group publishes the parameters)
+void v2_ps_lion(int ps, uint64_t units, uint64_t tiles, int tile0, int ntiles, int W, int nranks, int group,
+                bool final_group, int owner, uint64_t master, uint64_t mom, uint64_t vmom, uint64_t wshadow_mc,
+                uint64_t wshadow_peer, uint64_t vparams_local, uint64_t vparams_mc, uint64_t vparams_peer,
+                uint64_t vgrads_mc, uint64_t vgrads_peer, uint64_t stage_peer, uint64_t arenas, int64_t arena_floats,
+                uint64_t sig, uint64_t sig_peer, uint64_t ctrl, uint64_t group_counter, int64_t timeout,
+                uint64_t tstats, double inv_w, int grid, int max_level, int max_bucket) {
+  TORCH_CHECK(ps >= 0 && ps <= 6, "v2_ps_lion: unknown PS kernel");
+  TORCH_CHECK(W >= 1 && W <= 16, "too many workers for v2_ps_lion");
+  TORCH_CHECK(master != 0 && mom != 0 && vmom != 0, "v2_ps_lion: master / mom / vmom required");
+  if (ps == 1) check_qsgd_plan(max_level, max_bucket);
+  atomo_v2_launch_ps_lion(ps, P<const void>(units), P<const void>(tiles), tile0, ntiles, W, nranks, group,
+                          final_group ? 1 : 0, owner, P<float>(master), P<float>(mom), P<float>(vmom),
+                          P<void>(wshadow_mc), P<void* const>(wshadow_peer), P<float>(vparams_local),
+                          P<float>(vparams_mc), P<float* const>(vparams_peer), P<const float>(vgrads_mc),
+                          P<const float* const>(vgrads_peer), P<const void* const>(stage_peer), P<const float>(arenas),
+                          arena_floats, P<int>(sig), P<int* const>(sig_peer), P<void>(ctrl),
+                          P<unsigned int>(group_counter), timeout, P<long long>(tstats), (float)inv_w, grid,
+                          cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
 // gradient-norm clipping phase 2: the whole-model norm across tiles and owners, the clip coefficient, and the step of
 // every tile of the owner (with `layerwise`, LARS / LAMB's direction and tile partials instead; v2_layerwise follows)
 void v2_clip(bool layerwise, uint64_t units, uint64_t tiles, uint64_t owner_tiles, int ntiles, uint64_t gpart,
@@ -1308,6 +1338,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("v2_layerwise", &v2_layerwise);
   m.def("v2_layerwise_max_layers", &atomo_v2_layerwise_max_layers);
   m.def("v2_ps_gather", &v2_ps_gather);
+  m.def("v2_ps_lion", &v2_ps_lion);
   m.def("v2_clip", &v2_clip);
   m.def("v2_ema", &v2_ema);
   m.def("v2_decay", &v2_decay);

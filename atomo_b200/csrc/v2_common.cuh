@@ -76,7 +76,8 @@ struct Tile2 {
   int owner;
 };
 
-enum Opt : int { OPT_SGD = 0, OPT_ADAM = 1, OPT_AMSGRAD = 2, OPT_LARS = 3, OPT_LAMB = 4 };
+// OPT_LION is bookkeeping only: Lion runs the PS kernels' Lion instantiation (PsArgsLion), never the plain one
+enum Opt : int { OPT_SGD = 0, OPT_ADAM = 1, OPT_AMSGRAD = 2, OPT_LARS = 3, OPT_LAMB = 4, OPT_LION = 5 };
 
 struct Ctrl2 {
   int step;

@@ -160,6 +160,7 @@ __device__ __forceinline__ void ps_entry(const A& a) {
 __global__ void __launch_bounds__(EPS_THREADS) v2_ps_entry_kernel(const PsArgs2 a) { ps_entry(a); }
 __global__ void __launch_bounds__(EPS_THREADS, 1) v2_ps_entry_lw_kernel(const PsArgsLw a) { ps_entry(a); }
 __global__ void __launch_bounds__(EPS_THREADS, 1) v2_ps_entry_gather_kernel(const PsArgsGather a) { ps_entry(a); }
+__global__ void __launch_bounds__(EPS_THREADS, 1) v2_ps_entry_lion_kernel(const PsArgsLion a) { ps_entry(a); }
 
 extern "C" {
 
@@ -210,6 +211,11 @@ void atomo_v2_launch_ps_entry_lw(const void* args, int grid, cudaStream_t stream
 void atomo_v2_launch_ps_entry_gather(const void* args, int grid, cudaStream_t stream) {
   const PsArgsGather& a = *static_cast<const PsArgsGather*>(args);
   v2_ps_entry_gather_kernel<<<ps_grid(grid, a.ntiles), EPS_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_entry_lion(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsLion& a = *static_cast<const PsArgsLion*>(args);
+  v2_ps_entry_lion_kernel<<<ps_grid(grid, a.ntiles), EPS_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

@@ -272,6 +272,7 @@ __device__ __forceinline__ void ps_fp8(const A& a) {
 __global__ void __launch_bounds__(FPS_THREADS) v2_ps_fp8_kernel(const PsArgs2 a) { ps_fp8(a); }
 __global__ void __launch_bounds__(FPS_THREADS, 1) v2_ps_fp8_lw_kernel(const PsArgsLw a) { ps_fp8(a); }
 __global__ void __launch_bounds__(FPS_THREADS, 1) v2_ps_fp8_gather_kernel(const PsArgsGather a) { ps_fp8(a); }
+__global__ void __launch_bounds__(FPS_THREADS, 1) v2_ps_fp8_lion_kernel(const PsArgsLion a) { ps_fp8(a); }
 
 // ---- --code-stats ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(FE_THREADS) v2_fp8_code_stats_kernel(const ScaleStatArgs a) {
@@ -380,6 +381,11 @@ void atomo_v2_launch_ps_fp8_lw(const void* args, int grid, cudaStream_t stream) 
 void atomo_v2_launch_ps_fp8_gather(const void* args, int grid, cudaStream_t stream) {
   const PsArgsGather& a = *static_cast<const PsArgsGather*>(args);
   v2_ps_fp8_gather_kernel<<<ps_grid(grid, a.ntiles), FPS_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_fp8_lion(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsLion& a = *static_cast<const PsArgsLion*>(args);
+  v2_ps_fp8_lion_kernel<<<ps_grid(grid, a.ntiles), FPS_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

@@ -434,6 +434,7 @@ __device__ __forceinline__ void ps_hadamard(const A& a) {
 __global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_kernel(const PsArgs2 a) { ps_hadamard(a); }
 __global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_lw_kernel(const PsArgsLw a) { ps_hadamard(a); }
 __global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_gather_kernel(const PsArgsGather a) { ps_hadamard(a); }
+__global__ void __launch_bounds__(HD_THREADS, 1) v2_ps_hadamard_lion_kernel(const PsArgsLion a) { ps_hadamard(a); }
 
 // ---- --code-stats ------------------------------------------------------------------------------------------
 struct HStatArgs {
@@ -557,6 +558,11 @@ void atomo_v2_launch_ps_hadamard_lw(const void* args, int grid, cudaStream_t str
 void atomo_v2_launch_ps_hadamard_gather(const void* args, int grid, cudaStream_t stream) {
   const PsArgsGather& a = *static_cast<const PsArgsGather*>(args);
   v2_ps_hadamard_gather_kernel<<<ps_grid(grid, a.ntiles), HD_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_hadamard_lion(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsLion& a = *static_cast<const PsArgsLion*>(args);
+  v2_ps_hadamard_lion_kernel<<<ps_grid(grid, a.ntiles), HD_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

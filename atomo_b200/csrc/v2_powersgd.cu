@@ -527,6 +527,7 @@ __device__ __forceinline__ void ps_powersgd(const A& a) {
 __global__ void __launch_bounds__(PW_THREADS) v2_ps_powersgd_kernel(const PsArgs2 a) { ps_powersgd(a); }
 __global__ void __launch_bounds__(PW_THREADS, 1) v2_ps_powersgd_lw_kernel(const PsArgsLw a) { ps_powersgd(a); }
 __global__ void __launch_bounds__(PW_THREADS, 1) v2_ps_powersgd_gather_kernel(const PsArgsGather a) { ps_powersgd(a); }
+__global__ void __launch_bounds__(PW_THREADS, 1) v2_ps_powersgd_lion_kernel(const PsArgsLion a) { ps_powersgd(a); }
 
 // ---- --code-stats ------------------------------------------------------------------------------------------------
 struct PwStatArgs {
@@ -674,6 +675,11 @@ void atomo_v2_launch_ps_powersgd_lw(const void* args, int grid, cudaStream_t str
 void atomo_v2_launch_ps_powersgd_gather(const void* args, int grid, cudaStream_t stream) {
   const PsArgsGather& a = *static_cast<const PsArgsGather*>(args);
   v2_ps_powersgd_gather_kernel<<<ps_grid(grid, a.ntiles), PW_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_powersgd_lion(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsLion& a = *static_cast<const PsArgsLion*>(args);
+  v2_ps_powersgd_lion_kernel<<<ps_grid(grid, a.ntiles), PW_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

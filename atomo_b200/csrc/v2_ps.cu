@@ -304,6 +304,7 @@ __device__ __forceinline__ void ps_spectral(const A& a) {
 __global__ void __launch_bounds__(PS2_THREADS) v2_ps_kernel(const PsArgs2 a) { ps_spectral(a); }
 __global__ void __launch_bounds__(PS2_THREADS, 1) v2_ps_lw_kernel(const PsArgsLw a) { ps_spectral(a); }
 __global__ void __launch_bounds__(PS2_THREADS, 1) v2_ps_gather_kernel(const PsArgsGather a) { ps_spectral(a); }
+__global__ void __launch_bounds__(PS2_THREADS, 1) v2_ps_lion_kernel(const PsArgsLion a) { ps_spectral(a); }
 
 // worker side: block the stream until every owner has delivered its shard of the parameters of `step`
 __global__ void v2_wait_params_kernel(const int* sig, int n_owners, Ctrl2* ctrl, long long timeout, long long* tstats) {
@@ -386,6 +387,16 @@ void atomo_v2_launch_ps_spectral_gather(const void* args, int grid, cudaStream_t
   }
   const PsArgsGather& a = *static_cast<const PsArgsGather*>(args);
   v2_ps_gather_kernel<<<ps_grid(grid, a.ntiles), PS2_THREADS, PS2_SMEM, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_spectral_lion(const void* args, int grid, cudaStream_t stream) {
+  static bool attr = false;
+  if (!attr) {
+    cudaFuncSetAttribute(v2_ps_lion_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PS2_SMEM);
+    attr = true;
+  }
+  const PsArgsLion& a = *static_cast<const PsArgsLion*>(args);
+  v2_ps_lion_kernel<<<ps_grid(grid, a.ntiles), PS2_THREADS, PS2_SMEM, stream>>>(a);
 }
 
 void atomo_v2_launch_wait_params(const int* sig, int n_owners, void* ctrl, long long timeout, long long* tstats,

@@ -230,6 +230,22 @@ __device__ __forceinline__ void mc_store16(void* mc, const uint4 v) {
                : "memory");
 }
 
+// the bf16 copy of 8 consecutive updated weights from element e (16-byte aligned in bf16) to every rank
+__device__ __forceinline__ void ps_bcast8(const PsArgs2& a, long long e, const float (&p)[8]) {
+  const uint4 packed = pack_bf16x8(p);
+  if (a.wshadow_mc != nullptr) {
+    mc_store16(a.wshadow_mc + e, packed);
+  } else {
+    for (int r = 0; r < a.nranks; ++r) *reinterpret_cast<uint4*>(a.wshadow_peer[r] + e) = packed;
+  }
+}
+
+// ... of one updated weight (the scalar tail: peer stores only)
+__device__ __forceinline__ void ps_bcast1(const PsArgs2& a, long long e, float p) {
+  const __nv_bfloat16 b = __float2bfloat16_rn(p);
+  for (int r = 0; r < a.nranks; ++r) a.wshadow_peer[r][e] = b;
+}
+
 // update 8 consecutive weight elements starting at element e (16-byte aligned in bf16), broadcast the bf16 copy
 __device__ __forceinline__ void update8(const PsArgs2& a, const OptC& c, long long e, const float (&g)[8]) {
   float p[8], m[8], v[8], vm[8];
@@ -254,12 +270,7 @@ __device__ __forceinline__ void update8(const PsArgs2& a, const OptC& c, long lo
 #pragma unroll
     for (int i = 0; i < 8; ++i) { a.sq[e + i] = v[i]; if (c.opt == OPT_AMSGRAD) a.sqmax[e + i] = vm[i]; }
   }
-  const uint4 packed = pack_bf16x8(p);
-  if (a.wshadow_mc != nullptr) {
-    mc_store16(a.wshadow_mc + e, packed);
-  } else {
-    for (int r = 0; r < a.nranks; ++r) *reinterpret_cast<uint4*>(a.wshadow_peer[r] + e) = packed;
-  }
+  ps_bcast8(a, e, p);
 }
 
 __device__ __forceinline__ void update1(const PsArgs2& a, const OptC& c, long long e, float g) {
@@ -268,8 +279,45 @@ __device__ __forceinline__ void update1(const PsArgs2& a, const OptC& c, long lo
   opt_update(g, p, m, v, vm, c);
   a.master[e] = p; a.mom[e] = m;
   if (c.opt != OPT_SGD) { a.sq[e] = v; if (c.opt == OPT_AMSGRAD) a.sqmax[e] = vm; }
-  const __nv_bfloat16 b = __float2bfloat16_rn(p);
-  for (int r = 0; r < a.nranks; ++r) a.wshadow_peer[r][e] = b;
+  ps_bcast1(a, e, p);
+}
+
+// ---- Lion (Chen et al. 2023), the fourth instantiation of every PS kernel -----------------------------------------
+// Per element, on the mean gradient g the plain instantiation hands to the optimizer, every operation rounded on its
+// own (no contraction), om1 = 1 - b1 and om2 = 1 - b2 formed in fp32:
+//   c = b1 m + om1 g;  p <- p - lr sign(c);  m <- b2 m + om2 g
+// sign(+-0) = 0, so an exact zero c leaves p as it was; a NaN c gives a NaN step (torch.sign would return 0 and hide
+// it).  m starts at zero; no bias correction.  The decoupled weight decay of the weights is the v2_decay launch before
+// this one (Ctrl2::decay_factor).  State: master and mom (vectors: vparams and vmom); sq / sqmax / vsq / vsqmax are
+// never touched.  Then the same bf16 (weights) or fp32 (vectors) broadcast as the plain instantiation.
+struct PsArgsLion : PsArgs2 {};
+
+__device__ __forceinline__ void lion_update(float g, float& p, float& m, const OptC& c) {
+  const float cc = __fadd_rn(__fmul_rn(c.b1, m), __fmul_rn(__fsub_rn(1.f, c.b1), g));
+  const float s = cc > 0.f ? 1.f : cc < 0.f ? -1.f : cc == 0.f ? 0.f : cc;
+  p = __fsub_rn(p, __fmul_rn(c.lr, s));
+  m = __fadd_rn(__fmul_rn(c.b2, m), __fmul_rn(__fsub_rn(1.f, c.b2), g));
+}
+
+__device__ __forceinline__ void update8(const PsArgsLion& a, const OptC& c, long long e, const float (&g)[8]) {
+  const float4 p0 = *reinterpret_cast<const float4*>(a.master + e), p1 = *reinterpret_cast<const float4*>(a.master + e + 4);
+  const float4 m0 = *reinterpret_cast<const float4*>(a.mom + e), m1 = *reinterpret_cast<const float4*>(a.mom + e + 4);
+  float p[8] = {p0.x, p0.y, p0.z, p0.w, p1.x, p1.y, p1.z, p1.w};
+  float m[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
+#pragma unroll
+  for (int i = 0; i < 8; ++i) lion_update(g[i], p[i], m[i], c);
+  *reinterpret_cast<float4*>(a.master + e) = make_float4(p[0], p[1], p[2], p[3]);
+  *reinterpret_cast<float4*>(a.master + e + 4) = make_float4(p[4], p[5], p[6], p[7]);
+  *reinterpret_cast<float4*>(a.mom + e) = make_float4(m[0], m[1], m[2], m[3]);
+  *reinterpret_cast<float4*>(a.mom + e + 4) = make_float4(m[4], m[5], m[6], m[7]);
+  ps_bcast8(a, e, p);
+}
+
+__device__ __forceinline__ void update1(const PsArgsLion& a, const OptC& c, long long e, float g) {
+  float p = a.master[e], m = a.mom[e];
+  lion_update(g, p, m, c);
+  a.master[e] = p; a.mom[e] = m;
+  ps_bcast1(a, e, p);
 }
 
 // ---- push wait (thread 0 of every CTA) ------------------------------------------------------------------
@@ -385,8 +433,11 @@ __device__ __forceinline__ OptC ps_opt_consts(const Ctrl2* ctrl, int step) {
 }
 
 // ---- fp32 vector tile (BN, biases): sum of the counted workers' gradients, optimizer, fp32 broadcast ------------
-__device__ __forceinline__ void ps_vec_tile(const PsArgs2& a, const OptC& c, const Unit2& u, const Tile2& t,
-                                            unsigned int wmask, bool all_workers, float inv_w) {
+// The walk is shared by the plain and the Lion instantiation: step4(e, g, p) / step1(e, g, p) update the vector
+// element(s) at e in p (read from vparams_local) from the workers' gradient sum g and write their own state.
+template <class Step4, class Step1>
+__device__ __forceinline__ void ps_vec_walk(const PsArgs2& a, const Unit2& u, const Tile2& t, unsigned int wmask,
+                                            bool all_workers, Step4 step4, Step1 step1) {
   const int tid = threadIdx.x;
   const long long e0 = u.w_off + t.a;
   const int nvec = t.b >> 2;
@@ -404,21 +455,7 @@ __device__ __forceinline__ void ps_vec_tile(const PsArgs2& a, const OptC& c, con
       }
     }
     float4 p = *reinterpret_cast<float4*>(a.vparams_local + e);
-    float4 m = *reinterpret_cast<float4*>(a.vmom + e);
-    float4 q = make_float4(0.f, 0.f, 0.f, 0.f), qm = q;
-    if (c.opt != OPT_SGD) {
-      q = *reinterpret_cast<float4*>(a.vsq + e);
-      if (c.opt == OPT_AMSGRAD) qm = *reinterpret_cast<float4*>(a.vsqmax + e);
-    }
-    opt_update(g.x * inv_w, p.x, m.x, q.x, qm.x, c);
-    opt_update(g.y * inv_w, p.y, m.y, q.y, qm.y, c);
-    opt_update(g.z * inv_w, p.z, m.z, q.z, qm.z, c);
-    opt_update(g.w * inv_w, p.w, m.w, q.w, qm.w, c);
-    *reinterpret_cast<float4*>(a.vmom + e) = m;
-    if (c.opt != OPT_SGD) {
-      *reinterpret_cast<float4*>(a.vsq + e) = q;
-      if (c.opt == OPT_AMSGRAD) *reinterpret_cast<float4*>(a.vsqmax + e) = qm;
-    }
+    step4(e, g, p);
     if (a.vparams_mc != nullptr) {
       multimem_st_f4(reinterpret_cast<float4*>(a.vparams_mc + e), p);
     } else {
@@ -430,13 +467,60 @@ __device__ __forceinline__ void ps_vec_tile(const PsArgs2& a, const OptC& c, con
     float g = 0.f;
     for (int w = 0; w < a.W; ++w)
       if ((wmask >> w) & 1u) g += ld_cg_f(a.vgrads_peer[w] + e);
-    float p = a.vparams_local[e], m = a.vmom[e], q = 0.f, qm = 0.f;
-    if (c.opt != OPT_SGD) { q = a.vsq[e]; if (c.opt == OPT_AMSGRAD) qm = a.vsqmax[e]; }
-    opt_update(g * inv_w, p, m, q, qm, c);
-    a.vmom[e] = m;
-    if (c.opt != OPT_SGD) { a.vsq[e] = q; if (c.opt == OPT_AMSGRAD) a.vsqmax[e] = qm; }
+    float p = a.vparams_local[e];
+    step1(e, g, p);
     for (int r = 0; r < a.nranks; ++r) a.vparams_peer[r][e] = p;
   }
+}
+
+__device__ __forceinline__ void ps_vec_tile(const PsArgs2& a, const OptC& c, const Unit2& u, const Tile2& t,
+                                            unsigned int wmask, bool all_workers, float inv_w) {
+  ps_vec_walk(
+      a, u, t, wmask, all_workers,
+      [&](long long e, const float4& g, float4& p) {
+        float4 m = *reinterpret_cast<float4*>(a.vmom + e);
+        float4 q = make_float4(0.f, 0.f, 0.f, 0.f), qm = q;
+        if (c.opt != OPT_SGD) {
+          q = *reinterpret_cast<float4*>(a.vsq + e);
+          if (c.opt == OPT_AMSGRAD) qm = *reinterpret_cast<float4*>(a.vsqmax + e);
+        }
+        opt_update(g.x * inv_w, p.x, m.x, q.x, qm.x, c);
+        opt_update(g.y * inv_w, p.y, m.y, q.y, qm.y, c);
+        opt_update(g.z * inv_w, p.z, m.z, q.z, qm.z, c);
+        opt_update(g.w * inv_w, p.w, m.w, q.w, qm.w, c);
+        *reinterpret_cast<float4*>(a.vmom + e) = m;
+        if (c.opt != OPT_SGD) {
+          *reinterpret_cast<float4*>(a.vsq + e) = q;
+          if (c.opt == OPT_AMSGRAD) *reinterpret_cast<float4*>(a.vsqmax + e) = qm;
+        }
+      },
+      [&](long long e, float g, float& p) {
+        float m = a.vmom[e], q = 0.f, qm = 0.f;
+        if (c.opt != OPT_SGD) { q = a.vsq[e]; if (c.opt == OPT_AMSGRAD) qm = a.vsqmax[e]; }
+        opt_update(g * inv_w, p, m, q, qm, c);
+        a.vmom[e] = m;
+        if (c.opt != OPT_SGD) { a.vsq[e] = q; if (c.opt == OPT_AMSGRAD) a.vsqmax[e] = qm; }
+      });
+}
+
+// Lion: the same walk, the Lion step on vparams / vmom (vectors take no weight decay)
+__device__ __forceinline__ void ps_vec_tile(const PsArgsLion& a, const OptC& c, const Unit2& u, const Tile2& t,
+                                            unsigned int wmask, bool all_workers, float inv_w) {
+  ps_vec_walk(
+      a, u, t, wmask, all_workers,
+      [&](long long e, const float4& g, float4& p) {
+        float4 m = *reinterpret_cast<float4*>(a.vmom + e);
+        lion_update(g.x * inv_w, p.x, m.x, c);
+        lion_update(g.y * inv_w, p.y, m.y, c);
+        lion_update(g.z * inv_w, p.z, m.z, c);
+        lion_update(g.w * inv_w, p.w, m.w, c);
+        *reinterpret_cast<float4*>(a.vmom + e) = m;
+      },
+      [&](long long e, float g, float& p) {
+        float m = a.vmom[e];
+        lion_update(g * inv_w, p, m, c);
+        a.vmom[e] = m;
+      });
 }
 
 // layer-wise: vectors take momentum-SGD (LARS) or Adam (LAMB) without weight decay and trust ratio

@@ -360,6 +360,7 @@ __device__ __forceinline__ void ps_qsgd(const A& a) {
 __global__ void __launch_bounds__(QPS_THREADS) v2_ps_qsgd_kernel(const PsArgs2 a) { ps_qsgd(a); }
 __global__ void __launch_bounds__(QPS_THREADS, 1) v2_ps_qsgd_lw_kernel(const PsArgsLw a) { ps_qsgd(a); }
 __global__ void __launch_bounds__(QPS_THREADS, 1) v2_ps_qsgd_gather_kernel(const PsArgsGather a) { ps_qsgd(a); }
+__global__ void __launch_bounds__(QPS_THREADS, 1) v2_ps_qsgd_lion_kernel(const PsArgsLion a) { ps_qsgd(a); }
 
 extern "C" {
 
@@ -411,6 +412,11 @@ void atomo_v2_launch_ps_qsgd_lw(const void* args, int grid, cudaStream_t stream)
 void atomo_v2_launch_ps_qsgd_gather(const void* args, int grid, cudaStream_t stream) {
   const PsArgsGather& a = *static_cast<const PsArgsGather*>(args);
   v2_ps_qsgd_gather_kernel<<<ps_grid(grid, a.ntiles), QPS_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_qsgd_lion(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsLion& a = *static_cast<const PsArgsLion*>(args);
+  v2_ps_qsgd_lion_kernel<<<ps_grid(grid, a.ntiles), QPS_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

@@ -210,6 +210,7 @@ __device__ __forceinline__ void ps_sign(const A& a) {
 __global__ void __launch_bounds__(SPS_THREADS) v2_ps_sign_kernel(const PsArgs2 a) { ps_sign(a); }
 __global__ void __launch_bounds__(SPS_THREADS, 1) v2_ps_sign_lw_kernel(const PsArgsLw a) { ps_sign(a); }
 __global__ void __launch_bounds__(SPS_THREADS, 1) v2_ps_sign_gather_kernel(const PsArgsGather a) { ps_sign(a); }
+__global__ void __launch_bounds__(SPS_THREADS, 1) v2_ps_sign_lion_kernel(const PsArgsLion a) { ps_sign(a); }
 
 // ---- --code-stats ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(SE_THREADS) v2_sign_code_stats_kernel(const ScaleStatArgs a) {
@@ -310,6 +311,11 @@ void atomo_v2_launch_ps_sign_lw(const void* args, int grid, cudaStream_t stream)
 void atomo_v2_launch_ps_sign_gather(const void* args, int grid, cudaStream_t stream) {
   const PsArgsGather& a = *static_cast<const PsArgsGather*>(args);
   v2_ps_sign_gather_kernel<<<ps_grid(grid, a.ntiles), SPS_THREADS, 0, stream>>>(a);
+}
+
+void atomo_v2_launch_ps_sign_lion(const void* args, int grid, cudaStream_t stream) {
+  const PsArgsLion& a = *static_cast<const PsArgsLion*>(args);
+  v2_ps_sign_lion_kernel<<<ps_grid(grid, a.ntiles), SPS_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

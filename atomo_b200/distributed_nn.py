@@ -38,6 +38,7 @@ def _kwargs(args, role: str) -> dict:
         kw.update({"num_aggregate": args.num_aggregate, "lr_shrinkage": args.lr_shrinkage,
                    "optimizer": args.optimizer, "weight_decay": args.weight_decay, "nesterov": args.nesterov,
                    "trust_coefficient": getattr(args, "trust_coefficient", 0.001),
+                   "lion_betas": tuple(getattr(args, "lion_betas", (0.9, 0.99))),
                    "clip_grad_norm": getattr(args, "clip_grad_norm", 0.0),
                    "ema_decay": getattr(args, "ema_decay", 0.0),
                    "resume": args.resume, "kill_stragglers": args.straggler_kill})

@@ -795,6 +795,7 @@ def plan_digest(plan: "Plan2") -> str:
 
 
 OPT_SGD, OPT_ADAM, OPT_AMSGRAD, OPT_LARS, OPT_LAMB = 0, 1, 2, 3, 4
+OPT_LION = 5      # bookkeeping: Lion runs the PS kernels' Lion instantiation (v2_ps_lion), never the plain one
 LAYERWISE_OPTS = (OPT_LARS, OPT_LAMB)
 
 

@@ -22,7 +22,7 @@ import torch
 
 from .. import codings
 from ..models import build_model
-from ..optim import LAMB, LARS, SGD, Adam, AdamW
+from ..optim import LAMB, LARS, SGD, Adam, AdamW, Lion
 from ..parallel.transport import Transport, STOP_STEP
 from ..utils import checkpoint as ckpt
 from ..utils.flags import check_clip_grad_norm, check_ema_decay
@@ -162,6 +162,10 @@ class SyncReplicasMaster_NN(NN_Trainer):
         elif self._optimizer_name == "adamw":
             self.optimizer = AdamW(self.network.parameters(), lr=self.lr,
                                    weight_decay=self._kwargs.get("weight_decay", 0.0))
+        elif self._optimizer_name == "lion":
+            self.optimizer = Lion(self.network.parameters(), lr=self.lr,
+                                  betas=tuple(self._kwargs.get("lion_betas", (0.9, 0.99))),
+                                  weight_decay=self._kwargs.get("weight_decay", 0.0))
         elif self._optimizer_name == "lamb":
             self.optimizer = LAMB(self.network.parameters(), lr=self.lr,
                                   weight_decay=self._kwargs.get("weight_decay", 0.0))

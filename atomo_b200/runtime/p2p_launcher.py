@@ -103,6 +103,8 @@ def _build_engine(args, model, rank, world):
             kw["accumulate_steps"] = accum      # the engine refuses a value below 1
         if args.optimizer in ("lars", "lamb"):
             kw["trust_coefficient"] = getattr(args, "trust_coefficient", 0.001)
+        if args.optimizer == "lion":
+            kw["betas"] = tuple(getattr(args, "lion_betas", (0.9, 0.99)))     # the engine checks them
         if clip:
             kw["clip_grad_norm"] = clip
         if getattr(args, "momentum_correction", False):
@@ -123,9 +125,9 @@ def _build_engine(args, model, rank, world):
     if args.optimizer in ("lars", "lamb"):
         raise SystemExit("--optimizer %s runs on the bf16 engine (--engine shadow, --dtype bf16); the fp32-flat engine "
                          "has no layer-wise trust ratio" % args.optimizer)
-    if args.optimizer == "adamw":
-        raise SystemExit("--optimizer adamw runs on the bf16 engine (--engine shadow, --dtype bf16); the fp32-flat "
-                         "engine fuses momentum-SGD only and has no decoupled weight decay")
+    if args.optimizer in ("adamw", "lion"):
+        raise SystemExit("--optimizer %s runs on the bf16 engine (--engine shadow, --dtype bf16); the fp32-flat "
+                         "engine fuses momentum-SGD only and has no decoupled weight decay" % args.optimizer)
     from .engine import FusedEngine
     if accum != 1:
         raise SystemExit("--accumulate-steps runs on the bf16 engine (--dtype bf16, --engine auto|shadow, --code "

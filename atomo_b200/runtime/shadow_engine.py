@@ -96,6 +96,10 @@ one central PS kernel at the end of the step):
   ``Ctrl2.decay_factor``, which ``set_lr`` rewrites.  The PS kernels then run Adam (AMSGrad with ``amsgrad=True``)
   with weight decay 0.  1-D parameters (BN, biases) take no decay.  With ``weight_decay=0`` it is ``adam``, bit for
   bit, and launches nothing new.
+* Lion (``optimizer="lion"``, ``betas`` default ``(0.9, 0.99)``; ``optim/lion.py`` is the oracle): the code's PS
+  kernel runs its Lion instantiation (``v2_ps_lion``): ``p -= lr sign(b1 m + (1 - b1) g)``, ``m = b2 m + (1 - b2) g``
+  on ``master`` / ``mom`` and ``vparams`` / ``vmom``, no second moments allocated.  Weight decay is AdamW's decay
+  launch before it.  Clipping, Nesterov, AMSGrad, ``code="signum"`` and momentum correction are refused.
 
 Per step and rank: ``wait_params`` -> forward -> backward [group hooks -> encode, project+push on stream E;
 PS launch of the group on stream P] -> join -> ``advance_step``.  All cross-GPU ordering is carried by
@@ -129,7 +133,7 @@ def _dev_bytes(b: bytes, device) -> torch.Tensor:
 class ShadowEngine:
     def __init__(self, model: nn.Module, rank: int = 0, world: int = 1, code: str = "svd", svd_rank: int = 3,
                  lr: float = 0.01, momentum: float = 0.0, weight_decay: float = 0.0, nesterov: bool = False,
-                 dampening: float = 0.0, optimizer: str = "sgd", betas=(0.9, 0.999), eps: float = 1e-8,
+                 dampening: float = 0.0, optimizer: str = "sgd", betas=None, eps: float = 1e-8,
                  amsgrad: bool = False, ps_mode: str = "sharded", groups: int = 5, sampling: str = "bernoulli",
                  prob_rule: str = "reference", random_sample: bool = True, seed: int = 1, use_graph: bool = True,
                  group=None, multicast: bool = True, heap_mode: str = "auto", timeout_s: float = 30.0,
@@ -141,17 +145,38 @@ class ShadowEngine:
                  error_feedback: bool = False, accumulate_steps: int = 1, trust_coefficient: float = 0.001,
                  clip_grad_norm: float = 0.0, momentum_correction: bool = False, ema_decay: float = 0.0):
         self.optimizer = optimizer.lower()
-        if self.optimizer not in ("sgd", "adam", "adamw", "lars", "lamb"):      # checked before any CUDA work
-            raise ValueError("ShadowEngine optimizers: sgd | adam | adamw | lars | lamb (got %r)" % (optimizer,))
+        if self.optimizer not in ("sgd", "adam", "adamw", "lars", "lamb", "lion"):      # checked before any CUDA work
+            raise ValueError("ShadowEngine optimizers: sgd | adam | adamw | lars | lamb | lion (got %r)" % (optimizer,))
         self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
         self.signum = self.code == "signum"
-        # AdamW and Signum: the PS kernels run with weight_decay 0; the decoupled decay of the weights is its own pass
+        self.lion = self.optimizer == "lion"
+        if betas is None:
+            betas = (0.9, 0.99) if self.lion else (0.9, 0.999)
+        if self.lion:       # checked before any CUDA work
+            if len(betas) != 2 or not all(not isinstance(b, bool) and isinstance(b, numbers.Real) and 0 <= b < 1
+                                          for b in betas):
+                raise ValueError("lion: betas must be two finite numbers in [0, 1) (got %r)" % (betas,))
+            if nesterov:
+                raise ValueError("lion takes no Nesterov momentum: nesterov=False")
+            if amsgrad:
+                raise ValueError("lion keeps no second moment: amsgrad=False")
+            if self.signum:
+                raise ValueError("lion cannot be combined with code='signum': the owners step by the vote")
+            if momentum_correction:
+                raise ValueError("lion cannot be combined with momentum_correction: the parameter server must run "
+                                 "plain SGD")
+            if check_clip_grad_norm(clip_grad_norm) > 0:
+                raise ValueError("lion cannot be combined with clip_grad_norm yet: the clip launch steps Adam and "
+                                 "momentum-SGD only")
+        self.betas = (float(betas[0]), float(betas[1]))
+        # AdamW, Lion and Signum: the PS kernels run with weight_decay 0; the decoupled decay of the weights is its own
+        # pass
         self.adamw_wd = 0.0
-        if self.optimizer == "adamw" or self.signum:      # checked before any CUDA work
+        if self.optimizer in ("adamw", "lion") or self.signum:      # checked before any CUDA work
             if isinstance(weight_decay, bool) or not isinstance(weight_decay, numbers.Real) \
                     or not 0 <= weight_decay < math.inf:
                 raise ValueError("%s: weight_decay must be finite and >= 0 (got %r)"
-                                 % ("signum" if self.signum else "adamw", weight_decay))
+                                 % ("signum" if self.signum else self.optimizer, weight_decay))
             self.adamw_wd, weight_decay = float(weight_decay), 0.0
         self.decay_on = self.adamw_wd > 0     # with weight_decay 0 AdamW is Adam: nothing new is launched
         self.layerwise = self.optimizer in ("lars", "lamb")
@@ -306,7 +331,7 @@ class ShadowEngine:
         self.step, self.lr = 1, lr
         adam_opt = P2.OPT_AMSGRAD if amsgrad else P2.OPT_ADAM
         self.opt = {"sgd": P2.OPT_SGD, "adam": adam_opt, "adamw": adam_opt, "lars": P2.OPT_LARS,
-                    "lamb": P2.OPT_LAMB}[self.optimizer]
+                    "lamb": P2.OPT_LAMB, "lion": P2.OPT_LION}[self.optimizer]
         self.launches_per_step = 0
 
         # ---- model: NHWC activations, fused BN ------------------------------------------------------------
@@ -465,11 +490,11 @@ class ShadowEngine:
         self.cnt_ps_group = self.cnt_enc_group + 4 * P2.MAX_GROUPS
         # momentum correction: momentum, weight decay and Nesterov act on the workers (v2_mc_apply), the PS runs plain SGD
         self.mc_momentum, self.mc_weight_decay, self.mc_nesterov = float(momentum), float(weight_decay), bool(nesterov)
-        if self.momentum_correction or self.signum:
+        if self.momentum_correction or self.signum or self.lion:     # lion: --momentum is ignored, as for Adam
             momentum, dampening, weight_decay, nesterov = 0.0, 0.0, 0.0, False
         self.ctrl = _dev_bytes(P2.pack_ctrl2(step=1, lr=lr, momentum=momentum, dampening=dampening,
                                              weight_decay=weight_decay, nesterov=nesterov, first_step=1, seed=seed,
-                                             beta1=betas[0], beta2=betas[1], eps=eps, opt=self.opt,
+                                             beta1=self.betas[0], beta2=self.betas[1], eps=eps, opt=self.opt,
                                              num_aggregate=num_aggregate,
                                              trust_coefficient=self.trust_coefficient if self.layerwise else 0.0,
                                              clip_grad_norm=self.clip_grad_norm,
@@ -628,7 +653,7 @@ class ShadowEngine:
             self.ctrl_f32[17] = self.decay_factor(lr)      # Ctrl2::decay_factor, read by every decay launch
 
     def decay_factor(self, lr: float) -> float:
-        """AdamW and Signum: the factor of the decoupled weight decay at learning rate ``lr``, ``1 - lr * wd`` in double
+        """AdamW, Lion and Signum: the factor of the decoupled weight decay at learning rate ``lr``, ``1 - lr * wd`` in double
         (as torch.optim.AdamW computes it in Python) rounded to fp32 once."""
         return float(np.float32(1.0 - float(lr) * self.adamw_wd))
 
@@ -938,7 +963,10 @@ class ShadowEngine:
             self._launch_ps_layerwise(g, final, t0, nt)
         else:
             self._launch_decay(g)
-            self._launch_ps_code(g, final, t0, nt)
+            if self.lion:
+                self._launch_ps_lion(g, final, t0, nt)
+            else:
+                self._launch_ps_code(g, final, t0, nt)
             self._launch_ema(g)
 
     def _launch_ps_code(self, g: int, final: bool, t0: int, nt: int):
@@ -1007,6 +1035,20 @@ class ShadowEngine:
                 self.t_stage_peer.data_ptr(), self.heap.region_ptr("arena"), pl.arena_floats,
                 self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(), self.cnt_ps_group + 4 * g,
                 self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W, max(1, min(self.ps_grid, max(nt, 1))))
+        self._nlaunch += 1
+
+    def _launch_ps_lion(self, g: int, final: bool, t0: int, nt: int):
+        """Lion: the code's PS kernel with the Lion epilogue (decode and sum as the plain launch; ``master`` / ``mom``
+        and ``vparams`` / ``vmom`` stepped, the new parameters broadcast; the last group publishes them)."""
+        C, pl = self.C, self.plan
+        C.v2_ps_lion(self._ps_kind(), self.t_units.data_ptr(), self.t_ps_tiles.data_ptr(), t0, nt, self.W, self.world,
+                     g, final, self.owner_index, self.master.data_ptr(), self.mom.data_ptr(), self.vmom.data_ptr(),
+                     self.wshadow_mc, self.t_wshadow_peer.data_ptr(), self.vparams.data_ptr(), self.vparams_mc,
+                     self.t_vparams_peer.data_ptr(), self.vgrads_mc, self.t_vgrads_peer.data_ptr(),
+                     self.t_stage_peer.data_ptr(), self.heap.region_ptr("arena"), pl.arena_floats,
+                     self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
+                     self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
+                     max(1, min(self.ps_grid, max(nt, 1))), self.q_max_level, self.q_max_bucket)
         self._nlaunch += 1
 
     def _launch_ps_layerwise(self, g: int, final: bool, t0: int, nt: int):
@@ -1441,7 +1483,7 @@ class ShadowEngine:
         if self.world > 1:
             dist.all_reduce(vm, group=self.group)
         adam_state = {}
-        if self.opt != P2.OPT_SGD and self.opt != P2.OPT_LARS:      # Adam / AMSGrad / LAMB: second moments too
+        if self.opt in (P2.OPT_ADAM, P2.OPT_AMSGRAD, P2.OPT_LAMB):      # Adam / AMSGrad / LAMB: second moments too
             # (collective gathers, every rank takes part)
             names = [("sq", "vsq")] + ([("sqmax", "vsqmax")] if self.opt == P2.OPT_AMSGRAD else [])
             for wname, vname in names:
@@ -1475,6 +1517,8 @@ class ShadowEngine:
             side.update(momentum_correction=True)
         if self.signum:
             side.update(signum_momentum=self.mc_momentum, weight_decay=self.adamw_wd)
+        if self.lion:       # Lion's one state is mom_w / mom_v above
+            side.update(lion_betas=self.betas, weight_decay=self.adamw_wd)
         side.update(adam_state)
         torch.save(side, path + "_optim.tmp")
         os.replace(path + "_optim.tmp", path + "_optim")
@@ -1543,8 +1587,8 @@ class ShadowEngine:
         if os.path.exists(path + "_optim"):     # refused before any state changes
             side = torch.load(path + "_optim", map_location="cpu", weights_only=False)
             saved = side.get("optimizer", "sgd or adam")
-            layerwise = ("lars", "lamb")
-            if (self.layerwise or saved in layerwise) and saved != self.optimizer:
+            own_state = ("lars", "lamb", "lion")       # optimizers whose state no other optimizer can continue
+            if (self.optimizer in own_state or saved in own_state) and saved != self.optimizer:
                 raise ValueError("checkpoint %s was written by optimizer %s; this engine runs %s" % (path, saved,
                                                                                                   self.optimizer))
             if bool(side.get("momentum_correction", False)) != self.momentum_correction:

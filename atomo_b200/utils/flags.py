@@ -72,11 +72,17 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                    "elements below 1, else an atom count (top-k sends floor of it)")
     p.add_argument("--sampling", type=str, default="bernoulli", choices=["bernoulli", "systematic"])
     p.add_argument("--prob-rule", type=str, default="reference", choices=["reference", "waterfill"])
-    p.add_argument("--optimizer", type=str, default="sgd", choices=["sgd", "adam", "adamw", "lars", "lamb"],
+    p.add_argument("--optimizer", type=str, default="sgd", choices=["sgd", "adam", "adamw", "lars", "lamb", "lion"],
                    help="lars / lamb: layer-wise trust ratios (LARS on momentum-SGD, LAMB on Adam) for large batches; "
                         "adamw: Adam with decoupled weight decay (torch.optim.AdamW), every weight (2 or more "
                         "dimensions) scaled by 1 - lr * --weight-decay before the Adam step, BN / bias vectors not "
-                        "decayed; p2p backend on the bf16 engine (--engine shadow), or the gloo / nccl role path")
+                        "decayed; lion: Lion (Chen et al. 2023), w <- w - lr * sign(b1 m + (1 - b1) g) and m <- b2 m + "
+                        "(1 - b2) g with b1, b2 = --lion-betas, one fp32 state per weight and --weight-decay decoupled "
+                        "as in adamw; --momentum is ignored, and --nesterov, --clip-grad-norm and --code signum are "
+                        "refused; p2p backend on the bf16 engine (--engine shadow), or the gloo / nccl role path")
+    p.add_argument("--lion-betas", type=float, nargs=2, default=[0.9, 0.99], metavar=("B1", "B2"),
+                   help="--optimizer lion: the interpolation beta of the step's sign (b1) and the momentum's beta (b2), "
+                        "each in [0, 1); ignored by the other optimizers")
     p.add_argument("--trust-coefficient", type=float, default=0.001,
                    help="--optimizer lars: eta of the trust ratio eta ||w|| / (||g|| + wd ||w||)")
     p.add_argument("--clip-grad-norm", type=float, default=0.0,
