@@ -171,7 +171,14 @@ void atomo_v2_launch_ps_signum(const void* units, const void* tiles, int tile0, 
                                float* const* vparams_peer, const float* vgrads_mc, const float* const* vgrads_peer,
                                const float* arenas, long long arena_floats, int* sig, int* const* sig_peer, void* ctrl,
                                unsigned int* group_counter, long long timeout, long long* tstats, float inv_w, int grid,
-                               const float* vext, long long vext_stride, cudaStream_t stream);
+                               const float* vext, long long vext_stride, int mean, cudaStream_t stream);
+// v2_signum.cu (Distributed Lion on the bf16 engine: Signum's push and PS with Lion's worker rule)
+void atomo_v2_launch_dlion_encode(const void* units, const void* tiles, int tile0, int ntiles, const long long* gptr,
+                                  const void* vchunks, int nv, float* vgrads, float* mom, float* vmom, float b1,
+                                  float b2, float* const* arena_peer, int* const* sig_peer, int n_owners,
+                                  long long arena_floats, int worker, int group, const void* ctrl,
+                                  unsigned int* group_counter, long long* tstats, int final_group,
+                                  const float* ext_uniforms, cudaStream_t stream);
 // v2_fp8.cu (fp8 units of the bf16 engine)
 void atomo_v2_launch_fp8_encode(const void* units, const void* tiles, int tile0, int ntiles, const long long* gptr,
                                 float* const* arena_peer, int* const* sig_peer, int n_owners, long long arena_floats,
@@ -801,14 +808,36 @@ void v2_signum_encode(uint64_t units, uint64_t tiles, int tile0, int ntiles, uin
                                 P<long long>(tstats), final_group ? 1 : 0, P<const float>(ext_uniforms), cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
-// Signum PS: the arguments of v2_ps_sign, then the tests' vector coin uniforms ([worker][vparams index], 0 = Philox)
+// Distributed Lion: the arguments of v2_signum_encode with Lion's two betas in place of beta.  The pushed bit is the
+// sign of c = b1 m + (1 - b1) g, then m = b2 m + (1 - b2) g.  mom == 0 (b1 == 0): c = g, and no vector chunks.
+void v2_dlion_encode(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t vchunks, int nv,
+                     uint64_t vgrads, uint64_t mom, uint64_t vmom, double b1, double b2, uint64_t arena_peer,
+                     uint64_t sig_peer, int n_owners, int64_t arena_floats, int worker, int group, uint64_t ctrl,
+                     uint64_t group_counter, uint64_t tstats, bool final_group, uint64_t ext_uniforms) {
+  TORCH_CHECK(worker >= 0 && worker < 16, "v2_dlion_encode: worker index must be in [0, 16)");
+  TORCH_CHECK(ntiles >= 0 && nv >= 0 && tile0 >= 0, "v2_dlion_encode: bad tile / chunk range");
+  TORCH_CHECK(b1 >= 0.0 && b1 < 1.0 && b2 >= 0.0 && b2 < 1.0, "v2_dlion_encode: b1 and b2 must be in [0, 1)");
+  TORCH_CHECK(ntiles == 0 || (units != 0 && tiles != 0 && gptr != 0 && arena_peer != 0 && sig_peer != 0 && ctrl != 0),
+              "v2_dlion_encode: units / tiles / gptr / arena / signal tables required");
+  TORCH_CHECK(ntiles == 0 || (mom != 0) == (b1 > 0.0), "v2_dlion_encode: a momentum buffer exactly when b1 > 0");
+  TORCH_CHECK(nv == 0 || (b1 > 0.0 && vchunks != 0 && vgrads != 0 && vmom != 0),
+              "v2_dlion_encode: vector chunks need b1 > 0 and vgrads / vmom");
+  atomo_v2_launch_dlion_encode(P<const void>(units), P<const void>(tiles), tile0, ntiles, P<const long long>(gptr),
+                               P<const void>(vchunks), nv, P<float>(vgrads), P<float>(mom), P<float>(vmom), (float)b1,
+                               (float)b2, P<float* const>(arena_peer), P<int* const>(sig_peer), n_owners,
+                               arena_floats, worker, group, P<const void>(ctrl), P<unsigned int>(group_counter),
+                               P<long long>(tstats), final_group ? 1 : 0, P<const float>(ext_uniforms), cur_stream());
+  C10_CUDA_KERNEL_LAUNCH_CHECK();
+}
+// Signum PS: the arguments of v2_ps_sign, then the tests' vector coin uniforms ([worker][vparams index], 0 = Philox);
+// mean = true steps by the mean of the counted signs (Distributed Lion's Avg) instead of their vote
 void v2_ps_signum(uint64_t units, uint64_t tiles, int tile0, int ntiles, int W, int nranks, int group,
                   bool final_group, int owner, uint64_t master, uint64_t mom, uint64_t sq, uint64_t sqmax,
                   uint64_t vmom, uint64_t vsq, uint64_t vsqmax, uint64_t wshadow_mc, uint64_t wshadow_peer,
                   uint64_t vparams_local, uint64_t vparams_mc, uint64_t vparams_peer, uint64_t vgrads_mc,
                   uint64_t vgrads_peer, uint64_t arenas, int64_t arena_floats, uint64_t sig, uint64_t sig_peer,
                   uint64_t ctrl, uint64_t group_counter, int64_t timeout, uint64_t tstats, double inv_w, int grid,
-                  uint64_t vext, int64_t vext_stride) {
+                  uint64_t vext, int64_t vext_stride, bool mean) {
   TORCH_CHECK(W >= 1 && W <= 16, "too many workers for v2_ps_signum");
   TORCH_CHECK(ntiles >= 0 && tile0 >= 0, "v2_ps_signum: bad tile range");
   atomo_v2_launch_ps_signum(P<const void>(units), P<const void>(tiles), tile0, ntiles, W, nranks, group,
@@ -818,7 +847,8 @@ void v2_ps_signum(uint64_t units, uint64_t tiles, int tile0, int ntiles, int W, 
                             P<float* const>(vparams_peer), P<const float>(vgrads_mc),
                             P<const float* const>(vgrads_peer), P<const float>(arenas), arena_floats, P<int>(sig),
                             P<int* const>(sig_peer), P<void>(ctrl), P<unsigned int>(group_counter), timeout,
-                            P<long long>(tstats), (float)inv_w, grid, P<const float>(vext), vext_stride, cur_stream());
+                            P<long long>(tstats), (float)inv_w, grid, P<const float>(vext), vext_stride, mean ? 1 : 0,
+                            cur_stream());
   C10_CUDA_KERNEL_LAUNCH_CHECK();
 }
 void v2_sign_code_stats(uint64_t units, uint64_t tiles, int tile0, int ntiles, uint64_t gptr, uint64_t arena_peer,
@@ -1311,7 +1341,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("vparams_mc"), py::arg("vparams_peer"), py::arg("vgrads_mc"), py::arg("vgrads_peer"),
         py::arg("arenas"), py::arg("arena_floats"), py::arg("sig"), py::arg("sig_peer"), py::arg("ctrl"),
         py::arg("group_counter"), py::arg("timeout"), py::arg("tstats"), py::arg("inv_w"), py::arg("grid"),
-        py::arg("vext") = 0, py::arg("vext_stride") = 0);
+        py::arg("vext") = 0, py::arg("vext_stride") = 0, py::arg("mean") = false);
+  m.def("v2_dlion_encode", &v2_dlion_encode, py::arg("units"), py::arg("tiles"), py::arg("tile0"), py::arg("ntiles"),
+        py::arg("gptr"), py::arg("vchunks"), py::arg("nv"), py::arg("vgrads"), py::arg("mom"), py::arg("vmom"),
+        py::arg("b1"), py::arg("b2"), py::arg("arena_peer"), py::arg("sig_peer"), py::arg("n_owners"),
+        py::arg("arena_floats"), py::arg("worker"), py::arg("group"), py::arg("ctrl"), py::arg("group_counter"),
+        py::arg("tstats"), py::arg("final_group"), py::arg("ext_uniforms") = 0);
   m.def("v2_fp8_encode", &v2_fp8_encode, py::arg("units"), py::arg("tiles"), py::arg("tile0"), py::arg("ntiles"),
         py::arg("gptr"), py::arg("arena_peer"), py::arg("sig_peer"), py::arg("n_owners"), py::arg("arena_floats"),
         py::arg("worker"), py::arg("group"), py::arg("ctrl"), py::arg("group_counter"), py::arg("tstats"),

@@ -7,6 +7,7 @@
 #include <type_traits>
 
 #include "v2_common.cuh"
+#include "v2_momentum.cuh"
 
 namespace atomo {
 namespace v2 {
@@ -293,10 +294,10 @@ __device__ __forceinline__ void update1(const PsArgs2& a, const OptC& c, long lo
 struct PsArgsLion : PsArgs2 {};
 
 __device__ __forceinline__ void lion_update(float g, float& p, float& m, const OptC& c) {
-  const float cc = __fadd_rn(__fmul_rn(c.b1, m), __fmul_rn(__fsub_rn(1.f, c.b1), g));
+  const float cc = lion_direction(g, m, c.b1);      // v2_momentum.cuh: Distributed Lion's workers round the same way
   const float s = cc > 0.f ? 1.f : cc < 0.f ? -1.f : cc == 0.f ? 0.f : cc;
   p = __fsub_rn(p, __fmul_rn(c.lr, s));
-  m = __fadd_rn(__fmul_rn(c.b2, m), __fmul_rn(__fsub_rn(1.f, c.b2), g));
+  m = lion_momentum(g, m, c.b2);
 }
 
 __device__ __forceinline__ void update8(const PsArgsLion& a, const OptC& c, long long e, const float (&g)[8]) {

@@ -1,6 +1,6 @@
-// Signum with majority vote (Bernstein et al., ICML 2018 / ICLR 2019) on the overlapped, sharded bf16 engine (sm_90a):
-// the worker-side momentum, 1-bit encode and push of ONE backward group, and the owner-side vote and step.  The oracle
-// is codings/signum.py.
+// Signum with majority vote (Bernstein et al., ICML 2018 / ICLR 2019) and Distributed Lion (Liu et al., NeurIPS 2024) on
+// the overlapped, sharded bf16 engine (sm_90a): the worker-side momentum, 1-bit encode and push of ONE backward group,
+// and the owner-side vote (or mean) and step.  The oracles are codings/signum.py and codings/dlion.py.
 //
 //   v2_signum_encode_kernel  blocks [0, ntiles): one CTA per PS tile (one bucket of at most 4096 elements, one
 //                            destination owner), 16 consecutive elements per thread.  The bf16 gradient g is read in
@@ -15,6 +15,9 @@
 //                            and vgrads (the owners read vgrads).  The last CTA of the launch, tile or vector, publishes
 //                            flag[group][worker] = step.  The group's only launch.  Bandwidth bound: 2 bytes read, 4 + 4
 //                            read and written per weight element, 1/8 byte pushed.
+//   v2_dlion_encode_kernel   the same launch with Lion's two-beta worker rule (v2_momentum.cuh) in place of
+//                            the heavy-ball one: the bit is the sign of c = b1 m + (1 - b1) g, then m = b2 m + (1 - b2) g;
+//                            vgrads receives c and vmom m.  With b1 == 0, c = g: no buffer and no vector chunks.
 //   v2_ps_signum_kernel      one launch per (group, owner): the push wait / --num-aggregate mask and the stale-slot
 //                            check of v2_ps_common.cuh.  Per weight tile and element, the 1 bits (neg) of the counted
 //                            workers are summed by per-thread counters, pos = counted - neg, and
@@ -23,6 +26,8 @@
 //                            and weight decay 0, then the bf16 broadcast.  Vector tiles vote the same way on the sign of
 //                            every counted worker's fp32 vgrads value, zeros by the same coin, any NaN / Inf value making
 //                            the tile's vote NaN.
+//   v2_ps_signum_mean_kernel the same launch with Distributed Lion's mean in place of the vote:
+//                            v = (pos - neg) / counted (one rounded division; 0 when nothing is counted).
 #include "v2_entry_encode.cuh"
 #include "v2_momentum.cuh"
 
@@ -60,17 +65,45 @@ __device__ __forceinline__ float signum_vote(int pos, int neg) {
   return pos > neg ? 1.f : (neg > pos ? -1.f : 0.f);
 }
 
+// the owners' aggregate of pos positive and neg negative signs: the vote, or (MEAN) their mean, 0 when nothing is counted
+template <bool MEAN>
+__device__ __forceinline__ float signum_aggregate(int pos, int neg) {
+  if constexpr (MEAN)
+    return pos + neg == 0 ? 0.f : __fdiv_rn((float)(pos - neg), (float)(pos + neg));
+  else
+    return signum_vote(pos, neg);
+}
+
 struct SignumEncArgs : PushArgs {
   int ntiles;                  // blocks [0, ntiles) are PS tiles, the rest vector chunks
   const EfChunk* vchunks;      // the group's vector chunks (plan2.vec_chunks), or nullptr
   float* mom;                  // worker momentum indexed like wshadow, or nullptr (beta == 0)
   float* vgrads;
   float* vmom;                 // worker momentum indexed like vgrads
-  float beta;
+  float beta;                  // Distributed Lion: b1
   const float* ext_uniforms;   // tests: uniforms indexed like wshadow, replacing the coin's Philox
 };
 
-__device__ __forceinline__ void signum_encode_tile(const SignumEncArgs& a, int step) {
+struct DlionEncArgs : SignumEncArgs {
+  float b2;
+};
+
+// The worker rules: the direction whose sign is pushed, from the gradient g and the worker's momentum m (updated in place)
+struct HeavyBallRule {         // Signum: u = beta u + g, the direction is u
+  float beta;
+  __device__ __forceinline__ float operator()(float g, float& m) const { return mc_step(g, m, beta, false); }
+};
+struct LionRule {              // Distributed Lion: c = b1 m + (1 - b1) g, then m = b2 m + (1 - b2) g
+  float b1, b2;
+  __device__ __forceinline__ float operator()(float g, float& m) const {
+    const float c = lion_direction(g, m, b1);
+    m = lion_momentum(g, m, b2);
+    return c;
+  }
+};
+
+template <class Rule>
+__device__ __forceinline__ void signum_encode_tile(const SignumEncArgs& a, int step, const Rule& rule) {
   const Tile2 t = a.tiles[blockIdx.x];
   const Unit2 u = a.units[t.unit];
   const int tid = threadIdx.x, lane = tid & 31;
@@ -93,10 +126,10 @@ __device__ __forceinline__ void signum_encode_tile(const SignumEncArgs& a, int s
 #pragma unroll
       for (int j = 0; j < SG_PER_THREAD / 4; ++j) {
         float4 v = reinterpret_cast<const float4*>(up)[j];
-        x[4 * j] = mc_step(x[4 * j], v.x, a.beta, false);
-        x[4 * j + 1] = mc_step(x[4 * j + 1], v.y, a.beta, false);
-        x[4 * j + 2] = mc_step(x[4 * j + 2], v.z, a.beta, false);
-        x[4 * j + 3] = mc_step(x[4 * j + 3], v.w, a.beta, false);
+        x[4 * j] = rule(x[4 * j], v.x);
+        x[4 * j + 1] = rule(x[4 * j + 1], v.y);
+        x[4 * j + 2] = rule(x[4 * j + 2], v.z);
+        x[4 * j + 3] = rule(x[4 * j + 3], v.w);
         reinterpret_cast<float4*>(up)[j] = v;
       }
     } else {
@@ -104,7 +137,7 @@ __device__ __forceinline__ void signum_encode_tile(const SignumEncArgs& a, int s
       for (int i = 0; i < SG_PER_THREAD; ++i) {
         if (i < n) {
           float ui = up[i];
-          x[i] = mc_step(x[i], ui, a.beta, false);
+          x[i] = rule(x[i], ui);
           up[i] = ui;
         }
       }
@@ -139,11 +172,12 @@ __device__ __forceinline__ void signum_encode_tile(const SignumEncArgs& a, int s
   }
 }
 
-__global__ void __launch_bounds__(SG_THREADS) v2_signum_encode_kernel(const SignumEncArgs a) {
+template <class Rule>
+__device__ __forceinline__ void signum_encode(const SignumEncArgs& a, const Rule& rule) {
   if (blockIdx.x == 0 && threadIdx.x == 0 && a.tstats != nullptr) a.tstats[9 + a.group] = globaltimer_ns();
   const int step = a.ctrl->step;
   if ((int)blockIdx.x < a.ntiles) {
-    signum_encode_tile(a, step);
+    signum_encode_tile(a, step, rule);
     return;
   }
   const EfChunk c = a.vchunks[blockIdx.x - a.ntiles];
@@ -151,11 +185,19 @@ __global__ void __launch_bounds__(SG_THREADS) v2_signum_encode_kernel(const Sign
   float* um = a.vmom + c.w_off + c.start;
   for (int i = threadIdx.x; i < c.count; i += blockDim.x) {
     float ui = um[i];
-    s[i] = mc_step(s[i], ui, a.beta, false);
+    s[i] = rule(s[i], ui);
     um[i] = ui;
   }
   __syncthreads();
   if (threadIdx.x == 0) enc_push_flag(a, step);
+}
+
+__global__ void __launch_bounds__(SG_THREADS) v2_signum_encode_kernel(const SignumEncArgs a) {
+  signum_encode(a, HeavyBallRule{a.beta});
+}
+
+__global__ void __launch_bounds__(SG_THREADS) v2_dlion_encode_kernel(const DlionEncArgs a) {
+  signum_encode(a, LionRule{a.beta, a.b2});
 }
 
 // ---- PS: vote + step --------------------------------------------------------------------------------------------
@@ -164,8 +206,9 @@ struct SignumPsArgs : PsArgs2 {
   long long vext_stride;
 };
 
-// the vote of a vector tile into OUT (NaN everywhere when a counted value is not finite), then the step and the fp32
-// broadcast
+// the vote (or mean) of a vector tile into OUT (NaN everywhere when a counted value is not finite), then the step and
+// the fp32 broadcast
+template <bool MEAN>
 __device__ __forceinline__ void signum_vec_tile(const SignumPsArgs& a, const OptC& c, const Unit2& u, const Tile2& t,
                                                 int unit, unsigned int wmask, int step, float* OUT) {
   const int tid = threadIdx.x;
@@ -187,7 +230,7 @@ __device__ __forceinline__ void signum_vec_tile(const SignumPsArgs& a, const Opt
       bad |= cls == 3u;
       ++cnt;
     }
-    OUT[i] = signum_vote(cnt - neg, neg);
+    OUT[i] = signum_aggregate<MEAN>(cnt - neg, neg);
   }
   const int nonfinite = __syncthreads_or(bad);
   for (int i = tid; i < t.b; i += blockDim.x) {
@@ -198,7 +241,8 @@ __device__ __forceinline__ void signum_vec_tile(const SignumPsArgs& a, const Opt
   }
 }
 
-__global__ void __launch_bounds__(SG_THREADS) v2_ps_signum_kernel(const SignumPsArgs a) {
+template <bool MEAN>
+__device__ __forceinline__ void ps_signum(const SignumPsArgs& a) {
   __shared__ __align__(16) float OUT[SG_TILE_ELEMS];   // the votes of one tile, physical element order
   __shared__ int s_ok, s_bad, s_nf;
   __shared__ unsigned int s_mask, s_use;
@@ -210,7 +254,7 @@ __global__ void __launch_bounds__(SG_THREADS) v2_ps_signum_kernel(const SignumPs
   ps_wait(a, ctrl, step, s_ok, s_bad, s_mask, s_t_enter, s_t_ready);
   const bool ok = s_ok != 0;
   const unsigned int wmask = s_mask;
-  // the step is p - lr vote: the momentum lives on the workers, and the weight decay is v2_decay's launch before this one
+  // the step is p - lr vote (or mean): the momentum lives on the workers, and the weight decay is v2_decay's launch before this one
   OptC c = ps_opt_consts(ctrl, step);
   c.opt = OPT_SGD; c.mu = 0.f; c.wd = 0.f;
   const auto [t_begin, t_end] = ps_tile_range(a);
@@ -218,7 +262,7 @@ __global__ void __launch_bounds__(SG_THREADS) v2_ps_signum_kernel(const SignumPs
     const Tile2 t = a.tiles[ti];
     const Unit2 u = a.units[t.unit];
     if (u.kind == KIND_VEC) {
-      signum_vec_tile(a, c, u, t, t.unit, wmask, step, OUT);
+      signum_vec_tile<MEAN>(a, c, u, t, t.unit, wmask, step, OUT);
       continue;
     }
     if (u.kind != KIND_SIGNUM) continue;
@@ -253,7 +297,8 @@ __global__ void __launch_bounds__(SG_THREADS) v2_ps_signum_kernel(const SignumPs
       const bool nf = s_nf != 0;
 #pragma unroll
       for (int i = 0; i < SG_PER_THREAD; ++i)
-        if (i0 + i < t.b) OUT[i0 + i] = nf ? __int_as_float(0x7fffffff) : signum_vote(counted - neg[i], neg[i]);
+        if (i0 + i < t.b)
+          OUT[i0 + i] = nf ? __int_as_float(0x7fffffff) : signum_aggregate<MEAN>(counted - neg[i], neg[i]);
     }
     __syncthreads();
     // fused SGD epilogue + bf16 parameter broadcast
@@ -271,6 +316,10 @@ __global__ void __launch_bounds__(SG_THREADS) v2_ps_signum_kernel(const SignumPs
   __syncthreads();
   if (tid == 0) ps_complete(a, ctrl, step, s_bad != 0, s_t_enter, s_t_ready);
 }
+
+__global__ void __launch_bounds__(SG_THREADS) v2_ps_signum_kernel(const SignumPsArgs a) { ps_signum<false>(a); }
+
+__global__ void __launch_bounds__(SG_THREADS) v2_ps_signum_mean_kernel(const SignumPsArgs a) { ps_signum<true>(a); }
 
 extern "C" {
 
@@ -291,6 +340,23 @@ void atomo_v2_launch_signum_encode(const void* units, const void* tiles, int til
   v2_signum_encode_kernel<<<ntiles + nv, SG_THREADS, 0, stream>>>(a);
 }
 
+void atomo_v2_launch_dlion_encode(const void* units, const void* tiles, int tile0, int ntiles, const long long* gptr,
+                                  const void* vchunks, int nv, float* vgrads, float* mom, float* vmom, float b1,
+                                  float b2, float* const* arena_peer, int* const* sig_peer, int n_owners,
+                                  long long arena_floats, int worker, int group, const void* ctrl,
+                                  unsigned int* group_counter, long long* tstats, int final_group,
+                                  const float* ext_uniforms, cudaStream_t stream) {
+  if (ntiles + nv <= 0) return;
+  DlionEncArgs a;
+  a.units = (const Unit2*)units; a.tiles = (const Tile2*)tiles + tile0; a.gptr = gptr;
+  a.arena_peer = arena_peer; a.sig_peer = sig_peer; a.n_owners = n_owners; a.arena_floats = arena_floats;
+  a.worker = worker; a.group = group; a.ctrl = (const Ctrl2*)ctrl; a.group_counter = group_counter;
+  a.tstats = tstats; a.final_group = final_group; a.residual = nullptr;
+  a.ntiles = ntiles; a.vchunks = (const EfChunk*)vchunks; a.mom = mom; a.vgrads = vgrads; a.vmom = vmom; a.beta = b1;
+  a.b2 = b2; a.ext_uniforms = ext_uniforms;
+  v2_dlion_encode_kernel<<<ntiles + nv, SG_THREADS, 0, stream>>>(a);
+}
+
 void atomo_v2_launch_ps_signum(const void* units, const void* tiles, int tile0, int ntiles, int W, int nranks,
                                int group, int final_group, int owner, float* master, float* mom, float* sq,
                                float* sqmax, float* vmom, float* vsq, float* vsqmax, void* wshadow_mc,
@@ -298,7 +364,7 @@ void atomo_v2_launch_ps_signum(const void* units, const void* tiles, int tile0, 
                                float* const* vparams_peer, const float* vgrads_mc, const float* const* vgrads_peer,
                                const float* arenas, long long arena_floats, int* sig, int* const* sig_peer, void* ctrl,
                                unsigned int* group_counter, long long timeout, long long* tstats, float inv_w, int grid,
-                               const float* vext, long long vext_stride, cudaStream_t stream) {
+                               const float* vext, long long vext_stride, int mean, cudaStream_t stream) {
   SignumPsArgs a;
   static_cast<PsArgs2&>(a) =
       ps_args(units, tiles, tile0, ntiles, W, nranks, group, final_group, owner, master, mom, sq, sqmax, vmom, vsq,
@@ -306,7 +372,10 @@ void atomo_v2_launch_ps_signum(const void* units, const void* tiles, int tile0, 
               nullptr, arenas, arena_floats, sig, sig_peer, ctrl, group_counter, timeout, tstats, inv_w);
   a.vext = vext;
   a.vext_stride = vext_stride;
-  v2_ps_signum_kernel<<<ps_grid(grid, ntiles), SG_THREADS, 0, stream>>>(a);
+  if (mean)
+    v2_ps_signum_mean_kernel<<<ps_grid(grid, ntiles), SG_THREADS, 0, stream>>>(a);
+  else
+    v2_ps_signum_kernel<<<ps_grid(grid, ntiles), SG_THREADS, 0, stream>>>(a);
 }
 
 }  // extern "C"

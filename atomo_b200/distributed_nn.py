@@ -95,6 +95,10 @@ def run_rank(args) -> None:
         raise SystemExit("--code signum runs on the --backend p2p bf16 engine (--dtype bf16), which keeps each "
                          "worker's momentum and takes the owners' majority vote; the %s backend's coders keep neither"
                          % backend)
+    if args.code.lower() == "dlion":
+        raise SystemExit("--code dlion runs on the --backend p2p bf16 engine (--dtype bf16), which keeps each "
+                         "worker's Lion momentum and aggregates the signs on the owners; the %s backend's coders keep "
+                         "neither" % backend)
     if args.code.lower() == "topk":
         raise SystemExit("--code topk runs on the --backend p2p bf16 engine (--dtype bf16), which keeps the "
                          "error-feedback residual; top-k without it is biased, and the %s backend's coders keep none"

@@ -64,6 +64,10 @@ def build_coder(kwargs: dict, worker_side: bool):
     if code == "signum":
         raise ValueError("--code signum runs on the --backend p2p bf16 engine (--dtype bf16), which keeps each "
                          "worker's momentum and takes the owners' majority vote; the gloo / nccl coders keep neither")
+    if code == "dlion":
+        raise ValueError("--code dlion runs on the --backend p2p bf16 engine (--dtype bf16), which keeps each "
+                         "worker's Lion momentum and aggregates the signs on the owners; the gloo / nccl coders keep "
+                         "neither")
     if code == "topk":
         raise ValueError("--code topk runs on the --backend p2p bf16 engine (--dtype bf16), which keeps the "
                          "error-feedback residual; top-k without it is biased, and the gloo / nccl coders keep none")

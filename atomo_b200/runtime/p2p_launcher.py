@@ -59,6 +59,9 @@ def _build_engine(args, model, rank, world):
     if code == "signum" and (engine == "fused" or args.dtype != "bf16"):
         raise SystemExit("--code signum runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the "
                          "fp32-flat engine has no worker momentum or majority vote")
+    if code == "dlion" and (engine == "fused" or args.dtype != "bf16"):
+        raise SystemExit("--code dlion runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the "
+                         "fp32-flat engine has no worker momentum or sign aggregation")
     if code == "fp8" and (engine == "fused" or args.dtype != "bf16"):
         raise SystemExit("--code fp8 runs on the bf16 engine only (--dtype bf16, --engine auto|shadow); the fp32-flat "
                          "engine has no fp8 code")
@@ -73,14 +76,14 @@ def _build_engine(args, model, rank, world):
                          % args.svd_rank)
     if engine == "auto":
         shadow = args.dtype == "bf16" and code in ("svd", "qsvd", "sgd", "dense", "lossless", "topk", "sign",
-                                                   "signum", "powersgd", "fp8", "hadamard")
+                                                   "signum", "dlion", "powersgd", "fp8", "hadamard")
     elif engine == "shadow":
         if args.dtype != "bf16":
             raise SystemExit("--engine shadow trains bf16 weights: it needs --dtype bf16 (fp32 runs on --engine fused)")
         if code not in ("svd", "qsvd", "sgd", "dense", "lossless", "qsgd", "terngrad", "topk", "sign", "signum",
-                        "powersgd", "fp8", "hadamard"):
-            raise SystemExit("--engine shadow runs --code svd|qsvd|sgd|qsgd|terngrad|topk|sign|signum|powersgd|fp8|"
-                             "hadamard; --code %s runs on --engine fused" % args.code)
+                        "dlion", "powersgd", "fp8", "hadamard"):
+            raise SystemExit("--engine shadow runs --code svd|qsvd|sgd|qsgd|terngrad|topk|sign|signum|dlion|powersgd|"
+                             "fp8|hadamard; --code %s runs on --engine fused" % args.code)
         shadow = True
     else:
         shadow = False
@@ -103,8 +106,10 @@ def _build_engine(args, model, rank, world):
             kw["accumulate_steps"] = accum      # the engine refuses a value below 1
         if args.optimizer in ("lars", "lamb"):
             kw["trust_coefficient"] = getattr(args, "trust_coefficient", 0.001)
-        if args.optimizer == "lion":
+        if args.optimizer == "lion" or code == "dlion":
             kw["betas"] = tuple(getattr(args, "lion_betas", (0.9, 0.99)))     # the engine checks them
+        if code == "dlion":
+            kw["dlion_aggregate"] = getattr(args, "dlion_aggregate", "vote")
         if clip:
             kw["clip_grad_norm"] = clip
         if getattr(args, "momentum_correction", False):

@@ -42,6 +42,11 @@ one central PS kernel at the end of the step):
   ``p <- p - lr * vote``, ``vote`` in {-1, 0, +1} (NaN when a counted worker's tile is not finite); vectors are voted on
   the sign of each worker's ``vgrads``.  Weight decay is decoupled and owner-side, the pass of AdamW before the PS
   launch.  The momentum lives in momentum correction's buffers and checkpoint keys.
+* **Distributed Lion** (``code="dlion"``, ``betas`` = (b1, b2) default ``(0.9, 0.99)``, ``dlion_aggregate`` = ``"vote"``
+  or ``"mean"``; SGD only): Signum's plan, push, buffers and decay with Lion's worker rule.  Each worker pushes the sign
+  of ``c = b1 m + (1 - b1) g``, then ``m <- b2 m + (1 - b2) g`` (``v2_dlion_encode``; no buffer with ``b1 == 0``:
+  ``c = g``).  The owners step ``p <- p - lr * v`` with ``v`` the vote (Signum's PS kernel) or the mean
+  ``(pos - neg) / counted`` of the counted signs (``v2_ps_signum(mean=True)``).  ``momentum`` is ignored.
 * **PowerSGD** (``code="powersgd"``, ``svd_rank`` = r in ``[1, 4]``): every weight matrix (``[O][C]`` in its physical
   layout) is pushed as a rank-``r`` pair from one power step warm-started by the previous step's right factor
   (``csrc/v2_powersgd.cu``, two encode launches per group); the owners reconstruct ``P_hat Q'^T`` in worker order and
@@ -99,7 +104,7 @@ one central PS kernel at the end of the step):
 * Lion (``optimizer="lion"``, ``betas`` default ``(0.9, 0.99)``; ``optim/lion.py`` is the oracle): the code's PS
   kernel runs its Lion instantiation (``v2_ps_lion``): ``p -= lr sign(b1 m + (1 - b1) g)``, ``m = b2 m + (1 - b2) g``
   on ``master`` / ``mom`` and ``vparams`` / ``vmom``, no second moments allocated.  Weight decay is AdamW's decay
-  launch before it.  Clipping, Nesterov, AMSGrad, ``code="signum"`` and momentum correction are refused.
+  launch before it.  Clipping, Nesterov, AMSGrad, ``code="signum" | "dlion"`` and momentum correction are refused.
 
 Per step and rank: ``wait_params`` -> forward -> backward [group hooks -> encode, project+push on stream E;
 PS launch of the group on stream P] -> join -> ``advance_step``.  All cross-GPU ordering is carried by
@@ -143,23 +148,32 @@ class ShadowEngine:
                  side_priority: int = -1, resample_empty: bool = False, quantization_level: int = 4,
                  bucket_size: int = 512, entry_budget: float = 0.05, code_stats: bool = False,
                  error_feedback: bool = False, accumulate_steps: int = 1, trust_coefficient: float = 0.001,
-                 clip_grad_norm: float = 0.0, momentum_correction: bool = False, ema_decay: float = 0.0):
+                 clip_grad_norm: float = 0.0, momentum_correction: bool = False, ema_decay: float = 0.0,
+                 dlion_aggregate: str = "vote"):
         self.optimizer = optimizer.lower()
         if self.optimizer not in ("sgd", "adam", "adamw", "lars", "lamb", "lion"):      # checked before any CUDA work
             raise ValueError("ShadowEngine optimizers: sgd | adam | adamw | lars | lamb | lion (got %r)" % (optimizer,))
         self.code = {"dense": "sgd", "lossless": "sgd"}.get(code.lower(), code.lower())
-        self.signum = self.code == "signum"
+        # Signum and Distributed Lion: the workers push the 1-bit sign of their own momentum and the owners step by the
+        # aggregate; dlion differs only in the worker rule (two betas) and may average instead of voting
+        self.dlion = self.code == "dlion"
+        self.signum = self.code in ("signum", "dlion")
         self.lion = self.optimizer == "lion"
         if betas is None:
-            betas = (0.9, 0.99) if self.lion else (0.9, 0.999)
-        if self.lion:       # checked before any CUDA work
+            betas = (0.9, 0.99) if self.lion or self.dlion else (0.9, 0.999)
+        if self.lion or self.dlion:       # checked before any CUDA work
             if len(betas) != 2 or not all(not isinstance(b, bool) and isinstance(b, numbers.Real) and 0 <= b < 1
                                           for b in betas):
-                raise ValueError("lion: betas must be two finite numbers in [0, 1) (got %r)" % (betas,))
+                raise ValueError("%s: betas must be two finite numbers in [0, 1) (got %r)"
+                                 % ("lion" if self.lion else "dlion", betas))
+        if self.lion:       # checked before any CUDA work
             if nesterov:
                 raise ValueError("lion takes no Nesterov momentum: nesterov=False")
             if amsgrad:
                 raise ValueError("lion keeps no second moment: amsgrad=False")
+            if self.dlion:
+                raise ValueError("lion cannot be combined with code='dlion': the owners step by the aggregate of the "
+                                 "workers' Lion signs (code='dlion' alone runs Lion on the workers)")
             if self.signum:
                 raise ValueError("lion cannot be combined with code='signum': the owners step by the vote")
             if momentum_correction:
@@ -176,7 +190,7 @@ class ShadowEngine:
             if isinstance(weight_decay, bool) or not isinstance(weight_decay, numbers.Real) \
                     or not 0 <= weight_decay < math.inf:
                 raise ValueError("%s: weight_decay must be finite and >= 0 (got %r)"
-                                 % ("signum" if self.signum else self.optimizer, weight_decay))
+                                 % (self.code if self.signum else self.optimizer, weight_decay))
             self.adamw_wd, weight_decay = float(weight_decay), 0.0
         self.decay_on = self.adamw_wd > 0     # with weight_decay 0 AdamW is Adam: nothing new is launched
         self.layerwise = self.optimizer in ("lars", "lamb")
@@ -194,11 +208,31 @@ class ShadowEngine:
         self.clip_on = self.clip_grad_norm > 0
         self.ema_decay = check_ema_decay(ema_decay)      # checked before any CUDA work
         self.ema_w = float(np.float32(1.0 - self.ema_decay))    # the average's step weight, rounded once
-        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign", "signum",
+        if self.code not in ("svd", "sgd", "qsvd", "qsgd", "terngrad", "entrywise", "topk", "sign", "signum", "dlion",
                              "powersgd", "fp8", "hadamard"):
             raise ValueError("ShadowEngine codes: svd | qsvd | sgd | qsgd | terngrad | entrywise | topk | sign | signum "
-                             "| powersgd | fp8 | hadamard")
-        if self.signum:     # checked before any CUDA work
+                             "| dlion | powersgd | fp8 | hadamard")
+        self.dlion_aggregate = dlion_aggregate
+        if self.dlion:      # checked before any CUDA work; momentum is ignored, as Lion ignores it
+            if self.optimizer != "sgd":
+                raise ValueError("dlion runs Lion on the workers and steps the owners by the aggregate of their signs: "
+                                 "optimizer='sgd' only (got %r)" % (optimizer,))
+            if nesterov:
+                raise ValueError("dlion takes Lion's momentum on the workers: nesterov=False")
+            if dampening != 0:
+                raise ValueError("dlion takes dampening=0 (got %r)" % (dampening,))
+            if error_feedback:
+                raise ValueError("dlion sends the sign of the Lion direction without a residual: error_feedback=False")
+            if code_stats:
+                raise ValueError("code_stats has no estimator model for an aggregate of signs (dlion)")
+            if check_clip_grad_norm(clip_grad_norm) > 0:
+                raise ValueError("dlion cannot be combined with clip_grad_norm: the aggregate of signs has no gradient "
+                                 "norm to clip")
+            if momentum_correction:
+                raise ValueError("dlion keeps its own worker momentum: momentum_correction=False")
+            if dlion_aggregate not in ("vote", "mean"):
+                raise ValueError("dlion_aggregate: vote | mean (got %r)" % (dlion_aggregate,))
+        elif self.signum:     # checked before any CUDA work
             if self.optimizer != "sgd":
                 raise ValueError("signum steps the owners by the vote of the workers' momentum signs: optimizer='sgd' "
                                  "only (got %r)" % (optimizer,))
@@ -342,7 +376,7 @@ class ShadowEngine:
             self.fused_bn_layers, self.bn_arena = enable_fused_bn(self.model, True, arena_device=dev)
         self.params = list(self.model.parameters())
         shapes = [tuple(p.shape) for p in self.params]
-        self.plan = P2.build_plan2(shapes, self.code, self.svd_rank, self.systematic, n_owners=self.n_owners,
+        self.plan = P2.build_plan2(shapes, "signum" if self.dlion else self.code, self.svd_rank, self.systematic, n_owners=self.n_owners,
                                    n_groups=groups if overlap else 1, quantization_level=self.quantization_level,
                                    bucket_size=self.bucket_size, entry_budget=self.entry_budget)
         pl = self.plan
@@ -578,11 +612,12 @@ class ShadowEngine:
             self.t_aptr = torch.zeros((self.accum - 1, n_w), dtype=torch.int64, device=dev)
             self.host_aptr = np.zeros((self.accum - 1, n_w), dtype=np.int64)
         self.inv_n = float(np.float32(1.0 / self.accum))
-        # momentum correction (csrc/v2_momentum.cu) and Signum with beta > 0 (csrc/v2_signum.cu): the worker's fp32
-        # momentum per weight element (wshadow's physical order, the residual's offsets) and per vector element (vgrads'
-        # order)
+        # momentum correction (csrc/v2_momentum.cu), Signum with beta > 0 and Distributed Lion with b1 > 0
+        # (csrc/v2_signum.cu): the worker's fp32 momentum per weight element (wshadow's physical order, the residual's
+        # offsets) and per vector element (vgrads' order)
         self.mc_mom = self.mc_vmom = None
-        if (self.momentum_correction or (self.signum and self.mc_momentum > 0)) and self.is_worker:
+        worker_beta = self.betas[0] if self.dlion else self.mc_momentum
+        if (self.momentum_correction or (self.signum and worker_beta > 0)) and self.is_worker:
             self.mc_mom, self.mc_vmom = z(pl.w_total), z(pl.v_total)
         self.pw_warm = P2.pw_warm_ranges(pl) if self.power else []     # Q_w inside gpart (checkpointed)
         self._fresh_worker_state()
@@ -757,12 +792,12 @@ class ShadowEngine:
         return {"model": float(sum(sq)) ** 0.5, "tensors": {n: v ** 0.5 for (n, _), v in zip(ws, sq)}}
 
     def momentum_correction_norm(self) -> dict:
-        """``||u||`` of this worker's momentum (``momentum_correction=True``, or ``code="signum"`` with
-        ``momentum > 0``): per parameter tensor (weights and vectors) and for the whole model.  Reading it synchronises
-        the device."""
+        """``||u||`` of this worker's momentum (``momentum_correction=True``, ``code="signum"`` with
+        ``momentum > 0``, or ``code="dlion"`` with ``b1 > 0``): per parameter tensor (weights and vectors) and for the
+        whole model.  Reading it synchronises the device."""
         if self.mc_mom is None:
-            raise RuntimeError("momentum_correction_norm() needs ShadowEngine(..., momentum_correction=True) or "
-                               "code='signum' with momentum > 0, on a worker")
+            raise RuntimeError("momentum_correction_norm() needs ShadowEngine(..., momentum_correction=True), "
+                               "code='signum' with momentum > 0 or code='dlion' with b1 > 0, on a worker")
         names = {id(p): n for n, p in self.model.named_parameters()}
         ts = [(names.get(id(p), str(q.index)), (self.mc_mom if q.is_w else self.mc_vmom)[q.off:q.off + q.numel])
               for p, q in zip(self.params, self.plan.params)]
@@ -879,12 +914,20 @@ class ShadowEngine:
             if self.mc_vmom is None:
                 nv = 0
             p = lambda t: t.data_ptr() if t is not None else 0
-            C.v2_signum_encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
-                               self.t_vec_chunks.data_ptr() + cb * v0, nv, self.vgrads.data_ptr(), p(self.mc_mom),
-                               p(self.mc_vmom), self.mc_momentum, self.t_arena_peer.data_ptr(),
-                               self.t_sig_owner.data_ptr(), self.n_owners, pl.arena_floats, self.worker_index, g,
-                               self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g, self.tstats.data_ptr(),
-                               self._fired == self.G)
+            if self.dlion:      # Lion's worker rule: the sign of b1 m + (1 - b1) g, then m = b2 m + (1 - b2) g
+                C.v2_dlion_encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
+                                  self.t_vec_chunks.data_ptr() + cb * v0, nv, self.vgrads.data_ptr(), p(self.mc_mom),
+                                  p(self.mc_vmom), self.betas[0], self.betas[1], self.t_arena_peer.data_ptr(),
+                                  self.t_sig_owner.data_ptr(), self.n_owners, pl.arena_floats, self.worker_index, g,
+                                  self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g, self.tstats.data_ptr(),
+                                  self._fired == self.G)
+            else:
+                C.v2_signum_encode(self.t_units.data_ptr(), self.t_enc_tiles.data_ptr(), t0, nt, self.t_gptr.data_ptr(),
+                                   self.t_vec_chunks.data_ptr() + cb * v0, nv, self.vgrads.data_ptr(), p(self.mc_mom),
+                                   p(self.mc_vmom), self.mc_momentum, self.t_arena_peer.data_ptr(),
+                                   self.t_sig_owner.data_ptr(), self.n_owners, pl.arena_floats, self.worker_index, g,
+                                   self.ctrl.data_ptr(), self.cnt_enc_group + 4 * g, self.tstats.data_ptr(),
+                                   self._fired == self.G)
             self._nlaunch += 1
             return
         if self.power:
@@ -1014,7 +1057,7 @@ class ShadowEngine:
                            self.t_vgrads_peer.data_ptr(), self.heap.region_ptr("arena"), pl.arena_floats,
                            self.signals.data_ptr(), self.t_sig_all.data_ptr(), self.ctrl.data_ptr(),
                            self.cnt_ps_group + 4 * g, self.timeout_ticks, self.tstats.data_ptr(), 1.0 / self.W,
-                           max(1, min(self.ps_grid, max(nt, 1))))
+                           max(1, min(self.ps_grid, max(nt, 1))), mean=self.dlion and self.dlion_aggregate == "mean")
             self._nlaunch += 1
             return
         if self.entry:
@@ -1515,7 +1558,9 @@ class ShadowEngine:
             side.update(entry_budget=self.entry_budget)
         if self.momentum_correction:
             side.update(momentum_correction=True)
-        if self.signum:
+        if self.dlion:
+            side.update(dlion_betas=self.betas, dlion_aggregate=self.dlion_aggregate, weight_decay=self.adamw_wd)
+        elif self.signum:
             side.update(signum_momentum=self.mc_momentum, weight_decay=self.adamw_wd)
         if self.lion:       # Lion's one state is mom_w / mom_v above
             side.update(lion_betas=self.betas, weight_decay=self.adamw_wd)
@@ -1530,7 +1575,9 @@ class ShadowEngine:
                "warm_start": self.warm_start, "world": self.world, "ps_mode": self.ps_mode, "worker": self.worker_index}
         if self.momentum_correction:
             cfg["momentum_correction"] = True
-        if self.signum:
+        if self.dlion:
+            cfg["dlion_betas"] = self.betas
+        elif self.signum:
             cfg["signum_momentum"] = self.mc_momentum
         return cfg
 

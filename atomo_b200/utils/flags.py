@@ -40,7 +40,12 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "keeps a momentum with beta = --momentum in [0, 1) and sends its sign, one bit per element and "
                         "no scale; the owners step by lr times the vote; --backend p2p --dtype bf16 only, SGD without "
                         "--nesterov, --error-feedback, --clip-grad-norm or --code-stats; --weight-decay is decoupled, "
-                        "on the owners) | powersgd (rank --svd-rank in [1, 4] factors of every "
+                        "on the owners) | dlion (Distributed Lion: each worker keeps a Lion momentum with b1, b2 = "
+                        "--lion-betas and sends the sign of b1 m + (1 - b1) g, one bit per element; the owners step by "
+                        "lr times the vote or the mean of the signs, --dlion-aggregate; --backend p2p --dtype bf16 "
+                        "only, SGD without --nesterov, --error-feedback, --clip-grad-norm or --code-stats; --momentum "
+                        "is ignored; --weight-decay is decoupled, on the owners) | powersgd (rank --svd-rank in [1, 4] "
+                        "factors of every "
                         "weight matrix from one warm-started power step; --backend p2p --dtype bf16 only, meant for "
                         "--error-feedback 1) | fp8 (one e4m3 byte per element, stochastically rounded and so "
                         "unbiased, and one power-of-two fp32 scale per --bucket-size bucket, a multiple of 64 in "
@@ -78,11 +83,14 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "dimensions) scaled by 1 - lr * --weight-decay before the Adam step, BN / bias vectors not "
                         "decayed; lion: Lion (Chen et al. 2023), w <- w - lr * sign(b1 m + (1 - b1) g) and m <- b2 m + "
                         "(1 - b2) g with b1, b2 = --lion-betas, one fp32 state per weight and --weight-decay decoupled "
-                        "as in adamw; --momentum is ignored, and --nesterov, --clip-grad-norm and --code signum are "
-                        "refused; p2p backend on the bf16 engine (--engine shadow), or the gloo / nccl role path")
+                        "as in adamw; --momentum is ignored, and --nesterov, --clip-grad-norm and --code signum|dlion "
+                        "are refused (--code dlion runs Lion on the workers); p2p backend on the bf16 engine (--engine shadow), or the gloo / nccl role path")
     p.add_argument("--lion-betas", type=float, nargs=2, default=[0.9, 0.99], metavar=("B1", "B2"),
-                   help="--optimizer lion: the interpolation beta of the step's sign (b1) and the momentum's beta (b2), "
-                        "each in [0, 1); ignored by the other optimizers")
+                   help="--optimizer lion and --code dlion: the interpolation beta of the step's sign (b1) and the "
+                        "momentum's beta (b2), each in [0, 1); ignored by the other optimizers and codes")
+    p.add_argument("--dlion-aggregate", type=str, default="vote", choices=["vote", "mean"],
+                   help="--code dlion: how the owners combine the workers' signs, vote (majority vote, 0 on a tie) or "
+                        "mean (their average, a multiple of 1 / counted workers)")
     p.add_argument("--trust-coefficient", type=float, default=0.001,
                    help="--optimizer lars: eta of the trust ratio eta ||w|| / (||g|| + wd ||w||)")
     p.add_argument("--clip-grad-norm", type=float, default=0.0,
@@ -110,7 +118,7 @@ def add_fit_args(parser: argparse.ArgumentParser, argv=None):
                         "colocated = rank 0 hosts the whole PS and also trains; dedicated = rank 0 only serves")
     p.add_argument("--engine", type=str, default="auto", choices=["auto", "shadow", "fused"],
                    help="p2p backend: auto = the overlapped sharded bf16 engine for --dtype bf16 with --code "
-                        "svd|qsvd|sgd|topk|sign|powersgd|fp8|hadamard, the fp32-flat engine otherwise; shadow = the bf16 engine (also --code "
+                        "svd|qsvd|sgd|topk|sign|signum|dlion|powersgd|fp8|hadamard, the fp32-flat engine otherwise; shadow = the bf16 engine (also --code "
                         "qsgd|terngrad, needs --dtype bf16); fused = the fp32-flat engine")
     p.add_argument("--groups", type=int, default=5, help="p2p/bf16: backward groups pushed while backward runs")
     p.add_argument("--shrinkage-freq", type=int, default=50, help="steps between LR shrinkages (reference: 50)")

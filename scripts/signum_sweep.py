@@ -43,8 +43,9 @@ def push_bytes(pl):
     return pl.dense_bytes() + pl.qsgd_bytes() + pl.signum_bytes()
 
 
-def ps_vote_time(C, shapes, W, iters):
-    """Mean microseconds of one v2_ps_signum launch over every tile of ``shapes`` (one group, one owner)."""
+def ps_vote_time(C, shapes, W, iters, mean=False):
+    """Mean microseconds of one v2_ps_signum launch over every tile of ``shapes`` (one group, one owner); ``mean``
+    times the mean kernel of Distributed Lion instead of the vote."""
     from atomo_b200.ops import plan2 as P
     dev = torch.device("cuda", 0)
     pl = P.build_plan2(shapes, "signum", n_owners=1, n_groups=1)
@@ -81,7 +82,7 @@ def ps_vote_time(C, shapes, W, iters):
                        mom.data_ptr(), 0, 0, vmom.data_ptr(), 0, 0, 0, t_wsh.data_ptr(), vparams.data_ptr(), 0,
                        t_vp.data_ptr(), 0, t_vg.data_ptr(), arena.data_ptr(), pl.arena_floats, sig.data_ptr(),
                        t_sig.data_ptr(), ctrl.data_ptr(), counter.data_ptr(), int(5e9), 0, 1.0 / W,
-                       max(1, min(3 * sm, nt)))
+                       max(1, min(3 * sm, nt)), mean=mean)
     for _ in range(10):
         launch()
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
