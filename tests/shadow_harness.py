@@ -2,12 +2,21 @@
 engine, the single-GPU and multi-GPU training helpers and the launcher argv.  Not a test file itself: pytest puts this
 directory on ``sys.path``, and the tests import from here."""
 import argparse
+import math
 import os
+import subprocess
+import sys
+import types
 
+import numpy as np
+import pytest
 import torch
 import torch.nn as nn
 
+from atomo_b200.codings import signum as S
 from atomo_b200.ops import plan2 as P
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def ext():
@@ -293,6 +302,161 @@ class HE(LoopbackPS):
         return torch.cat(idx), torch.cat(val), torch.cat(flag)
 
 
+# -------------------------------------------------------------------------------------------- Signum / Distributed Lion
+# the 1728-element stem, 3x3 convs (one a multiple of the 4096-element tile, one with a half tile), fc layers, tensors
+# whose size is not a multiple of 64 (or of 16), vectors, an all-zero tensor (ZERO), one with +0 / -0 / bf16 subnormals
+# (SIGNED_ZERO) and one that gets a NaN (NAN)
+SIGNUM_SHAPES = [(64, 3, 3, 3), (64,), (64, 32, 3, 3), (128, 64, 3, 3), (128,), (96, 64, 3, 3), (10, 512), (7, 20),
+                 (5, 3), (10,), (32, 16, 3, 3), (40, 30), (48, 16, 3, 3)]
+ZERO, SIGNED_ZERO, NAN = 10, 11, 12
+
+
+class HSG(LoopbackPS):
+    """Signum: per virtual worker a momentum buffer (beta > 0) and the coin's external uniforms."""
+
+    PS = "v2_ps_signum"
+
+    def __init__(self, shapes, W=1, beta=0.0, lr=0.0625, seed=7, num_aggregate=0, n_groups=1, n_owners=1):
+        super().__init__(shapes, "signum", W, lr, 0.0, 0.0, False, 0, seed, num_aggregate, n_groups, n_owners)
+        pl, z = self.plan, self.zeros
+        self.beta = beta
+        self.wmom = [z(pl.w_total) for _ in range(W)] if beta > 0 else None
+        self.vmom_w = [z(pl.v_total) for _ in range(W)] if beta > 0 else None
+        chunks, self.vec_range = P.vec_chunks(pl)
+        self.t_vchunks = torch.frombuffer(bytearray(chunks or b"\0" * 24), dtype=torch.uint8).to(self.dev)
+        g = torch.Generator(device="cuda").manual_seed(seed + 1)
+        self.unif = [torch.rand(pl.w_total, device=self.dev, generator=g) for _ in range(W)]
+        self.vext = torch.rand(W * pl.v_total, device=self.dev, generator=g)
+        self.ps_tail = (self.vext.data_ptr(), pl.v_total)
+
+    def tensor(self, q, x, g, special=False, who=0, negate=None):
+        if special and q.index == ZERO:
+            x.zero_()
+        elif special and q.index == SIGNED_ZERO:
+            r = torch.rand(q.shape, device=self.dev, generator=g)
+            z = torch.zeros_like(x)
+            x = torch.where(r < 0.3, z, torch.where(r < 0.6, -z, torch.where(r < 0.7, x.sign() * 1e-39, x)))
+        if special and q.index == NAN and who == 0:
+            x = physical(x)
+            flat(x)[100] = float("nan")
+        return x
+
+    def encode(self, w, coin=False):
+        C, pl = self.C, self.plan
+        gptr = self.gptr(w)
+        for g in range(pl.n_groups):
+            t0, nt = pl.enc_range[g]
+            v0, nv = self.vec_range[g]
+            if self.beta == 0:
+                nv = 0
+            C.v2_signum_encode(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr,
+                               self.t_vchunks.data_ptr() + 24 * v0, nv, self.vgrads[w].data_ptr(),
+                               self.wmom[w].data_ptr() if self.wmom else 0,
+                               self.vmom_w[w].data_ptr() if self.vmom_w else 0, self.beta,
+                               self.t_arena_peer.data_ptr(), self.t_sig_peer.data_ptr(), self.n_owners,
+                               pl.arena_floats, w, g, self.ctrl.data_ptr(), self.counter(g), 0,
+                               g == pl.n_groups - 1, 0 if coin else self.unif[w].data_ptr())
+        torch.cuda.synchronize()
+
+
+class SignumOracle:
+    """The fp32 numpy oracle of a HSG run: the workers' momenta, the pushed bits per tile, the owners' state."""
+
+    def __init__(self, h):
+        pl = self.plan = h.plan
+        self.h = h
+        self.u = [np.zeros(pl.w_total, np.float32) for _ in range(h.W)]
+        self.uv = [np.zeros(pl.v_total, np.float32) for _ in range(h.W)]
+        self.x, self.xv = [None] * h.W, [None] * h.W
+        self.master = h.master.cpu().numpy().copy()
+        self.vparams = h.vparams.cpu().numpy().copy()
+        self.unif = [t.cpu().numpy() for t in h.unif]
+        self.vext = h.vext.cpu().numpy().reshape(h.W, pl.v_total)
+
+    def push(self, w, phys, coin=False):
+        pl, beta = self.plan, self.h.beta
+        x, xv = np.zeros(pl.w_total, np.float32), np.zeros(pl.v_total, np.float32)
+        for q in pl.params:
+            g = phys[q.index].cpu().numpy().astype(np.float32)
+            sl = slice(q.off, q.off + q.numel)
+            st, dst = (self.u[w], x) if q.is_w else (self.uv[w], xv)
+            if beta > 0:
+                st[sl] = S.momentum_step(st[sl], g, beta)
+                dst[sl] = st[sl]
+            else:
+                dst[sl] = g
+        self.x[w], self.xv[w] = x, xv
+        if coin:
+            self.unif[w] = np.zeros(pl.w_total, np.float32)
+            for u in pl.units:
+                if u.kind == P.KIND_SIGNUM:
+                    self.unif[w][u.w_off:u.w_off + u.numel] = S.coin_uniforms(self.h.seed, u.index,
+                                                                               np.arange(u.numel), self.h.step, w)
+
+    def tile_bits(self, w, u, a, b):
+        sl = slice(u.w_off + a, u.w_off + a + b)
+        return S.bits(self.x[w][sl], self.unif[w][sl]), S.nonfinite(self.x[w][sl])
+
+    def vec_bits(self, w, u, a, b, coin=False):
+        sl = slice(u.w_off + a, u.w_off + a + b)
+        un = S.coin_uniforms(self.h.seed, u.index, np.arange(a, a + b), self.h.step, w) if coin else self.vext[w][sl]
+        return S.bits(self.xv[w][sl], un), S.nonfinite(self.xv[w][sl])
+
+    def ps(self, counted, coin=False):
+        pl, lr = self.plan, np.float32(self.h_lr())
+        for (ui, a, b, o) in pl.ps_tiles:
+            u = pl.units[ui]
+            rows, bad = [], []
+            for w in counted:
+                r, nf = self.vec_bits(w, u, a, b, coin) if u.kind == P.KIND_VEC else self.tile_bits(w, u, a, b)
+                rows.append(r)
+                bad.append(nf)
+            v = S.vote(rows, b, bad)
+            dst = self.vparams if u.kind == P.KIND_VEC else self.master
+            dst[u.w_off + a:u.w_off + a + b] = S.step(dst[u.w_off + a:u.w_off + a + b], v, lr)
+
+    def h_lr(self):
+        return float(self.h.ctrl.view(torch.float32)[2])
+
+
+def signum_check_push(h, o, w):
+    """Worker w's words, status words and stamps in the owners' arenas, and its momenta, against the oracle."""
+    pl = h.plan
+    arenas = [t.cpu().numpy() for t in h.arenas]
+    for u in pl.units:
+        if u.kind != P.KIND_SIGNUM:
+            continue
+        for j in range(u.n_ps):
+            a, b = 4096 * j, min(4096, u.numel - 4096 * j)
+            ar = arenas[(u.own0 + j) % h.n_owners]
+            base = w * pl.arena_floats + u.slot_off
+            bits, nf = o.tile_bits(w, u, a, b)
+            wo = base + P.qsgd_words_off(u.n_ps, u.rows) + 2 * j * u.cols
+            nw = -(-b // 64)
+            got = ar[wo:wo + 2 * nw].view(np.uint64)
+            assert np.array_equal(got, S.pack(bits)), (u.index, j, w)
+            status = ar[base + P.qsgd_norms_off(u.n_ps) + j]
+            assert (math.isnan(status) if nf else status == 0.0), (u.index, j, w, status)
+            assert int(ar[base:base + u.n_ps].view(np.int32)[j]) == h.step
+    if h.beta > 0:
+        used = np.zeros(pl.w_total, bool)
+        for q in pl.params:
+            if q.is_w:
+                used[q.off:q.off + q.numel] = True
+        got = h.wmom[w].cpu().numpy()
+        assert np.array_equal(got[used], o.u[w][used], equal_nan=True)
+        assert np.array_equal(h.vmom_w[w].cpu().numpy(), o.uv[w], equal_nan=True)
+    assert np.array_equal(h.vgrads[w].cpu().numpy(), o.xv[w], equal_nan=True)
+
+
+def signum_check_ps(h, o):
+    assert int(h.ctrl.view(torch.int32)[1]) == 0
+    assert np.array_equal(h.master.cpu().numpy(), o.master, equal_nan=True)
+    assert np.array_equal(h.vparams.cpu().numpy(), o.vparams, equal_nan=True)
+    a, b = h.wshadow.float(), torch.from_numpy(o.master).cuda().bfloat16().float()
+    assert torch.equal(a.isnan(), b.isnan()) and torch.equal(a.nan_to_num(), b.nan_to_num())
+
+
 def opt_ref(p, g, m, s2, s2m, step, lr, momentum, nesterov, wd, opt):
     """One PS optimizer step in fp32 PyTorch: (new params, new momentum) for SGD (opt 0), Adam (1), AMSGrad (2)."""
     g = g + wd * p
@@ -454,6 +618,64 @@ class Loopback:
 
 
 # ---------------------------------------------------------------------------------------------------- engine
+@pytest.fixture
+def deterministic_cudnn(monkeypatch):
+    """cuDNN with deterministic, heuristically chosen algorithms (as bench.py runs it) for one test."""
+    monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)
+    monkeypatch.setattr(torch.backends.cudnn, "benchmark", False)
+
+
+_BATCHES = {}
+
+
+def engine_batch(net, step, n=32, seed=0, period=4):
+    """The device batch of training step `step`: n synthetic samples of `net`'s input shape drawn with seed
+    ``seed + step % period``, the same tensors on every call.  Test files share the cache, so its key holds the seed."""
+    from atomo_b200.data import SyntheticImageDataset
+    from atomo_b200.models import input_shape
+    k = (net, seed, step % period, n)
+    if k not in _BATCHES:
+        x, y = SyntheticImageDataset(input_shape(net), 10, 4096, seed=seed + k[2]).materialize(n)
+        _BATCHES[k] = (x.cuda(), y.cuda())
+    return _BATCHES[k]
+
+
+def make_engine(net="ResNet18", rank=0, world=1, seed=7, prepare_n=None, data_seed=0, **kw):
+    """ShadowEngine(**kw) on device `rank` for ``build_model(net)`` drawn from torch seed 0.  With `prepare_n` it is
+    prepared without warm-up on the step-0 `engine_batch` of prepare_n samples drawn from `data_seed`."""
+    from atomo_b200.models import build_model
+    from atomo_b200.runtime.shadow_engine import ShadowEngine
+    torch.manual_seed(0)
+    torch.cuda.set_device(rank)
+    eng = ShadowEngine(build_model(net, 10), rank, world, seed=seed, **kw)
+    if prepare_n is not None:
+        x, y = engine_batch(net, 0, prepare_n, data_seed)
+        eng.prepare(x, y, warmup=0)
+    return eng
+
+
+def step(eng, batch, check=True):
+    """One synchronized training step on `batch` (x, y); the loss.  With `check` the device error must be clear."""
+    loss = eng.train_step(*batch)
+    torch.cuda.synchronize()
+    if check:
+        assert eng.error_code() == 0
+    return float(loss[0])
+
+
+def state(eng, keys):
+    """Copies of the engine tensors named in `keys`, skipping those the engine does not allocate."""
+    return {k: getattr(eng, k).clone() for k in keys if getattr(eng, k, None) is not None}
+
+
+def differs(a, b, keys=None):
+    """The names among `keys` (default: all of a's, which must be b's) whose tensors are not bitwise equal."""
+    if keys is None:
+        assert a.keys() == b.keys()
+        keys = a.keys()
+    return [k for k in keys if not torch.equal(a[k], b[k])]
+
+
 def batch(net, n=32, seed=0):
     """n synthetic samples of the input shape of `net`, in pinned memory."""
     from atomo_b200.data import SyntheticImageDataset
@@ -495,14 +717,37 @@ MODELS = {"ResNet18": ("ResNet18", ""), "VGG11": ("VGG11", ""), "ResNet50-ImageN
 
 
 # ---------------------------------------------------------------------------------------------------- multi GPU
-def mp_worker(rank, world, port, cfg, out):
+def nccl_init(rank, world, port):
+    """Join the NCCL process group of `world` local ranks on 127.0.0.1:`port` as `rank`, on device `rank`."""
     import torch.distributed as dist
-    from atomo_b200.models import build_model
-    from atomo_b200.runtime.shadow_engine import ShadowEngine
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
                       LOCAL_RANK=str(rank))
     torch.cuda.set_device(rank)
     dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
+
+
+def spawn(world, target, *args, timeout=600):
+    """Run ``target(rank, world, *args, out)`` in `world` spawned processes; each puts one result tuple that starts
+    with its rank on the queue `out`.  The results are taken before the processes are joined (a full queue would
+    keep a process from exiting) and returned sorted by rank; every process must exit with code 0."""
+    import torch.multiprocessing as mp
+    ctx = mp.get_context("spawn")
+    out = ctx.Queue()
+    procs = [ctx.Process(target=target, args=(r, world, *args, out)) for r in range(world)]
+    for p in procs:
+        p.start()
+    res = sorted((out.get(timeout=timeout) for _ in range(world)), key=lambda r: r[0])
+    for p in procs:
+        p.join(timeout)
+        assert p.exitcode == 0
+    return res
+
+
+def mp_worker(rank, world, port, cfg, out):
+    import torch.distributed as dist
+    from atomo_b200.models import build_model
+    from atomo_b200.runtime.shadow_engine import ShadowEngine
+    nccl_init(rank, world, port)
     torch.manual_seed(0)
     net = cfg.get("net", "ResNet18")
     eng = ShadowEngine(build_model(net, 10), rank, world, code=cfg["code"], svd_rank=3, lr=0.05, momentum=0.9,
@@ -551,19 +796,13 @@ def mp_worker(rank, world, port, cfg, out):
 
 def run_mp(world, cfg, port):
     """`world` spawned ranks of ``mp_worker``; their result tuples sorted by rank."""
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    out = ctx.Queue()
-    procs = [ctx.Process(target=mp_worker, args=(r, world, port, cfg, out)) for r in range(world)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(300)
-        assert p.exitcode == 0
-    return sorted(out.get() for _ in range(world))
+    return spawn(world, mp_worker, port, cfg, timeout=300)
 
 
 # ---------------------------------------------------------------------------------------------------- launcher
+SVD3 = ("--code", "svd", "--svd-rank", "3")     # launcher flags of spectral ATOMO at rank 3
+
+
 def fit_args(tmp_path, *extra):
     """Launcher flags of a short synthetic LeNet / MNIST run writing to tmp_path, then `extra`."""
     from atomo_b200.utils.flags import add_fit_args
@@ -572,6 +811,75 @@ def fit_args(tmp_path, *extra):
         "--batch-size", "32", "--test-batch-size", "64", "--lr", "0.05", "--log-interval", "1", "--eval-freq", "100",
         "--train-dir", str(tmp_path) + "/", *extra])
 
+
+
+class StandInEngine:
+    """Plain SGD on the CPU behind the engine interface the launcher uses.  Every instance is appended to `instances`,
+    which a test clears before it runs the launcher; subclasses record what their test reads."""
+    first_worker, W, is_worker, is_ps, is_owner = 0, 1, True, True, True
+    instances = []
+
+    def __init__(self, model, args):
+        self.model, self.lr, self.step, self.args = model, args.lr, 1, args
+        self.opt = torch.optim.SGD(model.parameters(), lr=args.lr)
+        self.plan = types.SimpleNamespace(factor_bytes_per_worker=lambda: 1 << 20, dense_bytes=lambda: 1 << 18,
+                                          expected_factor_bytes=lambda: 1 << 20)
+        StandInEngine.instances.append(self)
+
+    def prepare(self, x, y, warmup=3):
+        for _ in range(warmup):
+            self.train_step(x, y)
+
+    def set_lr(self, lr):
+        self.lr = lr
+
+    def train_step(self, x, y):
+        self.opt.zero_grad()
+        out = self.model(x)
+        loss = torch.nn.functional.cross_entropy(out, y)
+        loss.backward()
+        self.opt.step()
+        self.step += 1
+        hit = out.argmax(1).eq(y).float().mean() * 100
+        return torch.stack([loss.detach(), hit, hit])
+
+    def phase_stats(self, reset=True):
+        return {"param_wait_us": 10.0, "encode_us": 300.0, "to_push_us": 1500.0}
+
+    def error_code(self):
+        return 0
+
+    def save_checkpoint(self, train_dir, step):
+        pass
+
+    def load_checkpoint(self, train_dir, step):
+        pass
+
+    def close(self):
+        pass
+
+
+def role_master(tmp_path, **kw):
+    """The gloo role path's master (``SyncReplicasMaster_NN``) of a 2-process LeNet / MNIST run writing to tmp_path,
+    with the settings `kw`, its model built from torch seed 0."""
+    from atomo_b200.runtime import master as M
+    m = M.SyncReplicasMaster_NN(types.SimpleNamespace(world_size=2), network="LeNet", dataset="MNIST",
+                                train_dir=str(tmp_path) + "/", **kw)
+    torch.manual_seed(0)
+    return m.build_model(10)
+
+
+def role_run(d, port, max_steps, *flags):
+    """A 2-process gloo role-path run (``distributed_nn``) of synthetic LeNet / MNIST with the dense code, writing to
+    d and evaluating every step, then `flags`; its stdout.  It must exit with code 0."""
+    cmd = [sys.executable, "-m", "atomo_b200.distributed_nn", "--synthetic", "1", "--train-len", "512",
+           "--test-len", "128", "--batch-size", "32", "--lr", "0.01", "--test-batch-size", "64", "--nproc", "2",
+           "--network", "LeNet", "--dataset", "MNIST", "--code", "sgd", "--max-steps", str(max_steps), "--eval-freq",
+           "1", "--train-dir", d, "--master-port", str(port), *flags]
+    env = dict(os.environ, ATOMO_HANG_DUMP_S="400", PYTHONPATH=ROOT, OMP_NUM_THREADS="2", MKL_NUM_THREADS="2")
+    r = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=420)
+    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
+    return r.stdout
 
 def forbid_cuda(monkeypatch):
     """Make ShadowEngine fail on its first CUDA work, so a refusal is shown to come before any."""

@@ -5,9 +5,6 @@
 import argparse
 import os
 import struct
-import subprocess
-import sys
-import types
 
 import numpy as np
 import pytest
@@ -19,7 +16,7 @@ from atomo_b200.runtime import master as M
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
 
-from shadow_harness import fit_args, forbid_cuda
+from shadow_harness import fit_args, forbid_cuda, role_master, role_run
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SHAPES = [(6, 3, 3, 3), (6,), (10, 24), (10,), (4, 5)]
@@ -151,11 +148,7 @@ def test_set_lr_rewrites_the_decay_factor():
 
 # ---------------------------------------------------------------------------------------------------- role path
 def _master(tmp_path, wd=0.05, resume=False):
-    m = M.SyncReplicasMaster_NN(types.SimpleNamespace(world_size=2), learning_rate=0.01, network="LeNet",
-                                dataset="MNIST", optimizer="adamw", weight_decay=wd, train_dir=str(tmp_path) + "/",
-                                resume=resume)
-    torch.manual_seed(0)
-    return m.build_model(10)
+    return role_master(tmp_path, learning_rate=0.01, optimizer="adamw", weight_decay=wd, resume=resume)
 
 
 def test_role_path_update_is_adamw(tmp_path):
@@ -177,22 +170,13 @@ def test_role_path_update_is_adamw(tmp_path):
         assert all(torch.equal(a, b) for a, b in zip(m.network.parameters(), params))
 
 
-def _role_run(d, port, max_steps, *extra):
-    cmd = [sys.executable, "-m", "atomo_b200.distributed_nn", "--synthetic", "1", "--train-len", "512",
-           "--test-len", "128", "--batch-size", "32", "--lr", "0.01", "--test-batch-size", "64", "--nproc", "2",
-           "--network", "LeNet", "--dataset", "MNIST", "--code", "sgd", "--optimizer", "adamw", "--weight-decay",
-           "0.05", "--max-steps", str(max_steps), "--eval-freq", "1", "--train-dir", d, "--master-port", str(port),
-           *extra]
-    env = dict(os.environ, ATOMO_HANG_DUMP_S="400", PYTHONPATH=ROOT, OMP_NUM_THREADS="2", MKL_NUM_THREADS="2")
-    r = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=420)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-    return r.stdout
+ROLE_FLAGS = ("--optimizer", "adamw", "--weight-decay", "0.05")
 
 
 def test_gloo_role_path_trains_and_resumes_adamw(tmp_path):
     d = str(tmp_path) + "/"
-    _role_run(d, 29581, 3)
-    out = _role_run(d, 29582, 5, "--resume", "1")
+    role_run(d, 29581, 3, *ROLE_FLAGS)
+    out = role_run(d, 29582, 5, *ROLE_FLAGS, "--resume", "1")
     assert "Master: Step: 5" in out and "Master: Step: 1," not in out
     load = lambda s: torch.load(d + "model_step_%d_optim" % s, map_location="cpu", weights_only=False)
     for s in range(1, 6):

@@ -18,14 +18,10 @@ from atomo_b200.runtime import master as M
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args, check_clip_grad_norm
 
-from shadow_harness import fit_args, forbid_cuda
+from shadow_harness import SVD3, StandInEngine, fit_args, forbid_cuda
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BAD = [-1.0, float("nan"), float("inf"), -float("inf"), True, "1.0"]
-
-
-def _args(tmp_path, *extra):
-    return fit_args(tmp_path, "--code", "svd", "--svd-rank", "3", *extra)
 
 
 def test_flag_parses_and_defaults_to_off():
@@ -51,7 +47,7 @@ def test_engine_refuses_before_cuda_work(bad, monkeypatch):
 @pytest.mark.parametrize("bad", ["-1", "nan", "inf"])
 def test_launcher_refuses_bad_values(bad, tmp_path):
     with pytest.raises(SystemExit, match="clip-grad-norm"):
-        L._build_engine(_args(tmp_path, "--clip-grad-norm", bad, "--dtype", "bf16"), torch.nn.Linear(4, 4), 0, 1)
+        L._build_engine(fit_args(tmp_path, *SVD3, "--clip-grad-norm", bad, "--dtype", "bf16"), torch.nn.Linear(4, 4), 0, 1)
 
 
 def test_fp32_flat_engine_refuses(tmp_path):
@@ -59,7 +55,7 @@ def test_fp32_flat_engine_refuses(tmp_path):
     for extra in (("--engine", "fused", "--dtype", "bf16"), ("--dtype", "fp32"),
                   ("--dtype", "bf16", "--code", "entrywise")):        # auto sends these to the fp32-flat engine
         with pytest.raises(SystemExit, match="--engine shadow"):
-            L._build_engine(_args(tmp_path, "--clip-grad-norm", "1.0", *extra), model, 0, 1)
+            L._build_engine(fit_args(tmp_path, *SVD3, "--clip-grad-norm", "1.0", *extra), model, 0, 1)
 
 
 @pytest.mark.parametrize("n_groups", [1, 2, 3, 5])
@@ -154,25 +150,12 @@ def test_gloo_role_path_trains_with_clipping(tmp_path):
     assert "Master: Step: 4" in r.stdout and os.path.isfile(d + "model_step_4")
 
 
-class StandInEngine:
-    """Plain SGD with torch's clipping on the CPU behind the engine interface the launcher uses."""
-    first_worker, W, is_worker, is_ps, is_owner = 0, 1, True, True, True
-    instances = []
+class ClipStandIn(StandInEngine):
+    """Clips with torch's ``clip_grad_norm_`` and counts the reads of the norm."""
 
     def __init__(self, model, args):
-        self.model, self.lr, self.step, self.args = model, args.lr, 1, args
-        self.opt = torch.optim.SGD(model.parameters(), lr=args.lr)
-        self.plan = types.SimpleNamespace(factor_bytes_per_worker=lambda: 1 << 20, dense_bytes=lambda: 1 << 18,
-                                          expected_factor_bytes=lambda: 1 << 20)
+        super().__init__(model, args)
         self.norm_reads, self.last = 0, (0.0, 1.0)
-        StandInEngine.instances.append(self)
-
-    def prepare(self, x, y, warmup=3):
-        for _ in range(warmup):
-            self.train_step(x, y)
-
-    def set_lr(self, lr):
-        self.lr = lr
 
     def train_step(self, x, y):
         self.opt.zero_grad()
@@ -190,27 +173,15 @@ class StandInEngine:
         self.norm_reads += 1
         return self.last
 
-    def phase_stats(self, reset=True):
-        return {"param_wait_us": 10.0, "encode_us": 300.0, "to_push_us": 1500.0}
-
-    def error_code(self):
-        return 0
-
-    def save_checkpoint(self, train_dir, step):
-        pass
-
-    def close(self):
-        pass
-
 
 def test_launcher_loop_records_the_norm_at_log_steps(tmp_path, monkeypatch, capsys):
     import json
     StandInEngine.instances.clear()
-    monkeypatch.setattr(L, "_build_engine", lambda args, model, rank, world: (StandInEngine(model, args), "shadow"))
+    monkeypatch.setattr(L, "_build_engine", lambda args, model, rank, world: (ClipStandIn(model, args), "shadow"))
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
     mf = str(tmp_path / "m")
-    L.run_p2p_training(_args(tmp_path, "--max-steps", "6", "--log-interval", "2", "--clip-grad-norm", "0.05",
+    L.run_p2p_training(fit_args(tmp_path, *SVD3, "--max-steps", "6", "--log-interval", "2", "--clip-grad-norm", "0.05",
                              "--dtype", "bf16", "--metrics-file", mf), device="cpu")
     eng = StandInEngine.instances[-1]
     assert eng.args.clip_grad_norm == 0.05 and eng.step == 7

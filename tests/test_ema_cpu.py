@@ -4,8 +4,6 @@ stand-in engine evaluating the averaged model at ``--eval-freq``, and the gloo r
 oracle, written beside each model file and restored on ``--resume``."""
 import argparse
 import os
-import subprocess
-import sys
 import types
 
 import numpy as np
@@ -17,7 +15,7 @@ from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils import checkpoint as ckpt
 from atomo_b200.utils.flags import add_fit_args, check_ema_decay
 
-from shadow_harness import fit_args, forbid_cuda
+from shadow_harness import StandInEngine, fit_args, forbid_cuda, role_master, role_run
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BAD = [1, 1.0, 1.5, -0.5, -1e-9, float("nan"), float("inf"), -float("inf"), True, False, "0.9"]
@@ -90,57 +88,21 @@ def test_evaluator_reads_the_average(tmp_path):
     assert all(not v.any() for v in plain.network.state_dict().values())
 
 
-class StandInEngine:
-    """Plain SGD on the CPU behind the engine interface the launcher uses; its average is a model of zeros, so that
-    the averaged model's test loss is exactly log(10)."""
-    first_worker, W, is_worker, is_ps, is_owner = 0, 1, True, True, True
-    instances = []
+class EmaStandIn(StandInEngine):
+    """Its average is a model of zeros, so that the averaged model's test loss is exactly log(10)."""
 
     def __init__(self, model, args):
-        self.model, self.lr, self.step, self.args = model, args.lr, 1, args
-        self.opt = torch.optim.SGD(model.parameters(), lr=args.lr)
-        self.plan = types.SimpleNamespace(factor_bytes_per_worker=lambda: 1 << 20, dense_bytes=lambda: 1 << 18,
-                                          expected_factor_bytes=lambda: 1 << 20)
+        super().__init__(model, args)
         self.ema_reads = []
-        StandInEngine.instances.append(self)
-
-    def prepare(self, x, y, warmup=3):
-        for _ in range(warmup):
-            self.train_step(x, y)
-
-    def set_lr(self, lr):
-        self.lr = lr
-
-    def train_step(self, x, y):
-        self.opt.zero_grad()
-        out = self.model(x)
-        loss = torch.nn.functional.cross_entropy(out, y)
-        loss.backward()
-        self.opt.step()
-        self.step += 1
-        hit = out.argmax(1).eq(y).float().mean() * 100
-        return torch.stack([loss.detach(), hit, hit])
 
     def ema_state_dict(self):
         self.ema_reads.append(self.step - 1)
         return {k: torch.zeros_like(v) for k, v in self.model.state_dict().items()}
 
-    def phase_stats(self, reset=True):
-        return {"param_wait_us": 10.0, "encode_us": 300.0, "to_push_us": 1500.0}
-
-    def error_code(self):
-        return 0
-
-    def save_checkpoint(self, train_dir, step):
-        pass
-
-    def close(self):
-        pass
-
 
 def test_launcher_loop_evaluates_the_average(tmp_path, monkeypatch, capsys):
     StandInEngine.instances.clear()
-    monkeypatch.setattr(L, "_build_engine", lambda args, model, rank, world: (StandInEngine(model, args), "shadow"))
+    monkeypatch.setattr(L, "_build_engine", lambda args, model, rank, world: (EmaStandIn(model, args), "shadow"))
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
     L.run_p2p_training(fit_args(tmp_path, "--code", "svd", "--dtype", "bf16", "--max-steps", "6", "--eval-freq", "3",
@@ -158,7 +120,7 @@ def test_launcher_loop_evaluates_the_average(tmp_path, monkeypatch, capsys):
 
 def test_launcher_loop_without_the_average(tmp_path, monkeypatch, capsys):
     StandInEngine.instances.clear()
-    monkeypatch.setattr(L, "_build_engine", lambda args, model, rank, world: (StandInEngine(model, args), "shadow"))
+    monkeypatch.setattr(L, "_build_engine", lambda args, model, rank, world: (EmaStandIn(model, args), "shadow"))
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
     L.run_p2p_training(fit_args(tmp_path, "--code", "svd", "--dtype", "bf16", "--max-steps", "3", "--eval-freq", "3"),
@@ -169,10 +131,7 @@ def test_launcher_loop_without_the_average(tmp_path, monkeypatch, capsys):
 
 # ---------------------------------------------------------------------------------------------------- role path
 def _master(tmp_path, decay, resume=False):
-    m = M.SyncReplicasMaster_NN(types.SimpleNamespace(world_size=2), learning_rate=0.1, momentum=0.9, network="LeNet",
-                                dataset="MNIST", ema_decay=decay, train_dir=str(tmp_path) + "/", resume=resume)
-    torch.manual_seed(0)
-    return m.build_model(10)
+    return role_master(tmp_path, learning_rate=0.1, momentum=0.9, ema_decay=decay, resume=resume)
 
 
 def test_role_path_average_is_the_fp32_oracle(tmp_path):
@@ -196,21 +155,13 @@ def test_role_path_without_the_average_keeps_none(tmp_path):
     assert _master(tmp_path, 0.0).ema is None
 
 
-def _role_run(d, port, max_steps, *extra):
-    cmd = [sys.executable, "-m", "atomo_b200.distributed_nn", "--synthetic", "1", "--train-len", "512",
-           "--test-len", "128", "--batch-size", "32", "--lr", "0.01", "--test-batch-size", "64", "--nproc", "2",
-           "--network", "LeNet", "--dataset", "MNIST", "--code", "sgd", "--momentum", "0.9", "--ema-decay", "0.8",
-           "--max-steps", str(max_steps), "--eval-freq", "1", "--train-dir", d, "--master-port", str(port), *extra]
-    env = dict(os.environ, ATOMO_HANG_DUMP_S="400", PYTHONPATH=ROOT, OMP_NUM_THREADS="2", MKL_NUM_THREADS="2")
-    r = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=420)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-    return r.stdout
+ROLE_FLAGS = ("--momentum", "0.9", "--ema-decay", "0.8")
 
 
 def test_gloo_role_path_writes_and_restores_the_average(tmp_path, capsys):
     d = str(tmp_path) + "/"
-    _role_run(d, 29571, 3)
-    out = _role_run(d, 29572, 5, "--resume", "1")
+    role_run(d, 29571, 3, *ROLE_FLAGS)
+    out = role_run(d, 29572, 5, *ROLE_FLAGS, "--resume", "1")
     assert "weight average starts" not in out
     w = np.float32(1.0 - 0.8)
     load = lambda name: torch.load(d + name, map_location="cpu")

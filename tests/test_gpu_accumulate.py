@@ -7,7 +7,7 @@ GPU: ``N = 1`` is the engine without the option; the buffer each encoder reads e
 batch of N b; a resume is bitwise; the peak memory falls.
 """
 import argparse
-import os
+import functools
 import types
 
 import numpy as np
@@ -17,7 +17,8 @@ import torch
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
 
-from shadow_harness import fit_args, forbid_cuda
+from shadow_harness import SVD3, StandInEngine, deterministic_cudnn, differs, engine_batch, fit_args, forbid_cuda, \
+    make_engine, nccl_init, spawn  # noqa: F401
 
 FLT_MIN = float(np.finfo(np.float32).tiny)
 
@@ -44,16 +45,12 @@ def test_prepare_refuses_an_indivisible_batch():
         ShadowEngine.prepare(eng, torch.zeros(8, 3, 4, 4), torch.zeros(8, dtype=torch.long))
 
 
-def _args(tmp_path, *extra):
-    return fit_args(tmp_path, "--code", "svd", "--svd-rank", "3", *extra)
-
-
 def test_fused_engine_and_fp32_refuse_the_flag(tmp_path):
     model = torch.nn.Linear(4, 4)
     for extra in (("--engine", "fused", "--dtype", "bf16"), ("--dtype", "fp32"),
                   ("--dtype", "bf16", "--code", "entrywise")):        # auto sends entrywise to the fp32-flat engine
         with pytest.raises(SystemExit, match="--accumulate-steps"):
-            L._build_engine(_args(tmp_path, "--accumulate-steps", "2", *extra), model, 0, 1)
+            L._build_engine(fit_args(tmp_path, *SVD3, "--accumulate-steps", "2", *extra), model, 0, 1)
 
 
 @pytest.mark.parametrize("backend", ["gloo", "nccl"])
@@ -62,59 +59,28 @@ def test_role_backends_refuse_the_flag(backend, monkeypatch, tmp_path):
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
     with pytest.raises(SystemExit, match="--accumulate-steps"):
-        distributed_nn.run_rank(_args(tmp_path, "--accumulate-steps", "2", "--backend", backend))
+        distributed_nn.run_rank(fit_args(tmp_path, *SVD3, "--accumulate-steps", "2", "--backend", backend))
 
 
-class StandInEngine:
-    """Plain SGD on the CPU behind the engine interface the launcher uses; records the batch sizes it is given."""
-    first_worker, W, is_worker, is_ps, is_owner = 0, 1, True, True, True
-    instances = []
+class BatchStandIn(StandInEngine):
+    """Records the batch sizes it is given."""
 
     def __init__(self, model, args):
-        self.model, self.lr, self.step = model, args.lr, 1
-        self.opt = torch.optim.SGD(model.parameters(), lr=args.lr)
-        self.plan = types.SimpleNamespace(factor_bytes_per_worker=lambda: 1 << 20, dense_bytes=lambda: 1 << 18)
+        super().__init__(model, args)
         self.batches = []
-        StandInEngine.instances.append(self)
-
-    def prepare(self, x, y, warmup=3):
-        for _ in range(warmup):
-            self.train_step(x, y)
-
-    def set_lr(self, lr):
-        self.lr = lr
 
     def train_step(self, x, y):
         self.batches.append(x.shape[0])
-        self.opt.zero_grad()
-        out = self.model(x)
-        loss = torch.nn.functional.cross_entropy(out, y)
-        loss.backward()
-        self.opt.step()
-        self.step += 1
-        hit = out.argmax(1).eq(y).float().mean() * 100
-        return torch.stack([loss.detach(), hit, hit])
-
-    def phase_stats(self, reset=True):
-        return {"param_wait_us": 10.0, "encode_us": 300.0, "to_push_us": 1500.0}
-
-    def error_code(self):
-        return 0
-
-    def save_checkpoint(self, train_dir, step):
-        pass
-
-    def close(self):
-        pass
+        return super().train_step(x, y)
 
 
 def test_launcher_draws_n_micro_batches_per_step(tmp_path, monkeypatch, capsys):
     import re
     StandInEngine.instances.clear()
-    monkeypatch.setattr(L, "_build_engine", lambda args, model, rank, world: (StandInEngine(model, args), "fused"))
+    monkeypatch.setattr(L, "_build_engine", lambda args, model, rank, world: (BatchStandIn(model, args), "fused"))
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
-    L.run_p2p_training(_args(tmp_path, "--max-steps", "6", "--accumulate-steps", "4"), device="cpu")
+    L.run_p2p_training(fit_args(tmp_path, *SVD3, "--max-steps", "6", "--accumulate-steps", "4"), device="cpu")
     eng = StandInEngine.instances[-1]
     assert eng.batches and set(eng.batches) == {4 * 32}
     recs = [re.match(r"Worker: 0, Step: (\d+), Epoch: \d+ \[(\d+)/(\d+)", l)
@@ -127,37 +93,16 @@ def test_launcher_draws_n_micro_batches_per_step(tmp_path, monkeypatch, capsys):
 
 
 # ---------------------------------------------------------------------------------------------------- GPU helpers
-@pytest.fixture
-def deterministic_cudnn(monkeypatch):
-    monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)
-    monkeypatch.setattr(torch.backends.cudnn, "benchmark", False)
-
-
 CODE_KW = {"svd": dict(svd_rank=3), "qsvd": dict(svd_rank=3), "sgd": {}, "qsgd": dict(quantization_level=2),
            "terngrad": {}, "entrywise": dict(entry_budget=0.05), "topk": dict(entry_budget=0.01), "sign": {},
            "powersgd": dict(svd_rank=2), "fp8": {}, "hadamard": dict(quantization_level=4)}
 EF_CODES = ("svd", "qsgd", "entrywise", "topk", "sign", "powersgd", "fp8", "hadamard")
 
-_BATCHES = {}
-
-
-def _batch(net, step, n):
-    from atomo_b200.data import SyntheticImageDataset
-    from atomo_b200.models import input_shape
-    k = (net, step % 4, n)
-    if k not in _BATCHES:
-        x, y = SyntheticImageDataset(input_shape(net), 10, 4096, seed=200 + k[1]).materialize(n)
-        _BATCHES[k] = (x.cuda(), y.cuda())
-    return _BATCHES[k]
+_batch = functools.partial(engine_batch, seed=200)
 
 
 def _engine(net, **kw):
-    from atomo_b200.models import build_model
-    from atomo_b200.runtime.shadow_engine import ShadowEngine
-    torch.manual_seed(0)
-    torch.cuda.set_device(0)
-    kw = dict(dict(lr=0.05, momentum=0.9, seed=7), **kw)
-    return ShadowEngine(build_model(net, 10), 0, 1, **kw)
+    return make_engine(net, **dict(dict(lr=0.05, momentum=0.9), **kw))
 
 
 def _state(eng) -> dict:
@@ -168,11 +113,6 @@ def _state(eng) -> dict:
     for name, t in eng._worker_tensors().items():
         out["worker:" + name] = t.clone()
     return out
-
-
-def _differs(a, b):
-    assert a.keys() == b.keys()
-    return [k for k in a if not torch.equal(a[k], b[k])]
 
 
 def _run(net, steps, batch, warmup=2, **kw):
@@ -198,7 +138,7 @@ def test_one_micro_batch_is_the_engine_without_the_option(code, ef, graph, deter
     a, na = _run("ResNet18", 4, 32, **kw)
     b, nb = _run("ResNet18", 4, 32, accumulate_steps=1, **kw)
     assert na == nb
-    assert _differs(a, b) == []
+    assert differs(a, b) == []
 
 
 def ftz(t):
@@ -293,7 +233,7 @@ def test_graph_replay_equals_eager(code, n, deterministic_cudnn):
         kw.pop("error_feedback")
     g, _ = _run("ResNet18", 4, 24, use_graph=True, **kw)
     e, _ = _run("ResNet18", 4, 24, use_graph=False, **kw)
-    assert _differs(g, e) == []
+    assert differs(g, e) == []
 
 
 @pytest.mark.gpu
@@ -365,11 +305,11 @@ def test_resume_is_bitwise(code, tmp_path, deterministic_cudnn, capsys):
 
     d = str(tmp_path) + "/"
     a = run(2 * K)
-    assert _differs(a, run(2 * K)) == [], "control: two uninterrupted runs differ"
+    assert differs(a, run(2 * K)) == [], "control: two uninterrupted runs differ"
     run(K, save=d)
     c = run(K, load=2 + K, save=d)
     assert "not restored" not in capsys.readouterr().out
-    assert _differs(a, c) == []
+    assert differs(a, c) == []
     assert bool(a["worker:residual"].ne(0).any())
     run(1, load=2 + K, save=d, accumulate_steps=1)      # the accumulators are scratch: N = 2 state loads at N = 1
     assert "not restored" not in capsys.readouterr().out
@@ -401,11 +341,8 @@ def test_peak_memory_falls():
 # ---------------------------------------------------------------------------------------------------- two GPUs
 def _mp_graph_eager(rank, world, port, out):
     import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
-                      LOCAL_RANK=str(rank))
-    torch.cuda.set_device(rank)
+    nccl_init(rank, world, port)
     torch.backends.cudnn.deterministic, torch.backends.cudnn.benchmark = True, False
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
     from atomo_b200.models import build_model
     from atomo_b200.runtime.shadow_engine import ShadowEngine
     res = []
@@ -430,14 +367,5 @@ def _mp_graph_eager(rank, world, port, out):
 def test_two_gpus_sharded_graph_equals_eager():
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    out = ctx.Queue()
-    procs = [ctx.Process(target=_mp_graph_eager, args=(r, 2, 29680, out)) for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(600)
-        assert p.exitcode == 0
-    res = sorted(out.get() for _ in range(2))
+    res = spawn(2, _mp_graph_eager, 29680)
     assert all(same and e1 == 0 and e2 == 0 for _, same, e1, e2 in res), res

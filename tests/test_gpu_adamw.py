@@ -12,7 +12,7 @@ followed by the engine's Adam with weight decay 0.
   clipping above the norm; ``accumulate_steps=2``; the weight average; bitwise resume (Adam and AMSGrad, and across
   ``adam`` / ``adamw``); the launcher.  The two-GPU test checks that the replicas agree.
 """
-import os
+import functools
 
 import numpy as np
 import pytest
@@ -20,7 +20,8 @@ import torch
 
 from atomo_b200.ops import plan2 as P2
 
-from shadow_harness import H2, ext, model_shapes
+from shadow_harness import H2, deterministic_cudnn, differs, engine_batch, ext, make_engine, model_shapes, nccl_init, \
+    spawn, state, step  # noqa: F401
 
 LR, WD = 2e-3, 0.05
 CODES = {
@@ -31,54 +32,19 @@ CODES = {
     "hadamard": dict(code="hadamard", quantization_level=4, bucket_size=256),
 }
 
-_BATCHES = {}
+DATA_SEED = 700
+_state = functools.partial(state, keys=("master", "vparams", "mom", "vmom", "sq", "vsq", "sqmax", "vsqmax", "wshadow"))
 
 
-def _batch(step, n=32):
-    from atomo_b200.data import SyntheticImageDataset
-    k = (step % 4, n)
-    if k not in _BATCHES:
-        x, y = SyntheticImageDataset((3, 32, 32), 10, 4096, seed=700 + k[0]).materialize(n)
-        _BATCHES[k] = (x.cuda(), y.cuda())
-    return _BATCHES[k]
-
-
-def _engine(graph=False, overlap=None, optimizer="adamw", lr=LR, weight_decay=WD, net="ResNet18", **kw):
-    from atomo_b200.models import build_model
-    from atomo_b200.runtime.shadow_engine import ShadowEngine
-    torch.manual_seed(0)
+def _engine(graph=False, overlap=None, optimizer="adamw", lr=LR, weight_decay=WD, **kw):
     kw = dict(CODES["svd"], **kw) if "code" not in kw else kw
-    eng = ShadowEngine(build_model(net, 10), 0, 1, use_graph=graph, overlap=graph if overlap is None else overlap,
-                       seed=7, optimizer=optimizer, lr=lr, weight_decay=weight_decay, **kw)
-    x, y = _batch(0, 32 * eng.accum)
-    eng.prepare(x, y, warmup=0)
-    return eng
+    return make_engine(use_graph=graph, overlap=graph if overlap is None else overlap, optimizer=optimizer, lr=lr,
+                       weight_decay=weight_decay, prepare_n=32 * kw.get("accumulate_steps", 1), data_seed=DATA_SEED,
+                       **kw)
 
 
 def _step(eng):
-    x, y = _batch(eng.step, 32 * eng.accum)
-    loss = eng.train_step(x, y)
-    torch.cuda.synchronize()
-    assert eng.error_code() == 0
-    return float(loss[0])
-
-
-def _state(eng):
-    out = {k: getattr(eng, k).clone() for k in ("master", "vparams", "mom", "vmom", "sq", "vsq")}
-    if eng.sqmax is not None:
-        out["sqmax"], out["vsqmax"] = eng.sqmax.clone(), eng.vsqmax.clone()
-    out["wshadow"] = eng.wshadow.clone()
-    return out
-
-
-def _differ(a, b):
-    return [k for k in a if not torch.equal(a[k], b[k])]
-
-
-@pytest.fixture
-def deterministic_cudnn(monkeypatch):
-    monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)
-    monkeypatch.setattr(torch.backends.cudnn, "benchmark", False)
+    return step(eng, engine_batch("ResNet18", eng.step, 32 * eng.accum, DATA_SEED))
 
 
 def _range_mask(pl, t0, nt, device="cuda"):
@@ -186,7 +152,7 @@ def test_step_is_torch_decay_then_the_ps_launch(code, amsgrad, deterministic_cud
             _step(eng)
         runs.append(_state(eng))
         eng.close()
-    assert _differ(runs[0], runs[1]) == []
+    assert differs(runs[0], runs[1]) == []
 
 
 @pytest.mark.gpu
@@ -233,7 +199,7 @@ def test_zero_decay_is_adam(amsgrad, deterministic_cudnn):
         losses = [_step(eng) for _ in range(5)]
         runs.append((losses, _state(eng), eng.launches_per_step))
         eng.close()
-    assert runs[0][0] == runs[1][0] and _differ(runs[0][1], runs[1][1]) == [] and runs[0][2] == runs[1][2]
+    assert runs[0][0] == runs[1][0] and differs(runs[0][1], runs[1][1]) == [] and runs[0][2] == runs[1][2]
 
 
 @pytest.mark.gpu
@@ -301,7 +267,7 @@ def test_eager_equals_graph_and_reruns(code, deterministic_cudnn):
             _step(eng)
         runs.append(_state(eng))
         eng.close()
-    assert all(_differ(runs[0], r) == [] for r in runs[1:])
+    assert all(differs(runs[0], r) == [] for r in runs[1:])
 
 
 @pytest.mark.gpu
@@ -317,8 +283,8 @@ def test_set_lr_between_replays_changes_the_decay(deterministic_cudnn):
             _step(eng)
         runs.append(_state(eng))
         eng.close()
-    assert _differ(runs[0], runs[1]) == []
-    assert "master" in _differ(runs[1], runs[2])
+    assert differs(runs[0], runs[1]) == []
+    assert "master" in differs(runs[1], runs[2])
 
 
 @pytest.mark.gpu
@@ -334,7 +300,7 @@ def test_clip_above_the_norm_is_unclipped_adamw(code, deterministic_cudnn):
             assert 0 < total < clip and coef == 1.0
         runs.append(_state(eng))
         eng.close()
-    assert _differ(runs[0], runs[1]) == []
+    assert differs(runs[0], runs[1]) == []
 
 
 @pytest.mark.gpu
@@ -352,9 +318,9 @@ def test_accumulate_steps_two(graph, deterministic_cudnn):
                                                               if eng.plan.ps_range[g][eng.owner_index][1] > 0))
         eng.close()
     assert runs["adamw"][1] == runs["adam"][1] + runs["adamw"][2]
-    assert "master" in _differ(runs["adam"][0], runs["adamw"][0])
+    assert "master" in differs(runs["adam"][0], runs["adamw"][0])
     if not graph:
-        assert _differ(runs["adamw"][0], runs["adamw-torch"][0]) == []
+        assert differs(runs["adamw"][0], runs["adamw-torch"][0]) == []
 
 
 @pytest.mark.gpu
@@ -401,7 +367,7 @@ def test_resume_is_bitwise(amsgrad, tmp_path, deterministic_cudnn):
     eng.load_checkpoint(d, 3)
     for _ in range(3):
         _step(eng)
-    assert _differ(want, _state(eng)) == []
+    assert differs(want, _state(eng)) == []
     eng.close()
 
 
@@ -418,7 +384,7 @@ def test_adam_and_adamw_checkpoints_load_into_each_other(tmp_path):
         eng = _engine(optimizer=loader)
         eng.load_checkpoint(d, 2)
         got = _state(eng)
-        assert _differ({k: want[k] for k in ("master", "mom", "sq", "vsq")},
+        assert differs({k: want[k] for k in ("master", "mom", "sq", "vsq")},
                        {k: got[k] for k in ("master", "mom", "sq", "vsq")}) == []
         _step(eng)
         eng.close()
@@ -449,19 +415,16 @@ def test_launcher_trains_checkpoints_and_resumes(tmp_path, monkeypatch, capsys):
 # ---------------------------------------------------------------------------------------------------- two GPUs
 def _mp(rank, world, port, out):
     import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
-                      LOCAL_RANK=str(rank))
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
+    nccl_init(rank, world, port)
     from atomo_b200.models import build_model
     from atomo_b200.runtime.shadow_engine import ShadowEngine
     torch.manual_seed(0)
     eng = ShadowEngine(build_model("ResNet18", 10), rank, world, use_graph=True, seed=7, ps_mode="sharded",
                        optimizer="adamw", lr=LR, weight_decay=WD, **CODES["svd"])
-    x, y = _batch(rank)
+    x, y = engine_batch("ResNet18", rank, seed=DATA_SEED)
     eng.prepare(x, y, warmup=0)
     for s in range(4):
-        x, y = _batch(1 + s + rank)
+        x, y = engine_batch("ResNet18", 1 + s + rank, seed=DATA_SEED)
         eng.train_step(x, y)
     torch.cuda.synchronize()
     dist.barrier()
@@ -476,16 +439,7 @@ def _mp(rank, world, port, out):
 def test_two_owners_keep_identical_replicas():
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    out = ctx.Queue()
-    procs = [ctx.Process(target=_mp, args=(r, 2, 29730, out)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = sorted((out.get(timeout=600) for _ in range(2)), key=lambda r: r[0])
-    for p in procs:
-        p.join(600)
-        assert p.exitcode == 0
+    res = spawn(2, _mp, 29730)
     assert all(r[1] == 0 for r in res)
     a, b = res
     assert torch.equal(a[2], b[2]) and torch.equal(a[3], b[3]) and torch.equal(a[4], b[4])

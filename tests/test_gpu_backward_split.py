@@ -3,18 +3,11 @@ Every value must stay bit for bit what the stock autograd node computes."""
 import pytest
 import torch
 
+from shadow_harness import deterministic_cudnn  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 
 CL = torch.channels_last
-
-
-@pytest.fixture
-def cudnn_deterministic():
-    """cuDNN as bench.py runs it: deterministic, heuristically chosen algorithms."""
-    old = torch.backends.cudnn.benchmark, torch.backends.cudnn.deterministic
-    torch.backends.cudnn.benchmark, torch.backends.cudnn.deterministic = False, True
-    yield
-    torch.backends.cudnn.benchmark, torch.backends.cudnn.deterministic = old
 
 
 def _bf16(shape):
@@ -23,7 +16,7 @@ def _bf16(shape):
 
 @pytest.mark.parametrize("k,stride", [(3, 1), (3, 2), (1, 2), (1, 1)])
 @pytest.mark.parametrize("graph", [False, True])
-def test_split_conv_backward_equals_convolution_backward(cudnn_deterministic, k, stride, graph):
+def test_split_conv_backward_equals_convolution_backward(deterministic_cudnn, k, stride, graph):
     from atomo_b200.ops.split_conv import Conv2d
     cin, cout = 64, 128
     conv = Conv2d(cin, cout, k, stride, k // 2, bias=False).cuda().to(torch.bfloat16).to(memory_format=CL)
@@ -60,7 +53,7 @@ def test_split_conv_backward_equals_convolution_backward(cudnn_deterministic, k,
 
 
 @pytest.mark.parametrize("use_graph,overlap", [(True, True), (False, False)])
-def test_shadow_engine_steps_equal_the_stock_backward(cudnn_deterministic, use_graph, overlap):
+def test_shadow_engine_steps_equal_the_stock_backward(deterministic_cudnn, use_graph, overlap):
     from atomo_b200.data import SyntheticImageDataset
     from atomo_b200.models import build_model
     from atomo_b200.ops.split_conv import enable_split_wgrad
@@ -84,7 +77,7 @@ def test_shadow_engine_steps_equal_the_stock_backward(cudnn_deterministic, use_g
     assert torch.equal(runs[0][1], runs[1][1])
 
 
-def test_trace_has_wgrad_on_a_second_stream(cudnn_deterministic):
+def test_trace_has_wgrad_on_a_second_stream(deterministic_cudnn):
     from torch.profiler import ProfilerActivity, profile
     from atomo_b200.models import build_model
     from atomo_b200.ops.fused_bn import enable_fused_bn

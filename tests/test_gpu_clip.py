@@ -12,14 +12,16 @@ bitwise comparison with the unclipped engine instead).  Runs are repeatable,
 graph replay equals eager, accumulation clips the step's mean once, error feedback is untouched, a resume is bitwise,
 and a non-finite norm raises the sticky error.  The two-GPU test exercises the cross-owner exchange.
 """
+import functools
 import math
-import os
 
 import numpy as np
 import pytest
 import torch
 
 from atomo_b200.optim import LAMB, LARS, SGD
+
+from shadow_harness import deterministic_cudnn, engine_batch, make_engine, nccl_init, spawn, state, step  # noqa: F401
 
 EPS32 = 2.0 ** -24
 TILE = 4608
@@ -43,41 +45,20 @@ OPTS = {
 HUGE = 1e30       # far above any norm: coef = 1
 TINY = 1e-3       # far below the norm of a ResNet-18 gradient: coef < 1
 
-_BATCHES = {}
-
-
-def _batch(step, n=32):
-    from atomo_b200.data import SyntheticImageDataset
-    k = (step % 4, n)
-    if k not in _BATCHES:
-        x, y = SyntheticImageDataset((3, 32, 32), 10, 4096, seed=500 + k[0]).materialize(n)
-        _BATCHES[k] = (x.cuda(), y.cuda())
-    return _BATCHES[k]
+DATA_SEED = 500
+_batch = functools.partial(engine_batch, "ResNet18", seed=DATA_SEED)
 
 
 def _engine(kw, graph=False, **extra):
-    from atomo_b200.models import build_model
-    from atomo_b200.runtime.shadow_engine import ShadowEngine
-    torch.manual_seed(0)
-    eng = ShadowEngine(build_model("ResNet18", 10), 0, 1, use_graph=graph, seed=7, **dict(kw, **extra))
-    x, y = _batch(0)
-    eng.prepare(x, y, warmup=0)
-    return eng
+    return make_engine(use_graph=graph, prepare_n=32, data_seed=DATA_SEED, **dict(kw, **extra))
 
 
 def _step(eng, check=True):
-    x, y = _batch(eng.step)
-    eng.train_step(x, y)
-    torch.cuda.synchronize()
-    if check:
-        assert eng.error_code() == 0
+    step(eng, _batch(eng.step), check)
 
 
 STATE = ("master", "mom", "sq", "sqmax", "vparams", "vmom", "vsq", "vsqmax", "wshadow")
-
-
-def _state(eng):
-    return {k: getattr(eng, k).clone() for k in STATE if getattr(eng, k, None) is not None}
+_state = functools.partial(state, keys=STATE)
 
 
 def _phys(t):
@@ -227,12 +208,6 @@ def _run(kw, graph, steps=4, **extra):
     return out, norms
 
 
-@pytest.fixture
-def deterministic_cudnn(monkeypatch):
-    monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)
-    monkeypatch.setattr(torch.backends.cudnn, "benchmark", False)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("opt,code", [("momentum", "svd"), ("lamb", "topk")])
 def test_bitwise_repeatable_and_graph_equals_eager(opt, code, deterministic_cudnn):
@@ -313,10 +288,7 @@ def test_a_non_finite_norm_sets_the_sticky_error():
 # ---------------------------------------------------------------------------------------------------- two GPUs
 def _mp(rank, world, port, mode, out):
     import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
-                      LOCAL_RANK=str(rank))
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
+    nccl_init(rank, world, port)
     from atomo_b200.models import build_model
     from atomo_b200.runtime.shadow_engine import ShadowEngine
     torch.manual_seed(0)
@@ -327,7 +299,7 @@ def _mp(rank, world, port, mode, out):
     x, y = _batch(1 + rank)
     eng.train_step(x, y)
     torch.cuda.synchronize()
-    out.put((mode, rank, eng.error_code(), eng.clip_norm.cpu(), eng.wshadow.cpu()))
+    out.put((rank, mode, eng.error_code(), eng.clip_norm.cpu(), eng.wshadow.cpu()))
     eng.close()
     dist.destroy_process_group()
 
@@ -337,21 +309,11 @@ def _mp(rank, world, port, mode, out):
 def test_two_owners_agree_on_the_norm():
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
     res = {}
     for i, mode in enumerate(("sharded", "colocated")):
-        out = ctx.Queue()
-        procs = [ctx.Process(target=_mp, args=(r, 2, 29690 + i, mode, out)) for r in range(2)]
-        for p in procs:
-            p.start()
-        for _ in range(2):
-            m, r, e, n, w = out.get(timeout=600)
+        for r, m, e, n, w in spawn(2, _mp, 29690 + i, mode):
             assert e == 0
             res[(m, r)] = (n, w)
-        for p in procs:
-            p.join(600)
-            assert p.exitcode == 0
     (n0, w0), (n1, w1) = res[("sharded", 0)], res[("sharded", 1)]
     assert torch.equal(n0, n1) and torch.equal(w0, w1)
     nc = res[("colocated", 0)][0]

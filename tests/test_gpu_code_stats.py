@@ -5,7 +5,6 @@ launcher's metrics record."""
 import argparse
 import json
 import math
-import os
 
 import numpy as np
 import pytest
@@ -13,7 +12,7 @@ import torch
 
 from atomo_b200.ops import plan2 as P
 
-from shadow_harness import Linear
+from shadow_harness import Linear, nccl_init, spawn
 
 pytestmark = pytest.mark.gpu
 
@@ -318,9 +317,7 @@ def _mp_worker(rank, world, port, code, out):
     from atomo_b200.data import SyntheticImageDataset
     from atomo_b200.models import build_model
     from atomo_b200.runtime.shadow_engine import ShadowEngine
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
+    nccl_init(rank, world, port)
     torch.manual_seed(0)
     x, y = SyntheticImageDataset((3, 32, 32), 10, 4096, seed=rank).materialize(32)
     eng = ShadowEngine(build_model("VGG11", 10), rank, world, code=code, lr=0.05, momentum=0.9, use_graph=False,
@@ -352,15 +349,6 @@ def test_code_stats_on_every_rank(code):
     n = torch.cuda.device_count()
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    out = ctx.Queue()
     port = 29840 + (3 if code == "entrywise" else 0)
-    procs = [ctx.Process(target=_mp_worker, args=(r, 2, port, code, out)) for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(300)
-        assert p.exitcode == 0
-    res = sorted(out.get() for _ in range(2))
+    res = spawn(2, _mp_worker, port, code, timeout=300)
     assert all(ok for _, ok in res), res

@@ -15,8 +15,8 @@ from atomo_b200.codings import signum as S
 from atomo_b200.ops import plan2 as P
 from atomo_b200.utils.flags import add_fit_args
 
-from shadow_harness import Linear, ef_grads, run_mp, train
-from test_gpu_signum import HSG, NAN, SHAPES, ZERO, Oracle, _check_ps, _check_push
+from shadow_harness import HSG, NAN, SIGNUM_SHAPES, ZERO, Linear, SignumOracle, ef_grads, run_mp, signum_check_ps, \
+    signum_check_push, train
 
 BETAS = [(0.0, 0.99), (0.9, 0.99), (0.95, 0.98)]
 
@@ -47,7 +47,7 @@ class HDL(HSG):
         torch.cuda.synchronize()
 
 
-class DOracle(Oracle):
+class DOracle(SignumOracle):
     """Signum's oracle with the Lion worker step (``u`` holds m, ``x`` the pushed direction c) and the aggregate."""
 
     def push(self, w, phys, coin=False):
@@ -94,10 +94,10 @@ def _run(h, steps, special=False, pushers=None, coin=False):
             phys = h.fill(w, 1000 * s + w, special=special, who=w)
             o.push(w, phys, coin)
             h.encode(w, coin)
-            _check_push(h, o, w)
+            signum_check_push(h, o, w)
         h.ps()
         o.ps(ws, coin)
-        _check_ps(h, o)
+        signum_check_ps(h, o)
     return h, o
 
 
@@ -109,7 +109,7 @@ def _run(h, steps, special=False, pushers=None, coin=False):
 @pytest.mark.parametrize("betas", BETAS)
 @pytest.mark.parametrize("agg", ["vote", "mean"])
 def test_encode_and_aggregate_match_oracle_bitwise(W, owners, groups, betas, agg):
-    h = HDL(SHAPES[:10], betas=betas, agg=agg, W=W, n_groups=groups, n_owners=owners, seed=W + 10 * owners)
+    h = HDL(SIGNUM_SHAPES[:10], betas=betas, agg=agg, W=W, n_groups=groups, n_owners=owners, seed=W + 10 * owners)
     _run(h, 3)
 
 
@@ -117,7 +117,7 @@ def test_encode_and_aggregate_match_oracle_bitwise(W, owners, groups, betas, agg
 @pytest.mark.parametrize("W,betas", [(2, (0.0, 0.99)), (4, (0.9, 0.99)), (3, (0.95, 0.98))])
 @pytest.mark.parametrize("agg", ["vote", "mean"])
 def test_designed_zeros_ties_nan_and_tails(W, betas, agg):
-    h = HDL(SHAPES, betas=betas, agg=agg, W=W, n_owners=2, n_groups=2)
+    h = HDL(SIGNUM_SHAPES, betas=betas, agg=agg, W=W, n_owners=2, n_groups=2)
     init = h.master.cpu().numpy().copy()
     _, o = _run(h, 3, special=True)
     # the NaN of worker 0 makes its tile NaN under either aggregate, on every step
@@ -132,7 +132,7 @@ def test_designed_zeros_ties_nan_and_tails(W, betas, agg):
 @pytest.mark.parametrize("agg", ["vote", "mean"])
 def test_even_w_ties_step_zero(agg):
     """W = 2, worker 1 pushes the negated gradient of worker 0 (b1 == 0): every nonzero element ties and stays."""
-    h = HDL(SHAPES[:10], betas=(0.0, 0.99), agg=agg, W=2)
+    h = HDL(SIGNUM_SHAPES[:10], betas=(0.0, 0.99), agg=agg, W=2)
     before = h.master.cpu().numpy().copy()
     o = DOracle(h)
     h.set_step(1)
@@ -142,10 +142,10 @@ def test_even_w_ties_step_zero(agg):
     for w, ph in ((0, phys0), (1, {k: -v for k, v in phys0.items()})):
         o.push(w, ph)
         h.encode(w)
-        _check_push(h, o, w)
+        signum_check_push(h, o, w)
     h.ps()
     o.ps([0, 1])
-    _check_ps(h, o)
+    signum_check_ps(h, o)
     x = o.x[0]
     tie = np.zeros(x.size, bool)
     for q in h.plan.params:
@@ -158,7 +158,7 @@ def test_even_w_ties_step_zero(agg):
 @pytest.mark.parametrize("betas", [(0.0, 0.99), (0.9, 0.99)])
 @pytest.mark.parametrize("agg", ["vote", "mean"])
 def test_philox_coin_matches_oracle(betas, agg):
-    h = HDL(SHAPES, betas=betas, agg=agg, W=3, n_owners=2)
+    h = HDL(SIGNUM_SHAPES, betas=betas, agg=agg, W=3, n_owners=2)
     _run(h, 2, special=True, coin=True)
 
 
@@ -167,7 +167,7 @@ def test_philox_coin_matches_oracle(betas, agg):
 @pytest.mark.parametrize("agg", ["vote", "mean"])
 def test_num_aggregate_counts_only_fresh_workers(betas, agg):
     """W = 3, --num-aggregate 2: worker 2 pushes at step 1 only, then goes stale; the owners count 0 and 1."""
-    h = HDL(SHAPES[:10], betas=betas, agg=agg, W=3, num_aggregate=2, n_owners=2)
+    h = HDL(SIGNUM_SHAPES[:10], betas=betas, agg=agg, W=3, num_aggregate=2, n_owners=2)
     _run(h, 3, pushers=lambda s: [0, 1, 2] if s == 1 else [0, 1])
 
 

@@ -9,11 +9,14 @@ strictly, ``latest_step`` skips it and the evaluator reads it with ``ema=True``;
 at ``--eval-freq`` and resumes it.  The two-GPU test checks the sharded average against the oracle on the gathered
 master.
 """
+import functools
 import os
 
 import numpy as np
 import pytest
 import torch
+
+from shadow_harness import deterministic_cudnn, engine_batch, make_engine, nccl_init, spawn, step  # noqa: F401
 
 DECAY = 0.9
 
@@ -29,46 +32,21 @@ OPTS = {
     "momentum+clip": dict(optimizer="sgd", lr=0.05, momentum=0.9, weight_decay=5e-4, clip_grad_norm=0.5),
 }
 
-_BATCHES = {}
-
-
-def _batch(step, n=32):
-    from atomo_b200.data import SyntheticImageDataset
-    k = (step % 4, n)
-    if k not in _BATCHES:
-        x, y = SyntheticImageDataset((3, 32, 32), 10, 4096, seed=500 + k[0]).materialize(n)
-        _BATCHES[k] = (x.cuda(), y.cuda())
-    return _BATCHES[k]
+DATA_SEED = 500
+_batch = functools.partial(engine_batch, "ResNet18", seed=DATA_SEED)
 
 
 def _engine(kw, graph=False, ema_decay=DECAY):
-    from atomo_b200.models import build_model
-    from atomo_b200.runtime.shadow_engine import ShadowEngine
-    torch.manual_seed(0)
-    eng = ShadowEngine(build_model("ResNet18", 10), 0, 1, use_graph=graph, overlap=graph, seed=7,
-                       ema_decay=ema_decay, **kw)
-    x, y = _batch(0)
-    eng.prepare(x, y, warmup=0)
-    return eng
+    return make_engine(use_graph=graph, overlap=graph, ema_decay=ema_decay, prepare_n=32, data_seed=DATA_SEED, **kw)
 
 
 def _step(eng):
-    x, y = _batch(eng.step)
-    loss = eng.train_step(x, y)
-    torch.cuda.synchronize()
-    assert eng.error_code() == 0
-    return float(loss[0])
+    return step(eng, _batch(eng.step))
 
 
 def _oracle(e, p, w):
     """One step of the average in numpy float32: three separately rounded operations."""
     return e + w * (p - e)
-
-
-@pytest.fixture
-def deterministic_cudnn(monkeypatch):
-    monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)
-    monkeypatch.setattr(torch.backends.cudnn, "benchmark", False)
 
 
 @pytest.mark.gpu
@@ -214,10 +192,7 @@ def test_launcher_evaluates_and_resumes_the_average(tmp_path, monkeypatch, capsy
 # ---------------------------------------------------------------------------------------------------- two GPUs
 def _mp(rank, world, port, out):
     import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
-                      LOCAL_RANK=str(rank))
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
+    nccl_init(rank, world, port)
     from atomo_b200.models import build_model
     from atomo_b200.runtime.shadow_engine import ShadowEngine
     torch.manual_seed(0)
@@ -248,16 +223,7 @@ def _mp(rank, world, port, out):
 def test_two_owners_average_their_shards():
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    out = ctx.Queue()
-    procs = [ctx.Process(target=_mp, args=(r, 2, 29710, out)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = sorted((out.get(timeout=600) for _ in range(2)), key=lambda r: r[0])
-    for p in procs:
-        p.join(600)
-        assert p.exitcode == 0
+    res = spawn(2, _mp, 29710)
     assert all(r[1] == 0 and r[2] for r in res)
     a, b = res[0][3], res[1][3]
     assert all(torch.equal(a[k], b[k]) for k in a)

@@ -1,10 +1,9 @@
 """Fused engine end-to-end on the GPU (1 GPU always; 2 GPUs when present)."""
-import os
 
 import pytest
 import torch
 
-from shadow_harness import batch
+from shadow_harness import batch, nccl_init, spawn
 
 pytestmark = pytest.mark.gpu
 
@@ -61,14 +60,11 @@ def test_dense_engine_matches_plain_sgd():
     eng.close()
 
 
-def _two_rank_worker(rank, world, code, port, out):
+def _two_rank_worker(rank, world, port, code, out):
     import torch.distributed as dist
     from atomo_b200.models import build_model
     from atomo_b200.runtime.engine import FusedEngine
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
-                      LOCAL_RANK=str(rank))
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
+    nccl_init(rank, world, port)
     torch.manual_seed(0)
     model = build_model("LeNet", 10)
     eng = FusedEngine(model, rank, world, code=code, svd_rank=3, lr=0.05, momentum=0.9, use_graph=True, seed=5,
@@ -96,17 +92,8 @@ def _two_rank_worker(rank, world, code, port, out):
 def test_two_gpu_engine_keeps_replicas_identical(code):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    out = ctx.Queue()
     port = 29620 + 3 * ["svd", "sgd", "qsgd", "entrywise"].index(code)
-    procs = [ctx.Process(target=_two_rank_worker, args=(r, 2, code, port, out)) for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(300)
-        assert p.exitcode == 0
-    res = sorted(out.get() for _ in range(2))
+    res = spawn(2, _two_rank_worker, port, code, timeout=300)
     for rank, err, same, l0, l1, mode, mc in res:
         assert err == 0 and same, res
         assert l1 < l0, res

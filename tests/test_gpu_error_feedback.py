@@ -12,7 +12,7 @@ import torch
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
 
-from shadow_harness import Loopback, ef_grads, fit_args, forbid_cuda
+from shadow_harness import SVD3, Loopback, ef_grads, fit_args, forbid_cuda
 
 
 # ---------------------------------------------------------------------------------------------------- CPU
@@ -37,15 +37,11 @@ def test_shadow_engine_refuses_codes_without_feedback(kw, match, monkeypatch):
         S.ShadowEngine(None, 0, world, error_feedback=True, **kw)
 
 
-def _args(tmp_path, *extra):
-    return fit_args(tmp_path, "--code", "svd", "--svd-rank", "3", *extra)
-
-
 def test_fused_engine_refuses_the_flag(tmp_path):
     model = torch.nn.Linear(4, 4)
     for extra in (("--engine", "fused", "--dtype", "bf16"), ("--dtype", "fp32")):
         with pytest.raises(SystemExit, match="--error-feedback"):
-            L._build_engine(_args(tmp_path, "--error-feedback", "1", *extra), model, 0, 1)
+            L._build_engine(fit_args(tmp_path, *SVD3, "--error-feedback", "1", *extra), model, 0, 1)
 
 
 def test_role_backends_refuse_the_flag(monkeypatch, tmp_path):
@@ -53,7 +49,7 @@ def test_role_backends_refuse_the_flag(monkeypatch, tmp_path):
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
     with pytest.raises(SystemExit, match="--error-feedback"):
-        distributed_nn.run_rank(_args(tmp_path, "--error-feedback", "1", "--backend", "gloo"))
+        distributed_nn.run_rank(fit_args(tmp_path, *SVD3, "--error-feedback", "1", "--backend", "gloo"))
 
 
 # ---------------------------------------------------------------------------------------------------- GPU harness

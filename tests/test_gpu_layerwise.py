@@ -6,8 +6,8 @@ On the dense code, where the PS's gradient is the worker's bf16 gradient exactly
 matches the fp64 ``optim/`` oracle.  Zero tensors give ratio 1; runs are bitwise repeatable and graph replay equals
 eager; accumulation, error feedback and a resume work.  The two-GPU test exercises the cross-owner exchange.
 """
+import functools
 import math
-import os
 
 import numpy as np
 import pytest
@@ -15,6 +15,8 @@ import torch
 
 from atomo_b200.optim import LAMB, LARS
 from atomo_b200.utils import checkpoint as ckpt
+
+from shadow_harness import deterministic_cudnn, engine_batch, make_engine, nccl_init, spawn, step  # noqa: F401
 
 EPS32 = 2.0 ** -24
 TILE = 4608            # the largest PS tile (elements): fp32 partial sums of at most this many terms
@@ -29,33 +31,16 @@ CODES = {
     "fp8": dict(code="fp8"), "hadamard": dict(code="hadamard", quantization_level=4, bucket_size=512),
 }
 
-_BATCHES = {}
+DATA_SEED = 300
+_batch = functools.partial(engine_batch, "ResNet18", seed=DATA_SEED)
 
 
-def _batch(step, n=32):
-    from atomo_b200.data import SyntheticImageDataset
-    k = (step % 4, n)
-    if k not in _BATCHES:
-        x, y = SyntheticImageDataset((3, 32, 32), 10, 4096, seed=300 + k[0]).materialize(n)
-        _BATCHES[k] = (x.cuda(), y.cuda())
-    return _BATCHES[k]
-
-
-def _engine(kw, graph=False, net="ResNet18", **extra):
-    from atomo_b200.models import build_model
-    from atomo_b200.runtime.shadow_engine import ShadowEngine
-    torch.manual_seed(0)
-    eng = ShadowEngine(build_model(net, 10), 0, 1, use_graph=graph, seed=7, **dict(kw, **extra))
-    x, y = _batch(0)
-    eng.prepare(x, y, warmup=0)
-    return eng
+def _engine(kw, graph=False, **extra):
+    return make_engine(use_graph=graph, prepare_n=32, data_seed=DATA_SEED, **dict(kw, **extra))
 
 
 def _step(eng):
-    x, y = _batch(eng.step)
-    eng.train_step(x, y)
-    torch.cuda.synchronize()
-    assert eng.error_code() == 0
+    step(eng, _batch(eng.step))
 
 
 def _weights(eng):
@@ -242,12 +227,6 @@ def _equal(a, b):
     return [k for k in a if not torch.equal(a[k], b[k])]
 
 
-@pytest.fixture
-def deterministic_cudnn(monkeypatch):
-    monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)
-    monkeypatch.setattr(torch.backends.cudnn, "benchmark", False)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("opt,code", [("lars", "svd"), ("lamb", "topk")])
 def test_bitwise_repeatable_and_graph_equals_eager(code, opt, deterministic_cudnn):
@@ -306,10 +285,7 @@ def test_resume_is_bitwise(opt, extra, tmp_path, deterministic_cudnn):
 # ---------------------------------------------------------------------------------------------------- two GPUs
 def _mp_sharded(rank, world, port, opt, out):
     import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
-                      LOCAL_RANK=str(rank))
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
+    nccl_init(rank, world, port)
     from atomo_b200.models import build_model
     from atomo_b200.runtime.shadow_engine import ShadowEngine
     torch.manual_seed(0)
@@ -332,17 +308,8 @@ def _mp_sharded(rank, world, port, opt, out):
 def test_two_owners_agree_on_the_ratios(opt):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    out = ctx.Queue()
     port = 29680 + (opt == "lamb")
-    procs = [ctx.Process(target=_mp_sharded, args=(r, 2, port, opt, out)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = sorted((out.get(timeout=600) for _ in range(2)), key=lambda t: t[0])
-    for p in procs:
-        p.join(600)
-        assert p.exitcode == 0
+    res = spawn(2, _mp_sharded, port, opt)
     (_, e0, r0, w0), (_, e1, r1, w1) = res
     assert e0 == 0 and e1 == 0
     assert torch.equal(r0, r1) and torch.equal(w0, w1)

@@ -12,7 +12,7 @@
   Lion weights; top-k with error feedback; resume is bitwise (svd, top-k + EF); cross-optimizer loads are refused;
   the launcher trains, checkpoints and resumes.  The two-GPU test checks that two owners keep identical replicas.
 """
-import os
+import functools
 
 import numpy as np
 import pytest
@@ -21,7 +21,8 @@ import torch
 from atomo_b200.ops import plan2 as P2
 from atomo_b200.optim import Lion
 
-from shadow_harness import H2, HE, SHAPES
+from shadow_harness import H2, HE, SHAPES, deterministic_cudnn, differs, engine_batch, make_engine, nccl_init, spawn, \
+    state, step  # noqa: F401
 
 LR, WD, BETAS = 1e-3, 0.1, (0.9, 0.99)
 FAMILY = {"svd": 0, "sgd": 0, "qsgd": 1, "terngrad": 1, "entrywise": 2, "topk": 2, "sign": 3, "fp8": 4,
@@ -156,50 +157,18 @@ CODES = {
     "powersgd": dict(code="powersgd", svd_rank=2), "fp8": dict(code="fp8"),
     "hadamard": dict(code="hadamard", quantization_level=4, bucket_size=256),
 }
-_BATCHES = {}
-
-
-def _batch(step, n=32):
-    from atomo_b200.data import SyntheticImageDataset
-    k = (step % 4, n)
-    if k not in _BATCHES:
-        x, y = SyntheticImageDataset((3, 32, 32), 10, 4096, seed=900 + k[0]).materialize(n)
-        _BATCHES[k] = (x.cuda(), y.cuda())
-    return _BATCHES[k]
+DATA_SEED = 900
+_state = functools.partial(state, keys=("master", "vparams", "mom", "vmom", "wshadow"))
 
 
 def _engine(graph=False, optimizer="lion", lr=LR, weight_decay=WD, **kw):
-    from atomo_b200.models import build_model
-    from atomo_b200.runtime.shadow_engine import ShadowEngine
-    torch.manual_seed(0)
     kw = dict(CODES["svd"], **kw) if "code" not in kw else kw
-    eng = ShadowEngine(build_model("ResNet18", 10), 0, 1, use_graph=graph, overlap=graph, seed=7,
-                       optimizer=optimizer, lr=lr, weight_decay=weight_decay, **kw)
-    x, y = _batch(0, 32 * eng.accum)
-    eng.prepare(x, y, warmup=0)
-    return eng
+    return make_engine(use_graph=graph, overlap=graph, optimizer=optimizer, lr=lr, weight_decay=weight_decay,
+                       prepare_n=32 * kw.get("accumulate_steps", 1), data_seed=DATA_SEED, **kw)
 
 
 def _step(eng):
-    x, y = _batch(eng.step, 32 * eng.accum)
-    loss = eng.train_step(x, y)
-    torch.cuda.synchronize()
-    assert eng.error_code() == 0
-    return float(loss[0])
-
-
-def _state(eng):
-    return {k: getattr(eng, k).clone() for k in ("master", "vparams", "mom", "vmom", "wshadow")}
-
-
-def _differ(a, b):
-    return [k for k in a if not torch.equal(a[k], b[k])]
-
-
-@pytest.fixture
-def deterministic_cudnn(monkeypatch):
-    monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)
-    monkeypatch.setattr(torch.backends.cudnn, "benchmark", False)
+    return step(eng, engine_batch("ResNet18", eng.step, 32 * eng.accum, DATA_SEED))
 
 
 @pytest.mark.gpu
@@ -213,7 +182,7 @@ def test_decay_is_the_torch_multiply_before_the_lion_step(code, deterministic_cu
         _step(a)
         b.master.mul_(f)          # weights only: vectors live in vparams
         _step(b)
-        assert not _differ(_state(a), _state(b)), (code, _differ(_state(a), _state(b)))
+        assert not differs(_state(a), _state(b)), (code, differs(_state(a), _state(b)))
     assert a.launches_per_step == b.launches_per_step + a.G      # one decay launch per group
     assert bool((a.mom != 0).any()) and bool((a.vmom != 0).any())
     a.close()
@@ -237,14 +206,14 @@ def _run(graph, steps=4, lr_at=None, **kw):
 @pytest.mark.parametrize("code", ["svd", "sgd", "topk"])
 def test_eager_equals_graph_and_reruns(code, deterministic_cudnn):
     e1, e2, g1 = _run(False, **CODES[code]), _run(False, **CODES[code]), _run(True, **CODES[code])
-    assert not _differ(e1, e2) and not _differ(e1, g1), (_differ(e1, e2), _differ(e1, g1))
+    assert not differs(e1, e2) and not differs(e1, g1), (differs(e1, e2), differs(e1, g1))
 
 
 @pytest.mark.gpu
 def test_set_lr_between_replays(deterministic_cudnn):
     eager, graph, plain = _run(False, lr_at=2), _run(True, lr_at=2), _run(True)
-    assert not _differ(eager, graph)
-    assert _differ(graph, plain)        # both the step and the decay factor changed
+    assert not differs(eager, graph)
+    assert differs(graph, plain)        # both the step and the decay factor changed
 
 
 @pytest.mark.gpu
@@ -302,7 +271,7 @@ def test_resume_is_bitwise(code, tmp_path, deterministic_cudnn):
     b.load_checkpoint(d, 2)
     for _ in range(2):
         _step(b)
-    assert not _differ(_state(b), want), _differ(_state(b), want)
+    assert not differs(_state(b), want), differs(_state(b), want)
     b.close()
 
 
@@ -352,19 +321,16 @@ def test_launcher_trains_checkpoints_and_resumes(tmp_path, monkeypatch, capsys):
 # ---------------------------------------------------------------------------------------------------- two GPUs
 def _mp(rank, world, port, out):
     import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
-                      LOCAL_RANK=str(rank))
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
+    nccl_init(rank, world, port)
     from atomo_b200.models import build_model
     from atomo_b200.runtime.shadow_engine import ShadowEngine
     torch.manual_seed(0)
     eng = ShadowEngine(build_model("ResNet18", 10), rank, world, use_graph=True, seed=7, ps_mode="sharded",
                        optimizer="lion", lr=LR, weight_decay=WD, **CODES["svd"])
-    x, y = _batch(rank)
+    x, y = engine_batch("ResNet18", rank, seed=DATA_SEED)
     eng.prepare(x, y, warmup=0)
     for s in range(4):
-        x, y = _batch(1 + s + rank)
+        x, y = engine_batch("ResNet18", 1 + s + rank, seed=DATA_SEED)
         eng.train_step(x, y)
     torch.cuda.synchronize()
     dist.barrier()
@@ -379,16 +345,7 @@ def _mp(rank, world, port, out):
 def test_two_owners_keep_identical_replicas():
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    out = ctx.Queue()
-    procs = [ctx.Process(target=_mp, args=(r, 2, 29740, out)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = sorted((out.get(timeout=600) for _ in range(2)), key=lambda r: r[0])
-    for p in procs:
-        p.join(600)
-        assert p.exitcode == 0
+    res = spawn(2, _mp, 29740)
     assert all(r[1] == 0 for r in res)
     a, b = res
     assert torch.equal(a[2], b[2]) and torch.equal(a[3], b[3]) and torch.equal(a[4], b[4])

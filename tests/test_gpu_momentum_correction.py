@@ -8,8 +8,8 @@ worker's arena words say an entry was sent; ``m = 0, wd = 0`` is top-k + error f
 bitwise; ResNet-18 trains; two ranks stay replicas.
 """
 import argparse
+import functools
 import math
-import os
 
 import numpy as np
 import pytest
@@ -21,7 +21,8 @@ from atomo_b200.optim import momentum_correction as MC
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
 
-from shadow_harness import fit_args, forbid_cuda
+from shadow_harness import deterministic_cudnn, differs, engine_batch, fit_args, forbid_cuda, make_engine, nccl_init, \
+    spawn  # noqa: F401
 
 
 # ---------------------------------------------------------------------------------------------------- CPU
@@ -286,32 +287,12 @@ def test_apply_and_masked_encode_equal_the_oracle_bitwise(nesterov, wd):
 
 
 # ---------------------------------------------------------------------------------------------------- GPU: engine
-@pytest.fixture
-def deterministic_cudnn(monkeypatch):
-    monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)
-    monkeypatch.setattr(torch.backends.cudnn, "benchmark", False)
-
-
-_BATCHES = {}
-
-
-def _batch(net, step, n):
-    from atomo_b200.data import SyntheticImageDataset
-    from atomo_b200.models import input_shape
-    k = (net, step % 4, n)
-    if k not in _BATCHES:
-        x, y = SyntheticImageDataset(input_shape(net), 10, 4096, seed=300 + k[1]).materialize(n)
-        _BATCHES[k] = (x.cuda(), y.cuda())
-    return _BATCHES[k]
+_batch = functools.partial(engine_batch, seed=300)
 
 
 def _engine(net, **kw):
-    from atomo_b200.models import build_model
-    from atomo_b200.runtime.shadow_engine import ShadowEngine
-    torch.manual_seed(0)
-    torch.cuda.set_device(0)
-    kw = dict(dict(code="topk", entry_budget=0.01, error_feedback=True, lr=0.05, momentum=0.9, seed=7), **kw)
-    return ShadowEngine(build_model(net, 10), 0, 1, **kw)
+    return make_engine(net, **dict(dict(code="topk", entry_budget=0.01, error_feedback=True, lr=0.05, momentum=0.9),
+                                   **kw))
 
 
 def _state(eng, losses) -> dict:
@@ -322,11 +303,6 @@ def _state(eng, losses) -> dict:
     for name, t in eng._worker_tensors().items():
         out["worker:" + name] = t.clone()
     return out
-
-
-def _differs(a, b, keys=None):
-    keys = keys or a.keys()
-    return [k for k in keys if not torch.equal(a[k], b[k])]
 
 
 def _run(net, steps, batch=32, warmup=2, load=None, save=None, **kw):
@@ -356,7 +332,7 @@ def test_without_momentum_it_is_top_k_with_error_feedback(net, deterministic_cud
     a, na = _run(net, 20, momentum=0.0, momentum_correction=True)
     b, nb = _run(net, 20, momentum=0.0)
     assert na == nb
-    assert _differs(a, b, ["master", "vparams", "wshadow", "worker:residual", "loss"]) == []
+    assert differs(a, b, ["master", "vparams", "wshadow", "worker:residual", "loss"]) == []
     assert math.isfinite(float(a["loss"][-1]))
 
 
@@ -366,11 +342,11 @@ def test_resume_is_bitwise(tmp_path, deterministic_cudnn, capsys):
     kw = dict(momentum_correction=True, weight_decay=5e-4, nesterov=True)
     d = str(tmp_path) + "/"
     a, _ = _run(net, 2 * K, **kw)
-    assert _differs(a, _run(net, 2 * K, **kw)[0]) == [], "control: two uninterrupted runs differ"
+    assert differs(a, _run(net, 2 * K, **kw)[0]) == [], "control: two uninterrupted runs differ"
     _run(net, K, save=d, **kw)
     c, _ = _run(net, K, load=2 + K, save=d, **kw)
     assert "not restored" not in capsys.readouterr().out
-    assert _differs(dict(a, loss=a["loss"][K:]), c) == []
+    assert differs(dict(a, loss=a["loss"][K:]), c) == []
     assert bool(a["worker:mom"].ne(0).any()) and bool(a["worker:vmom_w"].ne(0).any())
     eng = _engine(net, **dict(kw, momentum_correction=False))       # the sidecar refuses another setting
     try:
@@ -404,10 +380,7 @@ def test_resnet18_trains(deterministic_cudnn):
 # ---------------------------------------------------------------------------------------------------- two GPUs
 def _mp_replicas(rank, world, port, out):
     import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
-                      LOCAL_RANK=str(rank))
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
+    nccl_init(rank, world, port)
     from atomo_b200.data import SyntheticImageDataset
     from atomo_b200.models import build_model
     from atomo_b200.runtime.shadow_engine import ShadowEngine
@@ -439,15 +412,6 @@ def test_two_ranks_stay_replicas():
     every rank."""
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    out = ctx.Queue()
-    procs = [ctx.Process(target=_mp_replicas, args=(r, 2, 29870, out)) for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(300)
-        assert p.exitcode == 0
-    res = sorted(out.get() for _ in range(2))
+    res = spawn(2, _mp_replicas, 29870, timeout=300)
     for rank, err, same, mom in res:
         assert err == 0 and same and mom > 0, res

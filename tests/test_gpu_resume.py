@@ -18,6 +18,8 @@ import torch
 
 from atomo_b200.utils import checkpoint as ckpt
 
+from shadow_harness import deterministic_cudnn, differs, engine_batch, make_engine, nccl_init, spawn  # noqa: F401
+
 N = 3           # steps before and after the interruption
 WARMUP = 2      # eager warm-up steps of runs A and B (they count as steps, as in the launcher)
 
@@ -99,12 +101,6 @@ def test_powersgd_warm_ranges_are_the_tail_of_each_scratch():
 
 
 # ---------------------------------------------------------------------------------------------------- GPU
-@pytest.fixture
-def deterministic_cudnn(monkeypatch):
-    monkeypatch.setattr(torch.backends.cudnn, "deterministic", True)
-    monkeypatch.setattr(torch.backends.cudnn, "benchmark", False)
-
-
 # name -> (network, CUDA graph, warm-up steps of run C before its load, engine arguments)
 SGD = dict(lr=0.05, momentum=0.9)
 ADAM = dict(lr=1e-3, optimizer="adam")
@@ -132,26 +128,13 @@ CASES = {
     "hadamard-ef": ("ResNet18", True, WARMUP, dict(code="hadamard", quantization_level=4, error_feedback=True, **SGD)),
 }
 
-_BATCHES = {}
-
-
 def _batch(net, step):
     """The batch of training step ``step``: the same in every run, different from step to step."""
-    from atomo_b200.data import SyntheticImageDataset
-    from atomo_b200.models import input_shape
-    k = (net, step % 8)
-    if k not in _BATCHES:
-        x, y = SyntheticImageDataset(input_shape(net), 10, 4096, seed=100 + k[1]).materialize(32)
-        _BATCHES[k] = (x.cuda(), y.cuda())
-    return _BATCHES[k]
+    return engine_batch(net, step, seed=100, period=8)
 
 
 def _engine(net, graph, kw, rank=0, world=1, **extra):
-    from atomo_b200.models import build_model
-    from atomo_b200.runtime.shadow_engine import ShadowEngine
-    torch.manual_seed(0)
-    args = dict(kw, **extra)
-    return ShadowEngine(build_model(net, 10), rank, world, use_graph=graph, seed=11, **args)
+    return make_engine(net, rank, world, seed=11, use_graph=graph, **dict(kw, **extra))
 
 
 def _train(eng, net, steps):
@@ -182,11 +165,6 @@ def _state(eng) -> dict:
         out["worker:" + name] = t.cpu()
     out["device_step"] = torch.tensor(eng.device_step())
     return out
-
-
-def _differs(a: dict, b: dict) -> list:
-    assert a.keys() == b.keys()
-    return [k for k in a if not torch.equal(a[k], b[k])]
 
 
 def _run_a(net, graph, kw):
@@ -228,13 +206,13 @@ def test_resume_is_bitwise(case, tmp_path, deterministic_cudnn, capsys):
     net, graph, warm_c, kw = CASES[case]
     a, la = _run_a(net, graph, kw)
     a2, _ = _run_a(net, graph, kw)
-    assert _differs(a, a2) == [], "control: two uninterrupted runs differ"
+    assert differs(a, a2) == [], "control: two uninterrupted runs differ"
     d = str(tmp_path) + "/"
     step = _run_b(net, graph, kw, d)
     assert os.path.exists(ckpt.worker_path(d, step, 0))
     c, lc = _run_c(net, graph, warm_c, kw, d, step)
     assert "not restored" not in capsys.readouterr().out
-    assert _differs(a, c) == []
+    assert differs(a, c) == []
     assert torch.equal(la[N:], lc)
     want = {"svd": ["worker:vprev"], "qsvd": ["worker:vprev"], "powersgd": ["worker:pw_qw", "worker:pw_state"]}
     for k in want.get(kw["code"], []) + (["worker:residual"] if kw.get("error_feedback") else []):
@@ -252,7 +230,7 @@ def test_resume_without_worker_file_differs(tmp_path, deterministic_cudnn, capsy
     c, _ = _run_c(net, graph, warm_c, kw, d, step)
     out = capsys.readouterr().out
     assert out.count("per-worker state of step %d not restored (file missing)" % step) == 1, out
-    diff = _differs(a, c)
+    diff = differs(a, c)
     assert "worker:residual" in diff and "master" in diff, diff
 
 
@@ -278,7 +256,7 @@ def test_mismatched_worker_file_is_not_applied(other, tmp_path, deterministic_cu
     assert fresh.keys() == after.keys() and all(torch.equal(fresh[k], after[k]) for k in fresh)
     c1 = _state_after(eng, net)
     c2, _ = _run_c(net, graph, WARMUP, kw2, d2, step)
-    assert _differs(c1, c2) == []
+    assert differs(c1, c2) == []
 
 
 def _state_after(eng, net):
@@ -291,11 +269,8 @@ def _state_after(eng, net):
 # ---------------------------------------------------------------------------------------------------- two GPUs
 def _mp_resume(rank, world, port, case, d, out):
     import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world),
-                      LOCAL_RANK=str(rank))
-    torch.cuda.set_device(rank)
+    nccl_init(rank, world, port)
     torch.backends.cudnn.deterministic, torch.backends.cudnn.benchmark = True, False
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
     net, graph, warm_c, kw = CASES[case]
     kw = dict(kw, ps_mode="sharded")
 
@@ -315,7 +290,7 @@ def _mp_resume(rank, world, port, case, d, out):
     a = run(2 * N, WARMUP)
     run(N, WARMUP, save=True)
     c = run(N, warm_c, load=WARMUP + N)
-    out.put((rank, _differs(a, c), os.path.exists(ckpt.worker_path(d, WARMUP + N, rank))))
+    out.put((rank, differs(a, c), os.path.exists(ckpt.worker_path(d, WARMUP + N, rank))))
     dist.destroy_process_group()
 
 
@@ -325,15 +300,6 @@ def _mp_resume(rank, world, port, case, d, out):
 def test_resume_is_bitwise_two_gpus_sharded(case, tmp_path):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs >= 2 GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    out = ctx.Queue()
     port = 29610 + list(CASES).index(case)
-    procs = [ctx.Process(target=_mp_resume, args=(r, 2, port, case, str(tmp_path) + "/", out)) for r in range(2)]
-    for p in procs:
-        p.start()
-    for p in procs:
-        p.join(600)
-        assert p.exitcode == 0
-    res = sorted(out.get() for _ in range(2))
+    res = spawn(2, _mp_resume, port, case, str(tmp_path) + "/")
     assert all(diff == [] and has_file for _, diff, has_file in res), res

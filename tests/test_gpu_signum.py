@@ -11,167 +11,14 @@ import pytest
 import torch
 
 from atomo_b200.codings import signum as S
-from atomo_b200.ops import plan2 as P
 from atomo_b200.utils.flags import add_fit_args
 
-from shadow_harness import LoopbackPS, Linear, ef_grads, flat, physical, run_mp, train
-
-# the 1728-element stem, 3x3 convs (one a multiple of the 4096-element tile, one with a half tile), fc layers, tensors
-# whose size is not a multiple of 64 (or of 16), vectors, an all-zero tensor (ZERO), one with +0 / -0 / bf16 subnormals
-# (SIGNED_ZERO) and one that gets a NaN (NAN)
-SHAPES = [(64, 3, 3, 3), (64,), (64, 32, 3, 3), (128, 64, 3, 3), (128,), (96, 64, 3, 3), (10, 512), (7, 20), (5, 3),
-          (10,), (32, 16, 3, 3), (40, 30), (48, 16, 3, 3)]
-ZERO, SIGNED_ZERO, NAN = 10, 11, 12
-
-
-class HSG(LoopbackPS):
-    """Signum: per virtual worker a momentum buffer (beta > 0) and the coin's external uniforms."""
-
-    PS = "v2_ps_signum"
-
-    def __init__(self, shapes, W=1, beta=0.0, lr=0.0625, seed=7, num_aggregate=0, n_groups=1, n_owners=1):
-        super().__init__(shapes, "signum", W, lr, 0.0, 0.0, False, 0, seed, num_aggregate, n_groups, n_owners)
-        pl, z = self.plan, self.zeros
-        self.beta = beta
-        self.wmom = [z(pl.w_total) for _ in range(W)] if beta > 0 else None
-        self.vmom_w = [z(pl.v_total) for _ in range(W)] if beta > 0 else None
-        chunks, self.vec_range = P.vec_chunks(pl)
-        self.t_vchunks = torch.frombuffer(bytearray(chunks or b"\0" * 24), dtype=torch.uint8).to(self.dev)
-        g = torch.Generator(device="cuda").manual_seed(seed + 1)
-        self.unif = [torch.rand(pl.w_total, device=self.dev, generator=g) for _ in range(W)]
-        self.vext = torch.rand(W * pl.v_total, device=self.dev, generator=g)
-        self.ps_tail = (self.vext.data_ptr(), pl.v_total)
-
-    def tensor(self, q, x, g, special=False, who=0, negate=None):
-        if special and q.index == ZERO:
-            x.zero_()
-        elif special and q.index == SIGNED_ZERO:
-            r = torch.rand(q.shape, device=self.dev, generator=g)
-            z = torch.zeros_like(x)
-            x = torch.where(r < 0.3, z, torch.where(r < 0.6, -z, torch.where(r < 0.7, x.sign() * 1e-39, x)))
-        if special and q.index == NAN and who == 0:
-            x = physical(x)
-            flat(x)[100] = float("nan")
-        return x
-
-    def encode(self, w, coin=False):
-        C, pl = self.C, self.plan
-        gptr = self.gptr(w)
-        for g in range(pl.n_groups):
-            t0, nt = pl.enc_range[g]
-            v0, nv = self.vec_range[g]
-            if self.beta == 0:
-                nv = 0
-            C.v2_signum_encode(self.t_units.data_ptr(), self.t_enc.data_ptr(), t0, nt, gptr,
-                               self.t_vchunks.data_ptr() + 24 * v0, nv, self.vgrads[w].data_ptr(),
-                               self.wmom[w].data_ptr() if self.wmom else 0,
-                               self.vmom_w[w].data_ptr() if self.vmom_w else 0, self.beta,
-                               self.t_arena_peer.data_ptr(), self.t_sig_peer.data_ptr(), self.n_owners,
-                               pl.arena_floats, w, g, self.ctrl.data_ptr(), self.counter(g), 0,
-                               g == pl.n_groups - 1, 0 if coin else self.unif[w].data_ptr())
-        torch.cuda.synchronize()
-
-
-class Oracle:
-    """The fp32 numpy oracle of a HSG run: the workers' momenta, the pushed bits per tile, the owners' state."""
-
-    def __init__(self, h):
-        pl = self.plan = h.plan
-        self.h = h
-        self.u = [np.zeros(pl.w_total, np.float32) for _ in range(h.W)]
-        self.uv = [np.zeros(pl.v_total, np.float32) for _ in range(h.W)]
-        self.x, self.xv = [None] * h.W, [None] * h.W
-        self.master = h.master.cpu().numpy().copy()
-        self.vparams = h.vparams.cpu().numpy().copy()
-        self.unif = [t.cpu().numpy() for t in h.unif]
-        self.vext = h.vext.cpu().numpy().reshape(h.W, pl.v_total)
-
-    def push(self, w, phys, coin=False):
-        pl, beta = self.plan, self.h.beta
-        x, xv = np.zeros(pl.w_total, np.float32), np.zeros(pl.v_total, np.float32)
-        for q in pl.params:
-            g = phys[q.index].cpu().numpy().astype(np.float32)
-            sl = slice(q.off, q.off + q.numel)
-            st, dst = (self.u[w], x) if q.is_w else (self.uv[w], xv)
-            if beta > 0:
-                st[sl] = S.momentum_step(st[sl], g, beta)
-                dst[sl] = st[sl]
-            else:
-                dst[sl] = g
-        self.x[w], self.xv[w] = x, xv
-        if coin:
-            self.unif[w] = np.zeros(pl.w_total, np.float32)
-            for u in pl.units:
-                if u.kind == P.KIND_SIGNUM:
-                    self.unif[w][u.w_off:u.w_off + u.numel] = S.coin_uniforms(self.h.seed, u.index,
-                                                                               np.arange(u.numel), self.h.step, w)
-
-    def tile_bits(self, w, u, a, b):
-        sl = slice(u.w_off + a, u.w_off + a + b)
-        return S.bits(self.x[w][sl], self.unif[w][sl]), S.nonfinite(self.x[w][sl])
-
-    def vec_bits(self, w, u, a, b, coin=False):
-        sl = slice(u.w_off + a, u.w_off + a + b)
-        un = S.coin_uniforms(self.h.seed, u.index, np.arange(a, a + b), self.h.step, w) if coin else self.vext[w][sl]
-        return S.bits(self.xv[w][sl], un), S.nonfinite(self.xv[w][sl])
-
-    def ps(self, counted, coin=False):
-        pl, lr = self.plan, np.float32(self.h_lr())
-        for (ui, a, b, o) in pl.ps_tiles:
-            u = pl.units[ui]
-            rows, bad = [], []
-            for w in counted:
-                r, nf = self.vec_bits(w, u, a, b, coin) if u.kind == P.KIND_VEC else self.tile_bits(w, u, a, b)
-                rows.append(r)
-                bad.append(nf)
-            v = S.vote(rows, b, bad)
-            dst = self.vparams if u.kind == P.KIND_VEC else self.master
-            dst[u.w_off + a:u.w_off + a + b] = S.step(dst[u.w_off + a:u.w_off + a + b], v, lr)
-
-    def h_lr(self):
-        return float(self.h.ctrl.view(torch.float32)[2])
-
-
-def _check_push(h, o, w):
-    """Worker w's words, status words and stamps in the owners' arenas, and its momenta, against the oracle."""
-    pl = h.plan
-    arenas = [t.cpu().numpy() for t in h.arenas]
-    for u in pl.units:
-        if u.kind != P.KIND_SIGNUM:
-            continue
-        for j in range(u.n_ps):
-            a, b = 4096 * j, min(4096, u.numel - 4096 * j)
-            ar = arenas[(u.own0 + j) % h.n_owners]
-            base = w * pl.arena_floats + u.slot_off
-            bits, nf = o.tile_bits(w, u, a, b)
-            wo = base + P.qsgd_words_off(u.n_ps, u.rows) + 2 * j * u.cols
-            nw = -(-b // 64)
-            got = ar[wo:wo + 2 * nw].view(np.uint64)
-            assert np.array_equal(got, S.pack(bits)), (u.index, j, w)
-            status = ar[base + P.qsgd_norms_off(u.n_ps) + j]
-            assert (math.isnan(status) if nf else status == 0.0), (u.index, j, w, status)
-            assert int(ar[base:base + u.n_ps].view(np.int32)[j]) == h.step
-    if h.beta > 0:
-        used = np.zeros(pl.w_total, bool)
-        for q in pl.params:
-            if q.is_w:
-                used[q.off:q.off + q.numel] = True
-        got = h.wmom[w].cpu().numpy()
-        assert np.array_equal(got[used], o.u[w][used], equal_nan=True)
-        assert np.array_equal(h.vmom_w[w].cpu().numpy(), o.uv[w], equal_nan=True)
-    assert np.array_equal(h.vgrads[w].cpu().numpy(), o.xv[w], equal_nan=True)
-
-
-def _check_ps(h, o):
-    assert int(h.ctrl.view(torch.int32)[1]) == 0
-    assert np.array_equal(h.master.cpu().numpy(), o.master, equal_nan=True)
-    assert np.array_equal(h.vparams.cpu().numpy(), o.vparams, equal_nan=True)
-    a, b = h.wshadow.float(), torch.from_numpy(o.master).cuda().bfloat16().float()
-    assert torch.equal(a.isnan(), b.isnan()) and torch.equal(a.nan_to_num(), b.nan_to_num())
+from shadow_harness import HSG, NAN, SIGNUM_SHAPES, ZERO, Linear, SignumOracle, ef_grads, run_mp, signum_check_ps, \
+    signum_check_push, train
 
 
 def _run(h, steps, special=False, pushers=None, coin=False, negate=None):
-    o = Oracle(h)
+    o = SignumOracle(h)
     if coin:
         h.ps_tail = (0, 0)          # the owners draw the vectors' coins from Philox too
     for s in range(1, steps + 1):
@@ -187,10 +34,10 @@ def _run(h, steps, special=False, pushers=None, coin=False, negate=None):
                 phys[w] = {k: -v for k, v in phys[src].items()}
             o.push(w, phys[w], coin)
             h.encode(w, coin)
-            _check_push(h, o, w)
+            signum_check_push(h, o, w)
         h.ps()
         o.ps(ws, coin)
-        _check_ps(h, o)
+        signum_check_ps(h, o)
     return h, o
 
 
@@ -201,14 +48,14 @@ def _run(h, steps, special=False, pushers=None, coin=False, negate=None):
 @pytest.mark.parametrize("groups", [1, 3])
 @pytest.mark.parametrize("beta", [0.0, 0.9])
 def test_encode_and_vote_match_oracle_bitwise(W, owners, groups, beta):
-    h = HSG(SHAPES[:10], W=W, beta=beta, n_groups=groups, n_owners=owners, seed=W + 10 * owners)
+    h = HSG(SIGNUM_SHAPES[:10], W=W, beta=beta, n_groups=groups, n_owners=owners, seed=W + 10 * owners)
     _run(h, 3)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("W,beta", [(2, 0.0), (4, 0.9), (3, 0.9)])
 def test_designed_zeros_ties_nan_and_tails(W, beta):
-    h = HSG(SHAPES, W=W, beta=beta, n_owners=2, n_groups=2)
+    h = HSG(SIGNUM_SHAPES, W=W, beta=beta, n_owners=2, n_groups=2)
     init = h.master.cpu().numpy().copy()
     _, o = _run(h, 3, special=True)
     # the NaN of worker 0 makes its tile's vote NaN on every step; its momentum keeps it with beta > 0
@@ -222,14 +69,14 @@ def test_designed_zeros_ties_nan_and_tails(W, beta):
 @pytest.mark.gpu
 @pytest.mark.parametrize("beta", [0.0, 0.9])
 def test_philox_coin_matches_oracle(beta):
-    h = HSG(SHAPES, W=3, beta=beta, n_owners=2)
+    h = HSG(SIGNUM_SHAPES, W=3, beta=beta, n_owners=2)
     _run(h, 2, special=True, coin=True)
 
 
 @pytest.mark.gpu
 def test_nonfinite_vector_makes_its_tile_nan():
-    h = HSG(SHAPES[:10], W=3, beta=0.0)
-    o = Oracle(h)
+    h = HSG(SIGNUM_SHAPES[:10], W=3, beta=0.0)
+    o = SignumOracle(h)
     h.set_step(1)
     q = h.plan.params[1]
     for w in range(3):
@@ -241,7 +88,7 @@ def test_nonfinite_vector_makes_its_tile_nan():
         h.encode(w)
     h.ps()
     o.ps([0, 1, 2])
-    _check_ps(h, o)
+    signum_check_ps(h, o)
     v = h.vparams.cpu().numpy()
     assert np.isnan(v[q.off:q.off + q.numel]).all() and np.isfinite(v[h.plan.params[4].off]).all()
 
@@ -250,13 +97,13 @@ def test_nonfinite_vector_makes_its_tile_nan():
 @pytest.mark.parametrize("beta", [0.0, 0.9])
 def test_num_aggregate_counts_only_fresh_workers(beta):
     """W = 3, --num-aggregate 2: worker 2 pushes at step 1 only, then goes stale; the owners vote with 0 and 1."""
-    h = HSG(SHAPES[:10], W=3, beta=beta, num_aggregate=2, n_owners=2)
+    h = HSG(SIGNUM_SHAPES[:10], W=3, beta=beta, num_aggregate=2, n_owners=2)
     _run(h, 3, pushers=lambda s: [0, 1, 2] if s == 1 else [0, 1])
 
 
 @pytest.mark.gpu
 def test_one_negated_worker_cannot_move_a_three_of_four_majority():
-    h = HSG(SHAPES[:10], W=5, beta=0.0)
+    h = HSG(SIGNUM_SHAPES[:10], W=5, beta=0.0)
     before = h.master.cpu().numpy().copy()
     _, o = _run(h, 1, negate=(4, 0))
     x = np.stack([o.x[w] for w in range(4)])

@@ -6,7 +6,6 @@ import os
 import struct
 import subprocess
 import sys
-import types
 
 import numpy as np
 import pytest
@@ -17,7 +16,7 @@ from atomo_b200.optim import LAMB, LARS
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
 
-from shadow_harness import fit_args, forbid_cuda
+from shadow_harness import SVD3, StandInEngine, fit_args, forbid_cuda
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -127,10 +126,6 @@ def test_engine_refuses_before_cuda_work(kw, match, monkeypatch):
         S.ShadowEngine(None, 0, 1, **kw)
 
 
-def _args(tmp_path, *extra):
-    return fit_args(tmp_path, "--code", "svd", "--svd-rank", "3", *extra)
-
-
 def test_flags_parse():
     a = add_fit_args(argparse.ArgumentParser(), ["--optimizer", "lars", "--trust-coefficient", "0.02"])
     assert a.optimizer == "lars" and a.trust_coefficient == 0.02
@@ -143,7 +138,7 @@ def test_fp32_flat_engine_refuses(opt, tmp_path):
     for extra in (("--engine", "fused", "--dtype", "bf16"), ("--dtype", "fp32"),
                   ("--dtype", "bf16", "--code", "entrywise")):        # auto sends these to the fp32-flat engine
         with pytest.raises(SystemExit, match="--engine shadow"):
-            L._build_engine(_args(tmp_path, "--optimizer", opt, *extra), model, 0, 1)
+            L._build_engine(fit_args(tmp_path, *SVD3, "--optimizer", opt, *extra), model, 0, 1)
 
 
 def test_ctrl2_packing_keeps_every_offset():
@@ -185,54 +180,12 @@ def test_gloo_role_path_trains_with_lamb(tmp_path):
     assert "Master: Step: 6" in r.stdout and os.path.isfile(d + "model_step_6")
 
 
-class StandInEngine:
-    """Plain SGD on the CPU behind the engine interface the launcher uses; records the arguments it was built with."""
-    first_worker, W, is_worker, is_ps, is_owner = 0, 1, True, True, True
-    instances = []
-
-    def __init__(self, model, args):
-        self.model, self.lr, self.step, self.args = model, args.lr, 1, args
-        self.opt = torch.optim.SGD(model.parameters(), lr=args.lr)
-        self.plan = types.SimpleNamespace(factor_bytes_per_worker=lambda: 1 << 20, dense_bytes=lambda: 1 << 18,
-                                          expected_factor_bytes=lambda: 1 << 20)
-        StandInEngine.instances.append(self)
-
-    def prepare(self, x, y, warmup=3):
-        for _ in range(warmup):
-            self.train_step(x, y)
-
-    def set_lr(self, lr):
-        self.lr = lr
-
-    def train_step(self, x, y):
-        self.opt.zero_grad()
-        out = self.model(x)
-        loss = torch.nn.functional.cross_entropy(out, y)
-        loss.backward()
-        self.opt.step()
-        self.step += 1
-        hit = out.argmax(1).eq(y).float().mean() * 100
-        return torch.stack([loss.detach(), hit, hit])
-
-    def phase_stats(self, reset=True):
-        return {"param_wait_us": 10.0, "encode_us": 300.0, "to_push_us": 1500.0}
-
-    def error_code(self):
-        return 0
-
-    def save_checkpoint(self, train_dir, step):
-        pass
-
-    def close(self):
-        pass
-
-
 def test_launcher_loop_with_the_new_flags(tmp_path, monkeypatch, capsys):
     StandInEngine.instances.clear()
     monkeypatch.setattr(L, "_build_engine", lambda args, model, rank, world: (StandInEngine(model, args), "shadow"))
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
-    L.run_p2p_training(_args(tmp_path, "--max-steps", "4", "--optimizer", "lars", "--trust-coefficient", "0.02",
+    L.run_p2p_training(fit_args(tmp_path, *SVD3, "--max-steps", "4", "--optimizer", "lars", "--trust-coefficient", "0.02",
                              "--dtype", "bf16"), device="cpu")
     eng = StandInEngine.instances[-1]
     assert eng.args.optimizer == "lars" and eng.args.trust_coefficient == 0.02 and eng.step == 5

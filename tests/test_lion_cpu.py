@@ -3,9 +3,6 @@
 refusal, and the gloo role path's update against ``optim/lion.py``, with a 2-process run that trains and resumes."""
 import argparse
 import os
-import subprocess
-import sys
-import types
 
 import numpy as np
 import pytest
@@ -17,7 +14,7 @@ from atomo_b200.runtime import master as M
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils.flags import add_fit_args
 
-from shadow_harness import fit_args, forbid_cuda
+from shadow_harness import fit_args, forbid_cuda, role_master, role_run
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 f32 = np.float32
@@ -146,11 +143,7 @@ def test_fp32_flat_engine_refuses(tmp_path):
 
 # ---------------------------------------------------------------------------------------------------- role path
 def _master(tmp_path, wd=0.1, betas=(0.9, 0.99)):
-    m = M.SyncReplicasMaster_NN(types.SimpleNamespace(world_size=2), learning_rate=0.01, network="LeNet",
-                                dataset="MNIST", optimizer="lion", weight_decay=wd, lion_betas=betas,
-                                train_dir=str(tmp_path) + "/")
-    torch.manual_seed(0)
-    return m.build_model(10)
+    return role_master(tmp_path, learning_rate=0.01, optimizer="lion", weight_decay=wd, lion_betas=betas)
 
 
 def test_role_path_update_is_lion(tmp_path):
@@ -172,16 +165,7 @@ def test_role_path_update_is_lion(tmp_path):
         assert all(torch.equal(a, b) for a, b in zip(m.network.parameters(), params))
 
 
-def _role_run(d, port, max_steps, *extra):
-    cmd = [sys.executable, "-m", "atomo_b200.distributed_nn", "--synthetic", "1", "--train-len", "512",
-           "--test-len", "128", "--batch-size", "32", "--lr", "0.01", "--test-batch-size", "64", "--nproc", "2",
-           "--network", "LeNet", "--dataset", "MNIST", "--code", "sgd", "--optimizer", "lion", "--weight-decay",
-           "0.1", "--lion-betas", "0.9", "0.99", "--max-steps", str(max_steps), "--eval-freq", "1", "--train-dir", d,
-           "--master-port", str(port), *extra]
-    env = dict(os.environ, ATOMO_HANG_DUMP_S="400", PYTHONPATH=ROOT, OMP_NUM_THREADS="2", MKL_NUM_THREADS="2")
-    r = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=420)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-    return r.stdout
+ROLE_FLAGS = ("--optimizer", "lion", "--weight-decay", "0.1", "--lion-betas", "0.9", "0.99")
 
 
 def test_gloo_role_path_matches_the_oracle_and_resumes(tmp_path):
@@ -189,8 +173,8 @@ def test_gloo_role_path_matches_the_oracle_and_resumes(tmp_path):
     before by ``optim/lion.py`` on the gradient the momenta imply: with b2 = 0.99 the stored momenta give g exactly
     enough to fix the sign of every c that is not tiny, and the step is then checked bit for bit."""
     d = str(tmp_path) + "/"
-    _role_run(d, 29591, 3)
-    out = _role_run(d, 29592, 5, "--resume", "1")
+    role_run(d, 29591, 3, *ROLE_FLAGS)
+    out = role_run(d, 29592, 5, *ROLE_FLAGS, "--resume", "1")
     assert "Master: Step: 5" in out and "Master: Step: 1," not in out
     load = lambda s: torch.load(d + "model_step_%d_optim" % s, map_location="cpu", weights_only=False)
     net = M.build_model("LeNet", 10, "MNIST")

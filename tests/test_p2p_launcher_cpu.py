@@ -4,47 +4,29 @@ polling, metrics file.  The real engines are exercised by tests/test_gpu_*.py; t
 import argparse
 import json
 import os
-import types
 
 import pytest
-import torch
 
 from atomo_b200.runtime import p2p_launcher as L
 from atomo_b200.utils import checkpoint as ckpt
 from atomo_b200.utils.flags import add_fit_args
 
+import shadow_harness as harness
 
-class StandInEngine:
-    """Trains the model with plain SGD on the CPU behind the engine interface the launcher uses."""
-    first_worker, W, is_worker, is_ps, is_owner = 0, 1, True, True, True
-    instances = []
+
+class StandInEngine(harness.StandInEngine):
+    """Records the LR it is set to, its checkpoints and its close; reports device error 4 after step `fail_at`."""
 
     def __init__(self, model, args, fail_at=0):
-        self.model, self.lr, self.step, self.fail_at = model, args.lr, 1, fail_at
-        self.opt = torch.optim.SGD(model.parameters(), lr=args.lr, momentum=0.0)
-        self.plan = types.SimpleNamespace(factor_bytes_per_worker=lambda: 1 << 20, dense_bytes=lambda: 1 << 18)
+        super().__init__(model, args)
+        self.fail_at = fail_at
         self.lr_history, self.saved, self.closed, self.loaded = [], [], False, None
-        StandInEngine.instances.append(self)
-
-    def prepare(self, x, y, warmup=3):
-        for _ in range(warmup):
-            self.train_step(x, y)
 
     def set_lr(self, lr):
         self.lr = lr
         self.lr_history.append((self.step, lr))
         for g in self.opt.param_groups:
             g["lr"] = lr
-
-    def train_step(self, x, y):
-        self.opt.zero_grad()
-        out = self.model(x)
-        loss = torch.nn.functional.cross_entropy(out, y)
-        loss.backward()
-        self.opt.step()
-        self.step += 1
-        hit = out.argmax(1).eq(y).float().mean() * 100
-        return torch.stack([loss.detach(), hit, hit])
 
     def phase_stats(self, reset=True):
         return {"param_wait_us": 10.0, "encode_us": 300.0, "to_push_us": 1500.0, "to_params_us": 1600.0,
